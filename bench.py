@@ -6,7 +6,7 @@
 
 A "step" is one pass of the hot path (K1 scan -> K2 resolve -> K3 SHA-256 -> K4 probe) over one
 batch = BASELINE config[1]: 1024 x 64 MiB synthetic files per GPU, resident in HBM, generated on
-the device before the timed region (inputs are 64 GiB >> 126 MB L2, so no L2 flush is needed).
+the device before the timed region (inputs are 64 GiB >> the H100's 50 MB L2, so no L2 flush is needed).
 Steps are submitted asynchronously (the C ABI's submit/wait form) so the serial SHA-256 tail of
 one batch's longest chunk overlaps the next batch; all K steps complete inside the timed region.
 One JSON line on stdout (rank 0).  See DESIGN.md "Measurement".
@@ -42,7 +42,7 @@ def measured_peaks():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not a measured rate)"
 
 
 class ClockSampler:
@@ -97,17 +97,18 @@ class ClockSampler:
 
 
 def instr_ceiling(sm_total, sm_mhz, value_gbs):
-    """Integer-pipe bound of SHA-256 on this GPU.  Every one of the chip's SMs runs SHA work (124 the bulk kernel, 24
-    the long-chunk kernel), so the bound counts ALL of them: 64 ALU-pipe thread-instructions / clk / SM
-    (profiles/r01_microbench.txt) over the ALU instructions per byte of the shipped kernel
-    (profiles/r02_sass_mix.txt: loop of k_sha_tuned<2>, 1228 ALU-pipe instructions per 64 B block)."""
+    """Integer-pipe bound of SHA-256 on this GPU.  Every one of the chip's SMs runs SHA work (on an H100 108 the bulk
+    kernel, 24 the long-chunk kernel), so the bound counts ALL of them: 64 ALU-pipe thread-instructions / clk / SM
+    (4 x 16 INT32 lanes per SM) over the ALU instructions per byte of the shipped kernel (the 64 B block loop of
+    k_sha_tuned<2> in the sm_90a SASS holds 1228 ALU-pipe instructions: `python tools/sass_mix.py
+    pbs_plus_b200/_obj/sha256.cu.o k_sha_tuned`)."""
     if not sm_mhz:
         return None
     alu_per_block = 1228.0
     gbs = sm_total * 64 * float(sm_mhz) * 1e6 / (alu_per_block / 64.0) / 1e9
     return {"alu_pipe_GBps": gbs, "frac_of_alu_pipe": value_gbs / gbs if gbs else None, "sm_count": sm_total,
             "alu_instr_per_64B": alu_per_block,
-            "source": "profiles/r02_sass_mix.txt (SASS count), profiles/r01_microbench.txt (64 thread-ops/clk/SM)"}
+            "source": "tools/sass_mix.py on the sm_90a object (SASS count), 64 INT32 thread-ops/clk/SM"}
 
 
 def union_ms(intervals):
@@ -232,7 +233,7 @@ def h2d_roofline(torch, host_arr, nbytes=8 << 30):
     return best
 
 
-def run_distinct(args, eng, pg, torch, cfg, total_gib=768, batch_files=256, nbuf=7, early=True):
+def run_distinct(args, eng, pg, torch, cfg, total_gib=768, batch_files=256, nbuf=3, early=True):
     """value_distinct: the same path over NON-REPEATING data (the cfg3 corpus): every batch is generated on the device,
     hashed ONCE, and its buffer is refilled as soon as the device no longer reads it -- with `early` (the default,
     PBSGPU_BATCH_EARLY_INPUT) that is when the bulk pass and the copy of the long chunks into the library's arena are done,
@@ -327,6 +328,29 @@ def run_distinct(args, eng, pg, torch, cfg, total_gib=768, batch_files=256, nbuf
             "generation_share_if_serial": (n_batches * gen_alone) / wall,
             "workload": "cfg3 corpus (seed 3, 30 % duplicate 4 MiB blocks in runs of 8), every byte generated on the device and "
                         "hashed once; generation runs concurrently in a second context and is INSIDE the wall time"}
+
+
+DUMP_LIMIT = 64_000_000      # bytes of all files together, .npy headers included
+DUMP_HEADERS = 64 << 10      # reserved for the five .npy headers (128 B each in practice)
+
+
+def dump_outputs(out_dir, rec):
+    """Writes the chunk records the timed path returned for its last step, one float64 .npy per field (every value is
+    exact in float64: stream ids, flags, end offsets < 2^53, digest bytes), so two builds can be compared record for
+    record.  Where the files would exceed DUMP_LIMIT, a fixed seeded sample of the records is written with its row
+    indices."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    row_bytes = 8 * (3 + 32 + 1)
+    max_rows = (DUMP_LIMIT - DUMP_HEADERS) // row_bytes
+    rows = np.arange(len(rec))
+    if len(rec) > max_rows:
+        rows = np.sort(np.random.default_rng(0).choice(len(rec), max_rows, replace=False))
+    sel = rec[rows]
+    arrays = {"stream": sel["stream"], "flags": sel["flags"], "end_off": sel["end_off"], "digest": sel["digest"],
+              "rows": rows}
+    for name, a in arrays.items():
+        np.save(d / f"{name}.npy", np.asarray(a, dtype=np.float64))
 
 
 def expected_cfg4_hits(world, n_files, file_mib):
@@ -466,6 +490,8 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     step_bytes = n_files * file_len
     value = world * step_bytes * args.steps / (ms / 1e3) / GIB
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, results[-1][0])
     timings = [r[1] for r in results]
     n_chunks = int(timings[0]["chunks"])
     hit_last = float((results[-1][2] != 0).mean()) if len(results[-1][2]) else 0.0
@@ -474,7 +500,6 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     sha_union = union_ms([(t["sha_t0"], t["sha_t1"]) for t in timings])
     scan_union = union_ms([(t["scan_t0"], t["scan_t1"]) for t in timings])
     peak, peak_src = measured_peaks()
-    traffic = ncu_traffic() if (n_files == 1024 and args.file_mib == 64) else None
     # the roofline line follows from the SAME clock as `value`: algorithmic bytes of one step (per GPU) / ms_per_step
     step_gbs = step_bytes / (ms / args.steps / 1e3) / 1e9
     sha_gbs = step_bytes * args.steps / (sha_union / 1e3) / 1e9 if sha_union > 0 else 0.0
@@ -487,7 +512,7 @@ def run_ours(args, rank: int, local_rank: int, world: int):
         "config": {
             "workload": wl,
             "reduced_to_fit_hbm": reduced, "chunks_per_step": n_chunks, "parallelism": f"files sharded x{world}",
-            "l2": "inputs (>= 64 GiB) far exceed the 126 MB L2; no flush needed",
+            "l2": "inputs (>= 64 GiB) far exceed the H100's 50 MB L2; no flush needed",
             "pipelining": "K steps submitted asynchronously over the SAME resident batch (13 stream slots, FIFO per slot); all "
                           "complete inside the timed region; see value_distinct for non-repeating data",
             "inflight": args.inflight or args.steps, "sm_partition(long,bulk,scan)": list(eng.partition_info()) + [eng.scan_partition_sms()],
@@ -499,7 +524,6 @@ def run_ours(args, rank: int, local_rank: int, world: int):
         "roofline": {
             "bound": "hbm", "kernel": "k_sha_tuned / k_sha_split (K3, dominant; instruction-bound integer work, see DESIGN.md)",
             "achieved": step_gbs, "peak": peak, "unit": "GB/s", "frac": step_gbs / peak,
-            "traffic": traffic["total"] if traffic else None, "traffic_detail": traffic,
             "algorithmic_bytes_per_launch": step_bytes, "peak_source": peak_src,
             "how": "algorithmic bytes of one step on one GPU (1 per input byte) / ms_per_step (the driver-checkable clock: "
                    "CUDA events around the K timed steps, max over ranks); all kernels of the step included",
@@ -600,8 +624,8 @@ def run_ours(args, rank: int, local_rank: int, world: int):
 
 def run_cfg3(args):
     """BASELINE config[2]: a 10 TB synthetic corpus with 30 % duplicate 4 MiB blocks (runs of 8), streamed
-    through HBM in 32 GiB batches (3 in flight) generated on the device; reports throughput and the hit rate.
-    Not the default bench line (diagnostic / parity-at-scale run; see profiles/)."""
+    through HBM in 16 GiB batches (3 in flight, 48 GiB of an 80 GB H100) generated on the device; reports throughput
+    and the hit rate.  Not the default bench line (diagnostic / parity-at-scale run)."""
     import torch
 
     import pbs_plus_b200 as pg
@@ -609,7 +633,7 @@ def run_cfg3(args):
     torch.cuda.set_device(0)
     eng = pg.Engine(0, profiling=False)
     file_len = args.file_mib << 20
-    n_files = min(args.files, 512)                 # 32 GiB batches, NBUF of them in flight
+    n_files = min(args.files, 256)                 # 16 GiB batches, NBUF of them in flight
     NBUF = 3
     total = int(args.total_tb * 1e12)
     n_batches = max(1, total // (n_files * file_len))
@@ -674,11 +698,16 @@ def run_e2e(args, eng, cfg, pg, torch, first_file=0):
             if n <= 64:
                 return {"value": None, "unit": "GiB/s", "error": str(e)}
             n //= 2
-    # fill the pinned buffer with the same corpus (generated on the device, copied back once, untimed)
-    tmp = torch.empty(n * file_len, dtype=torch.uint8, device="cuda")
-    eng.corpus_fill(pg.corpus(seed=2, file_len=file_len), first_file, n, tmp, file_len)
-    torch.from_numpy(np.asarray(host)).copy_(tmp)
-    del tmp
+    # fill the pinned buffer with the same corpus (generated on the device, copied back once, untimed), 8 GiB at a
+    # time: the whole step does not fit on an 80 GB device next to the context's long-chunk arena
+    grp = max(1, min(n, (8 << 30) // file_len))
+    tmp = torch.empty(grp * file_len, dtype=torch.uint8, device="cuda")
+    host_t = torch.from_numpy(np.asarray(host))
+    for f0 in range(0, n, grp):
+        k = min(grp, n - f0)
+        eng.corpus_fill(pg.corpus(seed=2, file_len=file_len), first_file + f0, k, tmp, file_len)
+        host_t[f0 * file_len:(f0 + k) * file_len].copy_(tmp[:k * file_len])
+    del tmp, host_t
     torch.cuda.empty_cache()
     off = np.arange(n, dtype=np.uint64) * file_len
     ln = np.full(n, file_len, dtype=np.uint64)
@@ -725,34 +754,6 @@ def run_e2e(args, eng, cfg, pg, torch, first_file=0):
                          "peak_source": "pinned host -> device copy of 8 GiB measured in this run on this box (best of 3, CUDA events)"},
             "workload": f"{n} x {args.file_mib} MiB files of the cfg2 corpus per step (one blocking C-ABI call) from "
                         f"pinned host memory; PCIe-bound", "timer": "host wall clock around the blocking C-ABI calls"}
-
-
-def ncu_traffic():
-    """dram bytes (read + write) per launch of EVERY kernel class of the step, from the committed ncu --set full
-    summaries of one 64 GiB batch: K1 scan reads the input once, K3 (bulk + long-chunk kernel) reads it again."""
-    import re
-    files = {"K1_scan": ("r02_ncu_batch_k_scan_tuned.txt",), "K3_sha_bulk": ("r02_ncu_batch_k_sha_tuned.txt",), "K3_sha_long": ("r02_ncu_batch_k_sha_split.txt",)}
-    out, tot = {}, 0.0
-    for key, names in files.items():
-        for name in names:
-            p = ROOT / "profiles" / name
-            if not p.exists():
-                return None
-            txt = p.read_text()
-            b = 0.0
-            for m in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                mm = re.search(m + r"\s+(\w+)\s+([0-9.]+)", txt)
-                scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}.get(mm.group(1)) if mm else None
-                if scale is None:
-                    return None
-                b += float(mm.group(2)) * scale
-            out[key] = b
-            tot += b
-    alg = 1024 * (64 << 20)
-    out.update({"total": tot, "algorithmic": alg, "ratio_to_algorithmic": tot / alg,
-                "source": "profiles/r02_ncu_batch_k_scan_tuned.txt + r02_ncu_batch_k_sha_tuned.txt + r02_ncu_batch_k_sha_split.txt (ncu --set full of one launch each inside `bench.py --steps 2`, one 64 GiB batch); "
-                          "the input is read twice (K1, then K3): 2.0 x the algorithmic bytes; K7 (xxh3) is not part of the step"})
-    return out
 
 
 def run_cfg4verify(args):
@@ -806,7 +807,8 @@ def main():
     ap.add_argument("--no-verify", action="store_true", help="skip the untimed post-run comparison with the oracle")
     ap.add_argument("--no-distinct", action="store_true", help="skip the non-repeating-data figure (value_distinct)")
     ap.add_argument("--distinct-gib", type=int, default=768)
-    ap.add_argument("--distinct-bufs", type=int, default=7, help="16 GiB input buffers of the value_distinct run")
+    ap.add_argument("--distinct-bufs", type=int, default=3,
+                    help="16 GiB input buffers of the value_distinct run (3 leave room for the arena on an 80 GB H100)")
     ap.add_argument("--distinct-batch-files", type=int, default=256, help="files (of --file-mib) per batch of the value_distinct run")
     ap.add_argument("--distinct-early", type=int, default=1, help="0: value_distinct without PBSGPU_BATCH_EARLY_INPUT")
     ap.add_argument("--total-tb", type=float, default=10.0, help="cfg3 only")
@@ -816,6 +818,8 @@ def main():
                          "stream slots then queue them FIFO per stream, which keeps the GPU fed without the host)")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the chunk records of the last timed step to DIR/<field>.npy (float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

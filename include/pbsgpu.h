@@ -1,5 +1,5 @@
 /*
- * pbsgpu.h -- C ABI of libpbsgpu.so, the B200-native chunk + digest + probe engine.
+ * pbsgpu.h -- C ABI of libpbsgpu.so, the H100-native chunk + digest + probe engine.
  *
  * This is the drop-in boundary for the ONE hot path of pbs-plus that this repo
  * accelerates (SURVEY.md section 8): content-defined chunking (buzhash), per-chunk

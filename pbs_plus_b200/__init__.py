@@ -1,4 +1,4 @@
-"""pbs_plus_b200 -- B200-native chunk + digest + probe engine behind pbs-plus's chunker surface.
+"""pbs_plus_b200 -- H100-native chunk + digest + probe engine behind pbs-plus's chunker surface.
 
 Only the ONE hot path of SURVEY.md section 8: buzhash boundary scan, per-chunk SHA-256,
 known-digest probe.  The product is libpbsgpu.so (csrc/, C ABI in include/pbsgpu.h);

@@ -1,4 +1,4 @@
-"""Builds libpbsgpu.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libpbsgpu.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m pbs_plus_b200.build [--force]
 
@@ -19,8 +19,9 @@ LIB = HERE / "libpbsgpu.so"
 SOURCES = ["scan.cu", "resolve.cu", "sha256.cu", "digestset.cu", "crc32.cu", "xxh3.cu", "corpus.cu", "capi.cu", "capi_set.cu",
            "capi_stream.cu", "capi_aux.cu", "zframe.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    *ARCH, "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -32,6 +33,10 @@ def _deps(src: Path) -> float:
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     OBJ.mkdir(exist_ok=True)
+    # objects compiled with other flags (another architecture) are stale whatever their mtime
+    stamp = OBJ / "flags.txt"
+    if not stamp.exists() or stamp.read_text() != " ".join(FLAGS):
+        force = True
     jobs = []
     for name in SOURCES:
         src, obj = CSRC / name, OBJ / (name + ".o")
@@ -50,8 +55,8 @@ def build(force: bool = False, verbose: bool = False) -> Path:
                 print(out)
     objs = [str(OBJ / (n + ".o")) for n in SOURCES]
     if jobs or not LIB.exists():
-        run([NVCC, "-shared", "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a",
-             "-Xcompiler", "-fPIC", "-o", str(LIB), *objs, "-ldl"])
+        run([NVCC, "-shared", "-cudart", "static", *ARCH, "-Xcompiler", "-fPIC", "-o", str(LIB), *objs, "-ldl"])
+    stamp.write_text(" ".join(FLAGS))
     return LIB
 
 

@@ -299,7 +299,6 @@ extern "C" int pbsgpu_open(int device, pbsgpu_ctx **out) {
         // default: 24 SMs reserved for the long-chunk latency kernels (green contexts); 0 disables
         const int want_part = env_int("PBSGPU_PARTITION_SMS", 24);
         // + PBSGPU_SCAN_SMS SMs that run only the front halves (K1 scan / sort / K2); default 0 = scans share the bulk partition
-        // (measured: a dedicated scan partition of 16-32 SMs LOWERS the pipelined throughput by 15-25 %, profiles/r02_partition3.txt)
         const int want_scan = env_int("PBSGPU_SCAN_SMS", 0);
         const bool partitioned = want_part > 0 && want_part + 8 <= ctx->sm_count && make_partition(ctx, want_part, want_scan);
         bool ok = true;
@@ -583,7 +582,7 @@ static bool arena_reserve(pbsgpu_job *j, cudaStream_t side) {
 
 // The hybrid SHA launch pays off when the long-chunk kernels have SMs of their own (partition); without
 // a partition their CTAs pin shared memory for ~0.3 s and starve the whole-SM scan CTAs of later batches
-// (measured: 163 vs 143 ms/step).  PBSGPU_SHA_HYBRID=2 forces it on regardless, 0 turns it off.
+// and the pipelined step gets slower.  PBSGPU_SHA_HYBRID=2 forces it on regardless, 0 turns it off.
 static bool hybrid_for(const pbsgpu_ctx *ctx) {
     if (ctx->tune.mode >= 10 || ctx->tune.hybrid == 0) return false;
     return ctx->part_sms > 0 || ctx->tune.hybrid == 2;

@@ -73,7 +73,7 @@ struct pbsgpu_ctx {
     // kernels of long chunks (streams2), everything else runs on the remaining SMs (streams)
     // Round 2: an optional THIRD partition (PBSGPU_SCAN_SMS, default off) runs only the front halves: K1 is a whole-SM
     // persistent kernel (207 KB of shared memory, 49 k registers per CTA) that cannot be placed on an SM holding SHA
-    // blocks.  Measured 15-25 % SLOWER than sharing the bulk partition (profiles/r02_partition3.txt).
+    // blocks.
     int part_sms = 0, bulk_sms = 0, scan_sms = 0;
     CUgreenCtx g_long = nullptr, g_bulk = nullptr, g_scan = nullptr;
     // knobs, read from the environment ONCE PER CONTEXT in pbsgpu_open (never process-wide statics)
@@ -90,7 +90,7 @@ struct pbsgpu_ctx {
     struct ArenaRec { uint64_t lo, hi; cudaEvent_t ev; };
     uint8_t *arena = nullptr;
     uint64_t arena_bytes = 0, arena_cursor = 0;
-    uint64_t arena_want = 32ull << 30;        // PBSGPU_ARENA_MB
+    uint64_t arena_want = 16ull << 30;        // PBSGPU_ARENA_MB (a fifth of an 80 GB H100; halved until it fits)
     int arena_frac_x16 = 3;                   // PBSGPU_ARENA_FRAC_X16
     bool arena_failed = false;
     std::deque<ArenaRec> arena_recs;
@@ -110,8 +110,8 @@ int pbsgpu_fail(pbsgpu_ctx *c, int code, const char *fmt, ...);
 // one call at a time per ctx + device binding for this OS thread (goroutines migrate).  The caller's binding is restored
 // on exit so a host framework that tracks the current device (torch) is not retargeted behind its back -- but ONLY a
 // binding the thread really had: a thread that never touched CUDA reports "device 0" from cudaGetDevice, and restoring
-// that with cudaSetDevice(0) would CREATE a primary context on GPU 0 in every process of a multi-GPU job (measured: the
-// e2e leg of ranks 1..7 then waits seconds for context creation on rank 0's busy GPU, profiles/r02_e2e_multirank.txt).
+// that with cudaSetDevice(0) would CREATE a primary context on GPU 0 in every process of a multi-GPU job (the
+// e2e leg of ranks 1..7 then waits for context creation on rank 0's busy GPU).
 // Such a thread is returned to "no context" (cuCtxSetCurrent(NULL)).
 struct Guard {
     std::lock_guard<std::recursive_mutex> lk;

@@ -1,4 +1,4 @@
-// pbs_plus_b200/csrc/scan.cu -- K1: buzhash boundary-candidate scan (sm_100a).
+// pbs_plus_b200/csrc/scan.cu -- K1: buzhash boundary-candidate scan (sm_90a).
 //
 // Replaces the byte-at-a-time rolling-hash loop the reference runs inside
 // transfer.ArchiveWriter.WriteEntryReader (reference internal/pxarmount/commit.go:720,
@@ -580,7 +580,7 @@ cudaError_t launch_scan_lanes(const ScanArgs &a, const uint32_t *rot_table, int 
         encode = (tmap_encode_fn)fn;
     }
     // u8 tensor over the batch: dim0 = 128 contiguous bytes, dim1 = 128 B unit index, dim2 = lane (stride 2 KiB),
-    // dim3 = half (stride 128 B); overlapping strides on purpose (profiles/r02_tma_tensor_probe.txt)
+    // dim3 = half (stride 128 B); overlapping strides on purpose
     CUtensorMap tmap;
     const cuuint64_t units = extent / 128 ? extent / 128 : 1;
     const cuuint64_t dims[4] = {128, units, 32, 2};

@@ -1,4 +1,4 @@
-// pbs_plus_b200/csrc/sha256.cu -- K3: batched per-chunk SHA-256 (FIPS 180-4), sm_100a.
+// pbs_plus_b200/csrc/sha256.cu -- K3: batched per-chunk SHA-256 (FIPS 180-4), sm_90a.
 //
 // Replaces the per-chunk digest the reference's dedup writer computes for every chunk
 // cut inside transfer.ArchiveWriter.WriteEntryReader (reference
@@ -156,7 +156,7 @@ cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st) {
 //     though the kernel is ALU bound), next block prefetched while the current one is
 //     compressed; the per-lane word misalignment is undone by a 2-stage SEL network and
 //     the byte misalignment + endian swap by ONE PRMT per word;
-//   * pipe balancing: B200's integer work splits over the ALU pipe (LOP3/SHF/PRMT/IADD3)
+//   * pipe balancing: the SM's integer work splits over the ALU pipe (LOP3/SHF/PRMT/IADD3)
 //     and the FMA pipe (IMAD), 64 lanes/clk/SM each.  ptxas puts almost all of SHA-256 on
 //     the ALU pipe.  Multiplying by constants the compiler cannot see (kernel arguments
 //     1, 2^29, 2^22, 2^7) forces the additions (a*1+b), the two logical shifts of the
@@ -441,7 +441,7 @@ cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t
 
 // latency kernel (producer/consumer warps).
 // When it is launched next to a kernel that already occupies every SM, the CTA scheduler packs its
-// few CTAs onto a handful of SMs (measured: 4x slower than on an empty GPU).  In the hybrid launch
+// few CTAs onto a handful of SMs, where they run several times slower than on an empty GPU.  In the hybrid launch
 // (part 1) each CTA therefore also asks for `spread_kb` KiB of dummy dynamic shared memory, which caps the
 // CTAs per SM (30 -> 4, 85 -> 2, 112 -> 1) and forces the spread; the throughput kernel uses no shared
 // memory and still co-resides.
@@ -585,7 +585,7 @@ __global__ void __launch_bounds__(256) k_arena_gather(ShaArgs a, uint8_t *arena,
 }
 cudaError_t launch_arena_gather(const ShaArgs &a, uint8_t *arena, const uint64_t *arena_off, int sms, cudaStream_t st) {
     if (a.chunk_cap == 0) return cudaSuccess;
-    k_arena_gather<<<(unsigned)(sms > 0 ? sms : 148) * 4, 256, 0, st>>>(a, arena, arena_off);
+    k_arena_gather<<<(unsigned)(sms > 0 ? sms : 132) * 4, 256, 0, st>>>(a, arena, arena_off);
     return cudaGetLastError();
 }
 

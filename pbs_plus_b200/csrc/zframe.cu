@@ -1,4 +1,4 @@
-// f3: zstd framing of constant runs for DataBlobs (sm_100a).
+// f3: zstd framing of constant runs for DataBlobs (sm_90a).
 //
 // PBS stores a chunk as a zstd-compressed DataBlob when that is smaller than the raw one (upstream pbs-datastore
 // data_blob.rs `DataBlob::encode`; magic = sha256("Proxmox Backup zstd compressed blob v1.0")[0..8]).  The entropy

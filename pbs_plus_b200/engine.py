@@ -1,9 +1,9 @@
-"""Host-side front end of the B200 chunk + digest + probe engine.
+"""Host-side front end of the H100 chunk + digest + probe engine.
 
 Thin, allocation-free wrappers over the C ABI (include/pbsgpu.h).  Device memory
 comes from the caller (e.g. a torch CUDA tensor -- torch is plumbing only) or the
 library stages host memory itself.  No CPU fallback: everything below runs the
-sm_100a kernels in pbs_plus_b200/csrc/.
+sm_90a kernels in pbs_plus_b200/csrc/.
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # a fresh checkout has no built artefacts (they are git-ignored): build them once, in-tree
     lib = ROOT / "pbs_plus_b200" / "libpbsgpu.so"
     if not lib.exists() or not (ROOT / "tests" / "cxx" / "driver.bin").exists():

@@ -660,7 +660,7 @@ def test_calls_leave_the_callers_current_device_alone(eng, torch):
     eng.sha256_batch(rnd(1000, 1), [0], [1000])
     assert torch.cuda.current_device() == before
     # a thread that never touched CUDA must be left WITHOUT a context: "restoring" cudaGetDevice()'s default 0 would create
-    # a primary context on GPU 0 in every rank of a multi-GPU job (profiles/r02_e2e_multirank.txt)
+    # a primary context on GPU 0 in every rank of a multi-GPU job
     try:
         from cuda import cuda as cu
     except Exception:

@@ -9,7 +9,7 @@ mkdir -p gpurun_out
 export CUDA_DEVICE_MAX_CONNECTIONS=32
 timeout 900 python -m pytest tests -x -q -m gpu > gpurun_out/r2_pytest_gpu.txt 2>&1; echo "pytest rc=$?" >> gpurun_out/r2_pytest_gpu.txt; tail -3 gpurun_out/r2_pytest_gpu.txt
 timeout 300 python __graft_entry__.py smoke 2>&1 | tail -1 | tee gpurun_out/r2_smoke.txt
-[ -x tools/tma_tensor_probe.bin ] || nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/tma_tensor_probe.bin tools/tma_tensor_probe.cu
+[ -x tools/tma_tensor_probe.bin ] || nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/tma_tensor_probe.bin tools/tma_tensor_probe.cu
 timeout 120 ./tools/tma_tensor_probe.bin 2>&1 | tee gpurun_out/r2_tma_tensor_probe.txt
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:k_xxh3_ -c 2 -f -o gpurun_out/prof_xxh3 \
     python tools/xxh3_bench.py 8 > gpurun_out/r2_ncu_xxh3.log 2>&1; tail -2 gpurun_out/r2_ncu_xxh3.log

@@ -1,6 +1,6 @@
 #!/bin/bash
-# Round 2, call R: CTAs per SM of the latency kernel (PBSGPU_SPLIT_SPREAD_KB 30 -> 4, 85 -> 2) x size of its partition: the load
-# curve (profiles/r02_sha_lab_load_split.txt) says 4 CTAs per SM run a chain at 2.25 us per block, 2 at 1.37.
+# Round 2, call R: CTAs per SM of the latency kernel (PBSGPU_SPLIT_SPREAD_KB 30 -> 4, 85 -> 2) x size of its partition: fewer CTAs
+# per SM run each chain faster.
 mkdir -p gpurun_out
 export CUDA_DEVICE_MAX_CONNECTIONS=32
 PBSGPU_PARTITION_SMS=32 PBSGPU_SPLIT_SPREAD_KB=85 timeout 600 python -m pytest tests/test_gpu_round2.py tests/test_gpu_parity.py -q -x -k "cfg2 or early or async or knobs or partition or stream" > gpurun_out/r2r_pytest_p32s85.txt 2>&1; echo "pytest rc=$?" >> gpurun_out/r2r_pytest_p32s85.txt; tail -3 gpurun_out/r2r_pytest_p32s85.txt

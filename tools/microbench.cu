@@ -1,5 +1,5 @@
 // tools/microbench.cu -- pipe-throughput and TMA-capability probes for design decisions
-// (measurement aid, not product).  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench.bin tools/microbench.cu
+// (measurement aid, not product).  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench.bin tools/microbench.cu
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,12 +1,12 @@
 // tools/sha_lab.cu -- K3 instruction-mix laboratory (measurement aid, not product).
 //
 // SHA-256 on CUDA cores is bound by the two integer pipes of an SM sub-partition (ALU: SHF/LOP3/IADD3/PRMT/SEL,
-// FMA: IMAD; one warp instruction per 2 clk each, one issue per clk in total -- profiles/r01_microbench.txt).
+// FMA: IMAD).
 // This program times variants of the one-lane-per-range kernel that differ ONLY in which pipe their additions and
 // logical shifts are sent to and in the launch shape, on N equal ranges (no length imbalance), and checks every
 // digest against variant 0 (which is checked against a host SHA-256).  `tools/sass_mix.py` counts the loop's SASS
 // per pipe for the same variants.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o tools/sha_lab.bin tools/sha_lab.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o tools/sha_lab.bin tools/sha_lab.cu
 //   ./tools/sha_lab.bin mix [range_kib=256] [total_gib=16] [only_variant=-1]   instruction mixes at saturation
 //   ./tools/sha_lab.bin load [chain_kib=1024]                                  chain latency and GB/s vs number of concurrent chains
 #include <cuda_runtime.h>
@@ -294,7 +294,7 @@ int main(int argc, char **argv) {
         }
     } else if (!strcmp(mode, "load")) {
         // load curve: C concurrent chains of equal length; time per 64 B block of a chain = the chain latency that bounds
-        // a batch's makespan, GB/s = throughput at that load.  C = 148 SMs x 4 sub-partitions x 32 lanes x {1/4 .. 8} warps.
+        // a batch's makespan, GB/s = throughput at that load.  C = 132 SMs x 4 sub-partitions x 32 lanes x {1/4 .. 8} warps.
         const uint64_t chain = (argc > 2 ? atoll(argv[2]) : 1024) << 10;   // bytes per chain
         int picks[7] = {0, 3, 4, -1, -1, -1, -1};                               // v0, v11, v27, then tuned<2>, split<3,0>, split<3,1> by name
         for (int v = 0; v < NV; v++) {

@@ -1,9 +1,8 @@
-// tools/tma_tensor_probe.cu -- round-2 planning aid for K1 (DESIGN.md 5c item 2).  NOT RUN YET (written after the
-// round-1 GPU budget was spent): first thing to run in round 2:
-//     nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/tma_tensor_probe.bin tools/tma_tensor_probe.cu
-//     gpurun -- ./tools/tma_tensor_probe.bin
+// tools/tma_tensor_probe.cu -- planning aid for K1's lane-contiguous variant.
+//     nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/tma_tensor_probe.bin tools/tma_tensor_probe.cu
+//     ./tools/tma_tensor_probe.bin
 // Question: can ONE tensor-map TMA per warp step replace the 32 per-lane bulk copies of k_scan_lanes (which cost
-// ~560 warp-instructions per step, profiles/r01_scan_lanes.txt)?  The copy has to gather, for step k of a 64 KiB
+// ~560 warp-instructions per step)?  The copy has to gather, for step k of a 64 KiB
 // super-tile, the 256 B piece [L*2048 + k*256, +256) of every lane L and lay it out so that a quarter-warp's
 // LDS.128 is bank-conflict free.
 //   tensor map (u8): dim0 = 128 contiguous bytes, dim1 = 128 B unit index (stride 128: any 128 B aligned start),
