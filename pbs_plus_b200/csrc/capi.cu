@@ -270,7 +270,6 @@ extern "C" int pbsgpu_open(int device, pbsgpu_ctx **out) {
     pbsgpu_ctx *ctx = new pbsgpu_ctx();
     ctx->device = device;
     ctx->dev.pinned = false; ctx->pin.pinned = true;
-    memset(&ctx->last_timing, 0, sizeof ctx->last_timing);
     int rc = PBSGPU_OK;
     do {
         if (cudaSetDevice(device) != cudaSuccess || cudaGetDeviceProperties(&ctx->prop, device) != cudaSuccess) { rc = PBSGPU_ENODEV; break; }
@@ -385,26 +384,30 @@ cudaError_t pbsgpu_job_sync(pbsgpu_job *j) {   // everything the job enqueued, o
     if (j->st && (r = cudaStreamSynchronize(j->st)) != cudaSuccess) e = r;
     if (j->st2 && (r = cudaStreamSynchronize(j->st2)) != cudaSuccess) e = r;
     if (j->st3 && (r = cudaStreamSynchronize(j->st3)) != cudaSuccess) e = r;
-    if (j->enqueued && j->have_events && (r = cudaEventSynchronize(j->ev[EV_END])) != cudaSuccess) e = r;
+    if (j->state == JOB_ENQUEUED && (r = cudaEventSynchronize(j->ev[EV_END])) != cudaSuccess) e = r;   // the tail may run on the tail stream
     if (e != cudaSuccess) (void)cudaGetLastError();
     return e;
 }
 
+// The job's fused probe (if any) is done: move its insertions from the set's pending bound into its count.
+static void job_settle_set(pbsgpu_job *j) {
+    if (j->set && j->state == JOB_ENQUEUED) pbsgpu_set_reconcile(j->set, j->chunk_cap, j->h_counters[CTR_NEW]);
+}
+
+// A finished job is not synchronised again: its streams are slot streams shared with later jobs.
 void pbsgpu_job_release(pbsgpu_job *j) {
     if (!j) return;
     pbsgpu_ctx *c = j->ctx;
-    if (j->enqueued && j->have_events) { cudaEventSynchronize(j->ev[EV_END]); (void)cudaGetLastError(); }   // the tail may run on the tail stream
-    if (j->set && j->enqueued && !j->reconciled) {   // abandoned after its probe was enqueued: settle the set's bookkeeping
+    if (j->state == JOB_FRONT || j->state == JOB_ENQUEUED) {   // abandoned, or an enqueue failed midway
         pbsgpu_job_sync(j);
-        pbsgpu_set_reconcile(j->set, j->chunk_cap, j->h_counters ? j->h_counters[3] : 0);
-        j->reconciled = true;
+        job_settle_set(j);
     }
     void *devp[] = {j->d_off, j->d_len, j->d_tile_first, j->d_cand, j->d_cand_sorted, j->d_forced, j->d_counters, j->d_counts,
                     j->d_chunk_first, j->d_consumed, j->d_chunks, j->d_keys, j->d_keys2, j->d_vals, j->d_vals2,
                     j->d_digests, j->d_hit, j->d_out, j->d_temp, j->d_set_scratch, j->d_arena_off};
     for (void *p : devp) c->dev.put(p);
     c->pin.put(j->h_counters); c->pin.put(j->h_out); c->pin.put(j->h_consumed); c->pin.put(j->h_early);
-    if (j->have_events) for (int i = 0; i < EV_COUNT; i++) cudaEventDestroy(j->ev[i]);
+    for (cudaEvent_t e : j->ev) if (e) cudaEventDestroy(e);
     delete j;
 }
 
@@ -440,7 +443,7 @@ static int job_alloc(pbsgpu_job *j) {
     DALLOC(j->d_cand, uint64_t, j->cand_cap);
     DALLOC(j->d_cand_sorted, uint64_t, j->cand_cap);
     if (!j->forced_keys.empty()) DALLOC(j->d_forced, uint64_t, j->forced_keys.size());
-    DALLOC(j->d_counters, unsigned long long, 8);
+    DALLOC(j->d_counters, unsigned long long, CTR_DEVICE);
     DALLOC(j->d_counts, uint32_t, n + 1);
     DALLOC(j->d_chunk_first, uint64_t, n + 2);
     DALLOC(j->d_consumed, uint64_t, n + 1);
@@ -455,16 +458,16 @@ static int job_alloc(pbsgpu_job *j) {
     }
     if (j->set) {
         DALLOC(j->d_hit, uint8_t, j->chunk_cap + 1);
-        DALLOC(j->d_set_scratch, uint8_t, pbsgpu_set_fused_scratch_bytes(j->chunk_cap));
+        DALLOC(j->d_set_scratch, uint8_t, pbsgpu_set_scratch_bytes(j->chunk_cap));
     }
     j->temp_bytes = sort_temp_bytes(j);
     DALLOC(j->d_temp, uint8_t, j->temp_bytes);
 #undef DALLOC
-    j->h_counters = (unsigned long long *)ctx->pin.get(4 * sizeof(unsigned long long));
+    j->h_counters = (unsigned long long *)ctx->pin.get(CTR_HOST * sizeof(unsigned long long));
     j->h_out = (pbsgpu_chunk *)ctx->pin.get(sizeof(pbsgpu_chunk) * (j->chunk_cap + 1));
     j->h_consumed = (uint64_t *)ctx->pin.get(sizeof(uint64_t) * (n + 1));
     if (!j->h_counters || !j->h_out || !j->h_consumed) return fail(ctx, PBSGPU_ENOMEM, "pinned host allocation failed");
-    memset(j->h_counters, 0, 4 * sizeof(unsigned long long));
+    memset(j->h_counters, 0, CTR_HOST * sizeof(unsigned long long));
     return PBSGPU_OK;
 }
 
@@ -526,13 +529,12 @@ int pbsgpu_job_create(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base_d
     else j->ss = j->st;
     int rc = job_alloc(j);
     if (rc) { pbsgpu_job_release(j); return rc; }
-    for (int i = 0; i < EV_COUNT; i++)
-        if (cudaEventCreateWithFlags(&j->ev[i], j->profiling ? cudaEventDefault : cudaEventDisableTiming) != cudaSuccess) {
-            for (int k = 0; k < i; k++) cudaEventDestroy(j->ev[k]);
+    for (cudaEvent_t &e : j->ev)
+        if (cudaEventCreateWithFlags(&e, j->profiling ? cudaEventDefault : cudaEventDisableTiming) != cudaSuccess) {
+            e = nullptr;
             pbsgpu_job_release(j);
             return fail(ctx, PBSGPU_ECUDA, "cudaEventCreate failed");
         }
-    j->have_events = true;
     *out = j;
     return PBSGPU_OK;
 }
@@ -593,6 +595,7 @@ int pbsgpu_job_enqueue_front(pbsgpu_job *j) {
     pbsgpu_ctx *ctx = j->ctx;
     cudaStream_t st = j->ss;   // the scan partition's stream (= the job's own stream when the GPU has no scan partition)
     const uint32_t n = j->n;
+    j->state = JOB_FRONT;
     int rc = upload_table(ctx, &j->cfg, st);
     if (rc) return rc;
     if (n) {
@@ -601,14 +604,14 @@ int pbsgpu_job_enqueue_front(pbsgpu_job *j) {
     }
     CK(cudaMemcpyAsync(j->d_tile_first, j->tile_first.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
     if (j->d_forced) CK(cudaMemcpyAsync(j->d_forced, j->forced_keys.data(), j->forced_keys.size() * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(j->d_counters, 0, 8 * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(j->d_counters, 0, CTR_DEVICE * sizeof(unsigned long long), st));
     CK(cudaMemsetAsync(j->d_cand, 0xFF, j->cand_cap * 8, st));   // KEY_SENTINEL padding for the sort
     if (j->profiling) CK(cudaEventRecord(j->ev[EV_START], st));
     // K1
     ScanArgs sa;
     sa.base = j->base; sa.off = j->d_off; sa.len = j->d_len; sa.tile_first = j->d_tile_first; sa.n_streams = n;
     sa.total_tiles = j->total_tiles; sa.mask = j->cfg.mask; sa.break_min = j->cfg.break_min; sa.table = ctx->d_table;
-    sa.cand = j->d_cand; sa.cand_cap = j->cand_cap; sa.cand_count = &j->d_counters[0];
+    sa.cand = j->d_cand; sa.cand_cap = j->cand_cap; sa.cand_count = &j->d_counters[CTR_CANDIDATES];
     if (j->variant == 1) CK(launch_scan_simple(sa, st));
     else if (j->scan_lanes) {
         uint64_t extent = 0;
@@ -616,7 +619,7 @@ int pbsgpu_job_enqueue_front(pbsgpu_job *j) {
         CK(launch_scan_lanes(sa, ctx->d_rot, ctx->scan_sms > 0 ? ctx->scan_sms : ctx->sm_count, extent, st));
     }
     else CK(launch_scan_tuned(sa, ctx->d_rot, ctx->scan_sms > 0 ? ctx->scan_sms : ctx->sm_count, st));
-    if (j->d_forced) CK(launch_append_keys(j->d_forced, j->forced_keys.size(), j->d_cand, j->cand_cap, &j->d_counters[0], st));
+    if (j->d_forced) CK(launch_append_keys(j->d_forced, j->forced_keys.size(), j->d_cand, j->cand_cap, &j->d_counters[CTR_CANDIDATES], st));
     CK(cudaEventRecord(j->ev[EV_SCAN], st));
     // candidates -> sorted by (stream, position)
     size_t tb = j->temp_bytes;
@@ -624,14 +627,12 @@ int pbsgpu_job_enqueue_front(pbsgpu_job *j) {
     if (j->profiling) CK(cudaEventRecord(j->ev[EV_SORT], st));
     // K2
     ResolveArgs ra;
-    ra.keys_sorted = j->d_cand_sorted; ra.cand_count = &j->d_counters[0]; ra.cand_cap = j->cand_cap; ra.len = j->d_len;
+    ra.keys_sorted = j->d_cand_sorted; ra.cand_count = &j->d_counters[CTR_CANDIDATES]; ra.cand_cap = j->cand_cap; ra.len = j->d_len;
     ra.n_streams = n; ra.cmin = j->cfg.min; ra.cmax = j->cfg.max; ra.eof = j->eof; ra.counts = j->d_counts;
     ra.chunk_first = j->d_chunk_first; ra.chunks = j->d_chunks; ra.chunk_cap = j->chunk_cap; ra.consumed = j->d_consumed;
-    ra.n_chunks = &j->d_counters[1];
+    ra.n_chunks = &j->d_counters[CTR_CHUNKS];
     CK(launch_resolve(ra, st));
     CK(cudaEventRecord(j->ev[EV_RESOLVE], st));
-    j->front_done = true;
-    j->back_done = false;
     return PBSGPU_OK;
 }
 
@@ -645,13 +646,13 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
     if (j->ss != st) CK(cudaStreamWaitEvent(st, j->ev[EV_RESOLVE], 0));   // the chunk list comes from the scan partition
     if (j->profiling) CK(cudaEventRecord(j->ev[EV_BACK], st));
     if (j->want_digests && j->chunk_cap) {
-        CK(launch_len_keys(j->d_chunks, &j->d_counters[1], j->chunk_cap, j->d_keys, j->d_vals, st));
+        CK(launch_len_keys(j->d_chunks, &j->d_counters[CTR_CHUNKS], j->chunk_cap, j->d_keys, j->d_vals, st));
         tb = j->temp_bytes;
         CK(cub::DeviceRadixSort::SortPairsDescending(j->d_temp, tb, j->d_keys, j->d_keys2, j->d_vals, j->d_vals2,
                                                      (int)j->chunk_cap, 0, 32, st));
         ShaArgs ha;
         ha.base = j->base; ha.off = j->d_off; ha.chunks = j->d_chunks; ha.order = j->d_vals2;
-        ha.n_chunks = &j->d_counters[1]; ha.chunk_cap = j->chunk_cap; ha.digests = j->d_digests;
+        ha.n_chunks = &j->d_counters[CTR_CHUNKS]; ha.chunk_cap = j->chunk_cap; ha.digests = j->d_digests;
         ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
         if (j->variant == 1) CK(launch_sha_simple(ha, st));
         else if (!hybrid_for(ctx)) CK(launch_sha_tuned(ha, ctx->tune, st));
@@ -667,21 +668,21 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
             const bool use_mid = ctx->tune.mid_x10 > 0 && j->st3 != nullptr;
             uint64_t thr_mid64 = (uint64_t)j->cfg.avg * (uint64_t)ctx->tune.mid_x10 / 10;
             uint32_t thr_mid = thr_mid64 > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)thr_mid64;
-            CK(launch_split_point(j->d_keys2, &j->d_counters[1], j->chunk_cap, thr, max_head, &j->d_counters[2], thr_mid,
-                                  use_mid ? &j->d_counters[4] : nullptr, st));
-            ha.n_head = &j->d_counters[2];
+            CK(launch_split_point(j->d_keys2, &j->d_counters[CTR_CHUNKS], j->chunk_cap, thr, max_head, &j->d_counters[CTR_HEAD], thr_mid,
+                                  use_mid ? &j->d_counters[CTR_MID] : nullptr, st));
+            ha.n_head = &j->d_counters[CTR_HEAD];
             // early input release: the head chunks are copied to the arena and hashed from there
             // (the copy runs HERE, on the job's own stream and the big partition -- a few ms -- not on the side stream,
             // where it would queue behind the 0.3 s latency kernel of the slot's previous job)
             early = j->early && !serial && !use_mid && arena_reserve(j, st);
             if (early) {
-                CK(launch_arena_plan(ha, &j->d_counters[2], j->arena_len, j->d_arena_off, st));
+                CK(launch_arena_plan(ha, &j->d_counters[CTR_HEAD], j->arena_len, j->d_arena_off, st));
                 CK(launch_arena_gather(ha, ctx->arena + j->arena_lo, j->d_arena_off, ctx->sm_count, st));
                 ha.arena = ctx->arena + j->arena_lo; ha.arena_off = j->d_arena_off;
             }
             CK(cudaEventRecord(j->ev[EV_FORK], st));
             if (!serial) CK(cudaStreamWaitEvent(side, j->ev[EV_FORK], 0));
-            ha.n_mid = use_mid ? &j->d_counters[4] : nullptr;
+            ha.n_mid = use_mid ? &j->d_counters[CTR_MID] : nullptr;
             ha.part = 1; CK(launch_sha_split(ha, ctx->tune, side));
             ha.arena = nullptr; ha.arena_off = nullptr;
             CK(cudaEventRecord(j->ev[EV_JOIN], side));
@@ -699,7 +700,7 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
             if (early) {
                 // the caller's buffer is free once the bulk pass and the gather are done -- provided the candidate buffer
                 // did not overflow (then the job is rerun from the input; pbsgpu_batch_wait_input checks the count)
-                CK(cudaMemcpyAsync(j->h_early, &j->d_counters[0], sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+                CK(cudaMemcpyAsync(j->h_early, &j->d_counters[CTR_CANDIDATES], sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
                 CK(cudaEventRecord(j->ev[EV_INPUT], st));
             } else if (!serial) CK(cudaStreamWaitEvent(st, j->ev[EV_JOIN], 0));
         }
@@ -719,21 +720,19 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
         if (ts != st) CK(cudaStreamWaitEvent(ts, j->ev[EV_SHA], 0));
     }
     if (j->set && j->want_digests) {
-        int rc = pbsgpu_set_enqueue_fused(j->set, j->d_digests, &j->d_counters[1], j->chunk_cap, &j->d_counters[0], j->cand_cap,
-                                          j->d_hit, &j->d_counters[3], j->d_set_scratch, ts);
+        int rc = pbsgpu_set_enqueue(j->set, j->d_digests, &j->d_counters[CTR_CHUNKS], j->chunk_cap, 1, &j->d_counters[CTR_CANDIDATES],
+                                    j->cand_cap, j->d_hit, &j->d_counters[CTR_NEW], j->d_set_scratch, ts);
         if (rc) return rc;
     }
     if (j->profiling) CK(cudaEventRecord(j->ev[EV_SET], ts));
     if (j->want_digests)
-        CK(launch_pack_chunks(j->d_chunks, j->d_digests, j->set ? j->d_hit : nullptr, &j->d_counters[1], j->chunk_cap, j->d_out, ts));
-    CK(cudaMemcpyAsync(j->h_counters, j->d_counters, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ts));
+        CK(launch_pack_chunks(j->d_chunks, j->d_digests, j->set ? j->d_hit : nullptr, &j->d_counters[CTR_CHUNKS], j->chunk_cap, j->d_out, ts));
+    CK(cudaMemcpyAsync(j->h_counters, j->d_counters, CTR_HOST * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ts));
     if (j->want_digests)
         CK(cudaMemcpyAsync(j->h_out, j->d_out, sizeof(pbsgpu_chunk) * j->chunk_cap, cudaMemcpyDeviceToHost, ts));
     if (!j->eof && n) CK(cudaMemcpyAsync(j->h_consumed, j->d_consumed, n * 8, cudaMemcpyDeviceToHost, ts));
     CK(cudaEventRecord(j->ev[EV_END], ts));
-    j->enqueued = true;
-    j->back_done = true;
-    j->reconciled = false;
+    j->state = JOB_ENQUEUED;
     return PBSGPU_OK;
 }
 
@@ -744,8 +743,12 @@ int pbsgpu_job_enqueue(pbsgpu_job *j) {
 }
 
 // dense candidates (adversarial / highly structured data): replace the candidate buffers by exactly sized ones
-int pbsgpu_job_grow_cands(pbsgpu_job *j, unsigned long long nc) {
+int pbsgpu_job_prepare_rerun(pbsgpu_job *j, unsigned long long nc) {
     pbsgpu_ctx *ctx = j->ctx;
+    // K4 skipped itself on the device (its guard is this very counter), so the set is untouched: settle the bookkeeping
+    // of the skipped pass
+    job_settle_set(j);
+    j->state = JOB_CREATED;
     ctx->dev.put(j->d_cand); ctx->dev.put(j->d_cand_sorted); ctx->dev.put(j->d_temp);
     j->d_cand = j->d_cand_sorted = nullptr; j->d_temp = nullptr;
     j->cand_cap = nc + nc / 8 + 4096;
@@ -755,6 +758,7 @@ int pbsgpu_job_grow_cands(pbsgpu_job *j, unsigned long long nc) {
     j->temp_bytes = sort_temp_bytes(j);
     j->d_temp = ctx->dev.get(j->temp_bytes);
     if (!j->d_cand || !j->d_cand_sorted || !j->d_temp) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed (rerun)");
+    j->reruns++;
     return PBSGPU_OK;
 }
 
@@ -762,23 +766,19 @@ int pbsgpu_job_grow_cands(pbsgpu_job *j, unsigned long long nc) {
 // (statistically sized) one overflowed -- results are exact either way.
 int pbsgpu_job_finish(pbsgpu_job *j) {
     pbsgpu_ctx *ctx = j->ctx;
+    if (j->state == JOB_FINISHED) return PBSGPU_OK;
     for (;;) {
         CK(cudaEventSynchronize(j->ev[EV_END]));
-        unsigned long long nc = j->h_counters[0];
-        if (nc <= j->cand_cap) break;
-        // overflow: K4 skipped itself on the device (its guard is this very counter), so the set is untouched; settle the
-        // bookkeeping of the skipped pass, then rerun with room for every candidate
-        if (j->set && !j->reconciled) { pbsgpu_set_reconcile(j->set, j->chunk_cap, j->h_counters[3]); j->reconciled = true; }
-        int grc = pbsgpu_job_grow_cands(j, nc);
-        if (grc) return grc;
-        j->reruns++;
-        int rc = pbsgpu_job_enqueue(j);
+        const unsigned long long nc = j->h_counters[CTR_CANDIDATES];
+        if (!pbsgpu_job_overflowed(j, nc)) break;
+        int rc = pbsgpu_job_prepare_rerun(j, nc);
+        if (rc == PBSGPU_OK) rc = pbsgpu_job_enqueue(j);
         if (rc) return rc;
     }
-    if (j->set && !j->reconciled) { pbsgpu_set_reconcile(j->set, j->chunk_cap, j->h_counters[3]); j->reconciled = true; }
-    pbsgpu_timing &t = ctx->last_timing;
-    memset(&t, 0, sizeof t);
-    t.bytes = j->total_bytes; t.chunks = j->h_counters[1]; t.candidates = j->h_counters[0]; t.reruns = j->reruns;
+    job_settle_set(j);
+    j->state = JOB_FINISHED;
+    pbsgpu_timing &t = j->timing;
+    t.bytes = j->total_bytes; t.chunks = j->h_counters[CTR_CHUNKS]; t.candidates = j->h_counters[CTR_CANDIDATES]; t.reruns = j->reruns;
     t.scan_launches = 1;
     const bool hyb = j->variant == 0 && hybrid_for(ctx);
     t.sha_launches = j->want_digests ? (hyb ? 2 : 1) : 0;
@@ -825,7 +825,7 @@ extern "C" int pbsgpu_batch_submit_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, co
     if (rc) return rc;
     j->early = (o.flags & PBSGPU_BATCH_EARLY_INPUT) != 0;
     rc = pbsgpu_job_enqueue(j);
-    if (rc) { pbsgpu_job_sync(j); pbsgpu_job_release(j); return rc; }
+    if (rc) { pbsgpu_job_release(j); return rc; }
     *job = j;
     return PBSGPU_OK;
 }
@@ -840,14 +840,12 @@ extern "C" int pbsgpu_batch_wait(pbsgpu_job *j, pbsgpu_chunk *out, uint64_t cap,
     Guard g(ctx);
     int rc = pbsgpu_job_finish(j);
     if (rc == PBSGPU_OK) {
-        uint64_t nch = j->h_counters[1];
+        uint64_t nch = j->h_counters[CTR_CHUNKS];
         if (n_out) *n_out = nch;
-        if (timing) *timing = ctx->last_timing;
+        if (timing) *timing = j->timing;
         if (nch > cap || (nch && !out))   // the job stays valid: call again with room for *n_out records (or pbsgpu_batch_free)
             return fail(ctx, PBSGPU_ERANGE, "output capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)nch);
         if (nch) memcpy(out, j->h_out, nch * sizeof(pbsgpu_chunk));
-    } else {
-        pbsgpu_job_sync(j);
     }
     pbsgpu_job_release(j);
     return rc;
@@ -863,8 +861,8 @@ extern "C" int pbsgpu_batch_input_done(pbsgpu_job *j) {
     cudaError_t e = cudaEventQuery(j->ev[j->early_active ? EV_INPUT : EV_END]);
     if (e == cudaErrorNotReady) { (void)cudaGetLastError(); return 0; }
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "cudaEventQuery -> %s", cudaGetErrorString(e)); }
-    const unsigned long long nc = j->early_active ? *j->h_early : j->h_counters[0];
-    return nc <= j->cand_cap ? 1 : 0;
+    const unsigned long long nc = j->early_active ? *j->h_early : j->h_counters[CTR_CANDIDATES];
+    return pbsgpu_job_overflowed(j, nc) ? 0 : 1;
 }
 extern "C" int pbsgpu_batch_wait_input(pbsgpu_job *j) {
     if (!j) return PBSGPU_EINVAL;
@@ -872,7 +870,7 @@ extern "C" int pbsgpu_batch_wait_input(pbsgpu_job *j) {
     Guard g(ctx);
     if (j->early_active) {
         CK(cudaEventSynchronize(j->ev[EV_INPUT]));
-        if (*j->h_early <= j->cand_cap) return PBSGPU_OK;
+        if (!pbsgpu_job_overflowed(j, *j->h_early)) return PBSGPU_OK;
     }
     return pbsgpu_job_finish(j);   // no early release (or a rerun is due): the input is free when the job is done
 }
@@ -889,6 +887,27 @@ extern "C" void pbsgpu_batch_free(pbsgpu_job *j) {
 // H2D of group k+1 overlapping the kernels of group k.
 // ---------------------------------------------------------------------------
 struct Group { uint32_t first, count; uint64_t bytes; uint64_t f_lo, f_hi; };
+
+// Finishes and releases one job of the synchronous batch (j becomes NULL).  `first` is the job's first stream in the
+// caller's numbering: its records go to out[*produced...] with `stream` rebased by it, and the XXH3 run `xr` (when
+// stream_xxh3 is set) to stream_xxh3 + first.  *produced counts every record; those that do not fit into `cap` are not
+// copied (the caller reports ERANGE).
+static int batch_collect(pbsgpu_job *&j, uint32_t first, XxhRun *xr, uint64_t *stream_xxh3, pbsgpu_chunk *out, uint64_t cap,
+                         uint64_t *produced) {
+    int rc = pbsgpu_job_finish(j);
+    if (stream_xxh3) { int rx = pbsgpu_xxh3_collect(j->ctx, xr, stream_xxh3 + first, j->st); if (rc == PBSGPU_OK) rc = rx; }
+    if (rc == PBSGPU_OK) {
+        const uint64_t nch = j->h_counters[CTR_CHUNKS];
+        if (*produced + nch <= cap && nch) {
+            memcpy(out + *produced, j->h_out, nch * sizeof(pbsgpu_chunk));
+            if (first) for (uint64_t k = 0; k < nch; k++) out[*produced + k].stream += first;
+        }
+        *produced += nch;
+    }
+    pbsgpu_job_release(j);
+    j = nullptr;
+    return rc;
+}
 
 static int batch_host(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const uint8_t *base, const uint64_t *off,
                       const uint64_t *len, uint32_t n, const pbsgpu_batch_opts &o, pbsgpu_chunk *out, uint64_t cap, uint64_t *n_out) {
@@ -931,35 +950,18 @@ static int batch_host(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const uint8_t *bas
         if (!bufs.p[b]) return fail(ctx, PBSGPU_ENOMEM, "staging buffer of %llu bytes failed", (unsigned long long)buf_bytes);
     }
     std::vector<pbsgpu_job *> jobs(groups.size(), nullptr);
-    std::vector<XxhRun> xruns(o.stream_xxh3 ? groups.size() : 0);   // f2: per-file XXH3-64 from the same staged bytes
+    std::vector<XxhRun> xruns(groups.size());   // f2: per-file XXH3-64 from the same staged bytes
     std::vector<cudaEvent_t> copied(groups.size(), nullptr);
     for (auto &e : copied) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     int rc = PBSGPU_OK;
     uint64_t produced = 0;
-    bool overflow = false;
-    auto collect = [&](size_t gi) -> int {
-        pbsgpu_job *j = jobs[gi];
-        int r = pbsgpu_job_finish(j);
-        if (o.stream_xxh3) { int rx = pbsgpu_xxh3_collect(ctx, &xruns[gi], o.stream_xxh3 + groups[gi].first, j->st); if (r == PBSGPU_OK) r = rx; }
-        if (r == PBSGPU_OK) {
-            uint64_t nch = j->h_counters[1];
-            if (produced + nch > cap) overflow = true;
-            else {
-                for (uint64_t k = 0; k < nch; k++) {
-                    pbsgpu_chunk c = j->h_out[k];
-                    c.stream += groups[gi].first;
-                    out[produced + k] = c;
-                }
-            }
-            produced += nch;
-        } else pbsgpu_job_sync(j);
-        pbsgpu_job_release(j);
-        jobs[gi] = nullptr;
-        return r;
-    };
     std::vector<uint32_t> fs;
     for (size_t gi = 0; gi < groups.size() && rc == PBSGPU_OK; gi++) {
-        if (gi >= (size_t)nbuf) { rc = collect(gi - nbuf); if (rc) break; }   // frees the buffer we are about to reuse
+        if (gi >= (size_t)nbuf) {   // frees the buffer we are about to reuse
+            const size_t c = gi - nbuf;
+            rc = batch_collect(jobs[c], groups[c].first, &xruns[c], o.stream_xxh3, out, cap, &produced);
+            if (rc) break;
+        }
         const Group &g = groups[gi];
         uint8_t *buf = bufs.p[gi % nbuf];
         std::vector<uint64_t> goff(g.count), glen(g.count);
@@ -984,16 +986,14 @@ static int batch_host(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const uint8_t *bas
         cudaStreamWaitEvent(j->ss, copied[gi], 0);
         rc = pbsgpu_job_enqueue(j);
         if (rc == PBSGPU_OK && o.stream_xxh3) rc = pbsgpu_xxh3_enqueue(ctx, buf, goff.data(), glen.data(), g.count, j->st, &xruns[gi]);
-        if (rc) { pbsgpu_job_sync(j); pbsgpu_job_release(j); break; }
+        if (rc) { pbsgpu_job_release(j); break; }
         jobs[gi] = j;
     }
     for (size_t gi = 0; gi < groups.size(); gi++)
-        if (jobs[gi]) { int r = collect(gi); if (rc == PBSGPU_OK) rc = r; }
+        if (jobs[gi]) { int r = batch_collect(jobs[gi], groups[gi].first, &xruns[gi], o.stream_xxh3, out, cap, &produced); if (rc == PBSGPU_OK) rc = r; }
     cudaStreamSynchronize(ctx->copy_stream);
     for (auto &e : copied) if (e) cudaEventDestroy(e);
     if (n_out) *n_out = produced;
-    if (rc == PBSGPU_OK && overflow)
-        rc = fail(ctx, PBSGPU_ERANGE, "output capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)produced);
     return rc;
 }
 
@@ -1009,25 +1009,21 @@ extern "C" int pbsgpu_chunk_digest_batch_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *c
     if (!pbsgpu_cfg_ok(cfg)) return fail(ctx, PBSGPU_EINVAL, "invalid pbsgpu_cfg (use pbsgpu_config)");
     uint64_t produced = 0;
     if (n == 0) { if (n_out) *n_out = 0; return PBSGPU_OK; }
-    if (pbsgpu_is_device_ptr(base)) {
+    if (pbsgpu_is_device_ptr(base)) {   // device input: one job over all streams
         pbsgpu_job *j = nullptr;
         rc = pbsgpu_job_create(ctx, cfg, base, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j);
         if (rc) return rc;
         XxhRun xr;
         rc = pbsgpu_job_enqueue(j);
         if (rc == PBSGPU_OK && o.stream_xxh3) rc = pbsgpu_xxh3_enqueue(ctx, (const uint8_t *)base, off, len, n, j->st, &xr);
-        if (rc == PBSGPU_OK) rc = pbsgpu_job_finish(j);
-        if (rc == PBSGPU_OK) {
-            produced = j->h_counters[1];
-            if (produced > cap) rc = fail(ctx, PBSGPU_ERANGE, "output capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)produced);
-            else if (produced) memcpy(out, j->h_out, produced * sizeof(pbsgpu_chunk));
-        } else pbsgpu_job_sync(j);
-        if (o.stream_xxh3) { int rx = pbsgpu_xxh3_collect(ctx, &xr, o.stream_xxh3, j->st); if (rc == PBSGPU_OK) rc = rx; }
-        pbsgpu_job_release(j);
+        if (rc == PBSGPU_OK) rc = batch_collect(j, 0, &xr, o.stream_xxh3, out, cap, &produced);
+        else pbsgpu_job_release(j);
     } else {
         rc = batch_host(ctx, cfg, (const uint8_t *)base, off, len, n, o, out, cap, &produced);
     }
     if (n_out) *n_out = produced;
+    if (rc == PBSGPU_OK && produced > cap)
+        rc = fail(ctx, PBSGPU_ERANGE, "output capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)produced);
     return rc;
 }
 
@@ -1057,7 +1053,7 @@ extern "C" int pbsgpu_scan_batch(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const v
     rc = pbsgpu_job_enqueue(j);
     if (rc == PBSGPU_OK) rc = pbsgpu_job_finish(j);
     if (rc == PBSGPU_OK) {
-        uint64_t nch = j->h_counters[1];
+        uint64_t nch = j->h_counters[CTR_CHUNKS];
         if (n_out) *n_out = nch;
         if (nch > cap) rc = fail(ctx, PBSGPU_ERANGE, "output capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)nch);
         else {
@@ -1071,7 +1067,7 @@ extern "C" int pbsgpu_scan_batch(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const v
                 memcpy(stream_first, first.data(), (n + 1) * 8);
             }
         }
-    } else pbsgpu_job_sync(j);
+    }
     pbsgpu_job_release(j);
     return rc;
 }

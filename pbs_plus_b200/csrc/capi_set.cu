@@ -77,10 +77,10 @@ static int set_reserve(pbsgpu_set *s, uint64_t more, cudaStream_t st) {
     return PBSGPU_OK;
 }
 
-// scratch layout of one fused operation: tag[cap] tag2[cap] (u64) | idx[cap] idx2[cap] (u32) | miss[cap] | cub temp
-struct FusedLayout { size_t tag, tag2, idx, idx2, miss, temp, temp_bytes, total; };
-static FusedLayout fused_layout(uint64_t cap) {
-    FusedLayout L;
+// scratch layout of one operation: tag[cap] tag2[cap] (u64) | idx[cap] idx2[cap] (u32) | miss[cap] | cub temp
+struct SetLayout { size_t tag, tag2, idx, idx2, miss, temp, temp_bytes, total; };
+static SetLayout set_layout(uint64_t cap) {
+    SetLayout L;
     auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
     size_t tb = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tb, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr,
@@ -89,28 +89,27 @@ static FusedLayout fused_layout(uint64_t cap) {
     L.miss = al(L.idx2 + cap * 4); L.temp = al(L.miss + cap); L.temp_bytes = tb + 256; L.total = L.temp + L.temp_bytes;
     return L;
 }
-size_t pbsgpu_set_fused_scratch_bytes(uint64_t cap) { return fused_layout(cap).total; }
+size_t pbsgpu_set_scratch_bytes(uint64_t cap) { return set_layout(cap).total; }
 
-int pbsgpu_set_enqueue_fused(pbsgpu_set *s, const uint8_t *d_dig, const unsigned long long *n_dev, uint64_t cap,
-                             const unsigned long long *guard, uint64_t guard_max, uint8_t *d_hit, unsigned long long *d_new,
-                             void *scratch, cudaStream_t st) {
+int pbsgpu_set_enqueue(pbsgpu_set *s, const uint8_t *d_dig, const unsigned long long *n_dev, uint64_t cap, int do_insert,
+                       const unsigned long long *guard, uint64_t guard_max, uint8_t *d_hit, unsigned long long *d_new,
+                       void *scratch, cudaStream_t st) {
     pbsgpu_ctx *ctx = s->ctx;
     if (cap == 0) return PBSGPU_OK;
     if (cap >= (1ull << 31)) return fail(ctx, PBSGPU_EINVAL, "too many digests in one call");
-    int rc = set_reserve(s, cap, ctx->streams[0]);
-    if (rc) return rc;
+    if (do_insert) { int rc = set_reserve(s, cap, ctx->streams[0]); if (rc) return rc; }
     if (s->last_valid) CK(cudaStreamWaitEvent(st, s->last, 0));   // table operations are totally ordered
-    const FusedLayout L = fused_layout(cap);
+    const SetLayout L = set_layout(cap);
     uint8_t *b = (uint8_t *)scratch;
     uint64_t *tag = (uint64_t *)(b + L.tag), *tag2 = (uint64_t *)(b + L.tag2);
     uint32_t *idx = (uint32_t *)(b + L.idx), *idx2 = (uint32_t *)(b + L.idx2);
     size_t tb = L.temp_bytes;
-    CK(launch_set_make_keys_dev(d_dig, n_dev, cap, tag, idx, st));
+    CK(launch_set_make_keys(d_dig, n_dev, cap, tag, idx, st));
     CK(cub::DeviceRadixSort::SortPairs(b + L.temp, tb, tag, tag2, idx, idx2, (int)cap, 0, 64, st));   // stable
-    CK(launch_set_mark_probe_insert_dev(s->t, d_dig, tag2, idx2, n_dev, cap, guard, guard_max, d_hit, b + L.miss, d_new, st));
+    CK(launch_set_mark_probe_insert(s->t, d_dig, tag2, idx2, n_dev, cap, guard, guard_max, do_insert, d_hit, b + L.miss, d_new, st));
     CK(cudaEventRecord(s->last, st));
     s->last_valid = true;
-    s->pending_max += cap;
+    if (do_insert) s->pending_max += cap;
     return PBSGPU_OK;
 }
 
@@ -125,28 +124,17 @@ int pbsgpu_set_process_dev(pbsgpu_set *s, const uint8_t *d_dig, uint64_t n, int 
     cudaStream_t st = ctx->streams[0];
     if (n == 0) return PBSGPU_OK;
     if (n >= (1ull << 31)) return fail(ctx, PBSGPU_EINVAL, "too many digests in one call");
-    if (do_insert) { int rc = set_reserve(s, n, st); if (rc) return rc; }
-    if (s->last_valid) CK(cudaStreamWaitEvent(st, s->last, 0));
-    size_t tb = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tb, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint32_t *)nullptr,
-                                    (uint32_t *)nullptr, (int)n);
-    Scoped tag(ctx->dev, n * 8), tag2(ctx->dev, n * 8), idx(ctx->dev, n * 4), idx2(ctx->dev, n * 4), miss(ctx->dev, n),
-        d_new(ctx->dev, 8), temp(ctx->dev, tb + 256);
-    if (!tag || !tag2 || !idx || !idx2 || !miss || !d_new || !temp) return fail(ctx, PBSGPU_ENOMEM, "digest set scratch allocation failed");
+    Scoped scratch(ctx->dev, pbsgpu_set_scratch_bytes(n)), d_new(ctx->dev, 8);
+    if (!scratch || !d_new) return fail(ctx, PBSGPU_ENOMEM, "digest set scratch allocation failed");
+    CK(cudaMemsetAsync(d_new.p, 0, 8, st));
+    const int rc = pbsgpu_set_enqueue(s, d_dig, nullptr, n, do_insert, nullptr, 0, d_hit, d_new.as<unsigned long long>(), scratch.p, st);
     unsigned long long h_new = 0;
-    cudaError_t e = cudaMemsetAsync(d_new.p, 0, 8, st);
-    if (e == cudaSuccess) e = launch_set_make_keys(d_dig, n, tag.as<uint64_t>(), idx.as<uint32_t>(), st);
-    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(temp.p, tb, tag.as<uint64_t>(), tag2.as<uint64_t>(), idx.as<uint32_t>(),
-                                                              idx2.as<uint32_t>(), (int)n, 0, 64, st);   // stable
-    if (e == cudaSuccess) e = launch_set_mark_probe_insert(s->t, d_dig, tag2.as<uint64_t>(), idx2.as<uint32_t>(), n, do_insert, d_hit,
-                                                           miss.as<uint8_t>(), d_new.as<unsigned long long>(), st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_new, d_new.p, 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaEventRecord(s->last, st);
+    cudaError_t e = rc ? cudaSuccess : cudaMemcpyAsync(&h_new, d_new.p, 8, cudaMemcpyDeviceToHost, st);
     cudaError_t es = cudaStreamSynchronize(st);   // the scoped scratch must not return to the pool while kernels use it
+    if (rc) { (void)cudaGetLastError(); return rc; }
     if (e == cudaSuccess) e = es;
+    pbsgpu_set_reconcile(s, do_insert ? n : 0, e == cudaSuccess ? h_new : 0);   // the enqueue added n to pending_max
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "digest set: %s", cudaGetErrorString(e)); }
-    s->last_valid = true;
-    s->count += h_new;
     return PBSGPU_OK;
 }
 

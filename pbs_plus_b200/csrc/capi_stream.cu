@@ -86,11 +86,10 @@ static int stream_collect(pbsgpu_stream *s, bool block) {
             if (q == cudaErrorNotReady) { (void)cudaGetLastError(); break; }
         }
         int rc = pbsgpu_job_finish(sj.j);
-        if (rc != PBSGPU_OK) pbsgpu_job_sync(sj.j);
         s->inflight.pop_front();
         s->busy[sj.buf] = 0;
         if (rc != PBSGPU_OK) { pbsgpu_job_release(sj.j); return rc; }
-        const uint64_t nch = sj.j->h_counters[1];
+        const uint64_t nch = sj.j->h_counters[CTR_CHUNKS];
         for (uint64_t k = 0; k < nch; k++) {
             pbsgpu_chunk c = sj.j->h_out[k];          // flags already carry the fused probe's result
             c.stream = 0; c.end_off += sj.base_off;
@@ -117,25 +116,22 @@ static int stream_process(pbsgpu_stream *s, int eof) {
     int rc = pbsgpu_job_create(ctx, &s->cfg, s->buf[s->cur], &off0, &len0, 1, eof, 1, s->set, fstream.data(), foff.data(), foff.size(), &j);
     if (rc) return rc;
     CK(cudaStreamWaitEvent(j->ss, s->copied, 0));       // every byte of the window has arrived before K1 reads it
-    // front half now: the cut points decide what has to be carried over
-    unsigned long long *counters = j->h_counters;       // pinned
-    uint64_t *consumed_p = j->h_consumed;
-    uint64_t consumed = s->fill;
+    // front half now: the cut points decide what has to be carried over.  On a candidate overflow only the front half is
+    // rerun: the back half is enqueued once the carry is known.
     for (;;) {
         rc = pbsgpu_job_enqueue_front(j);
         if (rc == PBSGPU_OK) {
-            cudaError_t e = cudaMemcpyAsync(counters, j->d_counters, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, j->ss);
-            if (e == cudaSuccess && !eof) e = cudaMemcpyAsync(consumed_p, j->d_consumed, 8, cudaMemcpyDeviceToHost, j->ss);
+            cudaError_t e = cudaMemcpyAsync(j->h_counters, j->d_counters, CTR_HOST * sizeof(unsigned long long), cudaMemcpyDeviceToHost, j->ss);
+            if (e == cudaSuccess && !eof) e = cudaMemcpyAsync(j->h_consumed, j->d_consumed, 8, cudaMemcpyDeviceToHost, j->ss);
             if (e == cudaSuccess) e = cudaStreamSynchronize(j->ss);
             if (e != cudaSuccess) { (void)cudaGetLastError(); rc = fail(ctx, PBSGPU_ECUDA, "stream window: %s", cudaGetErrorString(e)); }
         }
-        if (rc != PBSGPU_OK) { pbsgpu_job_sync(j); pbsgpu_job_release(j); return rc; }
-        if (counters[0] <= j->cand_cap) break;
-        rc = pbsgpu_job_grow_cands(j, counters[0]);          // dense candidates: redo the front half with room for all
-        if (rc) { pbsgpu_job_release(j); return rc; }
-        j->reruns++;
+        const unsigned long long nc = j->h_counters[CTR_CANDIDATES];
+        if (rc == PBSGPU_OK && !pbsgpu_job_overflowed(j, nc)) break;
+        if (rc == PBSGPU_OK) rc = pbsgpu_job_prepare_rerun(j, nc);   // dense candidates: redo the front half with room for all
+        if (rc != PBSGPU_OK) { pbsgpu_job_release(j); return rc; }
     }
-    consumed = eof ? s->fill : consumed_p[0];
+    const uint64_t consumed = eof ? s->fill : j->h_consumed[0];
     const uint64_t rest = s->fill - consumed;
     // next buffer (wait for the oldest window if all are referenced)
     int next = -1;
@@ -146,20 +142,20 @@ static int stream_process(pbsgpu_stream *s, int eof) {
         StreamJob oldest = s->inflight.front();
         cudaEventSynchronize(oldest.j->ev[EV_END]);
         rc = stream_collect(s, false);
-        if (rc) { pbsgpu_job_sync(j); pbsgpu_job_release(j); return rc; }
+        if (rc) { pbsgpu_job_release(j); return rc; }
     }
-    if (next < 0) { pbsgpu_job_sync(j); pbsgpu_job_release(j); return fail(ctx, PBSGPU_ESTATE, "internal: no free stream buffer"); }
+    if (next < 0) { pbsgpu_job_release(j); return fail(ctx, PBSGPU_ESTATE, "internal: no free stream buffer"); }
     if (!s->buf[next]) {
         s->buf[next] = (uint8_t *)ctx->dev.get(s->cap);
-        if (!s->buf[next]) { pbsgpu_job_sync(j); pbsgpu_job_release(j); return fail(ctx, PBSGPU_ENOMEM, "stream buffer of %llu bytes failed", (unsigned long long)s->cap); }
+        if (!s->buf[next]) { pbsgpu_job_release(j); return fail(ctx, PBSGPU_ENOMEM, "stream buffer of %llu bytes failed", (unsigned long long)s->cap); }
     }
     if (rest) {   // carry: ordered on the copy stream in front of the next window's H2D copies, no host wait
         cudaError_t e = cudaMemcpyAsync(s->buf[next], s->buf[s->cur] + consumed, rest, cudaMemcpyDeviceToDevice, ctx->copy_stream);
         if (e == cudaSuccess) e = cudaEventRecord(s->copied, ctx->copy_stream);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); pbsgpu_job_sync(j); pbsgpu_job_release(j); return fail(ctx, PBSGPU_ECUDA, "carry copy: %s", cudaGetErrorString(e)); }
+        if (e != cudaSuccess) { (void)cudaGetLastError(); pbsgpu_job_release(j); return fail(ctx, PBSGPU_ECUDA, "carry copy: %s", cudaGetErrorString(e)); }
     }
     rc = pbsgpu_job_enqueue_back(j);                          // SHA-256 etc. run while the next window fills
-    if (rc != PBSGPU_OK) { pbsgpu_job_sync(j); pbsgpu_job_release(j); return rc; }
+    if (rc != PBSGPU_OK) { pbsgpu_job_release(j); return rc; }
     s->busy[s->cur] = 1;
     s->inflight.push_back(StreamJob{j, s->cur, s->base_off});
     s->cur = next; s->fill = rest; s->base_off += consumed;
@@ -305,7 +301,7 @@ extern "C" void pbsgpu_stream_close(pbsgpu_stream *s) {
     pbsgpu_ctx *ctx = s->ctx;
     Guard g(ctx);
     cudaStreamSynchronize(ctx->copy_stream);
-    for (auto &sj : s->inflight) { cudaEventSynchronize(sj.j->ev[EV_END]); pbsgpu_job_sync(sj.j); pbsgpu_job_release(sj.j); }
+    for (auto &sj : s->inflight) pbsgpu_job_release(sj.j);
     for (auto b : s->buf) ctx->dev.put(b);
     if (s->ring) ctx->pin.put(s->ring);
     for (auto e : s->slot_done) if (e) cudaEventDestroy(e);

@@ -33,25 +33,38 @@ __device__ __forceinline__ bool eq32(const uint64_t *a, const uint64_t *b) {
     return a[0] == b[0] && a[1] == b[1] && a[2] == b[2] && a[3] == b[3];
 }
 
-__global__ void k_set_make_keys(const uint8_t *d32, uint64_t n, uint64_t *tag, uint32_t *idx) {
+// The element count is *n_dev when n_dev is set (K4 as part of a batch job: the job's chunk count is only known on the
+// device) and `cap` otherwise; `cap` bounds every launch.  Entries at index >= n get the all-ones tag and sort behind the
+// real ones (a real digest whose first 8 bytes are all ones still works: the sort is stable, so it stays in front of the
+// padding and padding threads return at once).
+__device__ __forceinline__ uint64_t count_of(const unsigned long long *n_dev, uint64_t cap) {
+    const uint64_t n = n_dev ? *n_dev : cap;
+    return n < cap ? n : cap;
+}
+
+__global__ void k_set_make_keys(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    tag[i] = tag_of((const uint64_t *)(d32 + i * 32));
+    if (i >= cap) return;
+    tag[i] = i < count_of(n_dev, cap) ? tag_of((const uint64_t *)(d32 + i * 32)) : ~0ull;
     idx[i] = (uint32_t)i;
 }
-cudaError_t launch_set_make_keys(const uint8_t *d32, uint64_t n, uint64_t *tag, uint32_t *idx, cudaStream_t st) {
-    if (!n) return cudaSuccess;
-    k_set_make_keys<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d32, n, tag, idx);
+cudaError_t launch_set_make_keys(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx,
+                                 cudaStream_t st) {
+    if (!cap) return cudaSuccess;
+    k_set_make_keys<<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(d32, n_dev, cap, tag, idx);
     return cudaGetLastError();
 }
 
 // phase 0: mark in-batch duplicates + probe representatives.  phase 1: insert missing representatives.
+// `guard` (optional): candidate counter of the job; when it exceeds guard_max the job's chunk list is truncated and will be
+// recomputed, so this pass must not touch the table.
 template <int PHASE>
 __global__ void k_set_process(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted, const uint32_t *idx_sorted,
-                              uint64_t n, int do_insert, uint8_t *hit, uint8_t *is_rep_miss,
-                              unsigned long long *n_new) {
+                              const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard, uint64_t guard_max,
+                              int do_insert, uint8_t *hit, uint8_t *is_rep_miss, unsigned long long *n_new) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
+    if (j >= count_of(n_dev, cap)) return;   // the n real entries are the first n after the stable sort
+    if (guard && *guard > guard_max) { if (PHASE == 0 && hit) hit[idx_sorted[j]] = 0; return; }
     const uint32_t i = idx_sorted[j];
     const uint64_t *d = (const uint64_t *)(d32 + (uint64_t)i * 32);
     const uint64_t tag = tag_sorted[j];
@@ -96,14 +109,15 @@ __global__ void k_set_process(SetTable t, const uint8_t *d32, const uint64_t *ta
     }
 }
 
-cudaError_t launch_set_mark_probe_insert(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted,
-                                         const uint32_t *idx_sorted, uint64_t n, int do_insert, uint8_t *hit,
-                                         uint8_t *is_rep_miss /*[n] scratch*/, unsigned long long *n_new,
-                                         cudaStream_t st) {
-    if (!n) return cudaSuccess;
-    unsigned blocks = (unsigned)((n + 255) / 256);
-    k_set_process<0><<<blocks, 256, 0, st>>>(t, d32, tag_sorted, idx_sorted, n, do_insert, hit, is_rep_miss, n_new);
-    if (do_insert) k_set_process<1><<<blocks, 256, 0, st>>>(t, d32, tag_sorted, idx_sorted, n, do_insert, hit, is_rep_miss, n_new);
+cudaError_t launch_set_mark_probe_insert(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted, const uint32_t *idx_sorted,
+                                         const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard,
+                                         uint64_t guard_max, int do_insert, uint8_t *hit, uint8_t *is_rep_miss /*[cap] scratch*/,
+                                         unsigned long long *n_new, cudaStream_t st) {
+    if (!cap) return cudaSuccess;
+    unsigned blocks = (unsigned)((cap + 255) / 256);
+    k_set_process<0><<<blocks, 256, 0, st>>>(t, d32, tag_sorted, idx_sorted, n_dev, cap, guard, guard_max, do_insert, hit, is_rep_miss, n_new);
+    if (do_insert)
+        k_set_process<1><<<blocks, 256, 0, st>>>(t, d32, tag_sorted, idx_sorted, n_dev, cap, guard, guard_max, do_insert, hit, is_rep_miss, n_new);
     return cudaGetLastError();
 }
 
@@ -122,86 +136,6 @@ __global__ void k_set_rehash(SetTable from, SetTable to) {
 }
 cudaError_t launch_set_rehash(SetTable from, SetTable to, cudaStream_t st) {
     k_set_rehash<<<(unsigned)((from.cap + 255) / 256), 256, 0, st>>>(from, to);
-    return cudaGetLastError();
-}
-
-// ---------------------------------------------------------------------------
-// Fused form: K4 as part of a batch job, enqueued on the job's stream.  The number of digests (the job's chunk
-// count) is only known on the device, so launches are bounded by `cap` and every thread re-reads *n_dev; entries at
-// index >= n get the all-ones tag and sort behind the real ones (a real digest whose first 8 bytes are all ones
-// still works: the sort is stable, so it stays in front of the padding and padding threads return at once).
-// `guard`: candidate counter of the job; when it exceeds guard_max the job's chunk list is truncated and will be
-// recomputed, so this pass must not touch the table.
-// ---------------------------------------------------------------------------
-__global__ void k_set_make_keys_dev(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= cap) return;
-    unsigned long long n = *n_dev;
-    tag[i] = i < n ? tag_of((const uint64_t *)(d32 + i * 32)) : ~0ull;
-    idx[i] = (uint32_t)i;
-}
-cudaError_t launch_set_make_keys_dev(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx,
-                                     cudaStream_t st) {
-    if (!cap) return cudaSuccess;
-    k_set_make_keys_dev<<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(d32, n_dev, cap, tag, idx);
-    return cudaGetLastError();
-}
-
-template <int PHASE>
-__global__ void k_set_process_dev(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted, const uint32_t *idx_sorted,
-                                  const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard, uint64_t guard_max,
-                                  uint8_t *hit, uint8_t *is_rep_miss, unsigned long long *n_new) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned long long n = *n_dev;
-    if (n > cap) n = cap;
-    if (j >= n) return;                      // the n real entries are the first n after the stable sort
-    if (guard && *guard > guard_max) { if (PHASE == 0 && hit) hit[idx_sorted[j]] = 0; return; }
-    const uint32_t i = idx_sorted[j];
-    const uint64_t *d = (const uint64_t *)(d32 + (uint64_t)i * 32);
-    const uint64_t tag = tag_sorted[j];
-    if (PHASE == 0) {
-        bool dup = false;
-        if (j > 0 && tag_sorted[j - 1] == tag) {
-            for (uint64_t k = j; k > 0 && tag_sorted[k - 1] == tag; k--)
-                if (eq32(d, (const uint64_t *)(d32 + (uint64_t)idx_sorted[k - 1] * 32))) { dup = true; break; }
-        }
-        uint8_t h = 1, miss = 0;
-        if (!dup) {
-            h = 0;
-            uint64_t slot = slot_hash(tag) & (t.cap - 1);
-            for (;;) {
-                uint64_t cur = t.tags[slot];
-                if (cur == 0) break;
-                if (cur == tag && eq32(d, t.keys + slot * 4)) { h = 1; break; }
-                slot = (slot + 1) & (t.cap - 1);
-            }
-            miss = !h;
-        }
-        if (hit) hit[i] = h;
-        is_rep_miss[j] = miss;
-    } else {
-        if (!is_rep_miss[j]) return;
-        uint64_t slot = slot_hash(tag) & (t.cap - 1);
-        for (;;) {
-            unsigned long long cur = atomicCAS((unsigned long long *)&t.tags[slot], 0ull, (unsigned long long)tag);
-            if (cur == 0) {
-                uint64_t *k = t.keys + slot * 4;
-                k[0] = d[0]; k[1] = d[1]; k[2] = d[2]; k[3] = d[3];
-                atomicAdd(n_new, 1ull);
-                break;
-            }
-            slot = (slot + 1) & (t.cap - 1);
-        }
-    }
-}
-cudaError_t launch_set_mark_probe_insert_dev(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted, const uint32_t *idx_sorted,
-                                             const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard,
-                                             uint64_t guard_max, uint8_t *hit, uint8_t *is_rep_miss, unsigned long long *n_new,
-                                             cudaStream_t st) {
-    if (!cap) return cudaSuccess;
-    unsigned blocks = (unsigned)((cap + 255) / 256);
-    k_set_process_dev<0><<<blocks, 256, 0, st>>>(t, d32, tag_sorted, idx_sorted, n_dev, cap, guard, guard_max, hit, is_rep_miss, n_new);
-    k_set_process_dev<1><<<blocks, 256, 0, st>>>(t, d32, tag_sorted, idx_sorted, n_dev, cap, guard, guard_max, hit, is_rep_miss, n_new);
     return cudaGetLastError();
 }
 

@@ -67,7 +67,6 @@ struct pbsgpu_ctx {
     void *d_xxh_tab = nullptr;      // K7 secret words, uploaded on first use
     uint32_t table_cache[256];
     bool table_valid = false;
-    pbsgpu_timing last_timing;
     cudaEvent_t epoch = nullptr;   // recorded at open; kernel intervals are reported relative to it
     // optional spatial partition (CUDA green contexts): `part_sms` SMs are reserved for the latency
     // kernels of long chunks (streams2), everything else runs on the remaining SMs (streams)
@@ -136,20 +135,27 @@ struct pbsgpu_set {
     cudaEvent_t last = nullptr;   // completion of the most recent operation enqueued on the table (any stream)
     bool last_valid = false;
 };
-// Enqueue "probe + insert" of the digests of a job on stream `st`, in index order (n_dev = device count, cap = launch
-// bound).  d_hit[cap] receives the flags, d_new the number of new digests.  Scratch comes from `scratch` (>= set_fused_scratch_bytes(cap)).
-size_t pbsgpu_set_fused_scratch_bytes(uint64_t cap);
-// `guard`/`guard_max`: the kernels do nothing when *guard > guard_max (the job's candidate buffer overflowed and it will be rerun).
-int pbsgpu_set_enqueue_fused(pbsgpu_set *s, const uint8_t *d_dig, const unsigned long long *n_dev, uint64_t cap,
-                             const unsigned long long *guard, uint64_t guard_max, uint8_t *d_hit, unsigned long long *d_new,
-                             void *scratch, cudaStream_t st);
-void pbsgpu_set_reconcile(pbsgpu_set *s, uint64_t cap, uint64_t n_new);   // a fused operation finished: pending -> count
+// Enqueue "probe (+ insert when do_insert)" of digests on stream `st`, in index order.  The count is *n_dev (a job's chunk
+// count, known only on the device) or `cap` when n_dev is NULL; `cap` bounds the launch.  d_hit[cap] (or NULL) receives the
+// flags, *d_new is incremented by the number of new digests.  Scratch comes from `scratch` (>= pbsgpu_set_scratch_bytes(cap)).
+// `guard`/`guard_max` (optional): the kernels do nothing when *guard > guard_max (the job's candidate buffer overflowed and it
+// will be rerun).  An insertion adds `cap` to pending_max until pbsgpu_set_reconcile settles it.
+size_t pbsgpu_set_scratch_bytes(uint64_t cap);
+int pbsgpu_set_enqueue(pbsgpu_set *s, const uint8_t *d_dig, const unsigned long long *n_dev, uint64_t cap, int do_insert,
+                       const unsigned long long *guard, uint64_t guard_max, uint8_t *d_hit, unsigned long long *d_new,
+                       void *scratch, cudaStream_t st);
+void pbsgpu_set_reconcile(pbsgpu_set *s, uint64_t cap, uint64_t n_new);   // an insertion finished: pending -> count
 int pbsgpu_set_process_dev(pbsgpu_set *s, const uint8_t *d_dig, uint64_t n, int do_insert, uint8_t *d_hit);
 
 // ---------------------------------------------------------------------------
 // Job: one batch of device-resident streams through K1..K4 on one CUDA stream (capi.cu)
 // ---------------------------------------------------------------------------
 enum { EV_START, EV_SCAN, EV_SORT, EV_RESOLVE, EV_SHA, EV_END, EV_FORK, EV_JOIN, EV_BULK, EV_BACK, EV_SET, EV_MID, EV_INPUT, EV_COUNT };
+// Slots of j->d_counters, zeroed by every front half.  The first CTR_HOST slots are copied back to j->h_counters.
+enum { CTR_CANDIDATES, CTR_CHUNKS, CTR_HEAD, CTR_NEW, CTR_MID, CTR_HOST = CTR_MID, CTR_DEVICE = 8 };
+// CREATED: nothing in flight.  FRONT: the front half was (perhaps partly) enqueued.  ENQUEUED: both halves are enqueued,
+// EV_END recorded, and a fused probe still has to be settled with the set.  FINISHED: results are on the host.
+enum JobState { JOB_CREATED, JOB_FRONT, JOB_ENQUEUED, JOB_FINISHED };
 
 struct pbsgpu_job {
     pbsgpu_ctx *ctx = nullptr;
@@ -164,7 +170,7 @@ struct pbsgpu_job {
     pbsgpu_set *set = nullptr;      // fused probe + insert (NULL: none)
     // device
     uint64_t *d_off = nullptr, *d_len = nullptr, *d_tile_first = nullptr, *d_cand = nullptr, *d_cand_sorted = nullptr, *d_forced = nullptr;
-    unsigned long long *d_counters = nullptr;   // [0] cand_count [1] n_chunks [2] n_head [3] n_new (set) [4] n_mid
+    unsigned long long *d_counters = nullptr;   // [CTR_DEVICE], indexed by CTR_*
     uint32_t *d_counts = nullptr;
     uint64_t *d_chunk_first = nullptr, *d_consumed = nullptr;
     pbsgpu::ChunkRef *d_chunks = nullptr;
@@ -181,12 +187,14 @@ struct pbsgpu_job {
     uint64_t *d_arena_off = nullptr;
     unsigned long long *h_early = nullptr;   // pinned: candidate count as of EV_INPUT (overflow => the input is still needed)
     // pinned host
-    unsigned long long *h_counters = nullptr;
+    unsigned long long *h_counters = nullptr;   // [CTR_HOST]
     pbsgpu_chunk *h_out = nullptr;
     uint64_t *h_consumed = nullptr;
-    cudaEvent_t ev[EV_COUNT];
-    bool have_events = false, profiling = false, enqueued = false, front_done = false, back_done = false, reconciled = false;
+    cudaEvent_t ev[EV_COUNT] = {};
+    bool profiling = false;
+    JobState state = JOB_CREATED;
     uint32_t reruns = 0;
+    pbsgpu_timing timing = {};      // filled by pbsgpu_job_finish
 };
 
 int pbsgpu_job_create(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base_dev, const uint64_t *off, const uint64_t *len,
@@ -195,10 +203,14 @@ int pbsgpu_job_create(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base_d
 int pbsgpu_job_enqueue_front(pbsgpu_job *j);
 int pbsgpu_job_enqueue_back(pbsgpu_job *j);
 int pbsgpu_job_enqueue(pbsgpu_job *j);
-int pbsgpu_job_grow_cands(pbsgpu_job *j, unsigned long long nc);
-int pbsgpu_job_finish(pbsgpu_job *j);     // blocks; reruns on candidate overflow; fills ctx->last_timing
+// Candidate overflow: the candidate buffer is sized from statistics; a job whose `nc` candidates did not fit is rerun from
+// its input.  prepare_rerun is called once the overflowed pass is done: it settles the set for a probe that was
+// enqueued, grows the candidate buffers to fit `nc` and counts the rerun; the caller enqueues again.
+inline bool pbsgpu_job_overflowed(const pbsgpu_job *j, unsigned long long nc) { return nc > j->cand_cap; }
+int pbsgpu_job_prepare_rerun(pbsgpu_job *j, unsigned long long nc);
+int pbsgpu_job_finish(pbsgpu_job *j);     // blocks; reruns on candidate overflow; fills j->timing
 cudaError_t pbsgpu_job_sync(pbsgpu_job *j);
-void pbsgpu_job_release(pbsgpu_job *j);   // waits for nothing: call only after finish or after synchronising j->st
+void pbsgpu_job_release(pbsgpu_job *j);   // waits for what the job still has in flight unless it finished
 
 // K7 (capi_aux.cu): enqueue-only / collect pair so the fused batch call can put it on a job's stream
 struct XxhRun {

@@ -133,19 +133,16 @@ struct SetTable {
     uint64_t *keys;     // [cap][4]
     uint64_t cap;       // power of two
 };
-cudaError_t launch_set_make_keys(const uint8_t *d32, uint64_t n, uint64_t *tag, uint32_t *idx, cudaStream_t st);
-cudaError_t launch_set_mark_probe_insert(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted,
-                                         const uint32_t *idx_sorted, uint64_t n, int do_insert, uint8_t *hit,
-                                         uint8_t *is_rep_miss, unsigned long long *n_new, cudaStream_t st);
+// The element count is *n_dev (NULL: cap); `cap` bounds the launch.  Padding entries (index >= n) get the all-ones tag and
+// sort last.  Nothing happens when guard is set and *guard > guard_max.  Probe only (do_insert = 0): no in-batch duplicate
+// check and no insert launch.
+cudaError_t launch_set_make_keys(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx,
+                                 cudaStream_t st);
+cudaError_t launch_set_mark_probe_insert(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted, const uint32_t *idx_sorted,
+                                         const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard,
+                                         uint64_t guard_max, int do_insert, uint8_t *hit, uint8_t *is_rep_miss,
+                                         unsigned long long *n_new, cudaStream_t st);
 cudaError_t launch_set_rehash(SetTable from, SetTable to, cudaStream_t st);
-// fused form (K4 on a job's stream): the element count lives on the device, `cap` bounds the launch; nothing happens when
-// *guard > guard_max.  Padding entries (index >= *n_dev) get the all-ones tag and sort last.
-cudaError_t launch_set_make_keys_dev(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx,
-                                     cudaStream_t st);
-cudaError_t launch_set_mark_probe_insert_dev(SetTable t, const uint8_t *d32, const uint64_t *tag_sorted, const uint32_t *idx_sorted,
-                                             const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard,
-                                             uint64_t guard_max, uint8_t *hit, uint8_t *is_rep_miss, unsigned long long *n_new,
-                                             cudaStream_t st);
 // multi-GPU merge: compact the padded all-gather payload [rank][max_n][32] into global order [sum(counts)][32]
 cudaError_t launch_set_compact_gather(const uint8_t *padded, const uint64_t *counts_dev, uint32_t nranks, uint64_t max_n,
                                       uint8_t *dense, cudaStream_t st);

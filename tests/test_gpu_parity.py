@@ -116,6 +116,39 @@ def test_dense_candidates_overflow_rerun_is_exact(eng, torch):
     assert ends.tolist() == oracle.chunk_ends(oracle.config(512, t), data).tolist()
 
 
+@pytest.mark.parametrize("entry", ["device_batch", "staged_batch", "stream"])
+def test_dense_candidates_overflow_rerun_is_exact_in_every_entry_point(eng, torch, entry):
+    """The same overflow through the other entry points that rerun an overflowed job: one device job over all
+    streams, host input staged in several groups, and a stream cut into several windows (front half rerun only)."""
+    t = np.zeros(256, dtype=np.uint32)
+    t[0] = 0xFFFFFFFF
+    data = np.random.default_rng(3).integers(0, 2, size=600_000, dtype=np.uint8)
+    cfg, cfg_o = pg.make_config(512, t), oracle.config(512, t)
+    if entry == "device_batch":
+        arrs = [data[:250_000], data[250_000:]]
+        buf, off, ln = pack(arrs)
+        rec = eng.chunk_digest_batch(cfg, to_dev(torch, buf), off, ln)
+        assert rec.tobytes() == oracle.chunk_digest_streams(cfg_o, arrs).tobytes()
+    elif entry == "staged_batch":
+        arrs = [data[i:i + 150_000] for i in range(0, len(data), 150_000)]
+        e = _engine_with_env({"PBSGPU_STAGE_BYTES": str(1 << 18)})     # one stream per staging group
+        try:
+            rec = e.chunk_digest_streams(cfg, arrs)
+        finally:
+            e.close()
+        assert rec.tobytes() == oracle.chunk_digest_streams(cfg_o, arrs).tobytes()
+    else:
+        e = _engine_with_env({"PBSGPU_STREAM_WINDOW": str(1 << 17)})   # five windows
+        try:
+            st = e.stream(cfg)
+            st.write(data)
+            rec = st.finish()
+            st.close()
+        finally:
+            e.close()
+        assert rec.tobytes() == oracle.chunk_digest(cfg_o, data).tobytes()
+
+
 def test_custom_table(eng, torch):
     t = np.random.default_rng(9).integers(0, 2**32, size=256, dtype=np.uint32)
     data = rnd(2_000_000, 11)
