@@ -6,7 +6,7 @@
 // runtime; no torch types.  There is no CPU fallback anywhere in this file: every data
 // path launches the kernels in scan.cu / resolve.cu / sha256.cu / digestset.cu.
 // Sibling translation units: capi_set.cu (digest set, NCCL merge), capi_stream.cu (streaming form),
-// capi_aux.cu (dynamic index, DataBlob, XXH3).
+// capi_aux.cu (dynamic index and the blocking byte-range calls: SHA-256, CRC-32, DataBlob, XXH3).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -1070,41 +1070,6 @@ extern "C" int pbsgpu_scan_batch(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const v
     }
     pbsgpu_job_release(j);
     return rc;
-}
-
-extern "C" int pbsgpu_sha256_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
-                                   uint32_t n, uint8_t *digests) {
-    if (!ctx || (n && (!off || !len || !digests))) return PBSGPU_EINVAL;
-    Guard g(ctx);
-    if (n == 0) return PBSGPU_OK;
-    cudaStream_t st = ctx->streams[0];
-    std::vector<ChunkRef> refs(n);
-    uint64_t hi = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        if (len[i] >= (1ull << 32)) return fail(ctx, PBSGPU_EINVAL, "range %u longer than 4 GiB", i);
-        refs[i].stream = i; refs[i].len = (uint32_t)len[i]; refs[i].start = off[i];
-        hi = std::max(hi, off[i] + len[i]);
-    }
-    const bool on_dev = pbsgpu_is_device_ptr(base);
-    Scoped staged(ctx->dev, on_dev ? 0 : hi + 16), d_refs(ctx->dev, sizeof(ChunkRef) * (size_t)n), d_dig(ctx->dev, (uint64_t)n * 32), d_n(ctx->dev, 8);
-    if (!staged || !d_refs || !d_dig || !d_n) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed (%llu bytes staged)", (unsigned long long)hi);
-    const uint8_t *dbase = (const uint8_t *)base;
-    if (!on_dev) {
-        CK(cudaMemcpyAsync(staged.p, base, hi, cudaMemcpyHostToDevice, st));
-        dbase = staged.as<uint8_t>();
-    }
-    unsigned long long hn = n;
-    CK(cudaMemcpyAsync(d_refs.p, refs.data(), sizeof(ChunkRef) * n, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_n.p, &hn, 8, cudaMemcpyHostToDevice, st));
-    ShaArgs ha;
-    ha.base = dbase; ha.off = nullptr; ha.chunks = d_refs.as<ChunkRef>(); ha.order = nullptr; ha.n_chunks = d_n.as<unsigned long long>();
-    ha.chunk_cap = n; ha.digests = d_dig.as<uint8_t>(); ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
-    cudaError_t e = ctx->variant == 1 ? launch_sha_simple(ha, st) : launch_sha_tuned(ha, ctx->tune, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(digests, d_dig.p, (uint64_t)n * 32, cudaMemcpyDeviceToHost, st);
-    cudaError_t es = cudaStreamSynchronize(st);   // always: the scoped blocks must not return to the pool while in use
-    if (e == cudaSuccess) e = es;
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "sha256 batch: %s", cudaGetErrorString(e)); }
-    return PBSGPU_OK;
 }
 
 // ---------------------------------------------------------------------------

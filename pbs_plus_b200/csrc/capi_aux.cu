@@ -1,5 +1,6 @@
 // pbs_plus_b200/csrc/capi_aux.cu -- C ABI of the "next" rows of SURVEY.md section 8: dynamic index images (f1), the commit
-// walk's per-file XXH3-64 (f2) and DataBlob framing + CRC-32 for new chunks (f3).
+// walk's per-file XXH3-64 (f2) and DataBlob framing + CRC-32 for new chunks (f3); and the SHA-256 of byte ranges.
+// Except for the index images these are blocking calls (host.hpp, Blocking).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -9,10 +10,48 @@
 using namespace pbsgpu;
 
 // ---------------------------------------------------------------------------
+// blocking calls: completion, staging of the caller's bytes, constant tables
+// ---------------------------------------------------------------------------
+int pbsgpu_finish(pbsgpu_ctx *ctx, cudaStream_t st, cudaError_t e, const char *what) {
+    const cudaError_t es = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = es;
+    if (e == cudaSuccess) return PBSGPU_OK;
+    (void)cudaGetLastError();
+    return fail(ctx, PBSGPU_ECUDA, "%s: %s", what, cudaGetErrorString(e));
+}
+
+Blocking::~Blocking() {
+    if (blocks.empty()) return;
+    if (cudaStreamSynchronize(st) != cudaSuccess) (void)cudaGetLastError();
+    for (void *p : blocks) ctx->dev.put(p);
+}
+
+int Blocking::stage(const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, const uint8_t **dbase) {
+    uint64_t hi = 0;
+    for (uint32_t i = 0; i < n; i++) hi = std::max(hi, off[i] + len[i]);
+    *dbase = (const uint8_t *)base;
+    if (hi == 0 || pbsgpu_is_device_ptr(base)) return PBSGPU_OK;
+    uint8_t *p = get<uint8_t>(hi + 16);
+    if (!p) return fail(ctx, PBSGPU_ENOMEM, "staging of %llu bytes failed", (unsigned long long)hi);
+    *dbase = p;
+    if (ok()) e = cudaMemcpyAsync(p, base, hi, cudaMemcpyHostToDevice, st);
+    return ok() ? PBSGPU_OK : finish("H2D copy");
+}
+
+// K6 / K7 constant tables: built on the host and uploaded on the context's first use (freed with the context)
+static int upload_table_once(pbsgpu_ctx *ctx, void **d, size_t bytes, void (*fill)(void *)) {
+    if (*d) return PBSGPU_OK;
+    std::vector<uint8_t> h(bytes);
+    fill(h.data());
+    CK(cudaMalloc(d, bytes));
+    CK(cudaMemcpy(*d, h.data(), bytes, cudaMemcpyHostToDevice));
+    return PBSGPU_OK;
+}
+
+// ---------------------------------------------------------------------------
 // f1: dynamic index images
 // ---------------------------------------------------------------------------
 static const uint8_t DIDX_MAGIC[8] = {28, 145, 78, 165, 25, 186, 179, 205};
-extern "C" int pbsgpu_sha256_batch(pbsgpu_ctx *, const void *, const uint64_t *, const uint64_t *, uint32_t, uint8_t *);
 
 extern "C" uint64_t pbsgpu_didx_size(uint64_t n) { return 4096 + n * 40; }
 
@@ -71,34 +110,52 @@ extern "C" int pbsgpu_didx_parse(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t 
 }
 
 // ---------------------------------------------------------------------------
+// SHA-256 of n byte ranges (K3 without the chunker)
+// ---------------------------------------------------------------------------
+extern "C" int pbsgpu_sha256_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
+                                   uint32_t n, uint8_t *digests) {
+    if (!ctx || (n && (!off || !len || !digests))) return PBSGPU_EINVAL;
+    Guard g(ctx);
+    if (n == 0) return PBSGPU_OK;
+    std::vector<ChunkRef> refs(n);
+    for (uint32_t i = 0; i < n; i++) {
+        if (len[i] >= (1ull << 32)) return fail(ctx, PBSGPU_EINVAL, "range %u longer than 4 GiB", i);
+        refs[i].stream = i; refs[i].len = (uint32_t)len[i]; refs[i].start = off[i];
+    }
+    Blocking b(ctx, ctx->streams[0]);
+    ShaArgs ha;
+    if (int rc = b.stage(base, off, len, n, &ha.base)) return rc;
+    const unsigned long long hn = n;
+    ha.off = nullptr; ha.chunks = b.upload(refs.data(), n); ha.order = nullptr; ha.n_chunks = b.upload(&hn, 1);
+    ha.chunk_cap = n; ha.digests = b.get<uint8_t>((uint64_t)n * 32); ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
+    if (!ha.chunks || !ha.n_chunks || !ha.digests) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (b.ok()) b.e = ctx->variant == 1 ? launch_sha_simple(ha, b.st) : launch_sha_tuned(ha, ctx->tune, b.st);
+    if (b.ok()) b.e = cudaMemcpyAsync(digests, ha.digests, (uint64_t)n * 32, cudaMemcpyDeviceToHost, b.st);
+    return b.finish("sha256 batch");
+}
+
+// ---------------------------------------------------------------------------
 // f3: DataBlob checksums
 // ---------------------------------------------------------------------------
 static const uint8_t BLOB_MAGIC_UNCOMPRESSED[8] = {66, 171, 56, 7, 190, 131, 112, 161};
+static const uint8_t BLOB_MAGIC_COMPRESSED[8] = {49, 185, 88, 66, 111, 182, 163, 127};
 
-extern "C" void pbsgpu_blob_header(uint32_t crc, uint8_t out[12]) {
-    memcpy(out, BLOB_MAGIC_UNCOMPRESSED, 8);
+static void blob_header(const uint8_t magic[8], uint32_t crc, uint8_t *out) {
+    memcpy(out, magic, 8);
     for (int i = 0; i < 4; i++) out[8 + i] = (uint8_t)(crc >> (8 * i));
 }
+extern "C" void pbsgpu_blob_header(uint32_t crc, uint8_t out[12]) { blob_header(BLOB_MAGIC_UNCOMPRESSED, crc, out); }
 
 extern "C" int pbsgpu_crc32_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
                                   uint32_t n, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !crc_out))) return PBSGPU_EINVAL;
     Guard g(ctx);
     if (n == 0) return PBSGPU_OK;
-    cudaStream_t st = ctx->streams[0];
-    if (!ctx->d_crc_tables) {
-        std::vector<uint8_t> h(crc_tables_bytes());
-        crc_fill_tables_host(h.data());
-        CK(cudaMalloc(&ctx->d_crc_tables, h.size()));
-        CK(cudaMemcpy(ctx->d_crc_tables, h.data(), h.size(), cudaMemcpyHostToDevice));
-    }
+    if (int rc = upload_table_once(ctx, &ctx->d_crc_tables, crc_tables_bytes(), crc_fill_tables_host)) return rc;
     const int crc_variant = ctx->crc_variant;   // 0 = TMA-tiled kernel (default), 1 = simple lane-strided kernel (PBSGPU_CRC_VARIANT at open)
-    uint64_t hi = 0;
-    for (uint32_t i = 0; i < n; i++) hi = std::max(hi, off[i] + len[i]);
-    const bool on_dev = !hi || pbsgpu_is_device_ptr(base);
-    Scoped staged(ctx->dev, on_dev ? 0 : hi + 16);
-    if (!staged) return fail(ctx, PBSGPU_ENOMEM, "staging of %llu bytes failed", (unsigned long long)hi);
-    const uint8_t *dbase = on_dev ? (const uint8_t *)base : staged.as<uint8_t>();
+    Blocking b(ctx, ctx->streams[0]);
+    const uint8_t *dbase;
+    if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
     // work units: 128 KiB warp blocks (simple) or <= 576 KiB regions of the 16 B aligned body (tiled)
     const uint64_t UNIT = crc_variant ? crc_wb_bytes() : crc_region_bytes();
     std::vector<uint64_t> wb_first(n + 1);
@@ -113,76 +170,40 @@ extern "C" int pbsgpu_crc32_batch(pbsgpu_ctx *ctx, const void *base, const uint6
         }
     }
     wb_first[n] = total;
-    Scoped d_off(ctx->dev, n * 8), d_len(ctx->dev, n * 8), d_first(ctx->dev, (n + 1) * 8), d_part(ctx->dev, (total + 1) * 4), d_out(ctx->dev, (uint64_t)n * 4);
+    uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n), *d_first = b.upload(wb_first.data(), n + 1);
+    uint32_t *d_part = b.get<uint32_t>(total + 1), *d_out = b.get<uint32_t>(n);
     if (!d_off || !d_len || !d_first || !d_part || !d_out) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
-    cudaError_t e = on_dev ? cudaSuccess : cudaMemcpyAsync(staged.p, base, hi, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_off.p, off, n * 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_len.p, len, n * 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_first.p, wb_first.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess)
-        e = crc_variant ? launch_crc32(dbase, d_off.as<uint64_t>(), d_len.as<uint64_t>(), d_first.as<uint64_t>(), n, total, ctx->d_crc_tables,
-                                       d_part.as<uint32_t>(), d_out.as<uint32_t>(), ctx->sm_count, st)
-                        : launch_crc32_tiled(dbase, d_off.as<uint64_t>(), d_len.as<uint64_t>(), d_first.as<uint64_t>(), n, total,
-                                             ctx->d_crc_tables, d_part.as<uint32_t>(), d_out.as<uint32_t>(), ctx->sm_count, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(crc_out, d_out.p, (uint64_t)n * 4, cudaMemcpyDeviceToHost, st);
-    cudaError_t es = cudaStreamSynchronize(st);   // always: scoped blocks must be idle before they return to the pool
-    if (e == cudaSuccess) e = es;
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "crc32 batch: %s", cudaGetErrorString(e)); }
-    return PBSGPU_OK;
+    if (b.ok())
+        b.e = crc_variant ? launch_crc32(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st)
+                          : launch_crc32_tiled(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st);
+    if (b.ok()) b.e = cudaMemcpyAsync(crc_out, d_out, (uint64_t)n * 4, cudaMemcpyDeviceToHost, b.st);
+    return b.finish("crc32 batch");
 }
 
 uint64_t pbsgpu_blob_size_impl(uint64_t payload) { return payload + 12; }
 extern "C" uint64_t pbsgpu_blob_size(uint64_t payload_len) { return pbsgpu_blob_size_impl(payload_len); }
 
-// f3: complete uncompressed DataBlobs for the NEW chunks of a batch in one call (upstream pbs-datastore data_blob.rs:
-// magic[8] | crc32 LE over the payload | payload; uploaded by POST /dynamic_chunk, reference
-// internal/server/backup/log_cleanup.go:19-31).  The CRCs come from K6 on the device; payload bytes are copied once
-// (device -> host for resident data, host -> host otherwise) straight into their place behind the header.
-extern "C" int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
-                                        uint8_t *out, const uint64_t *out_off, uint32_t *crc_out) {
-    if (!ctx || (n && (!off || !len || !out || !out_off || !base))) return PBSGPU_EINVAL;
-    Guard g(ctx);
-    if (n == 0) return PBSGPU_OK;
-    std::vector<uint32_t> crc(n);
-    int rc = pbsgpu_crc32_batch(ctx, base, off, len, n, crc.data());
-    if (rc) return rc;
-    const bool on_dev = pbsgpu_is_device_ptr(base);
-    cudaStream_t st = ctx->copy_stream;
-    for (uint32_t i = 0; i < n; i++) {
-        uint8_t *b = out + out_off[i];
-        pbsgpu_blob_header(crc[i], b);
-        if (!len[i]) continue;
-        if (on_dev) {
-            cudaError_t e = cudaMemcpyAsync(b + 12, (const uint8_t *)base + off[i], len[i], cudaMemcpyDeviceToHost, st);
-            if (e != cudaSuccess) { (void)cudaGetLastError(); cudaStreamSynchronize(st); return fail(ctx, PBSGPU_ECUDA, "blob payload copy: %s", cudaGetErrorString(e)); }
-        } else memcpy(b + 12, (const uint8_t *)base + off[i], len[i]);
-    }
-    if (on_dev) CK(cudaStreamSynchronize(st));
-    if (crc_out) memcpy(crc_out, crc.data(), (size_t)n * 4);
-    return PBSGPU_OK;
+// CRC-32 (K6) of the ranges [src + o[i], + l[i]) of the blobs with comp[i] == want, into crc[i]
+static int crc_where(pbsgpu_ctx *ctx, const std::vector<uint8_t> &comp, uint8_t want, const void *src, const uint64_t *o,
+                     const uint64_t *l, std::vector<uint32_t> &crc) {
+    std::vector<uint64_t> so, sl;
+    std::vector<uint32_t> idx;
+    for (uint32_t i = 0; i < comp.size(); i++) if (comp[i] == want) { idx.push_back(i); so.push_back(o[i]); sl.push_back(l[i]); }
+    std::vector<uint32_t> c(idx.size());
+    int rc = pbsgpu_crc32_batch(ctx, src, so.data(), sl.data(), (uint32_t)idx.size(), c.data());
+    for (size_t k = 0; rc == PBSGPU_OK && k < idx.size(); k++) crc[idx[k]] = c[k];
+    return rc;
 }
 
-// f3, compressed form: DataBlobs whose payload is a zstd frame when that is smaller than the raw bytes (upstream
+// Compressed form: a blob's payload is a zstd frame when that is smaller than the raw bytes (upstream
 // `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device from RLE_Blocks (128 KiB
 // blocks of one repeated byte) and Raw_Blocks (zframe.cu) -- no match / entropy stage; the CRC (K6) covers the frame.
-static const uint8_t BLOB_MAGIC_COMPRESSED[8] = {49, 185, 88, 66, 111, 182, 163, 127};
-
-extern "C" int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
-                                          uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
-    if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
-    Guard g(ctx);
-    if (n == 0) return PBSGPU_OK;
-    cudaStream_t st = ctx->streams[0];
-    uint64_t hi = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        if (len[i] >= (1ull << 40)) return fail(ctx, PBSGPU_EINVAL, "blob %u longer than 2^40 bytes", i);
-        hi = std::max(hi, off[i] + len[i]);
-    }
-    const bool on_dev = !hi || pbsgpu_is_device_ptr(base);
-    Scoped staged(ctx->dev, on_dev ? 0 : hi + 16);
-    if (!staged) return fail(ctx, PBSGPU_ENOMEM, "staging of %llu bytes failed", (unsigned long long)hi);
-    const uint8_t *dbase = on_dev ? (const uint8_t *)base : staged.as<uint8_t>();
-    if (!on_dev) CK(cudaMemcpyAsync(staged.p, base, hi, cudaMemcpyHostToDevice, st));
+// Marks those blobs in comp[] and leaves their frames at *frames + frame_off[i] (frame_len[i] bytes, a block of `b`)
+// and their CRCs in crc[].
+static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n,
+                       std::vector<uint8_t> &comp, std::vector<uint64_t> &frame_off, std::vector<uint64_t> &frame_len,
+                       std::vector<uint32_t> &crc, const uint8_t **frames) {
+    pbsgpu_ctx *ctx = b.ctx;
     // K8a: which 128 KiB blocks are one repeated byte
     std::vector<uint64_t> blk_first(n + 1);
     uint64_t n_blocks = 0;
@@ -190,106 +211,105 @@ extern "C" int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, con
     blk_first[n] = n_blocks;
     if (n_blocks >= (1ull << 31)) return fail(ctx, PBSGPU_EINVAL, "too many 128 KiB blocks in one call (%llu)", (unsigned long long)n_blocks);
     std::vector<uint32_t> flags(n_blocks);
-    {
-        Scoped d_off(ctx->dev, n * 8), d_len(ctx->dev, n * 8), d_first(ctx->dev, (n + 1) * 8), d_flags(ctx->dev, (n_blocks + 1) * 4);
-        if (!d_off || !d_len || !d_first || !d_flags) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
-        cudaError_t e = cudaMemcpyAsync(d_off.p, off, n * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_len.p, len, n * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_first.p, blk_first.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = launch_zblock_scan(dbase, d_off.as<uint64_t>(), d_len.as<uint64_t>(), d_first.as<uint64_t>(), n, n_blocks, d_flags.as<uint32_t>(), st);
-        if (e == cudaSuccess && n_blocks) e = cudaMemcpyAsync(flags.data(), d_flags.p, n_blocks * 4, cudaMemcpyDeviceToHost, st);
-        cudaError_t es = cudaStreamSynchronize(st);
-        if (e == cudaSuccess) e = es;
-        if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "zstd block scan: %s", cudaGetErrorString(e)); }
-    }
-    // frame sizes; the chunks that come out smaller get a place in the stage and one emit entry per block
-    std::vector<uint8_t> comp(n, 0);
-    std::vector<uint64_t> frame_len(n, 0), frame_off, content, e_src, e_dst;
-    std::vector<uint32_t> e_hdr, comp_idx;
+    uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n), *d_first = b.upload(blk_first.data(), n + 1);
+    uint32_t *d_flags = b.get<uint32_t>(n_blocks + 1);
+    if (!d_off || !d_len || !d_first || !d_flags) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (b.ok()) b.e = launch_zblock_scan(dbase, d_off, d_len, d_first, n, n_blocks, d_flags, b.st);
+    if (b.ok() && n_blocks) b.e = cudaMemcpyAsync(flags.data(), d_flags, n_blocks * 4, cudaMemcpyDeviceToHost, b.st);
+    if (int rc = b.finish("zstd block scan")) return rc;
+    // frame sizes; the blobs that come out smaller get a place in the stage and one emit entry per block
+    std::vector<uint64_t> foff, content, e_src, e_dst;
+    std::vector<uint32_t> e_hdr;
     uint64_t cursor = 0;
     for (uint32_t i = 0; i < n; i++) {
         const uint64_t nb = blk_first[i + 1] - blk_first[i];
         uint64_t fl = ZFRAME_HEADER;
-        for (uint64_t b = 0; b < nb; b++) {
-            const uint64_t size = std::min<uint64_t>(ZFRAME_BLOCK, len[i] - b * ZFRAME_BLOCK);
-            fl += 3 + ((flags[blk_first[i] + b] & 0x100u) ? 1 : size);
+        for (uint64_t k = 0; k < nb; k++) {
+            const uint64_t size = std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK);
+            fl += 3 + ((flags[blk_first[i] + k] & 0x100u) ? 1 : size);
         }
-        frame_len[i] = fl;
         if (len[i] == 0 || fl >= len[i]) continue;
-        comp[i] = 1;
-        comp_idx.push_back(i);
-        frame_off.push_back(cursor);
+        comp[i] = 1; frame_off[i] = cursor; frame_len[i] = fl;
+        foff.push_back(cursor);
         content.push_back(len[i]);
         uint64_t pos = cursor + ZFRAME_HEADER;
-        for (uint64_t b = 0; b < nb; b++) {
-            const uint64_t size = std::min<uint64_t>(ZFRAME_BLOCK, len[i] - b * ZFRAME_BLOCK);
-            const uint32_t f = flags[blk_first[i] + b];
+        for (uint64_t k = 0; k < nb; k++) {
+            const uint64_t size = std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK);
+            const uint32_t f = flags[blk_first[i] + k];
             const bool rle = (f & 0x100u) != 0;
-            e_src.push_back(off[i] + b * ZFRAME_BLOCK);
+            e_src.push_back(off[i] + k * ZFRAME_BLOCK);
             e_dst.push_back(pos);
-            e_hdr.push_back((uint32_t)(b + 1 == nb) | ((rle ? 1u : 0u) << 1) | ((uint32_t)size << 3) | ((f & 0xFFu) << 24));
+            e_hdr.push_back((uint32_t)(k + 1 == nb) | ((rle ? 1u : 0u) << 1) | ((uint32_t)size << 3) | ((f & 0xFFu) << 24));
             pos += 3 + (rle ? 1 : size);
         }
         cursor = (pos + 15) & ~15ull;
     }
-    const uint32_t nc = (uint32_t)comp_idx.size();
-    Scoped stage(ctx->dev, nc ? cursor + 16 : 0);
+    const uint32_t nc = (uint32_t)foff.size();
+    if (nc == 0) return PBSGPU_OK;
+    const uint64_t ne = e_hdr.size();
+    uint8_t *stage = b.get<uint8_t>(cursor + 16);
     if (!stage) return fail(ctx, PBSGPU_ENOMEM, "frame staging of %llu bytes failed", (unsigned long long)cursor);
+    uint64_t *d_src = b.upload(e_src.data(), ne), *d_dst = b.upload(e_dst.data(), ne);
+    uint64_t *d_foff = b.upload(foff.data(), nc), *d_clen = b.upload(content.data(), nc);
+    uint32_t *d_hdr = b.upload(e_hdr.data(), ne);
+    if (!d_src || !d_dst || !d_hdr || !d_foff || !d_clen) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (b.ok()) b.e = launch_zframe_hdr(stage, d_foff, d_clen, nc, b.st);
+    if (b.ok()) b.e = launch_zframe_emit(dbase, stage, d_src, d_dst, d_hdr, ne, b.st);
+    if (int rc = b.finish("zstd frame emit")) return rc;
+    *frames = stage;
+    return crc_where(ctx, comp, 1, stage, frame_off.data(), frame_len.data(), crc);
+}
+
+// f3: complete DataBlobs for the NEW chunks of a batch in one call (upstream pbs-datastore data_blob.rs:
+// magic[8] | crc32 LE over the payload | payload; uploaded by POST /dynamic_chunk, reference
+// internal/server/backup/log_cleanup.go:19-31), with zstd frames as payloads where they are smaller when `compress`.
+// The CRCs come from K6 on the device; payload bytes are copied once (device -> host for resident data and frames,
+// host -> host otherwise) straight into their place behind the header.
+static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, bool compress,
+                       uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    Guard g(ctx);
+    if (n == 0) return PBSGPU_OK;
+    for (uint32_t i = 0; compress && i < n; i++)
+        if (len[i] >= (1ull << 40)) return fail(ctx, PBSGPU_EINVAL, "blob %u longer than 2^40 bytes", i);
+    Blocking b(ctx, ctx->streams[0]);
+    const uint8_t *dbase, *frames = nullptr;
+    if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
+    std::vector<uint8_t> comp(n, 0);
+    std::vector<uint64_t> frame_off(n), frame_len(n);
     std::vector<uint32_t> crc(n, 0);
-    if (nc) {
-        const uint64_t ne = e_hdr.size();
-        Scoped d_src(ctx->dev, ne * 8), d_dst(ctx->dev, ne * 8), d_hdr(ctx->dev, ne * 4), d_foff(ctx->dev, nc * 8), d_clen(ctx->dev, nc * 8);
-        if (!d_src || !d_dst || !d_hdr || !d_foff || !d_clen) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
-        cudaError_t e = cudaMemcpyAsync(d_src.p, e_src.data(), ne * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_dst.p, e_dst.data(), ne * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_hdr.p, e_hdr.data(), ne * 4, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_foff.p, frame_off.data(), nc * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_clen.p, content.data(), nc * 8, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = launch_zframe_hdr(stage.as<uint8_t>(), d_foff.as<uint64_t>(), d_clen.as<uint64_t>(), nc, st);
-        if (e == cudaSuccess) e = launch_zframe_emit(dbase, stage.as<uint8_t>(), d_src.as<uint64_t>(), d_dst.as<uint64_t>(), d_hdr.as<uint32_t>(), ne, st);
-        cudaError_t es = cudaStreamSynchronize(st);
-        if (e == cudaSuccess) e = es;
-        if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "zstd frame emit: %s", cudaGetErrorString(e)); }
-        // CRC over the frames
-        std::vector<uint64_t> flen(nc);
-        std::vector<uint32_t> fcrc(nc);
-        for (uint32_t k = 0; k < nc; k++) flen[k] = frame_len[comp_idx[k]];
-        int rc = pbsgpu_crc32_batch(ctx, stage.p, frame_off.data(), flen.data(), nc, fcrc.data());
+    if (compress) {
+        int rc = zstd_frames(b, dbase, off, len, n, comp, frame_off, frame_len, crc, &frames);
         if (rc) return rc;
-        for (uint32_t k = 0; k < nc; k++) crc[comp_idx[k]] = fcrc[k];
     }
-    if (nc < n) {   // CRC over the raw payloads of the rest
-        std::vector<uint64_t> roff, rlen;
-        std::vector<uint32_t> ridx;
-        for (uint32_t i = 0; i < n; i++) if (!comp[i]) { ridx.push_back(i); roff.push_back(off[i]); rlen.push_back(len[i]); }
-        std::vector<uint32_t> rcrc(ridx.size());
-        int rc = pbsgpu_crc32_batch(ctx, hi ? (const void *)dbase : base, roff.data(), rlen.data(), (uint32_t)ridx.size(), rcrc.data());
-        if (rc) return rc;
-        for (size_t k = 0; k < ridx.size(); k++) crc[ridx[k]] = rcrc[k];
-    }
-    // assemble in the caller's memory
-    cudaStream_t cs = ctx->copy_stream;
-    uint32_t k = 0;
+    if (int rc = crc_where(ctx, comp, 0, dbase, off, len, crc)) return rc;
+    // assemble in the caller's memory; staged payloads are copied from the caller's host memory
+    const bool staged = dbase != (const uint8_t *)base;
     cudaError_t e = cudaSuccess;
     for (uint32_t i = 0; i < n && e == cudaSuccess; i++) {
-        uint8_t *b = out + out_off[i];
-        memcpy(b, comp[i] ? BLOB_MAGIC_COMPRESSED : BLOB_MAGIC_UNCOMPRESSED, 8);
-        for (int q = 0; q < 4; q++) b[8 + q] = (uint8_t)(crc[i] >> (8 * q));
-        if (comp[i]) {
-            e = cudaMemcpyAsync(b + 12, stage.as<uint8_t>() + frame_off[k++], frame_len[i], cudaMemcpyDeviceToHost, cs);
-            out_len[i] = 12 + frame_len[i];
-        } else {
-            out_len[i] = 12 + len[i];
-            if (!len[i]) continue;
-            if (on_dev) e = cudaMemcpyAsync(b + 12, (const uint8_t *)base + off[i], len[i], cudaMemcpyDeviceToHost, cs);
-            else memcpy(b + 12, (const uint8_t *)base + off[i], len[i]);
-        }
+        uint8_t *blob = out + out_off[i];
+        blob_header(comp[i] ? BLOB_MAGIC_COMPRESSED : BLOB_MAGIC_UNCOMPRESSED, crc[i], blob);
+        const uint64_t plen = comp[i] ? frame_len[i] : len[i];
+        if (out_len) out_len[i] = 12 + plen;
+        if (plen == 0) continue;
+        if (comp[i]) e = cudaMemcpyAsync(blob + 12, frames + frame_off[i], plen, cudaMemcpyDeviceToHost, ctx->copy_stream);
+        else if (staged) memcpy(blob + 12, (const uint8_t *)base + off[i], plen);
+        else e = cudaMemcpyAsync(blob + 12, dbase + off[i], plen, cudaMemcpyDeviceToHost, ctx->copy_stream);
     }
-    cudaError_t es = cudaStreamSynchronize(cs);
-    if (e == cudaSuccess) e = es;
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "blob assembly copy: %s", cudaGetErrorString(e)); }
+    if (int rc = pbsgpu_finish(ctx, ctx->copy_stream, e, "blob assembly copy")) return rc;
     if (crc_out) memcpy(crc_out, crc.data(), (size_t)n * 4);
     return PBSGPU_OK;
+}
+
+extern "C" int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                        uint8_t *out, const uint64_t *out_off, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !out || !out_off || !base))) return PBSGPU_EINVAL;
+    return blob_encode(ctx, base, off, len, n, false, out, out_off, nullptr, crc_out);
+}
+
+extern "C" int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                          uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
+    return blob_encode(ctx, base, off, len, n, true, out, out_off, out_len, crc_out);
 }
 
 // ---------------------------------------------------------------------------
@@ -308,12 +328,7 @@ void pbsgpu_xxh3_release(pbsgpu_ctx *ctx, XxhRun *r) {
 
 int pbsgpu_xxh3_enqueue(pbsgpu_ctx *ctx, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n,
                         cudaStream_t st, XxhRun *r) {
-    if (!ctx->d_xxh_tab) {
-        std::vector<uint8_t> h(xxh3_tables_bytes());
-        xxh3_fill_tables_host(h.data());
-        CK(cudaMalloc(&ctx->d_xxh_tab, h.size()));
-        CK(cudaMemcpy(ctx->d_xxh_tab, h.data(), h.size(), cudaMemcpyHostToDevice));
-    }
+    if (int rc = upload_table_once(ctx, &ctx->d_xxh_tab, xxh3_tables_bytes(), xxh3_fill_tables_host)) return rc;
     const uint64_t cap_blocks = ctx->xxh3_cap_blocks;
     uint64_t total_all = 0, max_nb = 0, n_long = 0;
     std::vector<uint64_t> nb(n);
@@ -350,22 +365,17 @@ int pbsgpu_xxh3_enqueue(pbsgpu_ctx *ctx, const uint8_t *dbase, const uint64_t *o
         e = cudaMemcpyAsync(df, first.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st);
         if (e == cudaSuccess) e = launch_xxh3_pass(dbase, r->d_off, r->d_len, df, n, total, lo, win, ctx->d_xxh_tab, r->d_S, r->d_state, r->d_out, st);
     }
-    if (e != cudaSuccess) {
-        (void)cudaGetLastError();
-        cudaStreamSynchronize(st);
-        pbsgpu_xxh3_release(ctx, r);
-        return fail(ctx, PBSGPU_ECUDA, "xxh3: %s", cudaGetErrorString(e));
-    }
-    return PBSGPU_OK;
+    if (e == cudaSuccess) return PBSGPU_OK;
+    const int rc = pbsgpu_finish(ctx, st, e, "xxh3");   // the run's blocks go back once the stream is idle
+    pbsgpu_xxh3_release(ctx, r);
+    return rc;
 }
 
 int pbsgpu_xxh3_collect(pbsgpu_ctx *ctx, XxhRun *r, uint64_t *hash_out, cudaStream_t st) {
     if (!r->d_out) return PBSGPU_OK;
-    cudaError_t e = cudaMemcpyAsync(hash_out, r->d_out, (uint64_t)r->n * 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    const int rc = pbsgpu_finish(ctx, st, cudaMemcpyAsync(hash_out, r->d_out, (uint64_t)r->n * 8, cudaMemcpyDeviceToHost, st), "xxh3");
     pbsgpu_xxh3_release(ctx, r);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "xxh3: %s", cudaGetErrorString(e)); }
-    return PBSGPU_OK;
+    return rc;
 }
 
 extern "C" int pbsgpu_xxh3_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
@@ -373,20 +383,10 @@ extern "C" int pbsgpu_xxh3_batch(pbsgpu_ctx *ctx, const void *base, const uint64
     if (!ctx || (n && (!off || !len || !hash_out))) return PBSGPU_EINVAL;
     Guard g(ctx);
     if (n == 0) return PBSGPU_OK;
-    cudaStream_t st = ctx->streams[0];
-    uint64_t hi = 0;
-    for (uint32_t i = 0; i < n; i++) hi = std::max(hi, off[i] + len[i]);
-    const bool on_dev = !hi || pbsgpu_is_device_ptr(base);
-    Scoped staged(ctx->dev, on_dev ? 0 : hi + 16);
-    if (!staged) return fail(ctx, PBSGPU_ENOMEM, "staging of %llu bytes failed", (unsigned long long)hi);
-    const uint8_t *dbase = on_dev ? (const uint8_t *)base : staged.as<uint8_t>();
-    if (!on_dev) {
-        cudaError_t e = cudaMemcpyAsync(staged.p, base, hi, cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); cudaStreamSynchronize(st); return fail(ctx, PBSGPU_ECUDA, "H2D copy: %s", cudaGetErrorString(e)); }
-    }
+    Blocking b(ctx, ctx->streams[0]);
+    const uint8_t *dbase;
+    if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
     XxhRun run;
-    int rc = pbsgpu_xxh3_enqueue(ctx, dbase, off, len, n, st, &run);
-    if (rc == PBSGPU_OK) rc = pbsgpu_xxh3_collect(ctx, &run, hash_out, st);
-    else cudaStreamSynchronize(st);
-    return rc;
+    const int rc = pbsgpu_xxh3_enqueue(ctx, dbase, off, len, n, b.st, &run);
+    return rc ? rc : pbsgpu_xxh3_collect(ctx, &run, hash_out, b.st);
 }

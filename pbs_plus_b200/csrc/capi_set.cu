@@ -121,21 +121,19 @@ void pbsgpu_set_reconcile(pbsgpu_set *s, uint64_t cap, uint64_t n_new) {
 // d_dig: device pointer to n*32 bytes.  d_hit: device n bytes or NULL.  Synchronous (count known on return).
 int pbsgpu_set_process_dev(pbsgpu_set *s, const uint8_t *d_dig, uint64_t n, int do_insert, uint8_t *d_hit) {
     pbsgpu_ctx *ctx = s->ctx;
-    cudaStream_t st = ctx->streams[0];
     if (n == 0) return PBSGPU_OK;
     if (n >= (1ull << 31)) return fail(ctx, PBSGPU_EINVAL, "too many digests in one call");
-    Scoped scratch(ctx->dev, pbsgpu_set_scratch_bytes(n)), d_new(ctx->dev, 8);
+    Blocking b(ctx, ctx->streams[0]);
+    void *scratch = b.get<uint8_t>(pbsgpu_set_scratch_bytes(n));
+    unsigned long long *d_new = b.get<unsigned long long>(1), h_new = 0;
     if (!scratch || !d_new) return fail(ctx, PBSGPU_ENOMEM, "digest set scratch allocation failed");
-    CK(cudaMemsetAsync(d_new.p, 0, 8, st));
-    const int rc = pbsgpu_set_enqueue(s, d_dig, nullptr, n, do_insert, nullptr, 0, d_hit, d_new.as<unsigned long long>(), scratch.p, st);
-    unsigned long long h_new = 0;
-    cudaError_t e = rc ? cudaSuccess : cudaMemcpyAsync(&h_new, d_new.p, 8, cudaMemcpyDeviceToHost, st);
-    cudaError_t es = cudaStreamSynchronize(st);   // the scoped scratch must not return to the pool while kernels use it
-    if (rc) { (void)cudaGetLastError(); return rc; }
-    if (e == cudaSuccess) e = es;
-    pbsgpu_set_reconcile(s, do_insert ? n : 0, e == cudaSuccess ? h_new : 0);   // the enqueue added n to pending_max
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "digest set: %s", cudaGetErrorString(e)); }
-    return PBSGPU_OK;
+    b.e = cudaMemsetAsync(d_new, 0, 8, b.st);
+    if (!b.ok()) return b.finish("digest set");
+    if (int rc = pbsgpu_set_enqueue(s, d_dig, nullptr, n, do_insert, nullptr, 0, d_hit, d_new, scratch, b.st)) return rc;
+    b.e = cudaMemcpyAsync(&h_new, d_new, 8, cudaMemcpyDeviceToHost, b.st);
+    const int rc = b.finish("digest set");
+    pbsgpu_set_reconcile(s, do_insert ? n : 0, rc ? 0 : h_new);   // the enqueue added n to pending_max
+    return rc;
 }
 
 static int set_process(pbsgpu_set *s, const uint8_t *d32, uint64_t n, int do_insert, uint8_t *hit_host) {
@@ -143,20 +141,16 @@ static int set_process(pbsgpu_set *s, const uint8_t *d32, uint64_t n, int do_ins
     pbsgpu_ctx *ctx = s->ctx;
     Guard g(ctx);
     if (n == 0) return PBSGPU_OK;
-    cudaStream_t st = ctx->streams[0];
-    const bool on_dev = pbsgpu_is_device_ptr(d32);
-    Scoped staged(ctx->dev, on_dev ? 0 : n * 32), d_hit(ctx->dev, hit_host ? n : 0);
-    if (!staged || !d_hit) return fail(ctx, PBSGPU_ENOMEM, "digest staging allocation failed");
-    const uint8_t *d_dig = d32;
-    if (!on_dev) {
-        cudaError_t e = cudaMemcpyAsync(staged.p, d32, n * 32, cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); cudaStreamSynchronize(st); return fail(ctx, PBSGPU_ECUDA, "digest upload: %s", cudaGetErrorString(e)); }
-        d_dig = staged.as<uint8_t>();
-    }
-    int rc = pbsgpu_set_process_dev(s, d_dig, n, do_insert, hit_host ? d_hit.as<uint8_t>() : nullptr);
+    Blocking b(ctx, ctx->streams[0]);
+    const uint64_t zero = 0, bytes = n * 32;
+    const uint8_t *d_dig;
+    if (int rc = b.stage(d32, &zero, &bytes, 1, &d_dig)) return rc;
+    uint8_t *d_hit = hit_host ? b.get<uint8_t>(n) : nullptr;
+    if (hit_host && !d_hit) return fail(ctx, PBSGPU_ENOMEM, "hit flag allocation failed");
+    int rc = pbsgpu_set_process_dev(s, d_dig, n, do_insert, d_hit);
     if (rc == PBSGPU_OK && hit_host) {
-        cudaError_t e = cudaMemcpy(hit_host, d_hit.p, n, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); rc = fail(ctx, PBSGPU_ECUDA, "hit copy: %s", cudaGetErrorString(e)); }
+        b.e = cudaMemcpyAsync(hit_host, d_hit, n, cudaMemcpyDeviceToHost, b.st);
+        rc = b.finish("hit copy");
     }
     return rc;
 }
@@ -256,41 +250,41 @@ extern "C" int pbsgpu_set_allgather(pbsgpu_set *s, void *comm, const uint8_t *d3
     if (!N->h) return fail(ctx, PBSGPU_ENODEV, "NCCL unavailable: %s", N->why.c_str());
     int world = 0, rank = 0;
     if (N->CommCount(comm, &world) != 0 || N->CommUserRank(comm, &rank) != 0 || world < 1) return fail(ctx, PBSGPU_EINVAL, "bad NCCL communicator");
-    cudaStream_t st = ctx->streams[0];
-    if (s->last_valid) CK(cudaStreamWaitEvent(st, s->last, 0));
-    // 1. counts (one u64 per rank); the payload is padded to the largest, so the host needs them
-    Scoped d_counts(ctx->dev, (size_t)world * 8), h_counts_blk(ctx->pin, (size_t)world * 8 + 8);
-    if (!d_counts || !h_counts_blk) return fail(ctx, PBSGPU_ENOMEM, "allgather: allocation failed");
-    uint64_t *h_counts = h_counts_blk.as<uint64_t>();
-    h_counts[world] = n;
-    auto ncclck = [&](ncclResult r, const char *what) -> int {
-        if (r == 0) return PBSGPU_OK;
-        cudaStreamSynchronize(st);
-        return fail(ctx, PBSGPU_ECUDA, "%s: %s", what, N->GetErrorString ? N->GetErrorString(r) : "NCCL error");
+    Blocking b(ctx, ctx->streams[0]);
+    if (s->last_valid) CK(cudaStreamWaitEvent(b.st, s->last, 0));
+    auto ncclck = [&](ncclResult r, const char *what) {
+        return r == 0 ? PBSGPU_OK : fail(ctx, PBSGPU_ECUDA, "%s: %s", what, N->GetErrorString ? N->GetErrorString(r) : "NCCL error");
     };
-    CK(cudaMemcpyAsync(d_counts.as<uint64_t>() + rank, &h_counts[world], 8, cudaMemcpyHostToDevice, st));
-    int rc = ncclck(N->AllGather(d_counts.as<uint64_t>() + rank, d_counts.p, 1, NCCL_UINT64, comm, st), "ncclAllGather(counts)");
+    // 1. counts (one u64 per rank); the payload is padded to the largest, so the host needs them
+    uint64_t *d_counts = b.get<uint64_t>(world);
+    if (!d_counts) return fail(ctx, PBSGPU_ENOMEM, "allgather: allocation failed");
+    std::vector<uint64_t> h_counts(world);
+    b.e = cudaMemcpyAsync(d_counts + rank, &n, 8, cudaMemcpyHostToDevice, b.st);
+    if (!b.ok()) return b.finish("allgather counts");
+    int rc = ncclck(N->AllGather(d_counts + rank, d_counts, 1, NCCL_UINT64, comm, b.st), "ncclAllGather(counts)");
     if (rc) return rc;
-    CK(cudaMemcpyAsync(h_counts, d_counts.p, (size_t)world * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    b.e = cudaMemcpyAsync(h_counts.data(), d_counts, (size_t)world * 8, cudaMemcpyDeviceToHost, b.st);
+    rc = b.finish("allgather counts");
+    if (rc) return rc;
     uint64_t max_n = 0, total = 0, first = 0;
     for (int r = 0; r < world; r++) { max_n = std::max(max_n, h_counts[r]); if (r < rank) first += h_counts[r]; total += h_counts[r]; }
     if (total == 0) return PBSGPU_OK;
     if (total >= (1ull << 31)) return fail(ctx, PBSGPU_EINVAL, "too many digests in one merge");
     // 2. payload, padded to max_n rows per rank, then compacted into global (rank, index) order
-    Scoped padded(ctx->dev, (size_t)world * max_n * 32), dense(ctx->dev, total * 32), d_hit(ctx->dev, total), mine(ctx->dev, std::max<uint64_t>(max_n, 1) * 32);
-    if (!padded || !dense || !d_hit || !mine) return fail(ctx, PBSGPU_ENOMEM, "allgather: allocation of %llu digests failed", (unsigned long long)total);
-    uint8_t *slot = padded.as<uint8_t>() + (size_t)rank * max_n * 32;
-    if (n) CK(cudaMemcpyAsync(slot, d32, n * 32, pbsgpu_is_device_ptr(d32) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-    rc = ncclck(N->AllGather(slot, padded.p, max_n * 32, NCCL_UINT8, comm, st), "ncclAllGather(digests)");
+    uint8_t *padded = b.get<uint8_t>((uint64_t)world * max_n * 32), *dense = b.get<uint8_t>(total * 32), *d_hit = b.get<uint8_t>(total);
+    if (!padded || !dense || !d_hit) return fail(ctx, PBSGPU_ENOMEM, "allgather: allocation of %llu digests failed", (unsigned long long)total);
+    uint8_t *slot = padded + (size_t)rank * max_n * 32;
+    if (n) b.e = cudaMemcpyAsync(slot, d32, n * 32, pbsgpu_is_device_ptr(d32) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, b.st);
+    if (!b.ok()) return b.finish("allgather digests");
+    rc = ncclck(N->AllGather(slot, padded, max_n * 32, NCCL_UINT8, comm, b.st), "ncclAllGather(digests)");
     if (rc) return rc;
-    cudaError_t e = launch_set_compact_gather(padded.as<uint8_t>(), d_counts.as<uint64_t>(), (uint32_t)world, max_n, dense.as<uint8_t>(), st);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); cudaStreamSynchronize(st); return fail(ctx, PBSGPU_ECUDA, "allgather compaction: %s", cudaGetErrorString(e)); }
+    b.e = launch_set_compact_gather(padded, d_counts, (uint32_t)world, max_n, dense, b.st);
+    if (!b.ok()) return b.finish("allgather compaction");
     // 3. every rank inserts everything in the same order: replicas stay identical, flags equal a single-GPU run
-    rc = pbsgpu_set_process_dev(s, dense.as<uint8_t>(), total, 1, d_hit.as<uint8_t>());
+    rc = pbsgpu_set_process_dev(s, dense, total, 1, d_hit);
     if (rc == PBSGPU_OK && hit && n) {
-        e = cudaMemcpy(hit, d_hit.as<uint8_t>() + first, n, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); rc = fail(ctx, PBSGPU_ECUDA, "hit copy: %s", cudaGetErrorString(e)); }
+        b.e = cudaMemcpyAsync(hit, d_hit + first, n, cudaMemcpyDeviceToHost, b.st);
+        rc = b.finish("hit copy");
     }
     return rc;
 }

@@ -26,16 +26,6 @@ struct Pool {
     void trim();
     void destroy();
 };
-// scope guard for a pool block: error paths return without leaking the block
-struct Scoped {
-    Pool *pool; void *p;
-    Scoped(Pool &pl, size_t bytes) : pool(&pl), p(pl.get(bytes)) {}
-    ~Scoped() { if (p) pool->put(p); }
-    Scoped(const Scoped &) = delete;
-    Scoped &operator=(const Scoped &) = delete;
-    template <typename T> T *as() const { return (T *)p; }
-    explicit operator bool() const { return p != nullptr; }
-};
 
 constexpr int N_SCAN_STREAMS = 3;
 constexpr int N_STREAMS = 32;   // upper bound of stream slots (main + side stream each); beyond 15 slots streams share the 32 HW queues
@@ -123,6 +113,41 @@ struct Guard {
 bool pbsgpu_is_device_ptr(const void *p);
 bool pbsgpu_is_pinned_ptr(const void *p);
 bool pbsgpu_cfg_ok(const pbsgpu_cfg *c);
+
+// ---------------------------------------------------------------------------
+// Blocking calls (capi_aux.cu, capi_set.cu): the device work is a chain of enqueues on one stream and the call returns
+// once it is done.  pbsgpu_finish always synchronises `st`, then maps the chain's first error `e` (or the sync's) to
+// PBSGPU_ECUDA "what: ...".  A Blocking keeps that first error (enqueue only while ok()) and the call's pool blocks;
+// they go back to the pool in the destructor after one more synchronisation, so on every exit path no kernel still uses
+// a block the pool can hand out again.
+// ---------------------------------------------------------------------------
+int pbsgpu_finish(pbsgpu_ctx *ctx, cudaStream_t st, cudaError_t e, const char *what);
+struct Blocking {
+    pbsgpu_ctx *ctx;
+    cudaStream_t st;
+    cudaError_t e = cudaSuccess;
+    std::vector<void *> blocks;
+    Blocking(pbsgpu_ctx *c, cudaStream_t s) : ctx(c), st(s) {}
+    ~Blocking();
+    Blocking(const Blocking &) = delete;
+    Blocking &operator=(const Blocking &) = delete;
+    bool ok() const { return e == cudaSuccess; }
+    template <typename T> T *get(uint64_t count) {   // NULL when the pool is exhausted
+        void *p = ctx->dev.get(count * sizeof(T));
+        if (p) blocks.push_back(p);
+        return (T *)p;
+    }
+    template <typename T> T *upload(const T *h, uint64_t count) {   // get + H2D copy of h[0, count)
+        T *d = get<T>(count);
+        if (d && ok()) e = cudaMemcpyAsync(d, h, count * sizeof(T), cudaMemcpyHostToDevice, st);
+        return d;
+    }
+    // The caller's ranges [base + off[i], + len[i]) on the device, as one span [base, base + hi) with hi the largest
+    // range end: `base` itself when it is device memory or nothing is read (hi == 0: base is never dereferenced), else a
+    // block filled by an H2D copy of the span.  ENOMEM / ECUDA when that fails.
+    int stage(const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, const uint8_t **dbase);
+    int finish(const char *what) { return pbsgpu_finish(ctx, st, e, what); }
+};
 
 // ---------------------------------------------------------------------------
 // digest set (capi_set.cu)

@@ -165,9 +165,10 @@ def test_sha256_batch_all_small_lengths_and_alignments(eng, torch):
         for a in (0, 1, 2, 3, 5, 13):
             offs.append(a + 7 * (n % 11))
             lens.append(n)
-    for host in (False, True):
+    # the last input is a host base with every range empty at offset 0: nothing is staged and the base is not read
+    for host, offs, lens in ((False, offs, lens), (True, offs, lens), (True, [0] * 4, [0] * 4)):
         dig = eng.sha256_batch(data if host else to_dev(torch, data), offs, lens)
-        for o, n, d in zip(offs, lens, dig):
+        for o, n, d in zip(offs, lens, dig, strict=True):
             assert bytes(d) == hashlib.sha256(data[o:o + n].tobytes()).digest(), (o, n, host)
 
 
@@ -522,9 +523,10 @@ def test_crc32_batch_matches_zlib(eng, torch):
               131072, 131073, 262144, 589823, 589824, 589825, 1_000_003, 2_500_000]:
         for a in (0, 1, 2, 3, 15, 16, 17):
             offs.append(a); lens.append(n)
-    for host in (True, False):
+    # the first input is a host base with every range empty at offset 0: nothing is staged and the base is not read
+    for host, offs, lens in ((True, [0] * 4, [0] * 4), (True, offs, lens), (False, offs, lens)):
         crc = eng.crc32_batch(data if host else to_dev(torch, data), offs, lens)
-        for o, n, c in zip(offs, lens, crc):
+        for o, n, c in zip(offs, lens, crc, strict=True):
             assert int(c) == zlib.crc32(data[o:o + n].tobytes()), (o, n, host)
     hdr = eng.blob_header(int(crc[-1]))
     assert hdr[:8] == bytes([66, 171, 56, 7, 190, 131, 112, 161]) and int.from_bytes(hdr[8:], "little") == int(crc[-1])
