@@ -281,6 +281,12 @@ int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *
  * same input (no two zstd encoders are). */
 int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+/* pbsgpu_blob_encode_batch_z with a match stage: every 128 KiB block that is not one repeated byte is a zstd
+ * Compressed_Block -- a greedy LZ77 parse inside the block, raw literals and sequences coded with the predefined FSE
+ * tables -- when that is smaller than the block, else a Raw_Block.  Same arguments, limits and errors as _z; each blob is
+ * at most the size of its _z blob.  The output is a deterministic function of the chunk bytes. */
+int pbsgpu_blob_encode_batch_lz(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------
  * emitBackedFile tees every new file through `xxh3.New()` and keeps `h.Sum64()` (reference

@@ -196,11 +196,12 @@ static int crc_where(pbsgpu_ctx *ctx, const std::vector<uint8_t> &comp, uint8_t 
 }
 
 // Compressed form: a blob's payload is a zstd frame when that is smaller than the raw bytes (upstream
-// `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device from RLE_Blocks (128 KiB
-// blocks of one repeated byte) and Raw_Blocks (zframe.cu) -- no match / entropy stage; the CRC (K6) covers the frame.
-// Marks those blobs in comp[] and leaves their frames at *frames + frame_off[i] (frame_len[i] bytes, a block of `b`)
-// and their CRCs in crc[].
-static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n,
+// `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device (zframe.cu, zlz.cu): a
+// 128 KiB block of one repeated byte is an RLE_Block (K8a decides); with `lz` every other block goes through the match
+// stage (K9) and is a Compressed_Block when that is smaller than the block; the rest are Raw_Blocks.  The CRC (K6) covers
+// the frame.  Marks those blobs in comp[] and leaves their frames at *frames + frame_off[i] (frame_len[i] bytes, a block
+// of `b`) and their CRCs in crc[].
+static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, bool lz,
                        std::vector<uint8_t> &comp, std::vector<uint64_t> &frame_off, std::vector<uint64_t> &frame_len,
                        std::vector<uint32_t> &crc, const uint8_t **frames) {
     pbsgpu_ctx *ctx = b.ctx;
@@ -217,44 +218,95 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
     if (b.ok()) b.e = launch_zblock_scan(dbase, d_off, d_len, d_first, n, n_blocks, d_flags, b.st);
     if (b.ok() && n_blocks) b.e = cudaMemcpyAsync(flags.data(), d_flags, n_blocks * 4, cudaMemcpyDeviceToHost, b.st);
     if (int rc = b.finish("zstd block scan")) return rc;
-    // frame sizes; the blobs that come out smaller get a place in the stage and one emit entry per block
-    std::vector<uint64_t> foff, content, e_src, e_dst;
-    std::vector<uint32_t> e_hdr;
+    auto block_size = [&](uint32_t i, uint64_t k) { return (uint32_t)std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK); };
+    // K9: the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS
+    std::vector<uint32_t> info;
+    const uint8_t *slots = nullptr;
+    if (lz) {
+        std::vector<uint64_t> zsrc;
+        std::vector<uint32_t> zsize;
+        for (uint32_t i = 0; i < n; i++)
+            for (uint64_t k = 0; k < blk_first[i + 1] - blk_first[i]; k++)
+                if (!(flags[blk_first[i] + k] & 0x100u)) { zsrc.push_back(off[i] + k * ZFRAME_BLOCK); zsize.push_back(block_size(i, k)); }
+        const uint64_t nz = zsrc.size();
+        if (nz) {
+            if (int rc = upload_table_once(ctx, &ctx->d_lz_tab, sizeof(LzTables), lz_fill_tables_host)) return rc;
+            uint64_t *d_zsrc = b.upload(zsrc.data(), nz);
+            uint32_t *d_zsize = b.upload(zsize.data(), nz);
+            uint8_t *d_slots = b.get<uint8_t>(nz * LZ_SLOT);
+            uint64_t *d_seqs = b.get<uint64_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * LZ_MAX_SEQ);
+            uint32_t *d_nseq = b.get<uint32_t>(nz), *d_nlit = b.get<uint32_t>(nz), *d_info = b.get<uint32_t>(nz);
+            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info)
+                return fail(ctx, PBSGPU_ENOMEM, "match stage: device allocation failed");
+            for (uint64_t f = 0; b.ok() && f < nz; f += LZ_PASS_BLOCKS) {
+                const uint32_t pn = (uint32_t)std::min<uint64_t>(LZ_PASS_BLOCKS, nz - f);
+                b.e = launch_lz_parse(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit, b.st);
+                if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
+            }
+            info.resize(nz);
+            if (b.ok()) b.e = cudaMemcpyAsync(info.data(), d_info, nz * 4, cudaMemcpyDeviceToHost, b.st);
+            if (int rc = b.finish("zstd match stage")) return rc;
+            slots = d_slots;
+        }
+    }
+    // every block's Block_Header (bits 0..23; the RLE byte in 24..31), body size and body source (dbase + src, or
+    // slots + src for a Compressed_Block)
+    std::vector<uint32_t> bhdr(n_blocks), bbody(n_blocks);
+    std::vector<uint64_t> bsrc(n_blocks);
+    for (uint32_t i = 0, z = 0; i < n; i++) {
+        const uint64_t nb = blk_first[i + 1] - blk_first[i];
+        for (uint64_t k = 0; k < nb; k++) {
+            const uint64_t blk = blk_first[i] + k;
+            const uint32_t size = block_size(i, k), f = flags[blk], last = k + 1 == nb;
+            uint32_t type = 0, hsize = size, body = size;
+            bsrc[blk] = off[i] + k * ZFRAME_BLOCK;
+            if (f & 0x100u) { type = 1; body = 1; }
+            else if (lz) {
+                const uint32_t cs = info[z] & 0x3FFFFFFFu;
+                if (cs < size) { type = 2; hsize = body = cs; bsrc[blk] = (uint64_t)z * LZ_SLOT + (info[z] >> 30); }
+                z++;
+            }
+            bhdr[blk] = last | type << 1 | hsize << 3 | (f & 0xFFu) << 24;
+            bbody[blk] = body;
+        }
+    }
+    // frame sizes; the blobs that come out smaller get a place in the stage and one emit entry per block, in the list of
+    // their body's source
+    std::vector<uint64_t> foff, content, e_src[2], e_dst[2];
+    std::vector<uint32_t> e_hdr[2];
     uint64_t cursor = 0;
     for (uint32_t i = 0; i < n; i++) {
-        const uint64_t nb = blk_first[i + 1] - blk_first[i];
         uint64_t fl = ZFRAME_HEADER;
-        for (uint64_t k = 0; k < nb; k++) {
-            const uint64_t size = std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK);
-            fl += 3 + ((flags[blk_first[i] + k] & 0x100u) ? 1 : size);
-        }
+        for (uint64_t blk = blk_first[i]; blk < blk_first[i + 1]; blk++) fl += 3 + bbody[blk];
         if (len[i] == 0 || fl >= len[i]) continue;
         comp[i] = 1; frame_off[i] = cursor; frame_len[i] = fl;
         foff.push_back(cursor);
         content.push_back(len[i]);
         uint64_t pos = cursor + ZFRAME_HEADER;
-        for (uint64_t k = 0; k < nb; k++) {
-            const uint64_t size = std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK);
-            const uint32_t f = flags[blk_first[i] + k];
-            const bool rle = (f & 0x100u) != 0;
-            e_src.push_back(off[i] + k * ZFRAME_BLOCK);
-            e_dst.push_back(pos);
-            e_hdr.push_back((uint32_t)(k + 1 == nb) | ((rle ? 1u : 0u) << 1) | ((uint32_t)size << 3) | ((f & 0xFFu) << 24));
-            pos += 3 + (rle ? 1 : size);
+        for (uint64_t blk = blk_first[i]; blk < blk_first[i + 1]; blk++) {
+            const int from_slot = ((bhdr[blk] >> 1) & 3) == 2;
+            e_src[from_slot].push_back(bsrc[blk]);
+            e_dst[from_slot].push_back(pos);
+            e_hdr[from_slot].push_back(bhdr[blk]);
+            pos += 3 + bbody[blk];
         }
         cursor = (pos + 15) & ~15ull;
     }
     const uint32_t nc = (uint32_t)foff.size();
     if (nc == 0) return PBSGPU_OK;
-    const uint64_t ne = e_hdr.size();
     uint8_t *stage = b.get<uint8_t>(cursor + 16);
     if (!stage) return fail(ctx, PBSGPU_ENOMEM, "frame staging of %llu bytes failed", (unsigned long long)cursor);
-    uint64_t *d_src = b.upload(e_src.data(), ne), *d_dst = b.upload(e_dst.data(), ne);
     uint64_t *d_foff = b.upload(foff.data(), nc), *d_clen = b.upload(content.data(), nc);
-    uint32_t *d_hdr = b.upload(e_hdr.data(), ne);
-    if (!d_src || !d_dst || !d_hdr || !d_foff || !d_clen) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (!d_foff || !d_clen) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
     if (b.ok()) b.e = launch_zframe_hdr(stage, d_foff, d_clen, nc, b.st);
-    if (b.ok()) b.e = launch_zframe_emit(dbase, stage, d_src, d_dst, d_hdr, ne, b.st);
+    for (int s = 0; s < 2; s++) {
+        const uint64_t ne = e_hdr[s].size();
+        if (ne == 0) continue;
+        uint64_t *d_src = b.upload(e_src[s].data(), ne), *d_dst = b.upload(e_dst[s].data(), ne);
+        uint32_t *d_hdr = b.upload(e_hdr[s].data(), ne);
+        if (!d_src || !d_dst || !d_hdr) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+        if (b.ok()) b.e = launch_zframe_emit(s ? slots : dbase, stage, d_src, d_dst, d_hdr, ne, b.st);
+    }
     if (int rc = b.finish("zstd frame emit")) return rc;
     *frames = stage;
     return crc_where(ctx, comp, 1, stage, frame_off.data(), frame_len.data(), crc);
@@ -262,11 +314,12 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
 
 // f3: complete DataBlobs for the NEW chunks of a batch in one call (upstream pbs-datastore data_blob.rs:
 // magic[8] | crc32 LE over the payload | payload; uploaded by POST /dynamic_chunk, reference
-// internal/server/backup/log_cleanup.go:19-31), with zstd frames as payloads where they are smaller when `compress`.
+// internal/server/backup/log_cleanup.go:19-31), with zstd frames as payloads where they are smaller when `compress`
+// (with the match stage when `lz`).
 // The CRCs come from K6 on the device; payload bytes are copied once (device -> host for resident data and frames,
 // host -> host otherwise) straight into their place behind the header.
 static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, bool compress,
-                       uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+                       bool lz, uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     Guard g(ctx);
     if (n == 0) return PBSGPU_OK;
     for (uint32_t i = 0; compress && i < n; i++)
@@ -278,7 +331,7 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
     std::vector<uint64_t> frame_off(n), frame_len(n);
     std::vector<uint32_t> crc(n, 0);
     if (compress) {
-        int rc = zstd_frames(b, dbase, off, len, n, comp, frame_off, frame_len, crc, &frames);
+        int rc = zstd_frames(b, dbase, off, len, n, lz, comp, frame_off, frame_len, crc, &frames);
         if (rc) return rc;
     }
     if (int rc = crc_where(ctx, comp, 0, dbase, off, len, crc)) return rc;
@@ -303,13 +356,19 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
 extern "C" int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                         uint8_t *out, const uint64_t *out_off, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !base))) return PBSGPU_EINVAL;
-    return blob_encode(ctx, base, off, len, n, false, out, out_off, nullptr, crc_out);
+    return blob_encode(ctx, base, off, len, n, false, false, out, out_off, nullptr, crc_out);
 }
 
 extern "C" int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                           uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
-    return blob_encode(ctx, base, off, len, n, true, out, out_off, out_len, crc_out);
+    return blob_encode(ctx, base, off, len, n, true, false, out, out_off, out_len, crc_out);
+}
+
+extern "C" int pbsgpu_blob_encode_batch_lz(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                           uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
+    return blob_encode(ctx, base, off, len, n, true, true, out, out_off, out_len, crc_out);
 }
 
 // ---------------------------------------------------------------------------

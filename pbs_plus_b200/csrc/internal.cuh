@@ -126,6 +126,9 @@ cudaError_t launch_zblock_scan(const uint8_t *base, const uint64_t *off, const u
 cudaError_t launch_zframe_emit(const uint8_t *base, uint8_t *stage, const uint64_t *src_off, const uint64_t *dst_off,
                                const uint32_t *hdr, uint64_t n_entries, cudaStream_t st);
 cudaError_t launch_zframe_hdr(uint8_t *stage, const uint64_t *frame_off, const uint64_t *content_len, uint32_t n, cudaStream_t st);
+}  // namespace pbsgpu
+#include "zlz.cuh"   // f3: LZ77 match stage + Predefined_Mode sequences (K9)
+namespace pbsgpu {
 
 // ---- digest set (K4) ----------------------------------------------------------------
 struct SetTable {

@@ -1,6 +1,9 @@
-"""f3 microbench: DataBlob assembly for 4 MiB chunks of an 8 GiB device-resident image, half of it zero runs, into PINNED host
-memory through the raw C calls (no Python-side allocation or slicing inside the timed region)."""
-import ctypes as C
+"""f3 microbench: DataBlob assembly for 4 MiB chunks of an 8 GiB device-resident image into PINNED host memory through
+the raw C calls (no Python-side allocation or slicing inside the timed region).  Two images: random bytes with half of
+them zero runs, and a text-like image (tests/zstd_lz_ref.py text_corpus, 32 MiB repeated).  For each: GB/s of input and
+output / input of every encoder, and for context libzstd level 1 (pyarrow) on a 64 MiB host sample of the same image (8 MiB from each GiB),
+its ratio and single-thread rate on the HOST CPU."""
+import subprocess
 import sys
 import time
 from pathlib import Path
@@ -9,13 +12,15 @@ import numpy as np
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tests"))
 import pbs_plus_b200 as pg  # noqa: E402
+import zstd_lz_ref as lzref  # noqa: E402
 
+print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                     capture_output=True, text=True).stdout.strip())
 e = pg.Engine(0)
 L_ = e._L
 n = 8 << 30
-d = torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda")
-d[1 << 30: 5 << 30] = 0
 CH = 4 << 20
 off = np.arange(0, n, CH, dtype=np.uint64)
 ln = np.full(len(off), CH, dtype=np.uint64)
@@ -23,23 +28,50 @@ boff = (np.arange(len(off), dtype=np.uint64) * np.uint64(CH + 12))
 out = e.host_alloc(int(len(off)) * (CH + 12))
 blen = np.zeros(len(off), dtype=np.uint64)
 crc = np.zeros(len(off), dtype=np.uint32)
-for name in ("crc32_batch", "blob_encode_batch", "blob_encode_batch_z"):
-    for rep in range(3):
-        torch.cuda.synchronize()
+
+
+def images():
+    d = torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda")
+    d[1 << 30: 5 << 30] = 0
+    yield "half-zero random", d
+    del d
+    tile = torch.from_numpy(lzref.text_corpus(32 << 20, 1)).cuda()
+    yield "text-like", tile.repeat(n // len(tile))
+
+
+for label, d in images():
+    torch.cuda.synchronize()
+    print(f"-- {label} image, {n / 2**30:.0f} GiB")
+    for name in ("crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz"):
+        for rep in range(3):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            if name == "crc32_batch":
+                rc = L_.pbsgpu_crc32_batch(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), crc.ctypes.data)
+                size = 0
+            elif name == "blob_encode_batch":
+                rc = L_.pbsgpu_blob_encode_batch(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), out.ctypes.data,
+                                                 boff.ctypes.data, crc.ctypes.data)
+                size = len(off) * (CH + 12)
+            else:
+                rc = getattr(L_, "pbsgpu_" + name)(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), out.ctypes.data,
+                                                   boff.ctypes.data, blen.ctypes.data, crc.ctypes.data)
+                size = int(blen.sum())
+            dt = time.perf_counter() - t0
+            assert rc == 0, rc
+        ratio = f", output / input {size / n:.4f}" if size else ""
+        print(f"{name}: {n / dt / 1e9:.1f} GB/s of input ({dt * 1e3:.0f} ms, third run), {size / 2**30:.2f} GiB written to "
+              f"pinned host memory{ratio}")
+    try:
+        import pyarrow as pa
+        sample = b"".join(d[k * (n // 8): k * (n // 8) + (8 << 20)].cpu().numpy().tobytes() for k in range(8))
         t0 = time.perf_counter()
-        if name == "crc32_batch":
-            rc = L_.pbsgpu_crc32_batch(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), crc.ctypes.data)
-            size = 0
-        elif name == "blob_encode_batch":
-            rc = L_.pbsgpu_blob_encode_batch(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), out.ctypes.data,
-                                             boff.ctypes.data, crc.ctypes.data)
-            size = len(off) * (CH + 12)
-        else:
-            rc = L_.pbsgpu_blob_encode_batch_z(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), out.ctypes.data,
-                                               boff.ctypes.data, blen.ctypes.data, crc.ctypes.data)
-            size = int(blen.sum())
+        z = pa.Codec("zstd", compression_level=1).compress(sample, asbytes=True)
         dt = time.perf_counter() - t0
-        assert rc == 0, rc
-    print(f"{name}: {n / dt / 1e9:.1f} GB/s of input ({dt * 1e3:.0f} ms, third run), {size / 2**30:.2f} GiB written to pinned host memory")
+        print(f"libzstd level 1 (host CPU, one thread, 8 x 8 MiB sample): output / input {len(z) / len(sample):.4f}, "
+              f"{len(sample) / dt / 1e9:.2f} GB/s")
+    except ImportError:
+        print("libzstd level 1: pyarrow not available")
+    del d
 e.host_free(out)
 e.close()
