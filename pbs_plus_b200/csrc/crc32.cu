@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "device.cuh"
 #include "internal.cuh"
 
 namespace pbsgpu {
@@ -88,11 +89,10 @@ __global__ void __launch_bounds__(CRC_THREADS, 1) k_crc32_blocks(const uint8_t *
     };
     const uint64_t warps_total = ((uint64_t)gridDim.x * blockDim.x) >> 5;
     for (uint64_t gw = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; gw < total_wb; gw += warps_total) {
-        uint32_t lo = 0, hi = n;
-        while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (wb_first[mid] <= gw) lo = mid; else hi = mid; }
-        const uint64_t wb = gw - wb_first[lo], rlen = len[lo];
+        const uint32_t r = owner_of(wb_first, n, gw);
+        const uint64_t wb = gw - wb_first[r], rlen = len[r];
         const uint64_t done = wb * CRC_WB + (uint64_t)lane * CRC_SEG;
-        const uint8_t *p = base + off[lo] + done;
+        const uint8_t *p = base + off[r] + done;
         const uint32_t seg = done >= rlen ? 0u : (rlen - done < (uint64_t)CRC_SEG ? (uint32_t)(rlen - done) : (uint32_t)CRC_SEG);
         uint32_t c = 0xffffffffu, i = 0;
 #define CRC_BYTE(b) do { c = lut(0, (c ^ (b)) << 7) ^ (c >> 8); } while (0)
@@ -149,24 +149,6 @@ struct CrcTiledTables {
     uint32_t zt[4][256];   // state advance by (CT_TILE - CT_SPAN) zero bytes, per state byte
 };
 
-__device__ __forceinline__ uint32_t ct_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void ct_mbar_init(uint32_t bar) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void ct_mbar_expect(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void ct_mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n .reg .pred P1;\n LAB_WAIT:\n"
-        " mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        " @P1 bra DONE;\n bra LAB_WAIT;\n DONE:\n }" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void ct_tma(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-
 // region_first[r] = first region index of range r (prefix over ceil(tiles/CT_REGION_TILES), >= 1 per
 // non-empty range); part_crc[region] = standard CRC-32 of that region's bytes.
 __global__ void __launch_bounds__(CT_WARPS * 32, 1) k_crc32_tiled(const uint8_t *base, const uint64_t *off,
@@ -185,12 +167,8 @@ __global__ void __launch_bounds__(CT_WARPS * 32, 1) k_crc32_tiled(const uint8_t 
     if (threadIdx.x < 32) X2N[threadIdx.x] = tab->base.x2n[threadIdx.x];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lane4 = lane << 2;
     uint8_t *buf0 = bufs + warp * 2 * CT_TILE;
-    const uint32_t bar_s[2] = {ct_smem_u32(&bars[warp * 2]), ct_smem_u32(&bars[warp * 2 + 1])};
-    if (lane == 0) {
-        ct_mbar_init(bar_s[0]); ct_mbar_init(bar_s[1]);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    const uint32_t bar_s[2] = {smem_u32(&bars[warp * 2]), smem_u32(&bars[warp * 2 + 1])};
+    warp_bars_init(bar_s, lane);
     const uint8_t *TB = (const uint8_t *)TR;
     auto lut = [&](uint32_t k, uint32_t byte_shl7) -> uint32_t {
         return *(const uint32_t *)(TB + k * 32768u + ((byte_shl7 & 0x7f80u) | lane4));
@@ -200,10 +178,9 @@ __global__ void __launch_bounds__(CT_WARPS * 32, 1) k_crc32_tiled(const uint8_t 
     uint32_t uses[2] = {0, 0};                                // per-buffer use counters (mbarrier phase parity)
     const uint64_t warps_total = (uint64_t)gridDim.x * CT_WARPS;
     for (uint64_t g = (uint64_t)blockIdx.x * CT_WARPS + warp; g < total_regions; g += warps_total) {
-        uint32_t lo = 0, hi = n;
-        while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (region_first[mid] <= g) lo = mid; else hi = mid; }
-        const uint64_t reg = g - region_first[lo], rlen = len[lo];
-        const uint8_t *rstart = base + off[lo];
+        const uint32_t r = owner_of(region_first, n, g);
+        const uint64_t reg = g - region_first[r], rlen = len[r];
+        const uint8_t *rstart = base + off[r];
         const uint32_t head = (uint32_t)((16 - ((uintptr_t)rstart & 15)) & 15);     // bytes before the aligned body
         const uint64_t head_eff = head < rlen ? head : rlen;
         const uint64_t body = rlen - head_eff;                                       // aligned part, tiled
@@ -228,17 +205,13 @@ __global__ void __launch_bounds__(CT_WARPS * 32, 1) k_crc32_tiled(const uint8_t 
             const uint32_t bulk = valid & ~15u;
             for (uint32_t i = bulk + lane; i < valid; i += 32) dst[i] = src[i];
             __syncwarp();
-            if (lane == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                ct_mbar_expect(bar_s[b], bulk);
-                if (bulk) ct_tma(ct_smem_u32(dst), src, bulk, bar_s[b]);
-            }
+            if (lane == 0) stage_bulk(dst, src, bulk, bar_s[b]);
         };
         if (ntiles) issue(0, 0);
         for (uint32_t t = 0; t < ntiles; t++) {
             const int b = (int)(t & 1);
             if (t + 1 < ntiles) issue(t + 1, b ^ 1);
-            ct_mbar_wait(bar_s[b], uses[b] & 1);
+            mbar_wait(bar_s[b], uses[b] & 1);
             uses[b]++;
             const uint64_t tb = (uint64_t)t * CT_TILE;
             const uint32_t valid = r_bytes - tb < (uint64_t)CT_TILE ? (uint32_t)(r_bytes - tb) : (uint32_t)CT_TILE;

@@ -10,7 +10,7 @@
 //
 // Tuned kernel (k_scan_tuned), integer/byte work, no tensor cores:
 //   * one warp owns a tile of 32 x 272 B; the tile (+64 B halo) is brought into shared
-//     memory by ONE TMA bulk copy (cp.async.bulk + mbarrier, SASS UBLKCP), double
+//     memory by ONE TMA bulk copy (device.cuh stage_bulk, SASS UBLKCP), double
 //     buffered per warp, so HBM reads are fully coalesced and cost no issue slots;
 //   * each lane walks its own 272 B span (64 B warm-up from the halo);
 //   * de-rotated prefix form: A[p] = rotr(T[b[p]], (p+lane) mod 32), Q(p) = Q(p-1)^A[p],
@@ -26,6 +26,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "device.cuh"
 #include "internal.cuh"
 
 namespace pbsgpu {
@@ -36,16 +37,6 @@ __device__ __forceinline__ uint32_t rotr32(uint32_t x, uint32_t r) { return __fu
 __device__ __forceinline__ void emit_candidate(const ScanArgs &a, uint32_t stream, uint64_t pos) {
     unsigned long long i = atomicAdd(a.cand_count, 1ull);
     if (i < a.cand_cap) a.cand[i] = ((uint64_t)stream << KEY_POS_BITS) | pos;
-}
-
-// largest s with tile_first[s] <= t   (tile_first has n+1 entries, tile_first[n] = total)
-__device__ __forceinline__ uint32_t find_stream(const uint64_t *tile_first, uint32_t n, uint64_t t) {
-    uint32_t lo = 0, hi = n;  // invariant: tile_first[lo] <= t < tile_first[hi]
-    while (hi - lo > 1) {
-        uint32_t mid = (lo + hi) >> 1;
-        if (tile_first[mid] <= t) lo = mid; else hi = mid;
-    }
-    return lo;
 }
 
 // ============================================================================
@@ -59,7 +50,7 @@ __global__ void __launch_bounds__(256) k_scan_simple(ScanArgs a) {
     __syncthreads();
     uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= a.total_tiles) return;
-    uint32_t s = find_stream(a.tile_first, a.n_streams, g);
+    uint32_t s = owner_of(a.tile_first, a.n_streams, g);
     uint64_t j = g - a.tile_first[s];
     uint64_t len = a.len[s];
     const uint8_t *d = a.base + a.off[s];
@@ -101,26 +92,6 @@ __global__ void k_build_rot_table(const uint32_t *table, uint32_t *rot) {
 cudaError_t launch_build_rot_table(const uint32_t *table, uint32_t *rot, cudaStream_t st) {
     k_build_rot_table<<<64, 256, 0, st>>>(table, rot);
     return cudaGetLastError();
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n .reg .pred P1;\n LAB_WAIT:\n"
-        " mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        " @P1 bra DONE;\n bra LAB_WAIT;\n DONE:\n }" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
 }
 
 // d = ~(a^b) & c ;  acc = (d != 0) & acc      -> one LOP3.LUT.PAND
@@ -183,8 +154,10 @@ __device__ __noinline__ void lane_exact(const ScanArgs &a, const uint8_t *buf, c
     }
 }
 
+// Dynamic shared memory of both TMA-fed kernels: 1024 B aligned for k_scan_lanes' SWIZZLE_128B boxes.
+extern __shared__ __align__(1024) uint8_t smem[];
+
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_tuned(ScanArgs a, const uint32_t *__restrict__ rot_g) {
-    extern __shared__ __align__(128) uint8_t smem[];
     uint32_t *rot = (uint32_t *)smem;
     const uint8_t *rotb = smem;
     {   // 64 KiB table: coalesced 16 B loads, once per (persistent) CTA
@@ -196,12 +169,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_tuned(ScanArgs a
     uint8_t *buf0 = smem + ROT_BYTES + warp * 2 * BUF_STRIDE;
     uint64_t *bars = (uint64_t *)(smem + ROT_BYTES + WARPS_PER_CTA * 2 * BUF_STRIDE) + warp * 2;
     const uint32_t bar_s[2] = {smem_u32(&bars[0]), smem_u32(&bars[1])};
-    if (lane == 0) {
-        mbar_init(bar_s[0], 1);
-        mbar_init(bar_s[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    warp_bars_init(bar_s, lane);
 
     const uint64_t gw = (uint64_t)blockIdx.x * WARPS_PER_CTA + warp, nw = (uint64_t)gridDim.x * WARPS_PER_CTA;
     const uint64_t t0 = a.total_tiles * gw / nw, t1 = a.total_tiles * (gw + 1) / nw;
@@ -215,7 +183,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_tuned(ScanArgs a
     const uint32_t laneoff = lane * 4;
 
     // stream cursor (advances monotonically with t)
-    uint32_t s = find_stream(a.tile_first, a.n_streams, t0);
+    uint32_t s = owner_of(a.tile_first, a.n_streams, t0);
     uint64_t s_first = a.tile_first[s], s_next = a.tile_first[s + 1];
 
     auto tile_info = [&](uint64_t t, uint32_t &sc, uint64_t &sf, uint64_t &sn) {
@@ -241,11 +209,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_tuned(ScanArgs a
             uint32_t bulk = bytes & ~15u;
             for (uint32_t i = bulk + lane; i < bytes; i += 32) dst0[i] = src0[i];   // < 16 tail bytes
             __syncwarp();
-            if (lane == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                mbar_arrive_expect_tx(bar_s[b], bulk);
-                if (bulk) tma_bulk_g2s(smem_u32(dst0), src0, bulk, bar_s[b]);
-            }
+            if (lane == 0) stage_bulk(dst0, src0, bulk, bar_s[b]);
         } else {   // unaligned source: cooperative generic copy (slow path; TMA needs 16 B alignment)
             for (uint32_t i = lane; i < bytes; i += 32) dst0[i] = src0[i];
             __syncwarp();
@@ -373,7 +337,6 @@ struct LsUnit {
 
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_lanes(ScanArgs a, const uint32_t *__restrict__ rot_g,
                                                                        const __grid_constant__ CUtensorMap tmap) {
-    extern __shared__ __align__(1024) uint8_t smem[];
     uint32_t *rot = (uint32_t *)smem;
     const uint8_t *rotb = smem;
     {
@@ -385,12 +348,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_lanes(ScanArgs a
     uint8_t *buf0 = smem + ROT_BYTES + warp * 2 * LS_BUF;          // ROT_BYTES = 64 KiB: every step buffer is 1024 B aligned
     uint64_t *bars = (uint64_t *)(smem + ROT_BYTES + WARPS_PER_CTA * 2 * LS_BUF) + warp * 2;
     const uint32_t bar_s[2] = {smem_u32(&bars[0]), smem_u32(&bars[1])};
-    if (lane == 0) {
-        mbar_init(bar_s[0], 1);
-        mbar_init(bar_s[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    warp_bars_init(bar_s, lane);
     const uint64_t gw = (uint64_t)blockIdx.x * WARPS_PER_CTA + warp, nw = (uint64_t)gridDim.x * WARPS_PER_CTA;
     auto n_super_of = [&](uint32_t sc) -> uint64_t {
         return (a.off[sc] & (LS_ALIGN - 1)) == 0 ? a.len[sc] / LS_SUPER : 0;   // a.base itself is 128 B aligned (host checked)
@@ -398,7 +356,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_lanes(ScanArgs a
     // warps split the step list evenly, but a split inside a super-tile moves back to the super-tile's step 0
     auto round_unit = [&](uint64_t x) -> uint64_t {
         if (x >= a.total_tiles) return a.total_tiles;
-        const uint32_t sc = find_stream(a.tile_first, a.n_streams, x);
+        const uint32_t sc = owner_of(a.tile_first, a.n_streams, x);
         const uint64_t j = x - a.tile_first[sc];
         return j < n_super_of(sc) * LS_STEPS ? x - (j % LS_STEPS) : x;
     };
@@ -417,7 +375,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_lanes(ScanArgs a
 
     // unit cursor: tile_first[] counts STEPS (a super-tile is LS_STEPS of them, a plain tile one); all the bookkeeping
     // below runs once per UNIT (64 KiB), not once per step
-    uint32_t s = find_stream(a.tile_first, a.n_streams, u0);
+    uint32_t s = owner_of(a.tile_first, a.n_streams, u0);
     uint64_t s_first = a.tile_first[s], s_next = a.tile_first[s + 1];
     uint64_t s_ns = n_super_of(s), s_off = a.off[s], s_len = a.len[s];
     uint64_t u = u0;
@@ -453,24 +411,23 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_lanes(ScanArgs a
                 for (int i = 0; i < 16; i++) hz[i] = 0;                     // zero halo (positions < 63 are never reported)
             }
             const uint32_t any_first = __ballot_sync(0xffffffffu, first_of_stream);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             __syncwarp();
             if (lane == 0) {
                 mbar_arrive_expect_tx(bar_s[b], LS_BOX + (32 - __popc(any_first)) * 64);
-                const int c1 = (int)((un.soff + un.stream_pos) >> 7);
-                asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-                             ::"r"(smem_u32(buf)), "l"(&tmap), "r"(0), "r"(c1), "r"(0), "r"(0), "r"(bar_s[b]) : "memory");
+                tma_tensor4d_g2s(smem_u32(buf), &tmap, 0, (int)((un.soff + un.stream_pos) >> 7), 0, 0, bar_s[b]);
             }
             __syncwarp();
             if (!first_of_stream) tma_bulk_g2s(smem_u32(halo), a.base + un.soff + lane_start - 64, 64, bar_s[b]);
         } else if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             mbar_arrive_expect_tx(bar_s[b], LS_BOX);
             const int c1 = (int)((un.soff + un.stream_pos + (uint64_t)k * LS_PIECE) >> 7);   // 128 B unit of lane 0's piece
-            asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-                         ::"r"(smem_u32(buf)), "l"(&tmap), "r"(0), "r"(c1), "r"(0), "r"(0), "r"(bar_s[b]) : "memory");
+            tma_tensor4d_g2s(smem_u32(buf), &tmap, 0, c1, 0, 0, bar_s[b]);
         }
     };
+    // a plain tile: k_scan_tuned's `issue` written out again -- one function shared by both kernels raises this kernel
+    // from 208 to 212-214 registers
     auto issue_plain = [&](const LsUnit &un, int b) {
         uint8_t *buf = buf0 + b * LS_BUF;
         const uint8_t *src = a.base + un.soff + un.stream_pos;
@@ -483,11 +440,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 1) k_scan_lanes(ScanArgs a
             uint32_t bulk = bytes & ~15u;
             for (uint32_t i = bulk + lane; i < bytes; i += 32) dst0[i] = src0[i];
             __syncwarp();
-            if (lane == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                mbar_arrive_expect_tx(bar_s[b], bulk);
-                if (bulk) tma_bulk_g2s(smem_u32(dst0), src0, bulk, bar_s[b]);
-            }
+            if (lane == 0) stage_bulk(dst0, src0, bulk, bar_s[b]);
         } else {
             for (uint32_t i = lane; i < bytes; i += 32) dst0[i] = src0[i];
             __syncwarp();

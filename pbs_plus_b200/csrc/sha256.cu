@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "device.cuh"
 #include "internal.cuh"
 
 namespace pbsgpu {
@@ -275,20 +276,6 @@ __global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o) {
 // ---------------------------------------------------------------------------
 constexpr int SPLIT_STAGES = 3;
 
-__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n .reg .pred P1;\n LAB_WAIT:\n"
-        " mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        " @P1 bra DONE;\n bra LAB_WAIT;\n DONE:\n }" ::"r"(bar), "r"(parity) : "memory");
-}
-
 // consumer: 64 rounds with W+K supplied.  CMODE 0: IADD3 forms (fewest instructions),
 // CMODE 1: all additions on the FMA pipe (a*1+b with an opaque 1),
 // CMODE 2: the two additions on the chain (e', a') stay IADD3, everything that only depends on values known at the
@@ -345,11 +332,11 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o) {
     const uint32_t nblk_max = __reduce_max_sync(0xffffffffu, nblk);
     uint32_t full[SPLIT_STAGES], empty[SPLIT_STAGES];
 #pragma unroll
-    for (int k = 0; k < SPLIT_STAGES; k++) { full[k] = smem_addr(&bars[k]); empty[k] = smem_addr(&bars[SPLIT_STAGES + k]); }
+    for (int k = 0; k < SPLIT_STAGES; k++) { full[k] = smem_u32(&bars[k]); empty[k] = smem_u32(&bars[SPLIT_STAGES + k]); }
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int k = 0; k < SPLIT_STAGES; k++) { mbar_init(full[k], 32); mbar_init(empty[k], 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
     __syncthreads();
 

@@ -16,6 +16,7 @@
 // Streams of <= 1 KiB (all the short-length formulas, and long inputs with no full block) go through k_xxh3_small.
 // Scratch for S is bounded: a pass covers blocks [win_lo, win_lo + W) of every stream and the chain state is carried
 // between passes, so all streams stay parallel in every pass.
+#include "device.cuh"
 #include "internal.cuh"
 
 namespace pbsgpu {
@@ -96,15 +97,6 @@ struct XxhArgs {
 
 constexpr int XA_U = 8;   // blocks per 4-lane group (8 KiB): one stream search per group
 
-__device__ __forceinline__ uint32_t xfind(const uint64_t *first, uint32_t n, uint64_t g) {
-    uint32_t lo = 0, hi = n;   // largest s with first[s] <= g  (first[n] = total > g)
-    while (hi - lo > 1) {
-        uint32_t mid = (lo + hi) >> 1;
-        if (first[mid] <= g) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // ---- phase A ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_xxh3_blocks(XxhArgs a) {
     const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -115,7 +107,7 @@ __global__ void __launch_bounds__(256) k_xxh3_blocks(XxhArgs a) {
     const uint64_t *kw = (const uint64_t *)a.tab + 2 * j;
 #pragma unroll
     for (int t = 0; t < 17; t++) K[t] = __ldg(kw + t);
-    uint32_t s = xfind(a.first, a.n, g0);
+    uint32_t s = owner_of(a.first, a.n, g0);
     uint64_t s_first = a.first[s], s_next = a.first[s + 1];
 #pragma unroll 1
     for (int u = 0; u < XA_U; u++) {

@@ -12,6 +12,7 @@
 //   K8b k_zframe_emit : one CTA per block of the chunks that come out smaller: 3-byte Block_Header + 1 byte (RLE) or
 //                       + the raw bytes (funnel-shifted 4-byte copy: the 3-byte headers misalign source and target)
 //   K8c k_zframe_hdr  : the 13-byte Frame_Header of each such chunk
+#include "device.cuh"
 #include "internal.cuh"
 
 namespace pbsgpu {
@@ -19,15 +20,11 @@ namespace pbsgpu {
 __global__ void __launch_bounds__(256) k_zblock_scan(const uint8_t *base, const uint64_t *off, const uint64_t *len,
                                                      const uint64_t *blk_first, uint32_t n, uint32_t *flags) {
     const uint64_t b = blockIdx.x;
-    uint32_t lo = 0, hi = n;   // blk_first[lo] <= b < blk_first[hi]: the LAST such lo (chunks without blocks are skipped)
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (blk_first[mid] <= b) lo = mid; else hi = mid;
-    }
-    const uint64_t within = (b - blk_first[lo]) * (uint64_t)ZFRAME_BLOCK;
-    const uint64_t rem = len[lo] - within;
+    const uint32_t r = owner_of(blk_first, n, b);
+    const uint64_t within = (b - blk_first[r]) * (uint64_t)ZFRAME_BLOCK;
+    const uint64_t rem = len[r] - within;
     const uint32_t size = rem < ZFRAME_BLOCK ? (uint32_t)rem : ZFRAME_BLOCK;
-    const uint8_t *p = base + off[lo] + within;
+    const uint8_t *p = base + off[r] + within;
     const uint8_t c = p[0];
     const uint32_t cw = (uint32_t)c * 0x01010101u;
     uint32_t head = (uint32_t)((16 - ((uintptr_t)p & 15)) & 15);
