@@ -514,17 +514,33 @@ func (b *Batch) BlobEncode(off, length []uint64) ([][]byte, error) {
 // keeps a compressed payload only then).  The frames are built on the GPU from RLE and raw blocks -- they remove
 // the zero runs of disk images and sparse files; data without such runs stays uncompressed.
 func (b *Batch) BlobEncodeZ(off, length []uint64) ([][]byte, error) {
-	return b.blobEncodeCompressed(off, length, false)
+	return b.blobEncodeCompressed(off, length, blobZ)
 }
 
 // BlobEncodeLZ is BlobEncodeZ with a match stage: every 128 KiB block that is not one repeated byte becomes a zstd
 // Compressed_Block (greedy LZ77 inside the block, raw literals, predefined FSE tables) where that is smaller, so
 // text, logs and other compressible data shrink too.  Each blob is at most the size of its BlobEncodeZ blob.
 func (b *Batch) BlobEncodeLZ(off, length []uint64) ([][]byte, error) {
-	return b.blobEncodeCompressed(off, length, true)
+	return b.blobEncodeCompressed(off, length, blobLZ)
 }
 
-func (b *Batch) blobEncodeCompressed(off, length []uint64, lz bool) ([][]byte, error) {
+// BlobEncodeLZE is BlobEncodeLZ with zstd's entropy stage: each compressed block is the smaller of the BlobEncodeLZ
+// one and one with tables fitted to the block (FSE_Compressed_Mode sequences, Huffman literals).  Each blob is at most
+// the size of its BlobEncodeLZ blob.  Like the rest of this shim, it has not been compiled against a Go toolchain.
+func (b *Batch) BlobEncodeLZE(off, length []uint64) ([][]byte, error) {
+	return b.blobEncodeCompressed(off, length, blobLZE)
+}
+
+// which compressed DataBlob encoder blobEncodeCompressed calls
+type blobMode int
+
+const (
+	blobZ blobMode = iota
+	blobLZ
+	blobLZE
+)
+
+func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]byte, error) {
 	n := len(off)
 	if n == 0 {
 		return nil, nil
@@ -541,9 +557,12 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, lz bool) ([][]byte, e
 	out := make([]byte, total+1)
 	dst := (*C.uint8_t)(unsafe.Pointer(&out[0]))
 	var rc C.int
-	if lz {
+	switch mode {
+	case blobLZE:
+		rc = C.pbsgpu_blob_encode_batch_lze(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
+	case blobLZ:
 		rc = C.pbsgpu_blob_encode_batch_lz(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
-	} else {
+	default:
 		rc = C.pbsgpu_blob_encode_batch_z(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	}
 	if err := b.e.err(rc); err != nil {

@@ -287,6 +287,13 @@ int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, const uint64_t
  * at most the size of its _z blob.  The output is a deterministic function of the chunk bytes. */
 int pbsgpu_blob_encode_batch_lz(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                 uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+/* pbsgpu_blob_encode_batch_lz with zstd's entropy stage: the same parse, and each Compressed_Block is the smaller of the
+ * _lz content and one whose LL / OF / ML codes use tables fitted to the block (FSE_Compressed_Mode, or RLE_Mode for a
+ * single code) and whose literals are Huffman-coded (values up to 128), one repeated value (RLE) or raw.  Blocks stay
+ * independent (no Repeat_Mode, no Treeless literals).  Same arguments, limits and errors as _lz; each blob is at most the
+ * size of its _lz blob.  The output is a deterministic function of the chunk bytes. */
+int pbsgpu_blob_encode_batch_lze(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                 uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------
  * emitBackedFile tees every new file through `xxh3.New()` and keeps `h.Sum64()` (reference

@@ -195,13 +195,18 @@ static int crc_where(pbsgpu_ctx *ctx, const std::vector<uint8_t> &comp, uint8_t 
     return rc;
 }
 
+// Which DataBlob encoder a call is: uncompressed only, RLE / raw frames (_z), with the match stage (_lz), with the match
+// and entropy stages (_lze).
+enum class BlobMode { raw, z, lz, lze };
+
 // Compressed form: a blob's payload is a zstd frame when that is smaller than the raw bytes (upstream
-// `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device (zframe.cu, zlz.cu): a
-// 128 KiB block of one repeated byte is an RLE_Block (K8a decides); with `lz` every other block goes through the match
-// stage (K9) and is a Compressed_Block when that is smaller than the block; the rest are Raw_Blocks.  The CRC (K6) covers
+// `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device (zframe.cu, zlz.cu,
+// zent.cu): a 128 KiB block of one repeated byte is an RLE_Block (K8a decides); with lz / lze every other block goes
+// through the match stage (K9; lze adds the entropy stage, K10) and is a Compressed_Block when that is smaller than the
+// block; the rest are Raw_Blocks.  The CRC (K6) covers
 // the frame.  Marks those blobs in comp[] and leaves their frames at *frames + frame_off[i] (frame_len[i] bytes, a block
 // of `b`) and their CRCs in crc[].
-static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, bool lz,
+static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, BlobMode mode,
                        std::vector<uint8_t> &comp, std::vector<uint64_t> &frame_off, std::vector<uint64_t> &frame_len,
                        std::vector<uint32_t> &crc, const uint8_t **frames) {
     pbsgpu_ctx *ctx = b.ctx;
@@ -219,7 +224,8 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
     if (b.ok() && n_blocks) b.e = cudaMemcpyAsync(flags.data(), d_flags, n_blocks * 4, cudaMemcpyDeviceToHost, b.st);
     if (int rc = b.finish("zstd block scan")) return rc;
     auto block_size = [&](uint32_t i, uint64_t k) { return (uint32_t)std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK); };
-    // K9: the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS
+    // K9 (+ K10): the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS
+    const bool lz = mode == BlobMode::lz || mode == BlobMode::lze;
     std::vector<uint32_t> info;
     const uint8_t *slots = nullptr;
     if (lz) {
@@ -236,12 +242,16 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
             uint8_t *d_slots = b.get<uint8_t>(nz * LZ_SLOT);
             uint64_t *d_seqs = b.get<uint64_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * LZ_MAX_SEQ);
             uint32_t *d_nseq = b.get<uint32_t>(nz), *d_nlit = b.get<uint32_t>(nz), *d_info = b.get<uint32_t>(nz);
-            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info)
+            uint8_t *d_ent = mode == BlobMode::lze ? b.get<uint8_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * ENT_SCRATCH) : nullptr;
+            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info || (mode == BlobMode::lze && !d_ent))
                 return fail(ctx, PBSGPU_ENOMEM, "match stage: device allocation failed");
             for (uint64_t f = 0; b.ok() && f < nz; f += LZ_PASS_BLOCKS) {
                 const uint32_t pn = (uint32_t)std::min<uint64_t>(LZ_PASS_BLOCKS, nz - f);
                 b.e = launch_lz_parse(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit, b.st);
                 if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
+                if (b.ok() && d_ent)
+                    b.e = launch_ent_encode((const LzTables *)ctx->d_lz_tab, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
+                                            d_info, d_ent, b.st);
             }
             info.resize(nz);
             if (b.ok()) b.e = cudaMemcpyAsync(info.data(), d_info, nz * 4, cudaMemcpyDeviceToHost, b.st);
@@ -314,13 +324,14 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
 
 // f3: complete DataBlobs for the NEW chunks of a batch in one call (upstream pbs-datastore data_blob.rs:
 // magic[8] | crc32 LE over the payload | payload; uploaded by POST /dynamic_chunk, reference
-// internal/server/backup/log_cleanup.go:19-31), with zstd frames as payloads where they are smaller when `compress`
-// (with the match stage when `lz`).
+// internal/server/backup/log_cleanup.go:19-31), with zstd frames as payloads where they are smaller unless `mode` is
+// raw.
 // The CRCs come from K6 on the device; payload bytes are copied once (device -> host for resident data and frames,
 // host -> host otherwise) straight into their place behind the header.
-static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, bool compress,
-                       bool lz, uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, BlobMode mode,
+                       uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     Guard g(ctx);
+    const bool compress = mode != BlobMode::raw;
     if (n == 0) return PBSGPU_OK;
     for (uint32_t i = 0; compress && i < n; i++)
         if (len[i] >= (1ull << 40)) return fail(ctx, PBSGPU_EINVAL, "blob %u longer than 2^40 bytes", i);
@@ -331,7 +342,7 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
     std::vector<uint64_t> frame_off(n), frame_len(n);
     std::vector<uint32_t> crc(n, 0);
     if (compress) {
-        int rc = zstd_frames(b, dbase, off, len, n, lz, comp, frame_off, frame_len, crc, &frames);
+        int rc = zstd_frames(b, dbase, off, len, n, mode, comp, frame_off, frame_len, crc, &frames);
         if (rc) return rc;
     }
     if (int rc = crc_where(ctx, comp, 0, dbase, off, len, crc)) return rc;
@@ -356,19 +367,25 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
 extern "C" int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                         uint8_t *out, const uint64_t *out_off, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !base))) return PBSGPU_EINVAL;
-    return blob_encode(ctx, base, off, len, n, false, false, out, out_off, nullptr, crc_out);
+    return blob_encode(ctx, base, off, len, n, BlobMode::raw, out, out_off, nullptr, crc_out);
 }
 
 extern "C" int pbsgpu_blob_encode_batch_z(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                           uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
-    return blob_encode(ctx, base, off, len, n, true, false, out, out_off, out_len, crc_out);
+    return blob_encode(ctx, base, off, len, n, BlobMode::z, out, out_off, out_len, crc_out);
 }
 
 extern "C" int pbsgpu_blob_encode_batch_lz(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
-    return blob_encode(ctx, base, off, len, n, true, true, out, out_off, out_len, crc_out);
+    return blob_encode(ctx, base, off, len, n, BlobMode::lz, out, out_off, out_len, crc_out);
+}
+
+extern "C" int pbsgpu_blob_encode_batch_lze(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
+    return blob_encode(ctx, base, off, len, n, BlobMode::lze, out, out_off, out_len, crc_out);
 }
 
 // ---------------------------------------------------------------------------

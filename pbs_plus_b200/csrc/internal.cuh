@@ -128,6 +128,7 @@ cudaError_t launch_zframe_emit(const uint8_t *base, uint8_t *stage, const uint64
 cudaError_t launch_zframe_hdr(uint8_t *stage, const uint64_t *frame_off, const uint64_t *content_len, uint32_t n, cudaStream_t st);
 }  // namespace pbsgpu
 #include "zlz.cuh"   // f3: LZ77 match stage + Predefined_Mode sequences (K9)
+#include "zent.cuh"  // f3: entropy stage: FSE_Compressed_Mode sequences + Huffman literals (K10)
 namespace pbsgpu {
 
 // ---- digest set (K4) ----------------------------------------------------------------

@@ -1,0 +1,405 @@
+// f3: zstd's entropy stage for compressed DataBlobs (K10, sm_90a): FSE_Compressed_Mode sequences, Huffman literals.
+//
+// K10 re-encodes what K9a parsed.  Per block of a pass, after K9b: the literals K9a left at slot + 3 and the sequences
+// in the pass scratch are coded with the block's own tables, and that Block_Content replaces K9b's (in the slot and in
+// info[g]) when it is smaller than K9b's and than the block.  tests/zstd_ent_ref.py (block_content) states the format;
+// each rule below is also stated and commented there.
+//
+//   sequences  LL, OF, ML columns: RLE_Mode when every sequence has the same code, else FSE_Compressed_Mode with
+//              log = min(cap, max(5, bit_length(n) - 2)), raised until 2^log >= the codes present (caps LL 9, OF 8,
+//              ML 9), and the distribution normalised as in ent_table.  Offsets stay offset + 3, so no Repeat_Mode;
+//              the bitstream is K9b's with these tables, the last sequence starting in state enc[code][0].
+//   literals   RLE_Literals_Block when all have one value; Huffman (Compressed_Literals_Block, direct 4-bit weights) when
+//              there are >= 2 values, none above 128, and that section is smaller than the raw one; else raw.  Code
+//              lengths <= 11 (two-queue Huffman, counts halved until the longest fits), canonical codes.  One stream
+//              when the regenerated and compressed sizes both fit 10 bits, else four behind the jump table.
+//
+// One CTA of 256 threads per block: shared-memory histograms (all threads); then warp 0 builds the Huffman code while
+// lane 0 of warps 1..3 builds the LL / OF / ML tables; then lane 0 of warp 7 runs the serial FSE chain into the
+// scratch while warps 0..6 write the Huffman streams (a scan of the code lengths places every thread's run of literals;
+// 32-bit atomicOr into zeroed scratch, since neighbouring runs share words); finally the CTA copies the chosen content
+// over the slot.  The content never overwrites the literals it is still reading: it is built in scratch first.
+#include "internal.cuh"
+
+namespace pbsgpu {
+
+constexpr int ENT_THREADS = 256;
+constexpr int ENT_WRITERS = ENT_THREADS - 32;   // warps 0..6 write the literals; lane 0 of warp 7 runs the FSE chain
+enum : uint32_t { LIT_RAW = 0, LIT_RLE = 1, LIT_HUF = 2 };
+
+struct EntShared {
+    uint32_t lhist[256];
+    uint32_t chist[3][64];             // code counts of the LL, OF, ML columns
+    int16_t norm[3][64];
+    uint16_t stab[3][512];             // FSE encoder: the states of each code, in state order, grouped by code
+    int32_t dnb[3][64], dfs[3][64];    // per code: Number_of_Bits transform and offset into stab (zstd's symbolTT)
+    uint8_t spread[3][512];            // the code of every state (one table per warp building it)
+    uint8_t desc[3][96];
+    uint32_t desc_len[3], log[3], mode[3];
+    uint32_t llbase[36], mlbase[53];
+    uint8_t llbits[36], mlbits[53], llcode[64], mlcode[128];
+    // Huffman
+    uint32_t hc[129], hw[257];
+    uint16_t hparent[257], hcode[256];
+    uint8_t horder[129], hdepth[257], hlen[256];
+    uint8_t tree[72];
+    uint32_t wsum[ENT_WRITERS / 32], sbits[4];
+    uint8_t seqhdr[8];
+    uint32_t kind, top, nh, maxlen, tree_len, t1, hs, bitlen, take, co, seqpos, seqhdr_len;
+};
+
+// LL / ML / OF code, value and Offset_Value of a packed K9a sequence
+struct Seq {
+    uint32_t ll, ml, ov, lc, mc, oc;
+    __device__ Seq(uint64_t v, const EntShared &s) {
+        ll = (uint32_t)(v & 0xFFFFF); ml = (uint32_t)((v >> 20) & 0xFFFFF); ov = (uint32_t)(v >> 40) + 3;
+        lc = ll < 64 ? s.llcode[ll] : 31 - __clz(ll) + 19;
+        mc = ml - 3 < 128 ? s.mlcode[ml - 3] : 31 - __clz(ml - 3) + 36;
+        oc = 31 - __clz(ov);
+    }
+};
+
+__device__ __forceinline__ void writers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(ENT_WRITERS) : "memory"); }
+
+// exclusive prefix sum over the writer threads; *total = the sum of all
+__device__ uint32_t writers_scan(uint32_t v, uint32_t *wsum, uint32_t *total) {
+    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t x = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(~0u, x, d);
+        if (lane >= (uint32_t)d) x += y;
+    }
+    if (lane == 31) wsum[w] = x;
+    writers_sync();
+    uint32_t before = 0, all = 0;
+    for (uint32_t k = 0; k < ENT_WRITERS / 32; k++) { before += k < w ? wsum[k] : 0; all += wsum[k]; }
+    writers_sync();   // wsum is reused by the next scan
+    *total = all;
+    return before + x - v;
+}
+
+// One column's table (t = 0 LL, 1 OF, 2 ML) over n >= 1 sequences: mode, description, accuracy log and encoder form.
+__device__ void ent_table(EntShared &s, int t, uint32_t n) {
+    const int nsym = t == 0 ? 36 : t == 1 ? 32 : 53;
+    const int cap = t == 0 ? ENT_LL_MAXLOG : t == 1 ? ENT_OF_MAXLOG : ENT_ML_MAXLOG;
+    const uint32_t *cnt = s.chist[t];
+    int16_t *norm = s.norm[t];
+    uint8_t *d = s.desc[t];
+    int distinct = 0, one = 0;
+    for (int c = 0; c < nsym; c++) if (cnt[c]) { distinct++; one = c; }
+    int log = 0;
+    if (distinct == 1) {   // RLE_Mode: the code itself; as a table, one state of accuracy log 0
+        for (int c = 0; c < nsym; c++) norm[c] = c == one;
+        s.mode[t] = 1; d[0] = (uint8_t)one; s.desc_len[t] = 1;
+    } else {
+        // about 4 sequences per state, within [ENT_MIN_LOG, cap], and at least one state per code present
+        log = min(cap, max(ENT_MIN_LOG, 32 - __clz(n) - 2));
+        while ((1 << log) < distinct) log++;
+        const int size = 1 << log;
+        // normalisation: max(1, floor(count * 2^log / n)); while the sum is too large, decrement the largest entry
+        // (the lowest code on ties); if too small, the entry with the largest count (lowest code on ties) takes the rest
+        int sum = 0;
+        for (int c = 0; c < nsym; c++) {
+            norm[c] = cnt[c] ? (int16_t)max(1u, cnt[c] * (uint32_t)size / n) : 0;
+            sum += norm[c];
+        }
+        while (sum > size) {
+            int k = 0;
+            for (int c = 1; c < nsym; c++) if (norm[c] > norm[k]) k = c;
+            norm[k]--; sum--;
+        }
+        if (sum < size) {
+            int k = 0;
+            for (int c = 1; c < nsym; c++) if (cnt[c] > cnt[k]) k = c;
+            norm[k] += size - sum;
+        }
+        // description (RFC 8878 4.1.1): Accuracy_Log - 5, then count + 1 per code in a variable number of bits, a zero
+        // count followed by 2-bit repeat flags for the zero counts after it, until the counts reach 2^log
+        uint64_t acc = (uint64_t)(log - ENT_MIN_LOG);
+        uint32_t na = 4, q = 0;
+        auto put = [&](uint32_t v, uint32_t nb) {
+            acc |= (uint64_t)v << na;
+            na += nb;
+            while (na >= 8) { if (q < sizeof s.desc[0]) d[q] = (uint8_t)acc; q++; acc >>= 8; na -= 8; }
+        };
+        int remaining = size + 1, threshold = size, nbits = log + 1, c = 0;
+        bool prev0 = false;
+        while (c < nsym && remaining > 1) {
+            if (prev0) {
+                int start = c;
+                while (norm[c] == 0) c++;
+                while (c >= start + 3) { start += 3; put(3, 2); }
+                put(c - start, 2);
+            }
+            int v = norm[c++];
+            const int mx = 2 * threshold - 1 - remaining;
+            remaining -= v;
+            v++;
+            if (v >= threshold) v += mx;
+            put(v, nbits - (v < mx));
+            prev0 = v == 1;
+            while (remaining < threshold) { nbits--; threshold >>= 1; }
+        }
+        if (na) { if (q < sizeof s.desc[0]) d[q] = (uint8_t)acc; q++; }
+        s.mode[t] = 2; s.desc_len[t] = q;
+    }
+    s.log[t] = log;
+    // encoder form (zstd's FSE_buildCTable): spread the codes over the states (RFC 8878 4.1.1; no "less than 1"
+    // cells), list each code's states in state order, and per code the transform from the next state to the bits to
+    // write and the state to be in
+    const int size = 1 << log, step = (size >> 1) + (size >> 3) + 3;
+    for (int c = 0, pos = 0; c < nsym; c++)
+        for (int k = 0; k < norm[c]; k++) { s.spread[t][pos] = (uint8_t)c; pos = (pos + step) & (size - 1); }
+    int32_t *next = s.dnb[t];   // the next free place of each code in stab, before dnb takes its final value
+    for (int c = 0, cum = 0; c < nsym; c++) { next[c] = cum; cum += norm[c]; }
+    for (int u = 0; u < size; u++) s.stab[t][next[s.spread[t][u]]++] = (uint16_t)u;
+    for (int c = 0; c < nsym; c++) {
+        const int k = norm[c], start = next[c] - k;
+        if (k == 0) { s.dnb[t][c] = 0; s.dfs[t][c] = 0; continue; }
+        if (k == 1) { s.dnb[t][c] = (log << 16) - size; s.dfs[t][c] = start - 1; continue; }
+        const int out = log - (31 - __clz(k - 1));
+        s.dnb[t][c] = (out << 16) - (k << out);
+        s.dfs[t][c] = start - k;
+    }
+}
+
+// Huffman code of the literals (warp 0): lengths, canonical codes, tree description and the one-stream bit count.
+__device__ void ent_huffman(EntShared &s, uint32_t lane) {
+    const uint32_t top = s.top, m = s.nh;
+    for (uint32_t x = lane; x <= top; x += 32) s.hc[x] = s.lhist[x];
+    __syncwarp();
+    for (;;) {
+        // present symbols in (count, symbol) order
+        for (uint32_t x = lane; x <= top; x += 32) {
+            const uint32_t c = s.hc[x];
+            if (!c) continue;
+            uint32_t r = 0;
+            for (uint32_t y = 0; y <= top; y++) { const uint32_t e = s.hc[y]; r += e && (e < c || (e == c && y < x)); }
+            s.horder[r] = (uint8_t)x;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            // two-queue Huffman: leaves in that order, internal nodes in the order they are made; each step joins the two
+            // smallest fronts, a leaf before a node of equal count.  A parent is made after its children.
+            for (uint32_t k = 0; k < m; k++) s.hw[k] = s.hc[s.horder[k]];
+            uint32_t i = 0, j = m, nxt = m;
+            for (uint32_t k = 0; k + 1 < m; k++, nxt++) {
+                uint32_t a, b;
+                if (i < m && (j >= nxt || s.hw[i] <= s.hw[j])) a = i++; else a = j++;
+                if (i < m && (j >= nxt || s.hw[i] <= s.hw[j])) b = i++; else b = j++;
+                s.hw[nxt] = s.hw[a] + s.hw[b];
+                s.hparent[a] = s.hparent[b] = (uint16_t)nxt;
+            }
+            s.hdepth[2 * m - 2] = 0;
+            for (int k = 2 * (int)m - 3; k >= 0; k--) s.hdepth[k] = s.hdepth[s.hparent[k]] + 1;
+            uint32_t mx = 0;
+            for (uint32_t k = 0; k < m; k++) { s.hlen[s.horder[k]] = s.hdepth[k]; mx = max(mx, (uint32_t)s.hdepth[k]); }
+            s.maxlen = mx;
+        }
+        __syncwarp();
+        if (s.maxlen <= ENT_HUF_MAXBITS) break;
+        for (uint32_t x = lane; x <= top; x += 32) s.hc[x] = (s.hc[x] + 1) >> 1;   // a present symbol stays present
+        __syncwarp();
+    }
+    if (lane) return;
+    // canonical codes (RFC 8878 4.2.1.3): in (length descending, symbol ascending) order, consecutive prefixes in units
+    // of 2^(maxbits - length)
+    const uint32_t mx = s.maxlen;
+    uint32_t nxt = 0, t1 = 0;
+    for (uint32_t len = mx; len >= 1; len--)
+        for (uint32_t x = 0; x <= top; x++)
+            if (s.hlen[x] == len) { s.hcode[x] = (uint16_t)(nxt >> (mx - len)); nxt += 1u << (mx - len); }
+    // tree description, direct form: 127 + top, then the weights (maxbits + 1 - length, or 0) of symbols 0..top-1, two
+    // per byte, the first in the high nibble; the weight of `top` is implied
+    auto wt = [&](uint32_t x) -> uint32_t { return x < top && s.hlen[x] ? mx + 1 - s.hlen[x] : 0; };
+    s.tree[0] = (uint8_t)(127 + top);
+    for (uint32_t k = 0; k < top; k += 2) s.tree[1 + k / 2] = (uint8_t)(wt(k) << 4 | wt(k + 1));
+    s.tree_len = 1 + (top + 1) / 2;
+    for (uint32_t x = 0; x <= top; x++) t1 += s.lhist[x] * s.hlen[x];
+    s.t1 = t1;
+}
+
+// The Huffman literals section into A (writer threads).  Falls back to raw (s.kind) when it is not smaller.
+__device__ void ent_literals(EntShared &s, const uint8_t *lit, uint32_t nl, uint8_t *A) {
+    const uint32_t tid = threadIdx.x, tl = s.tree_len;
+    const uint32_t ns = nl <= 1023 && tl + s.t1 / 8 + 1 <= 1023 ? 1 : 4;
+    const uint32_t seg = ns == 1 ? nl : (nl + 3) / 4;
+    uint32_t start[4] = {0, 0, 0, 0};
+    // stream k holds literals [k * seg, + len) written from the last to the first, so the bit position of a literal
+    // is the sum of the code lengths of the literals after it in its stream
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        if (k == ns) break;
+        const uint32_t a = k * seg, len = min(nl, a + seg) - a, per = (len + ENT_WRITERS - 1) / ENT_WRITERS;
+        const uint32_t r0 = min(tid * per, len), r1 = min(r0 + per, len);
+        uint32_t v = 0, tot;
+        for (uint32_t r = r0; r < r1; r++) v += s.hlen[lit[a + len - 1 - r]];
+        start[k] = writers_scan(v, s.wsum, &tot);
+        if (tid == 0) s.sbits[k] = tot;
+    }
+    writers_sync();
+    uint32_t c = tl + (ns == 4 ? 6 : 0);
+    for (uint32_t k = 0; k < ns; k++) c += s.sbits[k] / 8 + 1;   // + the end mark
+    const uint32_t big = max(nl, c);
+    const uint32_t sf = ns == 1 ? 0 : big <= 1023 ? 1 : big <= 16383 ? 2 : 3, hl = sf < 2 ? 3 : sf + 2;
+    const uint32_t hs = hl + c, raw = (nl <= 31 ? 1 : nl <= 4095 ? 2 : 3) + nl;
+    if (hs >= raw) {
+        if (tid == 0) s.kind = LIT_RAW;
+        return;
+    }
+    const uint32_t hdr = hl + tl + (ns == 4 ? 6 : 0);
+    uint32_t *A32 = (uint32_t *)A;
+    for (uint32_t k = tid; k < (hs + 3) / 4; k += ENT_WRITERS) A32[k] = 0;
+    writers_sync();
+    uint32_t pos = hdr;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        if (k == ns) break;
+        const uint32_t a = k * seg, len = min(nl, a + seg) - a, per = (len + ENT_WRITERS - 1) / ENT_WRITERS;
+        const uint32_t r0 = min(tid * per, len), r1 = min(r0 + per, len);
+        const uint32_t bit = pos * 8 + start[k];
+        if (r0 < r1) {
+            uint32_t w = bit >> 5, na = bit & 31;
+            uint64_t acc = 0;
+            for (uint32_t r = r0; r < r1; r++) {
+                const uint32_t x = lit[a + len - 1 - r];
+                acc |= (uint64_t)s.hcode[x] << na;
+                na += s.hlen[x];
+                if (na >= 32) { atomicOr(A32 + w, (uint32_t)acc); acc >>= 32; na -= 32; w++; }
+            }
+            if (na) atomicOr(A32 + w, (uint32_t)acc);
+        }
+        const uint32_t end = pos * 8 + s.sbits[k];
+        if (tid == 0) atomicOr(A32 + (end >> 5), 1u << (end & 31));
+        pos += s.sbits[k] / 8 + 1;
+    }
+    writers_sync();
+    if (tid == 0) {
+        const uint64_t h = 2 | sf << 2 | (uint64_t)nl << 4 | (uint64_t)c << (sf < 2 ? 14 : sf == 2 ? 18 : 22);
+        for (uint32_t k = 0; k < hl; k++) A[k] = (uint8_t)(h >> (8 * k));
+        for (uint32_t k = 0; k < tl; k++) A[hl + k] = s.tree[k];
+        for (uint32_t k = 0; ns == 4 && k < 3; k++) {
+            const uint32_t b = s.sbits[k] / 8 + 1;
+            A[hl + tl + 2 * k] = (uint8_t)b; A[hl + tl + 2 * k + 1] = (uint8_t)(b >> 8);
+        }
+        s.hs = hs;
+    }
+}
+
+__global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab, const uint32_t *size, uint64_t first,
+                                                            uint8_t *slots, const uint64_t *seqs, const uint32_t *nseq,
+                                                            const uint32_t *nlit, uint32_t *info, uint8_t *scratch) {
+    __shared__ EntShared s;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint64_t g = first + blockIdx.x;
+    const uint32_t n = nseq[g], nl = nlit[g];
+    uint8_t *slot = slots + g * LZ_SLOT;
+    const uint8_t *lit = slot + 3;
+    const uint64_t *sq = seqs + (uint64_t)blockIdx.x * LZ_MAX_SEQ;
+    uint8_t *A = scratch + (uint64_t)blockIdx.x * ENT_SCRATCH, *B = A + LZ_SLOT;
+
+    for (uint32_t k = tid; k < 256; k += ENT_THREADS) { s.lhist[k] = 0; s.hlen[k] = 0; }
+    for (uint32_t k = tid; k < 3 * 64; k += ENT_THREADS) s.chist[k / 64][k % 64] = 0;
+    for (uint32_t k = tid; k < 128; k += ENT_THREADS) {
+        if (k < 36) { s.llbase[k] = __ldg(&tab->ll_base[k]); s.llbits[k] = __ldg(&tab->ll_bits[k]); }
+        if (k < 53) { s.mlbase[k] = __ldg(&tab->ml_base[k]); s.mlbits[k] = __ldg(&tab->ml_bits[k]); }
+        if (k < 64) s.llcode[k] = __ldg(&tab->ll_code[k]);
+        s.mlcode[k] = __ldg(&tab->ml_code[k]);
+    }
+    __syncthreads();
+    for (uint32_t i = tid; i < nl; i += ENT_THREADS) atomicAdd(&s.lhist[lit[i]], 1u);
+    for (uint32_t k = tid; k < n; k += ENT_THREADS) {
+        const Seq q(sq[k], s);
+        atomicAdd(&s.chist[0][q.lc], 1u); atomicAdd(&s.chist[1][q.oc], 1u); atomicAdd(&s.chist[2][q.mc], 1u);
+    }
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t cnt = 0, top = 0;
+        for (uint32_t x = lane; x < 256; x += 32) if (s.lhist[x]) { cnt++; top = x; }
+        cnt = __reduce_add_sync(~0u, cnt);
+        top = __reduce_max_sync(~0u, top);
+        const uint32_t kind = nl == 0 ? LIT_RAW : cnt == 1 ? LIT_RLE : top > ENT_HUF_MAXSYMBOL ? LIT_RAW : LIT_HUF;
+        if (lane == 0) { s.kind = kind; s.top = top; s.nh = cnt; }
+        __syncwarp();
+        if (kind == LIT_HUF) ent_huffman(s, lane);
+    } else if (warp <= 3 && lane == 0 && n) {
+        ent_table(s, warp - 1, n);
+    }
+    __syncthreads();
+    if (warp == ENT_WRITERS / 32) {
+        if (lane == 0 && n) {
+            // the FSE chain, as K9b's with the block's tables; a state is kept as 2^log + state (zstd's CState)
+            LzBits w{B, 0};
+            uint32_t X[3] = {0, 0, 0}, sz[3];
+#pragma unroll
+            for (int t = 0; t < 3; t++) sz[t] = 1u << s.log[t];
+            auto step = [&](int t, uint32_t c) {
+                const uint32_t nb = (uint32_t)((int)X[t] + s.dnb[t][c]) >> 16;
+                w.add(X[t] & ((1u << nb) - 1), nb);
+                X[t] = sz[t] + s.stab[t][(int)(X[t] >> nb) + s.dfs[t][c]];
+            };
+            for (uint32_t k = n; k-- > 0;) {
+                const Seq q(sq[k], s);
+                if (k + 1 == n) {   // enc[code][0]: the state from which the decoder goes to state 0
+                    X[0] = sz[0]; X[1] = sz[1]; X[2] = sz[2];
+                    const LzBits keep = w;
+                    step(0, q.lc); step(1, q.oc); step(2, q.mc);
+                    w = keep;
+                } else {
+                    step(1, q.oc); step(2, q.mc); step(0, q.lc);
+                }
+                w.add(q.ll - s.llbase[q.lc], s.llbits[q.lc]);
+                w.add(q.ml - s.mlbase[q.mc], s.mlbits[q.mc]);
+                w.add(q.ov - (1u << q.oc), q.oc);
+            }
+            w.add(X[2] - sz[2], s.log[2]); w.add(X[1] - sz[1], s.log[1]); w.add(X[0] - sz[0], s.log[0]); w.add(1, 1);
+            if (w.n) w.byte((uint32_t)w.acc);
+            s.bitlen = w.q;
+        }
+    } else if (s.kind == LIT_HUF) {
+        ent_literals(s, lit, nl, A);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        const uint32_t hl = nl <= 31 ? 1 : nl <= 4095 ? 2 : 3, kind = s.kind;
+        const uint32_t litlen = kind == LIT_HUF ? s.hs : kind == LIT_RLE ? hl + 1 : hl + nl;
+        uint32_t q = 0, seqlen = 1;
+        if (n == 0) s.seqhdr[q++] = 0;
+        else {
+            if (n < 128) s.seqhdr[q++] = (uint8_t)n;
+            else if (n < 0x7F00) { s.seqhdr[q++] = (uint8_t)((n >> 8) + 0x80); s.seqhdr[q++] = (uint8_t)n; }
+            else { s.seqhdr[q++] = 0xFF; s.seqhdr[q++] = (uint8_t)(n - 0x7F00); s.seqhdr[q++] = (uint8_t)((n - 0x7F00) >> 8); }
+            s.seqhdr[q++] = (uint8_t)(s.mode[0] << 6 | s.mode[1] << 4 | s.mode[2] << 2);   // LL, OF, ML
+            seqlen = q + s.desc_len[0] + s.desc_len[1] + s.desc_len[2] + s.bitlen;
+        }
+        const uint32_t E = litlen + seqlen, K = info[g] & 0x3FFFFFFFu;   // K9b wins ties
+        s.take = E < K && E < size[g];
+        s.seqhdr_len = q;
+        s.co = kind == LIT_HUF ? 0 : 3 - hl;
+        s.seqpos = s.co + litlen;
+        if (s.take) {
+            info[g] = E | s.co << 30;
+            if (kind == LIT_RLE) slot[s.co] |= 1;   // K9b's raw header with Literals_Block_Type 1; slot + 3 holds the value
+        }
+    }
+    __syncthreads();
+    if (!s.take) return;
+    if (s.kind == LIT_HUF)
+        for (uint32_t i = tid; i < s.hs; i += ENT_THREADS) slot[i] = A[i];
+    const uint32_t h = s.seqhdr_len, d0 = h + (n ? s.desc_len[0] : 0), d1 = d0 + (n ? s.desc_len[1] : 0);
+    const uint32_t d2 = d1 + (n ? s.desc_len[2] : 0), end = d2 + (n ? s.bitlen : 0);
+    uint8_t *out = slot + s.seqpos;
+    for (uint32_t i = tid; i < end; i += ENT_THREADS)
+        out[i] = i < h ? s.seqhdr[i] : i < d0 ? s.desc[0][i - h] : i < d1 ? s.desc[1][i - d0] : i < d2 ? s.desc[2][i - d1] : B[i - d2];
+}
+
+cudaError_t launch_ent_encode(const LzTables *tab, const uint32_t *size, uint64_t first, uint32_t nb, uint8_t *slots,
+                              const uint64_t *seqs, const uint32_t *nseq, const uint32_t *nlit, uint32_t *info,
+                              uint8_t *scratch, cudaStream_t st) {
+    if (nb == 0) return cudaSuccess;
+    k_ent_encode<<<nb, ENT_THREADS, 0, st>>>(tab, size, first, slots, seqs, nseq, nlit, info, scratch);
+    return cudaGetLastError();
+}
+
+}  // namespace pbsgpu

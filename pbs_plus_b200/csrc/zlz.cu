@@ -104,20 +104,6 @@ cudaError_t launch_lz_parse(const uint8_t *base, const uint64_t *src, const uint
     return cudaGetLastError();
 }
 
-// Bits are appended LSB first; bytes at or beyond LZ_SLOT are counted but not stored (such a block stays raw).
-struct LzBits {
-    uint8_t *slot;
-    uint32_t q;
-    uint64_t acc = 0;
-    uint32_t n = 0;
-    __device__ void byte(uint32_t v) { if (q < LZ_SLOT) slot[q] = (uint8_t)v; q++; }
-    __device__ void add(uint32_t v, uint32_t nb) {
-        acc |= (uint64_t)v << n;
-        n += nb;
-        while (n >= 8) { byte((uint32_t)acc); acc >>= 8; n -= 8; }
-    }
-};
-
 __global__ void __launch_bounds__(128) k_lz_encode(const LzTables *tab, uint64_t first, uint32_t nb, uint8_t *slots,
                                                    const uint64_t *seqs, const uint32_t *nseq, const uint32_t *nlit,
                                                    uint32_t *info) {

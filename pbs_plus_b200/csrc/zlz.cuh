@@ -27,6 +27,20 @@ struct LzTables {
 static_assert(sizeof(LzTables) % 16 == 0, "copied to shared memory in 16-byte words");
 void lz_fill_tables_host(void *dst);
 
+// Bits are appended LSB first; bytes at or beyond LZ_SLOT are counted but not stored (such a block stays raw).
+struct LzBits {
+    uint8_t *slot;
+    uint32_t q;
+    uint64_t acc = 0;
+    uint32_t n = 0;
+    __device__ void byte(uint32_t v) { if (q < LZ_SLOT) slot[q] = (uint8_t)v; q++; }
+    __device__ void add(uint32_t v, uint32_t nb) {
+        acc |= (uint64_t)v << n;
+        n += nb;
+        while (n >= 8) { byte((uint32_t)acc); acc >>= 8; n -= 8; }
+    }
+};
+
 // K9a: blocks [first, first + nb) of the list (src[], size[]); literals to slots + g * LZ_SLOT + 3, sequences to
 // seqs + (g - first) * LZ_MAX_SEQ, counts to nseq[g] / nlit[g].
 cudaError_t launch_lz_parse(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint64_t first, uint32_t nb,

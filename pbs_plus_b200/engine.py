@@ -256,6 +256,12 @@ class Engine:
         blobs, crc[n]."""
         return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lz, base, off, length)
 
+    def blob_encode_batch_lze(self, base, off, length):
+        """blob_encode_batch_lz with zstd's entropy stage: each compressed block is the smaller of the _lz one and one
+        with tables fitted to the block (FSE_Compressed_Mode sequences, Huffman literals) (pbsgpu_blob_encode_batch_lze)
+        -> list of n `bytes` blobs, crc[n]."""
+        return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lze, base, off, length)
+
     def _blob_encode_sized(self, fn, base, off, length):
         o, l = self._offlen(off, length)
         sizes = l + np.uint64(12)

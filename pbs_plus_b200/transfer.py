@@ -58,7 +58,8 @@ class DedupWriter:
     # chunks of a flush by ONE pbsgpu_blob_encode_batch_z call (zstd frame where smaller, CRC-32 from the GPU)
     upload_blob: Callable[[bytes, bytes], None] | None = None
     batch_bytes: int = 1 << 30
-    # "z": frames of RLE and raw blocks; "lz": also compressed blocks from the LZ77 match stage (pbsgpu_blob_encode_batch_lz)
+    # "z": frames of RLE and raw blocks; "lz": also compressed blocks from the LZ77 match stage (pbsgpu_blob_encode_batch_lz);
+    # "lze": those blocks also through zstd's entropy stage (pbsgpu_blob_encode_batch_lze)
     blob_compression: str = "z"
     index: list[IndexRecord] = field(default_factory=list)
     # relPath -> XXH3-64 of the file as uploaded: commitWalkState.backedHashes (commit.go:187, :725), computed on the
@@ -69,8 +70,8 @@ class DedupWriter:
     _finished: bool = False
 
     def __post_init__(self):
-        if self.blob_compression not in ("z", "lz"):
-            raise ValueError(f"transfer: blob_compression must be 'z' or 'lz', not {self.blob_compression!r}")
+        if self.blob_compression not in ("z", "lz", "lze"):
+            raise ValueError(f"transfer: blob_compression must be 'z', 'lz' or 'lze', not {self.blob_compression!r}")
 
     def WriteEntryReader(self, entry: Entry, reader: BinaryIO, size: int) -> None:
         """Pulls exactly `size` bytes from `reader` (error if it yields fewer, like io.ReadFull)."""
@@ -111,7 +112,7 @@ class DedupWriter:
         if self.upload_blob is not None and new_chunks:
             boff = np.array([int(offs[i]) + s0 for _, i, s0, _ in new_chunks], dtype=np.uint64)
             blen = np.array([e0 - s0 for _, _, s0, e0 in new_chunks], dtype=np.uint64)
-            encode = self.engine.blob_encode_batch_lz if self.blob_compression == "lz" else self.engine.blob_encode_batch_z
+            encode = getattr(self.engine, "blob_encode_batch_" + self.blob_compression)
             blobs, _crc = encode(buf, boff, blen)
             for (d, _i, _s, _e), blob in zip(new_chunks, blobs):
                 self.upload_blob(d, blob)

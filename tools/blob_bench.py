@@ -42,7 +42,8 @@ def images():
 for label, d in images():
     torch.cuda.synchronize()
     print(f"-- {label} image, {n / 2**30:.0f} GiB")
-    for name in ("crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz"):
+    for name in ("crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz",
+                 "blob_encode_batch_lze"):
         for rep in range(3):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
