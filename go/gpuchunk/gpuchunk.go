@@ -375,14 +375,90 @@ func (st *Stream) Finish() ([]Chunk, error) {
 
 func (st *Stream) Close() { C.pbsgpu_stream_close(st.s) }
 
+// Blob modes of SetBlobMode: the encoders of Batch.BlobEncode, BlobEncodeZ, BlobEncodeLZ and BlobEncodeLZE.
+const (
+	BlobNone = C.PBSGPU_BLOB_NONE
+	BlobRaw  = C.PBSGPU_BLOB_RAW
+	BlobZ    = C.PBSGPU_BLOB_Z
+	BlobLZ   = C.PBSGPU_BLOB_LZ
+	BlobLZE  = C.PBSGPU_BLOB_LZE
+)
+
+// SetBlobMode makes the stream encode a DataBlob for every new chunk on the GPU (before the first byte).
+func (st *Stream) SetBlobMode(mode int) error { return st.e.err(C.pbsgpu_stream_blob_mode(st.s, C.int(mode))) }
+
+// PollBlobs returns up to max blobs available now; blob k belongs to the k-th chunk without Known in Poll order.
+func (st *Stream) PollBlobs(buf []byte, max int) ([][]byte, error) {
+	var out [][]byte
+	lens := make([]C.uint64_t, 256)
+	for len(out) < max {
+		want := max - len(out)
+		if want > len(lens) {
+			want = len(lens)
+		}
+		var n C.uint64_t
+		if err := st.e.err(C.pbsgpu_stream_poll_blobs(st.s, (*C.uint8_t)(unsafe.Pointer(&buf[0])), C.uint64_t(len(buf)),
+			&lens[0], C.uint64_t(want), &n)); err != nil {
+			return out, err
+		}
+		if n == 0 {
+			break
+		}
+		pos := uint64(0)
+		for i := 0; i < int(n); i++ {
+			out = append(out, append([]byte(nil), buf[pos:pos+uint64(lens[i])]...))
+			pos += uint64(lens[i])
+		}
+	}
+	return out, nil
+}
+
+// HashRange registers [offset, offset+length) for XXH3-64 before its bytes are written.
+func (st *Stream) HashRange(offset, length uint64) error {
+	return st.e.err(C.pbsgpu_stream_hash_range(st.s, C.uint64_t(offset), C.uint64_t(length)))
+}
+
+// PollHashes returns the hashes of the registered ranges available now, in registration order.
+func (st *Stream) PollHashes() ([]uint64, error) {
+	var all []uint64
+	buf := make([]C.uint64_t, 4096)
+	for {
+		var n C.uint64_t
+		if err := st.e.err(C.pbsgpu_stream_poll_hashes(st.s, &buf[0], C.uint64_t(len(buf)), &n)); err != nil {
+			return all, err
+		}
+		if n == 0 {
+			return all, nil
+		}
+		for i := 0; i < int(n); i++ {
+			all = append(all, uint64(buf[i]))
+		}
+	}
+}
+
 // PayloadWriter produces the pxar v2 PAYLOAD stream the production chunker sees -- start marker, then per file a
 // 16-byte PAYLOAD header + content (internal/pxarmount/pxarfs.go:408-411) -- through ONE Stream, with a suggested
 // boundary at every file start.  WriteEntryReader returns the entry's payload offset (what the mpxar PAYLOAD_REF
 // stores).  This, not per-file batching, is the layout an existing .ppxar.didx describes.
+//
+// With PayloadOptions.BlobMode set, UploadBlob receives the DataBlob of every new chunk (encoded on the GPU from the
+// stream's windows: "upload only !Known chunks"); with HashFiles, BackedHashes maps each path to the file's XXH3-64
+// (commitWalkState.backedHashes, commit.go:725).
 type PayloadWriter struct {
-	st      *Stream
-	Chunks  []Chunk
-	started bool
+	st           *Stream
+	Chunks       []Chunk
+	started      bool
+	opt          PayloadOptions
+	blobBuf      []byte
+	pending      []Digest // digests of new chunks whose blob has not come back yet
+	hashed       []string // paths whose hash has not come back yet
+	BackedHashes map[string]uint64
+}
+
+type PayloadOptions struct {
+	BlobMode   int
+	UploadBlob func(digest Digest, blob []byte) error
+	HashFiles  bool
 }
 
 const (
@@ -401,19 +477,50 @@ func header(htype, fullSize uint64) []byte {
 }
 
 func (e *Engine) NewPayloadWriter(cfg Config, known *KnownSet) (*PayloadWriter, error) {
+	return e.NewPayloadWriterOpts(cfg, known, PayloadOptions{})
+}
+
+func (e *Engine) NewPayloadWriterOpts(cfg Config, known *KnownSet, opt PayloadOptions) (*PayloadWriter, error) {
 	st, err := e.NewStream(cfg, known)
 	if err != nil {
 		return nil, err
 	}
-	w := &PayloadWriter{st: st}
+	w := &PayloadWriter{st: st, opt: opt, BackedHashes: map[string]uint64{}}
+	if opt.BlobMode != BlobNone {
+		if opt.UploadBlob == nil {
+			st.Close()
+			return nil, fmt.Errorf("gpuchunk: a blob mode needs an UploadBlob callback")
+		}
+		if err := st.SetBlobMode(opt.BlobMode); err != nil {
+			st.Close()
+			return nil, err
+		}
+		w.blobBuf = make([]byte, uint64(C.pbsgpu_blob_size(cfg.c.max))+16<<20)
+	}
 	_, err = st.Write(header(pxarPayloadStartMarker, 16))
 	return w, err
 }
 
+// WriteEntryReader writes one file without a path; with HashFiles set, use WriteBackedEntry so that the hash has a key.
 func (w *PayloadWriter) WriteEntryReader(r io.Reader, size uint64) (payloadOffset uint64, err error) {
+	if w.opt.HashFiles {
+		return 0, fmt.Errorf("gpuchunk: with HashFiles, files are written through WriteBackedEntry(path, ...)")
+	}
+	return w.WriteBackedEntry("", r, size)
+}
+
+// WriteBackedEntry is WriteEntryReader for the file at path (relPath in emitBackedFile): with HashFiles set, its
+// XXH3-64 lands in BackedHashes[path].
+func (w *PayloadWriter) WriteBackedEntry(path string, r io.Reader, size uint64) (payloadOffset uint64, err error) {
 	payloadOffset = w.st.Position()
 	if err = w.st.Suggest(); err != nil {
 		return
+	}
+	if w.opt.HashFiles {
+		if err = w.st.HashRange(payloadOffset+16, size); err != nil {
+			return
+		}
+		w.hashed = append(w.hashed, path)
 	}
 	if _, err = w.st.Write(header(pxarPayload, 16+size)); err != nil {
 		return
@@ -422,8 +529,43 @@ func (w *PayloadWriter) WriteEntryReader(r io.Reader, size uint64) (payloadOffse
 		return
 	}
 	done, err := w.st.Poll()
-	w.Chunks = append(w.Chunks, done...)
+	if err == nil {
+		err = w.drain(done)
+	}
 	return
+}
+
+// drain records the chunks, uploads the blobs of the new ones whose records are here and stores the finished hashes.
+func (w *PayloadWriter) drain(done []Chunk) error {
+	w.Chunks = append(w.Chunks, done...)
+	if w.opt.BlobMode != BlobNone {
+		for _, c := range done {
+			if !c.Known {
+				w.pending = append(w.pending, c.Digest)
+			}
+		}
+		blobs, err := w.st.PollBlobs(w.blobBuf, len(w.pending))
+		for i, b := range blobs {
+			if err == nil {
+				err = w.opt.UploadBlob(w.pending[i], b)
+			}
+		}
+		w.pending = w.pending[len(blobs):]
+		if err != nil {
+			return err
+		}
+	}
+	if len(w.hashed) > 0 {
+		hs, err := w.st.PollHashes()
+		for i, h := range hs {
+			w.BackedHashes[w.hashed[i]] = h
+		}
+		w.hashed = w.hashed[len(hs):]
+		if err != nil {
+			return err
+		}
+	}
+	return nil
 }
 
 func (w *PayloadWriter) Finish() ([]Chunk, error) {
@@ -431,7 +573,9 @@ func (w *PayloadWriter) Finish() ([]Chunk, error) {
 		return nil, err
 	}
 	done, err := w.st.Finish()
-	w.Chunks = append(w.Chunks, done...)
+	if err == nil {
+		err = w.drain(done)
+	}
 	w.st.Close()
 	return w.Chunks, err
 }

@@ -211,6 +211,23 @@ uint64_t pbsgpu_stream_slot_bytes(const pbsgpu_stream *s);
 int pbsgpu_stream_suggest(pbsgpu_stream *s, uint64_t offset);
 /* Bytes written so far (= the payload offset the next entry will get in the mpxar PAYLOAD_REF). */
 uint64_t pbsgpu_stream_position(const pbsgpu_stream *s);
+/* DataBlobs of the stream's NEW chunks, encoded on the device from the window that holds them.  The mode is set before
+ * the first byte (PBSGPU_ESTATE after that) and has the meaning of pbsgpu_blob_encode_batch (RAW), _z, _lz and _lze;
+ * NONE, the default, encodes nothing.  Blob k belongs to the k-th record without PBSGPU_CHUNK_KNOWN in poll() order, so
+ * with a digest set every new digest gets exactly one blob.  A window's blobs become available when its records do, all
+ * of them after finish().  poll_blobs copies whole blobs back to back into out[0, out_cap) and their lengths into
+ * blob_len[0, cap); out_cap must be at least pbsgpu_blob_size(cfg.max), so every call makes progress. */
+enum { PBSGPU_BLOB_NONE = 0, PBSGPU_BLOB_RAW = 1, PBSGPU_BLOB_Z = 2, PBSGPU_BLOB_LZ = 3, PBSGPU_BLOB_LZE = 4 };
+int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode);
+int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
+                             uint64_t *n_out);
+/* XXH3-64 (seed 0) of the stream bytes [offset, offset + len), registered before they are written: offset at or after
+ * pbsgpu_stream_position, ranges ascending and not overlapping (PBSGPU_EINVAL otherwise).  The payload writer registers
+ * every file's content.  Each byte is hashed once on the device, in the window that holds it.  poll_hashes returns the
+ * hashes in registration order; a hash is available once the window holding the range's last byte has been collected.
+ * finish() fails with PBSGPU_EINVAL when a range extends past the end of the stream. */
+int pbsgpu_stream_hash_range(pbsgpu_stream *s, uint64_t offset, uint64_t len);
+int pbsgpu_stream_poll_hashes(pbsgpu_stream *s, uint64_t *out, uint64_t cap, uint64_t *n_out);
 
 /* ---- a4: known-digest set -------------------------------------------------------
  * Replaces the known-chunk bookkeeping of the reference's dedup session:

@@ -11,6 +11,7 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <deque>
 #include <functional>
 #include <map>
 #include <stdexcept>
@@ -140,14 +141,28 @@ class DedupWriter {
 // Start marker, then per file a 16-byte PAYLOAD header + content (reference internal/pxarmount/pxarfs.go:408-411),
 // chunker state carried across files, a suggested boundary at every file start, bytes read straight into the
 // library's pinned ring.  WriteEntryReader (commit.go:720) returns the entry's payload offset.
+// Optional: `blob_mode` (PBSGPU_BLOB_RAW .. _LZE) hands the DataBlob of every new chunk to `upload_blob(digest, blob,
+// len)`, encoded on the GPU from the stream's windows; `hash_files` records every file's XXH3-64 in BackedHashes()
+// (commitWalkState.backedHashes, commit.go:725).
 struct PayloadChunk { uint64_t end_off; uint8_t digest[32]; bool known; };
+using UploadBlob = std::function<void(const uint8_t digest[32], const uint8_t *blob, uint64_t len)>;
 
 class PayloadStreamWriter {
   public:
-    PayloadStreamWriter(Engine &e, const buzhash::Config &cfg, KnownSet *known, bool suggest = true)
-        : e_(e), suggest_(suggest) {
+    PayloadStreamWriter(Engine &e, const buzhash::Config &cfg, KnownSet *known, bool suggest = true,
+                        int blob_mode = PBSGPU_BLOB_NONE, UploadBlob upload_blob = nullptr, bool hash_files = false)
+        : e_(e), suggest_(suggest), upload_(std::move(upload_blob)), hash_(hash_files) {
+        if ((blob_mode != PBSGPU_BLOB_NONE) != (upload_ != nullptr))
+            throw Error(PBSGPU_EINVAL, "transfer: a blob mode and an upload_blob callback go together");
+        if (upload_) blob_buf_.resize(pbsgpu_blob_size(cfg.max) + (16u << 20));
         e.check(pbsgpu_stream_open(e.ctx(), &cfg, known ? known->handle() : nullptr, &s_));
-        raw(header(0x834c68c2194a4ed2ull, 16));                     // PXAR_PAYLOAD_START_MARKER
+        try {   // the destructor does not run for a constructor that throws
+            if (upload_) e.check(pbsgpu_stream_blob_mode(s_, blob_mode));
+            raw(header(0x834c68c2194a4ed2ull, 16));                 // PXAR_PAYLOAD_START_MARKER
+        } catch (...) {
+            pbsgpu_stream_close(s_);
+            throw;
+        }
     }
     ~PayloadStreamWriter() { pbsgpu_stream_close(s_); }
     PayloadStreamWriter(const PayloadStreamWriter &) = delete;
@@ -157,6 +172,7 @@ class PayloadStreamWriter {
         if (finished_) throw Error(PBSGPU_ESTATE, "transfer: writer already finished");
         const uint64_t off = pbsgpu_stream_position(s_);
         if (suggest_) e_.check(pbsgpu_stream_suggest(s_, off));
+        if (hash_) { e_.check(pbsgpu_stream_hash_range(s_, off + 16, size)); hashed_.push_back(entry.Path); }
         raw(header(0x28147a1b0b7c1a25ull, 16 + size));              // PXAR_PAYLOAD
         const uint64_t slot = pbsgpu_stream_slot_bytes(s_);
         uint64_t left = size;
@@ -185,6 +201,7 @@ class PayloadStreamWriter {
         }
         return index_;
     }
+    const std::map<std::string, uint64_t> &BackedHashes() const { return backed_hashes_; }
 
   private:
     static std::vector<uint8_t> header(uint64_t htype, uint64_t full) {
@@ -203,13 +220,38 @@ class PayloadStreamWriter {
                 PayloadChunk c; c.end_off = buf[i].end_off; std::memcpy(c.digest, buf[i].digest, 32);
                 c.known = (buf[i].flags & PBSGPU_CHUNK_KNOWN) != 0;
                 index_.push_back(c);
+                if (upload_ && !c.known) pending_.push_back(index_.size() - 1);
             }
+        }
+        // blob k belongs to the k-th new record: ask only for blobs whose records are here already
+        uint64_t lens[256];
+        while (!pending_.empty()) {
+            uint64_t n = 0;
+            const uint64_t cap = pending_.size() < 256 ? pending_.size() : 256;
+            e_.check(pbsgpu_stream_poll_blobs(s_, blob_buf_.data(), blob_buf_.size(), lens, cap, &n));
+            if (!n) break;
+            const uint8_t *b = blob_buf_.data();
+            for (uint64_t i = 0; i < n; b += lens[i], i++) {
+                upload_(index_[pending_.front()].digest, b, lens[i]);
+                pending_.pop_front();
+            }
+        }
+        uint64_t h[256];
+        for (uint64_t n = 1; n && !hashed_.empty();) {
+            e_.check(pbsgpu_stream_poll_hashes(s_, h, 256, &n));
+            for (uint64_t i = 0; i < n; i++) { backed_hashes_[hashed_.front()] = h[i]; hashed_.pop_front(); }
         }
     }
     Engine &e_;
     pbsgpu_stream *s_ = nullptr;
     bool suggest_, finished_ = false;
+    UploadBlob upload_;
+    bool hash_;
+    std::vector<uint8_t> blob_buf_;
     std::vector<PayloadChunk> index_;
+    std::deque<size_t> pending_;          // index_ positions of new chunks whose blob has not come back yet
+    std::deque<std::string> hashed_;      // paths whose hash has not come back yet
+    std::map<std::string, uint64_t> backed_hashes_;
 };
 
 }  // namespace transfer

@@ -36,6 +36,8 @@ class Chunk(C.Structure):
 CHUNK_DTYPE = np.dtype([("stream", "<u4"), ("flags", "<u4"), ("end_off", "<u8"), ("digest", "u1", (32,))])
 assert CHUNK_DTYPE.itemsize == C.sizeof(Chunk) == 48
 CHUNK_KNOWN = 1
+# pbsgpu_stream_blob_mode: the DataBlob encoder of a stream's new chunks (None = no blobs)
+BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4}
 
 
 class DevInfo(C.Structure):
@@ -75,7 +77,8 @@ SYMBOLS = [
     "pbsgpu_chunk_digest_batch_ex", "pbsgpu_batch_submit_ex", "pbsgpu_batch_free", "pbsgpu_batch_wait_input", "pbsgpu_batch_input_done",
     "pbsgpu_scan_batch", "pbsgpu_sha256_batch", "pbsgpu_stream_open", "pbsgpu_stream_write",
     "pbsgpu_stream_poll", "pbsgpu_stream_finish", "pbsgpu_stream_close", "pbsgpu_stream_reserve", "pbsgpu_stream_commit",
-    "pbsgpu_stream_slot_bytes", "pbsgpu_stream_suggest", "pbsgpu_stream_position", "pbsgpu_set_create",
+    "pbsgpu_stream_slot_bytes", "pbsgpu_stream_suggest", "pbsgpu_stream_position", "pbsgpu_stream_blob_mode",
+    "pbsgpu_stream_poll_blobs", "pbsgpu_stream_hash_range", "pbsgpu_stream_poll_hashes", "pbsgpu_set_create",
     "pbsgpu_set_destroy", "pbsgpu_set_insert", "pbsgpu_set_probe", "pbsgpu_set_count", "pbsgpu_set_seed_didx",
     "pbsgpu_set_allgather", "pbsgpu_nccl_unique_id", "pbsgpu_nccl_comm_create", "pbsgpu_nccl_comm_destroy",
     "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
@@ -136,6 +139,10 @@ def lib() -> C.CDLL:
     L.pbsgpu_stream_suggest.argtypes = [vp, C.c_uint64]
     L.pbsgpu_stream_position.argtypes = [vp]
     L.pbsgpu_stream_position.restype = C.c_uint64
+    L.pbsgpu_stream_blob_mode.argtypes = [vp, C.c_int]
+    L.pbsgpu_stream_poll_blobs.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, u64p]
+    L.pbsgpu_stream_hash_range.argtypes = [vp, C.c_uint64, C.c_uint64]
+    L.pbsgpu_stream_poll_hashes.argtypes = [vp, vp, C.c_uint64, u64p]
     L.pbsgpu_set_allgather.argtypes = [vp, vp, vp, C.c_uint64, vp]
     L.pbsgpu_nccl_unique_id.argtypes = [vp]
     L.pbsgpu_nccl_comm_create.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(vp)]

@@ -364,6 +364,13 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
     return PBSGPU_OK;
 }
 
+// The stream's blob mode (capi_stream.cu): PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZE are the four encoders in order.
+int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
+                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len) {
+    static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze};
+    return blob_encode(ctx, base, off, len, n, modes[mode - PBSGPU_BLOB_RAW], out, out_off, out_len, nullptr);
+}
+
 extern "C" int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                         uint8_t *out, const uint64_t *out_off, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !base))) return PBSGPU_EINVAL;
@@ -400,6 +407,12 @@ void pbsgpu_xxh3_release(pbsgpu_ctx *ctx, XxhRun *r) {
     ctx->dev.put(r->d_off); ctx->dev.put(r->d_len); ctx->dev.put(r->d_first); ctx->dev.put(r->d_out);
     ctx->dev.put(r->d_state); ctx->dev.put(r->d_S);
     *r = XxhRun();
+}
+
+int pbsgpu_xxh3_table(pbsgpu_ctx *ctx, const void **tab) {
+    const int rc = upload_table_once(ctx, &ctx->d_xxh_tab, xxh3_tables_bytes(), xxh3_fill_tables_host);
+    *tab = ctx->d_xxh_tab;
+    return rc;
 }
 
 int pbsgpu_xxh3_enqueue(pbsgpu_ctx *ctx, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n,

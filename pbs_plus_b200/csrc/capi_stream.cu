@@ -12,6 +12,15 @@
 // copied device-to-device behind the scan, and the window's SHA-256 half is enqueued asynchronously -- so the serial tail
 // of a window's longest chunk overlaps the copies and scans of the following windows (up to PBSGPU_STREAM_NBUF in
 // flight).  poll() hands out the chunks of finished windows in stream order.
+//
+// Two optional products of a window, made before its buffer is released:
+//  - DataBlobs of its new chunks (pbsgpu_stream_blob_mode): at collect time the window's chunks without
+//    PBSGPU_CHUNK_KNOWN are encoded in place by the batch encoders (capi_aux.cu) into a pinned arena of the stream.
+//  - XXH3-64 of registered byte ranges (pbsgpu_stream_hash_range): each window hashes the blocks, tails and short ranges
+//    that lie in its CONSUMED part [base_off, base_off + consumed) with K7's piece form, on the stream's own CUDA stream
+//    (window k+1 continues window k's chain).  Ranges do not overlap, so at most one range crosses a window end; the
+//    span of it that is still needed (a block, the tail or a short range: < 1 KiB) is copied device-to-device into the
+//    carry area in front of the next window's buffer, which makes it contiguous with the window's bytes.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -21,8 +30,20 @@
 
 using namespace pbsgpu;
 
-struct StreamJob { pbsgpu_job *j; int buf; uint64_t base_off; };
+// The hash work of one window: the pinned lists it was launched with (its results come back behind them), the device
+// block of lists, block sums and results, and the registration indices of the ranges it finishes.
+struct WindowHash {
+    void *host = nullptr, *dev = nullptr;
+    const uint64_t *h_out = nullptr;   // [n] hashes of the window's ranges
+    std::vector<uint64_t> seq;         // registration index of every range finished here ...
+    std::vector<uint32_t> slot;        // ... and its index in the window's list
+    cudaEvent_t done = nullptr;
+};
+struct StreamJob { pbsgpu_job *j; int buf; uint64_t base_off; WindowHash *wh; };
+struct BlobWindow { uint8_t *host; std::vector<uint64_t> off, len; size_t next; };   // one window's blobs, back to back
+struct HashRange { uint64_t off, len, h; bool done; };
 constexpr int RING_SLOTS = 8;
+constexpr uint64_t CARRY_BYTES = 2048;   // in front of every window buffer: the carried span of a hash range (< 1 KiB)
 
 struct pbsgpu_stream {
     pbsgpu_ctx *ctx;
@@ -47,6 +68,18 @@ struct pbsgpu_stream {
     bool slot_used[RING_SLOTS] = {};
     int slot_next = 0, slot_reserved = -1;
     cudaEvent_t copied = nullptr;     // after the most recent H2D copy into the current window
+    // DataBlobs of new chunks
+    int blob_mode = PBSGPU_BLOB_NONE;
+    std::deque<BlobWindow> blobs;
+    // XXH3-64 of registered ranges; hr[k] has registration index hr_base + k
+    std::deque<HashRange> hr;
+    uint64_t hr_base = 0;
+    uint64_t hr_work = 0;             // registration index of the first range with bytes still to hash
+    uint64_t hr_blk = 0;              // full blocks of that range hashed so far
+    uint64_t hr_end = 0;              // end of the last registered range
+    cudaStream_t hs = nullptr;        // every window's hash work, in window order
+    uint64_t *d_state = nullptr;      // [2][8] chain state of the range that crosses a window end: read from one slot,
+    int state_slot = 0;               // written to the other (state_slot is the one to read); swapped per hash launch
 };
 
 extern "C" int pbsgpu_stream_open(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, pbsgpu_set *set, pbsgpu_stream **out) {
@@ -66,14 +99,65 @@ extern "C" int pbsgpu_stream_open(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, pbsgpu
     return PBSGPU_OK;
 }
 
+// a window buffer with the hash carry area in front of it
+static uint8_t *buf_get(pbsgpu_ctx *ctx, uint64_t cap) {
+    uint8_t *p = (uint8_t *)ctx->dev.get(CARRY_BYTES + cap);
+    return p ? p + CARRY_BYTES : nullptr;
+}
+
 static int stream_start(pbsgpu_stream *s) {
     pbsgpu_ctx *ctx = s->ctx;
     if (s->started) return PBSGPU_OK;
     s->cap = s->window + s->cfg.max + 256;
-    s->buf[0] = (uint8_t *)ctx->dev.get(s->cap);      // further buffers are allocated when first needed
+    s->buf[0] = buf_get(ctx, s->cap);                 // further buffers are allocated when first needed
     if (!s->buf[0]) return fail(ctx, PBSGPU_ENOMEM, "stream buffer of %llu bytes failed", (unsigned long long)s->cap);
     if (cudaEventCreateWithFlags(&s->copied, cudaEventDisableTiming) != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "cudaEventCreate failed"); }
     s->started = true;
+    return PBSGPU_OK;
+}
+
+static void window_hash_release(pbsgpu_ctx *ctx, WindowHash *wh) {
+    if (!wh) return;
+    if (wh->done) { cudaEventSynchronize(wh->done); cudaEventDestroy(wh->done); }
+    ctx->dev.put(wh->dev); ctx->pin.put(wh->host);
+    (void)cudaGetLastError();
+    delete wh;
+}
+
+// the window's hashes: wait for its hash work and mark its finished ranges
+static int collect_hashes(pbsgpu_stream *s, WindowHash *wh) {
+    pbsgpu_ctx *ctx = s->ctx;
+    const cudaError_t e = cudaEventSynchronize(wh->done);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, PBSGPU_ECUDA, "stream hash: %s", cudaGetErrorString(e)); }
+    for (size_t k = 0; k < wh->seq.size(); k++) {
+        HashRange &r = s->hr[wh->seq[k] - s->hr_base];
+        r.h = wh->h_out[wh->slot[k]]; r.done = true;
+    }
+    return PBSGPU_OK;
+}
+
+// the window's new chunks -- [0, end) of the first, then from end to end (the carry put the first at offset 0) -- as
+// DataBlobs into a pinned block of the stream
+static int collect_blobs(pbsgpu_stream *s, const pbsgpu_job *j, const uint8_t *buf) {
+    pbsgpu_ctx *ctx = s->ctx;
+    const uint64_t nch = j->h_counters[CTR_CHUNKS];
+    std::vector<uint64_t> off, len, out_off;
+    uint64_t prev = 0, bytes = 0;
+    for (uint64_t k = 0; k < nch; k++) {
+        const uint64_t end = j->h_out[k].end_off;
+        if (!(j->h_out[k].flags & PBSGPU_CHUNK_KNOWN)) {
+            off.push_back(prev); len.push_back(end - prev); out_off.push_back(bytes);
+            bytes += pbsgpu_blob_size(end - prev);
+        }
+        prev = end;
+    }
+    if (off.empty()) return PBSGPU_OK;
+    BlobWindow bw{(uint8_t *)ctx->pin.get(bytes), std::move(out_off), std::vector<uint64_t>(off.size()), 0};
+    if (!bw.host) return fail(ctx, PBSGPU_ENOMEM, "pinned blob arena of %llu bytes failed", (unsigned long long)bytes);
+    const int rc = pbsgpu_blob_encode_mode(ctx, buf, off.data(), len.data(), (uint32_t)off.size(), s->blob_mode, bw.host,
+                                           bw.off.data(), bw.len.data());
+    if (rc) { ctx->pin.put(bw.host); return rc; }
+    s->blobs.push_back(std::move(bw));
     return PBSGPU_OK;
 }
 
@@ -87,7 +171,10 @@ static int stream_collect(pbsgpu_stream *s, bool block) {
         }
         int rc = pbsgpu_job_finish(sj.j);
         s->inflight.pop_front();
-        s->busy[sj.buf] = 0;
+        if (rc == PBSGPU_OK && sj.wh) rc = collect_hashes(s, sj.wh);
+        if (rc == PBSGPU_OK && s->blob_mode != PBSGPU_BLOB_NONE) rc = collect_blobs(s, sj.j, s->buf[sj.buf]);
+        window_hash_release(s->ctx, sj.wh);
+        s->busy[sj.buf] = 0;                          // the window's bytes are no longer needed
         if (rc != PBSGPU_OK) { pbsgpu_job_release(sj.j); return rc; }
         const uint64_t nch = sj.j->h_counters[CTR_CHUNKS];
         for (uint64_t k = 0; k < nch; k++) {
@@ -96,6 +183,99 @@ static int stream_collect(pbsgpu_stream *s, bool block) {
             s->ready.push_back(c);
         }
         pbsgpu_job_release(sj.j);
+    }
+    return PBSGPU_OK;
+}
+
+// K7's piece form over the window's list, on the stream's hash stream behind the window's bytes
+static int hash_enqueue(pbsgpu_stream *s, const std::vector<uint64_t> &off, const std::vector<uint64_t> &len,
+                        const std::vector<uint64_t> &first, const std::vector<uint64_t> &blo, const std::vector<uint8_t> &fin,
+                        WindowHash &&wh, WindowHash **out) {
+    pbsgpu_ctx *ctx = s->ctx;
+    const uint32_t n = (uint32_t)off.size();
+    // one pinned block: off | len | first | blo | fin, then the results; one device block: the same lists, the results,
+    // the block sums
+    const uint64_t total = first.back(), fin_words = (n + 7) / 8, list_words = 4ull * n + 1 + fin_words;
+    const uint64_t s_word = (list_words + n + 1) & ~1ull;   // 16 B aligned block sums
+    const void *tab = nullptr;
+    if (int rc = pbsgpu_xxh3_table(ctx, &tab)) return rc;
+    if (!s->hs) CK(cudaStreamCreateWithFlags(&s->hs, cudaStreamNonBlocking));
+    if (!s->d_state && !(s->d_state = (uint64_t *)ctx->dev.get(128))) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    WindowHash *w = new WindowHash(std::move(wh));
+    w->host = ctx->pin.get((list_words + n) * 8);
+    w->dev = ctx->dev.get((s_word + total * 8) * 8);
+    if (!w->host || !w->dev || cudaEventCreateWithFlags(&w->done, cudaEventDisableTiming) != cudaSuccess) {
+        (void)cudaGetLastError(); window_hash_release(ctx, w);
+        return fail(ctx, PBSGPU_ENOMEM, "stream hash: allocation failed");
+    }
+    uint64_t *h = (uint64_t *)w->host, *d = (uint64_t *)w->dev;
+    memcpy(h, off.data(), n * 8); memcpy(h + n, len.data(), n * 8); memcpy(h + 2 * n, first.data(), (n + 1) * 8);
+    memcpy(h + 3 * n + 1, blo.data(), n * 8); memcpy(h + 4 * n + 1, fin.data(), n);
+    w->h_out = h + list_words;
+    cudaError_t e = cudaStreamWaitEvent(s->hs, s->copied, 0);   // every byte of the window and of its carry is there
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d, h, list_words * 8, cudaMemcpyHostToDevice, s->hs);
+    if (e == cudaSuccess)
+        e = launch_xxh3_pieces(s->buf[s->cur], d, d + n, d + 2 * n, d + 3 * n + 1, (const uint8_t *)(d + 4 * n + 1), n, total,
+                               tab, d + s_word, s->d_state + 8 * s->state_slot, s->d_state + 8 * (1 - s->state_slot),
+                               d + list_words, s->hs);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h + list_words, d + list_words, n * 8, cudaMemcpyDeviceToHost, s->hs);
+    if (e == cudaSuccess) e = cudaEventRecord(w->done, s->hs);
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError(); window_hash_release(ctx, w);
+        return fail(ctx, PBSGPU_ECUDA, "stream hash: %s", cudaGetErrorString(e));
+    }
+    // the range that goes on (if any) saved its state in the other slot; a window without a launch has no range that
+    // goes on other than the carried one, whose state stays where it is
+    s->state_slot = 1 - s->state_slot;
+    *out = w;
+    return PBSGPU_OK;
+}
+
+// Enqueue the hash work of the current window, whose consumed part ends `consumed` bytes into buf[cur], and copy the span
+// a later window still needs into the carry area of buf[next].  *out = NULL when the window has nothing to hash.
+static int stream_hash(pbsgpu_stream *s, uint64_t consumed, int next, WindowHash **out) {
+    pbsgpu_ctx *ctx = s->ctx;
+    *out = nullptr;
+    const uint64_t w0 = s->base_off, w1 = w0 + consumed;
+    std::vector<uint64_t> off, len, first(1, 0), blo;
+    std::vector<uint8_t> fin;
+    WindowHash wh;
+    uint64_t keep = w1;          // first byte a later window still needs
+    uint64_t q = s->hr_work, blk = s->hr_blk;
+    for (; q < s->hr_base + s->hr.size(); q++, blk = 0) {
+        const HashRange &r = s->hr[q - s->hr_base];
+        if (r.len == 0) continue;                     // a constant, set when registered
+        if (r.off >= w1) break;
+        const uint64_t nb = r.len > 240 ? (r.len - 1) >> 10 : 0;
+        const uint64_t blk1 = std::min(nb, (w1 - r.off) >> 10);   // full blocks that end in this window
+        const bool done = r.off + r.len <= w1;
+        if (blk1 > blk || done) {
+            if (done) { wh.seq.push_back(q); wh.slot.push_back((uint32_t)off.size()); }
+            off.push_back(r.off - w0);                // modulo 2^64: the range may have begun in an earlier window
+            len.push_back(r.len); blo.push_back(blk); fin.push_back(done);
+            first.push_back(first.back() + (blk1 - blk));
+        }
+        if (!done) {   // crosses the window end: keep its next block, or its tail, or all of a short range
+            keep = nb == 0 ? r.off : blk1 < nb ? r.off + (blk1 << 10) : r.off + std::min(nb << 10, r.len - 64);
+            blk = blk1;
+            break;
+        }
+    }
+    s->hr_work = q; s->hr_blk = q < s->hr_base + s->hr.size() ? blk : 0;
+    const uint32_t n = (uint32_t)off.size();
+    if (n) {
+        int rc = hash_enqueue(s, off, len, first, blo, fin, std::move(wh), out);
+        if (rc) return rc;
+    }
+    const uint64_t carry = w1 - keep;   // stream bytes [keep, w1) go in front of buf[next]
+    if (carry) {
+        cudaError_t e = cudaMemcpyAsync(s->buf[next] - carry, s->buf[s->cur] + (int64_t)(keep - w0), carry,
+                                        cudaMemcpyDeviceToDevice, ctx->copy_stream);
+        if (e == cudaSuccess) e = cudaEventRecord(s->copied, ctx->copy_stream);
+        if (e != cudaSuccess) {
+            (void)cudaGetLastError(); window_hash_release(ctx, *out); *out = nullptr;
+            return fail(ctx, PBSGPU_ECUDA, "hash carry copy: %s", cudaGetErrorString(e));
+        }
     }
     return PBSGPU_OK;
 }
@@ -146,18 +326,21 @@ static int stream_process(pbsgpu_stream *s, int eof) {
     }
     if (next < 0) { pbsgpu_job_release(j); return fail(ctx, PBSGPU_ESTATE, "internal: no free stream buffer"); }
     if (!s->buf[next]) {
-        s->buf[next] = (uint8_t *)ctx->dev.get(s->cap);
+        s->buf[next] = buf_get(ctx, s->cap);
         if (!s->buf[next]) { pbsgpu_job_release(j); return fail(ctx, PBSGPU_ENOMEM, "stream buffer of %llu bytes failed", (unsigned long long)s->cap); }
     }
+    WindowHash *wh = nullptr;
+    rc = stream_hash(s, consumed, next, &wh);      // reads buf[cur] behind the window's copies; before the carry below
+    if (rc) { pbsgpu_job_release(j); return rc; }
     if (rest) {   // carry: ordered on the copy stream in front of the next window's H2D copies, no host wait
         cudaError_t e = cudaMemcpyAsync(s->buf[next], s->buf[s->cur] + consumed, rest, cudaMemcpyDeviceToDevice, ctx->copy_stream);
         if (e == cudaSuccess) e = cudaEventRecord(s->copied, ctx->copy_stream);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); pbsgpu_job_release(j); return fail(ctx, PBSGPU_ECUDA, "carry copy: %s", cudaGetErrorString(e)); }
+        if (e != cudaSuccess) { (void)cudaGetLastError(); window_hash_release(ctx, wh); pbsgpu_job_release(j); return fail(ctx, PBSGPU_ECUDA, "carry copy: %s", cudaGetErrorString(e)); }
     }
     rc = pbsgpu_job_enqueue_back(j);                          // SHA-256 etc. run while the next window fills
-    if (rc != PBSGPU_OK) { pbsgpu_job_release(j); return rc; }
+    if (rc != PBSGPU_OK) { window_hash_release(ctx, wh); pbsgpu_job_release(j); return rc; }
     s->busy[s->cur] = 1;
-    s->inflight.push_back(StreamJob{j, s->cur, s->base_off});
+    s->inflight.push_back(StreamJob{j, s->cur, s->base_off, wh});
     s->cur = next; s->fill = rest; s->base_off += consumed;
     return stream_collect(s, false);
 }
@@ -271,11 +454,79 @@ extern "C" int pbsgpu_stream_suggest(pbsgpu_stream *s, uint64_t offset) {
     return PBSGPU_OK;
 }
 
+extern "C" int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode) {
+    if (!s) return PBSGPU_EINVAL;
+    Guard g(s->ctx);
+    if (mode < PBSGPU_BLOB_NONE || mode > PBSGPU_BLOB_LZE) return fail(s->ctx, PBSGPU_EINVAL, "unknown blob mode %d", mode);
+    if (s->started || s->finished) return fail(s->ctx, PBSGPU_ESTATE, "the blob mode is set before the first byte");
+    s->blob_mode = mode;
+    return PBSGPU_OK;
+}
+
+extern "C" int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
+                                        uint64_t *n_out) {
+    if (!s || !n_out || (cap && (!out || !blob_len))) return PBSGPU_EINVAL;
+    pbsgpu_ctx *ctx = s->ctx;
+    Guard g(ctx);
+    if (out_cap < pbsgpu_blob_size(s->cfg.max))
+        return fail(ctx, PBSGPU_EINVAL, "blob buffer of %llu bytes is smaller than one blob of the largest chunk (%llu)",
+                    (unsigned long long)out_cap, (unsigned long long)pbsgpu_blob_size(s->cfg.max));
+    int rc = stream_collect(s, false);
+    if (rc) return rc;
+    uint64_t k = 0, used = 0;
+    while (!s->blobs.empty()) {
+        BlobWindow &bw = s->blobs.front();
+        for (; bw.next < bw.len.size() && k < cap && used + bw.len[bw.next] <= out_cap; bw.next++, k++) {
+            memcpy(out + used, bw.host + bw.off[bw.next], bw.len[bw.next]);
+            blob_len[k] = bw.len[bw.next];
+            used += bw.len[bw.next];
+        }
+        if (bw.next < bw.len.size()) break;
+        ctx->pin.put(bw.host);
+        s->blobs.pop_front();
+    }
+    *n_out = k;
+    return PBSGPU_OK;
+}
+
+extern "C" int pbsgpu_stream_hash_range(pbsgpu_stream *s, uint64_t offset, uint64_t len) {
+    if (!s) return PBSGPU_EINVAL;
+    pbsgpu_ctx *ctx = s->ctx;
+    Guard g(ctx);
+    if (s->finished) return fail(ctx, PBSGPU_ESTATE, "stream already finished");
+    const uint64_t pos = s->base_off + s->fill;
+    if (offset < pos) return fail(ctx, PBSGPU_EINVAL, "hash range at %llu lies behind the write position %llu", (unsigned long long)offset, (unsigned long long)pos);
+    if (offset < s->hr_end) return fail(ctx, PBSGPU_EINVAL, "hash range at %llu overlaps the previous one (ranges must ascend)", (unsigned long long)offset);
+    if (offset + len < offset) return fail(ctx, PBSGPU_EINVAL, "hash range overflows");
+    s->hr.push_back(HashRange{offset, len, len ? 0 : xxh3_empty_host(), len == 0});
+    s->hr_end = offset + len;
+    return PBSGPU_OK;
+}
+
+extern "C" int pbsgpu_stream_poll_hashes(pbsgpu_stream *s, uint64_t *out, uint64_t cap, uint64_t *n_out) {
+    if (!s || !n_out || (cap && !out)) return PBSGPU_EINVAL;
+    Guard g(s->ctx);
+    int rc = stream_collect(s, false);
+    if (rc) return rc;
+    uint64_t k = 0;
+    for (; k < cap && !s->hr.empty() && s->hr.front().done; k++) {
+        out[k] = s->hr.front().h;
+        s->hr.pop_front(); s->hr_base++;
+    }
+    // an empty range is done when registered, so the work cursor may sit on one that was just handed out
+    if (s->hr_work < s->hr_base) { s->hr_work = s->hr_base; s->hr_blk = 0; }
+    *n_out = k;
+    return PBSGPU_OK;
+}
+
 extern "C" int pbsgpu_stream_finish(pbsgpu_stream *s) {
     if (!s) return PBSGPU_EINVAL;
     Guard g(s->ctx);
     if (s->finished) return PBSGPU_OK;
     if (s->slot_reserved >= 0) return fail(s->ctx, PBSGPU_ESTATE, "a reserved slot is still uncommitted");
+    if (s->hr_end > s->base_off + s->fill)
+        return fail(s->ctx, PBSGPU_EINVAL, "a hash range ends at %llu, past the end of the stream (%llu)",
+                    (unsigned long long)s->hr_end, (unsigned long long)(s->base_off + s->fill));
     int rc = stream_process(s, 1);
     if (rc == PBSGPU_OK) rc = stream_collect(s, true);
     if (rc == PBSGPU_OK) s->finished = true;
@@ -301,8 +552,11 @@ extern "C" void pbsgpu_stream_close(pbsgpu_stream *s) {
     pbsgpu_ctx *ctx = s->ctx;
     Guard g(ctx);
     cudaStreamSynchronize(ctx->copy_stream);
-    for (auto &sj : s->inflight) pbsgpu_job_release(sj.j);
-    for (auto b : s->buf) ctx->dev.put(b);
+    for (auto &sj : s->inflight) { window_hash_release(ctx, sj.wh); pbsgpu_job_release(sj.j); }
+    for (auto b : s->buf) if (b) ctx->dev.put(b - CARRY_BYTES);
+    for (auto &bw : s->blobs) ctx->pin.put(bw.host);
+    ctx->dev.put(s->d_state);
+    if (s->hs) cudaStreamDestroy(s->hs);
     if (s->ring) ctx->pin.put(s->ring);
     for (auto e : s->slot_done) if (e) cudaEventDestroy(e);
     if (s->copied) cudaEventDestroy(s->copied);

@@ -168,6 +168,10 @@ cudaError_t launch_xxh3_pass(const uint8_t *base, const uint64_t *off, const uin
                              uint64_t *out, cudaStream_t st);
 cudaError_t launch_xxh3_small(const uint8_t *base, const uint64_t *off, const uint64_t *len, uint32_t n, const void *tab,
                               uint64_t *out, cudaStream_t st);
+cudaError_t launch_xxh3_pieces(const uint8_t *base, const uint64_t *off, const uint64_t *len, const uint64_t *first,
+                               const uint64_t *blo, const uint8_t *fin, uint32_t n, uint64_t total, const void *tab,
+                               uint64_t *S, uint64_t *state_in, uint64_t *state_out, uint64_t *out, cudaStream_t st);
+uint64_t xxh3_empty_host();
 void crc_fill_tables_host(void *dst);
 uint64_t crc_wb_bytes();
 

@@ -16,6 +16,15 @@
 // Streams of <= 1 KiB (all the short-length formulas, and long inputs with no full block) go through k_xxh3_small.
 // Scratch for S is bounded: a pass covers blocks [win_lo, win_lo + W) of every stream and the chain state is carried
 // between passes, so all streams stay parallel in every pass.
+//
+// Piece form (pbsgpu_stream_hash_range): each range of a pass starts at its own block index blo[s], and off[s] is the
+// position of the range's byte 0 relative to `base` taken modulo 2^64 -- it lies before `base` when the range began in an
+// earlier window (only bytes at or after blo[s]'s block, or the tail, are read, and those are in the window or in the
+// carry in front of it).  fin[s] says whether the tail is in this pass.  Ranges never overlap, so at most one range is
+// unfinished at a window end and carries chain state into the next pass.  That state is read from state[0..8) (by the
+// pass's first range, when it began earlier) and written to state_out[0..8) (by its last range, when it goes on): two
+// slots, so a pass whose first range reads the carried state while its last range saves its own has no
+// read-after-write race between their threads.  The caller swaps the slots between passes.
 #include "device.cuh"
 #include "internal.cuh"
 
@@ -93,6 +102,9 @@ struct XxhArgs {
     uint64_t *S;             // [total][8]
     uint64_t *state;         // [n][8] chain state between passes
     uint64_t *out;           // [n]
+    const uint64_t *blo;     // piece form: [n] first block of the range in this pass (NULL: win_lo for every stream)
+    const uint8_t *fin;      // piece form: [n] the range ends in this pass
+    uint64_t *state_out;     // piece form: [8] chain state of the range that goes on after this pass
 };
 
 constexpr int XA_U = 8;   // blocks per 4-lane group (8 KiB): one stream search per group
@@ -114,7 +126,8 @@ __global__ void __launch_bounds__(256) k_xxh3_blocks(XxhArgs a) {
         const uint64_t g = g0 + u;
         if (g >= a.total) break;
         while (g >= s_next) { s++; s_first = s_next; s_next = a.first[s + 1]; }
-        const uint8_t *p = a.base + a.off[s] + ((a.win_lo + (g - s_first)) << 10) + j * 16;
+        const uint64_t lo = a.blo ? a.blo[s] : a.win_lo;
+        const uint8_t *p = a.base + (a.off[s] + ((lo + (g - s_first)) << 10) + j * 16);
         uint64_t a0 = 0, a1 = 0;
         if ((((uintptr_t)p) & 15) == 0) {
             ulonglong2 d[16];
@@ -150,14 +163,25 @@ __global__ void __launch_bounds__(256) k_xxh3_chain(XxhArgs a) {
     const uint32_t s = in_range ? (uint32_t)sidx : 0;
     const uint64_t len = in_range ? a.len[s] : 0;
     const uint64_t nb = full_blocks(len);
-    const uint64_t lo = nb < a.win_lo ? nb : a.win_lo;
-    const uint64_t hi = nb < a.win_lo + a.win ? nb : a.win_lo + a.win;
-    const bool active = in_range && lo < hi;
-    const bool last = active && hi == nb;
+    uint64_t lo, hi;
+    bool active, last;
+    if (a.blo) {   // piece form: a range may have no block in the pass and only its tail
+        lo = in_range ? a.blo[s] : 0;
+        hi = in_range ? lo + (a.first[s + 1] - a.first[s]) : 0;
+        last = in_range && nb != 0 && a.fin[s];
+        active = in_range && (lo < hi || last);
+    } else {
+        lo = nb < a.win_lo ? nb : a.win_lo;
+        hi = nb < a.win_lo + a.win ? nb : a.win_lo + a.win;
+        active = in_range && lo < hi;
+        last = active && hi == nb;
+    }
     const uint8_t *sec = a.tab + XT_WORDS * 8;
+    const uint64_t *state_in = a.state + (a.blo ? 0 : (uint64_t)s * 8) + i;
+    uint64_t *state_out = (a.blo ? a.state_out : a.state + (uint64_t)s * 8) + i;
     uint64_t acc = 0;
     if (active) {
-        acc = a.win_lo == 0 ? acc_init(i) : a.state[(uint64_t)s * 8 + i];
+        acc = lo == 0 ? acc_init(i) : *state_in;
         const uint64_t ks = ld64u(sec + 128 + 8 * i);
         const uint64_t *sp = a.S + a.first[s] * 8 + i;
         // The loads do not depend on the chain: keep the next 16 block sums in flight while the current 16 are
@@ -186,12 +210,12 @@ __global__ void __launch_bounds__(256) k_xxh3_chain(XxhArgs a) {
 #pragma unroll
             for (int k = 0; k < PB; k++) cur[k] = nxt[k];
         }
-        if (!last) a.state[(uint64_t)s * 8 + i] = acc;
+        if (!last) *state_out = acc;
         else {
-            const uint8_t *d = a.base + a.off[s];
+            const uint64_t d = a.off[s];
             const uint64_t ns = ((len - 1) - (nb << 10)) >> 6;
-            for (uint64_t st = 0; st < ns; st++) acc += stripe_term(d + (nb << 10) + 64 * st, sec + 8 * st, i);
-            acc += stripe_term(d + len - 64, sec + 192 - 64 - 7, i);
+            for (uint64_t st = 0; st < ns; st++) acc += stripe_term(a.base + (d + (nb << 10) + 64 * st), sec + 8 * st, i);
+            acc += stripe_term(a.base + (d + len - 64), sec + 192 - 64 - 7, i);
         }
     }
     // merge: accumulators of one stream sit in 8 consecutive lanes
@@ -212,7 +236,7 @@ __global__ void __launch_bounds__(128) k_xxh3_small(XxhArgs a) {
     const uint32_t s = (uint32_t)tid;
     const uint64_t len = a.len[s];
     if (full_blocks(len) != 0) return;
-    const uint8_t *in = a.base + a.off[s];
+    const uint8_t *in = a.base + (int64_t)a.off[s];   // piece form: a carried range starts in front of `base`
     const uint8_t *S = a.tab + XT_WORDS * 8;
     uint64_t h;
     if (len == 0) h = aval64(ld64u(S + 56) ^ ld64u(S + 64));
@@ -263,7 +287,7 @@ __global__ void __launch_bounds__(128) k_xxh3_small(XxhArgs a) {
 cudaError_t launch_xxh3_pass(const uint8_t *base, const uint64_t *off, const uint64_t *len, const uint64_t *first, uint32_t n,
                              uint64_t total, uint64_t win_lo, uint64_t win, const void *tab, uint64_t *S, uint64_t *state,
                              uint64_t *out, cudaStream_t st) {
-    XxhArgs a{base, off, len, first, n, total, win_lo, win, (const uint8_t *)tab, S, state, out};
+    XxhArgs a{base, off, len, first, n, total, win_lo, win, (const uint8_t *)tab, S, state, out, nullptr, nullptr, nullptr};
     if (total) {
         const uint64_t groups = (total + XA_U - 1) / XA_U, threads = groups * 4;
         k_xxh3_blocks<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a);
@@ -277,9 +301,39 @@ cudaError_t launch_xxh3_pass(const uint8_t *base, const uint64_t *off, const uin
 
 cudaError_t launch_xxh3_small(const uint8_t *base, const uint64_t *off, const uint64_t *len, uint32_t n, const void *tab,
                               uint64_t *out, cudaStream_t st) {
-    XxhArgs a{base, off, len, nullptr, n, 0, 0, 0, (const uint8_t *)tab, nullptr, nullptr, out};
+    XxhArgs a{base, off, len, nullptr, n, 0, 0, 0, (const uint8_t *)tab, nullptr, nullptr, out, nullptr, nullptr, nullptr};
     k_xxh3_small<<<(n + 127) / 128, 128, 0, st>>>(a);
     return cudaGetLastError();
+}
+
+// Piece form: the ranges' blocks in this pass (prefix `first`, from block blo[s]), the chain carried in from state_in[0..8)
+// and out to state_out[0..8) (distinct slots), and the finish of every range with fin[s] -- long ranges in the chain
+// kernel, ranges of <= 1 KiB in k_xxh3_small.
+cudaError_t launch_xxh3_pieces(const uint8_t *base, const uint64_t *off, const uint64_t *len, const uint64_t *first,
+                               const uint64_t *blo, const uint8_t *fin, uint32_t n, uint64_t total, const void *tab,
+                               uint64_t *S, uint64_t *state_in, uint64_t *state_out, uint64_t *out, cudaStream_t st) {
+    XxhArgs a{base, off, len, first, n, total, 0, 0, (const uint8_t *)tab, S, state_in, out, blo, fin, state_out};
+    if (n == 0) return cudaSuccess;
+    if (total) {
+        const uint64_t groups = (total + XA_U - 1) / XA_U, threads = groups * 4;
+        k_xxh3_blocks<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    k_xxh3_chain<<<(unsigned)(((uint64_t)n * 8 + 255) / 256), 256, 0, st>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    k_xxh3_small<<<(n + 127) / 128, 128, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+// XXH3-64 of the empty input (a constant of the secret), for empty ranges that no window holds
+uint64_t xxh3_empty_host() {
+    uint64_t a = 0, b = 0;
+    for (int i = 0; i < 8; i++) { a |= (uint64_t)XSECRET[56 + i] << (8 * i); b |= (uint64_t)XSECRET[64 + i] << (8 * i); }
+    uint64_t h = a ^ b;
+    h ^= h >> 33; h *= XP64_2; h ^= h >> 29; h *= XP64_3; h ^= h >> 32;
+    return h;
 }
 
 }  // namespace pbsgpu

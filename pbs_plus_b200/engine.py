@@ -13,7 +13,7 @@ from typing import Iterable, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import CHUNK_DTYPE, CHUNK_KNOWN, BatchOpts, Cfg, Corpus, DevInfo, PbsGpuError, Timing
+from ._lib import BLOB_MODES, CHUNK_DTYPE, CHUNK_KNOWN, BatchOpts, Cfg, Corpus, DevInfo, PbsGpuError, Timing
 
 
 def _ptr(x) -> int:
@@ -459,6 +459,7 @@ class Stream:
 
     def __init__(self, eng: Engine, cfg: Cfg, digest_set: DigestSet | None):
         self._eng = eng
+        self._max = int(cfg.max)
         h = C.c_void_p()
         eng._ck(eng._L.pbsgpu_stream_open(eng._h, C.byref(cfg), digest_set._h if digest_set else None, C.byref(h)))
         self._h = h
@@ -490,6 +491,47 @@ class Stream:
         n = C.c_uint64()
         self._eng._ck(self._eng._L.pbsgpu_stream_poll(self._h, out.ctypes.data, cap, C.byref(n)))
         return out[: n.value]
+
+    def blob_mode(self, mode: str | None):
+        """DataBlobs for the new chunks (pbsgpu_stream_blob_mode), set before the first byte: None (no blobs), "raw",
+        "z", "lz" or "lze" -- the encoders of Engine.blob_encode_batch, _z, _lz and _lze."""
+        if mode not in BLOB_MODES:
+            raise ValueError(f"blob mode must be one of {list(BLOB_MODES)}, not {mode!r}")
+        self._eng._ck(self._eng._L.pbsgpu_stream_blob_mode(self._h, BLOB_MODES[mode]))
+
+    def poll_blobs(self, out_cap: int = 0) -> list[bytes]:
+        """Every blob available now, in order: blob k belongs to the k-th record without CHUNK_KNOWN."""
+        L = self._eng._L
+        want = max(int(out_cap), int(L.pbsgpu_blob_size(self._max)), 1 << 24)
+        if getattr(self, "_blob_buf", None) is None or len(self._blob_buf) < want:
+            self._blob_buf = np.empty(want, dtype=np.uint8)
+        out = self._blob_buf
+        lens = np.zeros(4096, dtype=np.uint64)
+        n = C.c_uint64()
+        blobs = []
+        while True:
+            self._eng._ck(L.pbsgpu_stream_poll_blobs(self._h, out.ctypes.data, len(out), lens.ctypes.data, len(lens), C.byref(n)))
+            pos = 0
+            for k in range(n.value):
+                blobs.append(out[pos: pos + int(lens[k])].tobytes())
+                pos += int(lens[k])
+            if n.value == 0:
+                return blobs
+
+    def hash_range(self, offset: int, length: int):
+        """Register [offset, offset + length) for XXH3-64 before its bytes are written (pbsgpu_stream_hash_range)."""
+        self._eng._ck(self._eng._L.pbsgpu_stream_hash_range(self._h, int(offset), int(length)))
+
+    def poll_hashes(self, cap: int = 1 << 16) -> np.ndarray:
+        """Every XXH3-64 of the registered ranges available now, in registration order (`cap` per C call)."""
+        out = np.zeros(cap, dtype=np.uint64)
+        n = C.c_uint64()
+        parts = []
+        while True:
+            self._eng._ck(self._eng._L.pbsgpu_stream_poll_hashes(self._h, out.ctypes.data, cap, C.byref(n)))
+            if n.value == 0:
+                return np.concatenate(parts) if parts else np.zeros(0, dtype=np.uint64)
+            parts.append(out[: n.value].copy())
 
     def finish(self) -> np.ndarray:
         self._eng._ck(self._eng._L.pbsgpu_stream_finish(self._h))

@@ -23,6 +23,7 @@ Two writers:
 from __future__ import annotations
 
 import io
+from collections import deque
 from dataclasses import dataclass, field
 from typing import BinaryIO, Callable
 
@@ -70,8 +71,7 @@ class DedupWriter:
     _finished: bool = False
 
     def __post_init__(self):
-        if self.blob_compression not in ("z", "lz", "lze"):
-            raise ValueError(f"transfer: blob_compression must be 'z', 'lz' or 'lze', not {self.blob_compression!r}")
+        _check_blob_compression(self.blob_compression)
 
     def WriteEntryReader(self, entry: Entry, reader: BinaryIO, size: int) -> None:
         """Pulls exactly `size` bytes from `reader` (error if it yields fewer, like io.ReadFull)."""
@@ -137,6 +137,11 @@ class DedupWriter:
         return self.index
 
 
+def _check_blob_compression(c: str) -> None:
+    if c not in ("z", "lz", "lze"):
+        raise ValueError(f"transfer: blob_compression must be 'z', 'lz' or 'lze', not {c!r}")
+
+
 # pxar v2 format constants (upstream pxar crate format/mod.rs; restated, UNVERIFIED against the Go module)
 PXAR_PAYLOAD = 0x28147A1B0B7C1A25
 PXAR_PAYLOAD_START_MARKER = 0x834C68C2194A4ED2
@@ -162,18 +167,33 @@ class PayloadStreamWriter:
     suggest: bool = True             # suggested boundary at every file start (upstream PayloadChunker); False = plain chunker
     index: list[tuple[int, bytes, bool]] = field(default_factory=list)   # (end offset in the NEW stream, digest, known)
     payload_offsets: dict[str, int] = field(default_factory=dict)        # entry path -> offset of its PAYLOAD header
+    # (digest, DataBlob) for NEW chunks, encoded on the GPU from the stream's windows (pbsgpu_stream_blob_mode) with the
+    # encoder `blob_compression` names ("z", "lz" or "lze", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
+    upload_blob: Callable[[bytes, bytes], None] | None = None
+    blob_compression: str = "z"
+    # hash_files: relPath -> XXH3-64 of every file written through WriteEntryReader in backed_hashes
+    # (commitWalkState.backedHashes, commit.go:725), hashed on the GPU from the stream's windows
+    # (pbsgpu_stream_hash_range).  Off by default: a stream with no hash ranges does no hashing work.
+    hash_files: bool = False
+    backed_hashes: dict[str, int] = field(default_factory=dict)
     _stream: object = None
     _seg_base: int = 0               # offset in the new stream at which the current pbsgpu stream starts
     _last_ref: int = -1
     _finished: bool = False
+    _new: list = field(default_factory=list)          # digests of new records still waiting for their blob
+    _blobs: list = field(default_factory=list)        # blobs still waiting for their record
+    _hashed: deque = field(default_factory=deque)     # paths whose hash the stream has not returned yet
 
     def __post_init__(self):
+        _check_blob_compression(self.blob_compression)
         self._open()
         self._raw(PXAR_PAYLOAD_START_MARKER.to_bytes(8, "little") + (16).to_bytes(8, "little"))
 
     # -- plumbing ---------------------------------------------------------------------------------------------
     def _open(self):
         self._stream = self.engine.stream(self.config, self.known)
+        if self.upload_blob is not None:
+            self._stream.blob_mode(self.blob_compression)
 
     def _raw(self, data: bytes):
         self._stream.write(np.frombuffer(data, dtype=np.uint8))
@@ -185,7 +205,22 @@ class PayloadStreamWriter:
     def _drain(self, final: bool):
         rec = self._stream.finish() if final else self._stream.poll(1 << 16)
         for r in rec:
-            self.index.append((self._seg_base + int(r["end_off"]), bytes(r["digest"]), bool(r["flags"] & CHUNK_KNOWN)))
+            known = bool(r["flags"] & CHUNK_KNOWN)
+            self.index.append((self._seg_base + int(r["end_off"]), bytes(r["digest"]), known))
+            if self.upload_blob is not None and not known:
+                self._new.append(bytes(r["digest"]))
+        if self.upload_blob is not None:
+            # blob k belongs to the k-th new record; either side may run ahead of the other between polls
+            self._blobs += self._stream.poll_blobs()
+            k = min(len(self._new), len(self._blobs))
+            for d, b in zip(self._new[:k], self._blobs[:k]):
+                self.upload_blob(d, b)
+            del self._new[:k], self._blobs[:k]
+        if self._hashed:
+            for h in self._stream.poll_hashes():
+                self.backed_hashes[self._hashed.popleft()] = int(h)
+        if final and (self._new or self._blobs or self._hashed):
+            raise RuntimeError("transfer: the stream finished with blobs or hashes unaccounted for")
 
     # -- ArchiveWriter surface (commit.go:183) -------------------------------------------------------------------
     def WriteEntryReader(self, entry: Entry, reader: BinaryIO, size: int) -> int:
@@ -195,6 +230,9 @@ class PayloadStreamWriter:
         off = self.position
         if self.suggest and self._stream.position > 0:
             self._stream.suggest(self._stream.position)
+        if self.hash_files:
+            self._stream.hash_range(self._stream.position + 16, size)
+            self._hashed.append(entry.Path)
         self._raw(payload_header(size))
         left = size
         while left:
@@ -246,10 +284,12 @@ class PayloadStreamWriter:
     def Finish(self) -> list[tuple[int, bytes, bool]]:
         """commit.go:383: tail marker, final short chunk, index complete."""
         if not self._finished:
-            self._raw(PXAR_PAYLOAD_TAIL_MARKER.to_bytes(8, "little") + (16).to_bytes(8, "little"))
-            self._drain(True)
-            self._stream.close()
-            self._finished = True
+            try:
+                self._raw(PXAR_PAYLOAD_TAIL_MARKER.to_bytes(8, "little") + (16).to_bytes(8, "little"))
+                self._drain(True)
+            finally:
+                self._stream.close()
+                self._finished = True
         return self.index
 
     def didx(self, uuid: bytes = b"\0" * 16, ctime: int = 0) -> bytes:
