@@ -375,13 +375,15 @@ func (st *Stream) Finish() ([]Chunk, error) {
 
 func (st *Stream) Close() { C.pbsgpu_stream_close(st.s) }
 
-// Blob modes of SetBlobMode: the encoders of Batch.BlobEncode, BlobEncodeZ, BlobEncodeLZ and BlobEncodeLZE.
+// Blob modes of SetBlobMode: the encoders of Batch.BlobEncode, BlobEncodeZ, BlobEncodeLZ, BlobEncodeLZE and
+// BlobEncodeLZH.
 const (
 	BlobNone = C.PBSGPU_BLOB_NONE
 	BlobRaw  = C.PBSGPU_BLOB_RAW
 	BlobZ    = C.PBSGPU_BLOB_Z
 	BlobLZ   = C.PBSGPU_BLOB_LZ
 	BlobLZE  = C.PBSGPU_BLOB_LZE
+	BlobLZH  = C.PBSGPU_BLOB_LZH
 )
 
 // SetBlobMode makes the stream encode a DataBlob for every new chunk on the GPU (before the first byte).
@@ -675,6 +677,14 @@ func (b *Batch) BlobEncodeLZE(off, length []uint64) ([][]byte, error) {
 	return b.blobEncodeCompressed(off, length, blobLZE)
 }
 
+// BlobEncodeLZH is BlobEncodeLZE with Huffman literals whatever their largest byte value: the tree is written in the
+// direct or the FSE-compressed weight form, the smaller one, so binary data gets entropy-coded literals too.  Each blob
+// is at most the size of its BlobEncodeLZE blob.  Like the rest of this shim, it has not been compiled against a Go
+// toolchain.
+func (b *Batch) BlobEncodeLZH(off, length []uint64) ([][]byte, error) {
+	return b.blobEncodeCompressed(off, length, blobLZH)
+}
+
 // which compressed DataBlob encoder blobEncodeCompressed calls
 type blobMode int
 
@@ -682,6 +692,7 @@ const (
 	blobZ blobMode = iota
 	blobLZ
 	blobLZE
+	blobLZH
 )
 
 func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]byte, error) {
@@ -702,6 +713,8 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]b
 	dst := (*C.uint8_t)(unsafe.Pointer(&out[0]))
 	var rc C.int
 	switch mode {
+	case blobLZH:
+		rc = C.pbsgpu_blob_encode_batch_lzh(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	case blobLZE:
 		rc = C.pbsgpu_blob_encode_batch_lze(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	case blobLZ:

@@ -212,12 +212,13 @@ int pbsgpu_stream_suggest(pbsgpu_stream *s, uint64_t offset);
 /* Bytes written so far (= the payload offset the next entry will get in the mpxar PAYLOAD_REF). */
 uint64_t pbsgpu_stream_position(const pbsgpu_stream *s);
 /* DataBlobs of the stream's NEW chunks, encoded on the device from the window that holds them.  The mode is set before
- * the first byte (PBSGPU_ESTATE after that) and has the meaning of pbsgpu_blob_encode_batch (RAW), _z, _lz and _lze;
+ * the first byte (PBSGPU_ESTATE after that) and has the meaning of pbsgpu_blob_encode_batch (RAW), _z, _lz, _lze and _lzh;
  * NONE, the default, encodes nothing.  Blob k belongs to the k-th record without PBSGPU_CHUNK_KNOWN in poll() order, so
  * with a digest set every new digest gets exactly one blob.  A window's blobs become available when its records do, all
  * of them after finish().  poll_blobs copies whole blobs back to back into out[0, out_cap) and their lengths into
  * blob_len[0, cap); out_cap must be at least pbsgpu_blob_size(cfg.max), so every call makes progress. */
-enum { PBSGPU_BLOB_NONE = 0, PBSGPU_BLOB_RAW = 1, PBSGPU_BLOB_Z = 2, PBSGPU_BLOB_LZ = 3, PBSGPU_BLOB_LZE = 4 };
+enum { PBSGPU_BLOB_NONE = 0, PBSGPU_BLOB_RAW = 1, PBSGPU_BLOB_Z = 2, PBSGPU_BLOB_LZ = 3, PBSGPU_BLOB_LZE = 4,
+       PBSGPU_BLOB_LZH = 5 };
 int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode);
 int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
                              uint64_t *n_out);
@@ -310,6 +311,14 @@ int pbsgpu_blob_encode_batch_lz(pbsgpu_ctx *ctx, const void *base, const uint64_
  * independent (no Repeat_Mode, no Treeless literals).  Same arguments, limits and errors as _lz; each blob is at most the
  * size of its _lz blob.  The output is a deterministic function of the chunk bytes. */
 int pbsgpu_blob_encode_batch_lze(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                 uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+/* pbsgpu_blob_encode_batch_lze with Huffman-coded literals whatever their largest value: the tree description is the
+ * smaller of the direct 4-bit weight form (values up to 128) and the FSE-compressed weight form, so blocks of binary
+ * data, whose literals almost always reach above 128, get entropy-coded literals too.  The same parse and sequence
+ * tables; each Compressed_Block is the smallest of the _lz content, the _lze content and this one.  Same arguments,
+ * limits and errors as _lze; each blob is at most the size of its _lze blob.  The output is a deterministic function
+ * of the chunk bytes. */
+int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                  uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------

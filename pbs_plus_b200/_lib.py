@@ -37,7 +37,7 @@ CHUNK_DTYPE = np.dtype([("stream", "<u4"), ("flags", "<u4"), ("end_off", "<u8"),
 assert CHUNK_DTYPE.itemsize == C.sizeof(Chunk) == 48
 CHUNK_KNOWN = 1
 # pbsgpu_stream_blob_mode: the DataBlob encoder of a stream's new chunks (None = no blobs)
-BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4}
+BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5}
 
 
 class DevInfo(C.Structure):
@@ -83,6 +83,7 @@ SYMBOLS = [
     "pbsgpu_set_allgather", "pbsgpu_nccl_unique_id", "pbsgpu_nccl_comm_create", "pbsgpu_nccl_comm_destroy",
     "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
+    "pbsgpu_blob_encode_batch_lzh",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
 ]
@@ -154,6 +155,7 @@ def lib() -> C.CDLL:
     L.pbsgpu_blob_encode_batch_z.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lz.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lze.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.pbsgpu_blob_encode_batch_lzh.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_set_create.argtypes = [vp, C.c_uint64, C.POINTER(vp)]
     L.pbsgpu_set_destroy.argtypes = [vp]
     L.pbsgpu_set_destroy.restype = None

@@ -196,15 +196,14 @@ static int crc_where(pbsgpu_ctx *ctx, const std::vector<uint8_t> &comp, uint8_t 
 }
 
 // Which DataBlob encoder a call is: uncompressed only, RLE / raw frames (_z), with the match stage (_lz), with the match
-// and entropy stages (_lze).
-enum class BlobMode { raw, z, lz, lze };
+// and entropy stages (_lze), and with Huffman literals over every byte value (_lzh).
+enum class BlobMode { raw, z, lz, lze, lzh };
 
 // Compressed form: a blob's payload is a zstd frame when that is smaller than the raw bytes (upstream
 // `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device (zframe.cu, zlz.cu,
-// zent.cu): a 128 KiB block of one repeated byte is an RLE_Block (K8a decides); with lz / lze every other block goes
-// through the match stage (K9; lze adds the entropy stage, K10) and is a Compressed_Block when that is smaller than the
-// block; the rest are Raw_Blocks.  The CRC (K6) covers
-// the frame.  Marks those blobs in comp[] and leaves their frames at *frames + frame_off[i] (frame_len[i] bytes, a block
+// zent.cu): a 128 KiB block of one repeated byte is an RLE_Block (K8a decides); with lz / lze / lzh every other block
+// goes through the match stage (K9; lze and lzh add the entropy stage, K10, lzh with its full-alphabet flag) and is a
+// Compressed_Block when that is smaller than the block; the rest are Raw_Blocks.  The CRC (K6) covers the frame.  Marks those blobs in comp[] and leaves their frames at *frames + frame_off[i] (frame_len[i] bytes, a block
 // of `b`) and their CRCs in crc[].
 static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, BlobMode mode,
                        std::vector<uint8_t> &comp, std::vector<uint64_t> &frame_off, std::vector<uint64_t> &frame_len,
@@ -225,7 +224,7 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
     if (int rc = b.finish("zstd block scan")) return rc;
     auto block_size = [&](uint32_t i, uint64_t k) { return (uint32_t)std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK); };
     // K9 (+ K10): the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS
-    const bool lz = mode == BlobMode::lz || mode == BlobMode::lze;
+    const bool ent = mode == BlobMode::lze || mode == BlobMode::lzh, lz = mode == BlobMode::lz || ent;
     std::vector<uint32_t> info;
     const uint8_t *slots = nullptr;
     if (lz) {
@@ -242,8 +241,8 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
             uint8_t *d_slots = b.get<uint8_t>(nz * LZ_SLOT);
             uint64_t *d_seqs = b.get<uint64_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * LZ_MAX_SEQ);
             uint32_t *d_nseq = b.get<uint32_t>(nz), *d_nlit = b.get<uint32_t>(nz), *d_info = b.get<uint32_t>(nz);
-            uint8_t *d_ent = mode == BlobMode::lze ? b.get<uint8_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * ENT_SCRATCH) : nullptr;
-            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info || (mode == BlobMode::lze && !d_ent))
+            uint8_t *d_ent = ent ? b.get<uint8_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * ENT_SCRATCH) : nullptr;
+            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info || (ent && !d_ent))
                 return fail(ctx, PBSGPU_ENOMEM, "match stage: device allocation failed");
             for (uint64_t f = 0; b.ok() && f < nz; f += LZ_PASS_BLOCKS) {
                 const uint32_t pn = (uint32_t)std::min<uint64_t>(LZ_PASS_BLOCKS, nz - f);
@@ -251,7 +250,7 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
                 if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
                 if (b.ok() && d_ent)
                     b.e = launch_ent_encode((const LzTables *)ctx->d_lz_tab, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
-                                            d_info, d_ent, b.st);
+                                            d_info, d_ent, mode == BlobMode::lzh, b.st);
             }
             info.resize(nz);
             if (b.ok()) b.e = cudaMemcpyAsync(info.data(), d_info, nz * 4, cudaMemcpyDeviceToHost, b.st);
@@ -364,10 +363,10 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
     return PBSGPU_OK;
 }
 
-// The stream's blob mode (capi_stream.cu): PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZE are the four encoders in order.
+// The stream's blob mode (capi_stream.cu): PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH are the five encoders in order.
 int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len) {
-    static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze};
+    static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze, BlobMode::lzh};
     return blob_encode(ctx, base, off, len, n, modes[mode - PBSGPU_BLOB_RAW], out, out_off, out_len, nullptr);
 }
 
@@ -393,6 +392,12 @@ extern "C" int pbsgpu_blob_encode_batch_lze(pbsgpu_ctx *ctx, const void *base, c
                                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
     return blob_encode(ctx, base, off, len, n, BlobMode::lze, out, out_off, out_len, crc_out);
+}
+
+extern "C" int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
+    return blob_encode(ctx, base, off, len, n, BlobMode::lzh, out, out_off, out_len, crc_out);
 }
 
 // ---------------------------------------------------------------------------

@@ -13,6 +13,9 @@
 //              there are >= 2 values, none above 128, and that section is smaller than the raw one; else raw.  Code
 //              lengths <= 11 (two-queue Huffman, counts halved until the longest fits), canonical codes.  One stream
 //              when the regenerated and compressed sizes both fit 10 bits, else four behind the jump table.
+//   full       (FULL, the _lzh encoder; tests/zstd_huf_ref.py): Huffman literals whatever their largest value, the
+//              tree in the smaller allowed form of the direct one and the FSE-compressed weights (ent_fse_tree), the
+//              direct one on ties; raw when neither is allowed.  Never larger than the content with FULL off.
 //
 // One CTA of 256 threads per block: shared-memory histograms (all threads); then warp 0 builds the Huffman code while
 // lane 0 of warps 1..3 builds the LL / OF / ML tables; then lane 0 of warp 7 runs the serial FSE chain into the
@@ -39,10 +42,16 @@ struct EntShared {
     uint32_t llbase[36], mlbase[53];
     uint8_t llbits[36], mlbits[53], llcode[64], mlcode[128];
     // Huffman
-    uint32_t hc[129], hw[257];
-    uint16_t hparent[257], hcode[256];
-    uint8_t horder[129], hdepth[257], hlen[256];
-    uint8_t tree[72];
+    uint32_t hc[256], hw[511];
+    uint16_t hparent[511], hcode[256];
+    uint8_t horder[256], hdepth[511], hlen[256];
+    uint8_t tree[ENT_FSE_TREE_MAX + 1];
+    // FSE table of the Huffman weights 0..ENT_HUF_MAXBITS (full-alphabet mode)
+    uint32_t whist[ENT_HUF_MAXBITS + 1];
+    int16_t wnorm[ENT_HUF_MAXBITS + 1];
+    int32_t wdnb[ENT_HUF_MAXBITS + 1], wdfs[ENT_HUF_MAXBITS + 1];
+    uint16_t wstab[1 << ENT_WEIGHT_MAXLOG];
+    uint8_t wspread[1 << ENT_WEIGHT_MAXLOG];
     uint32_t wsum[ENT_WRITERS / 32], sbits[4];
     uint8_t seqhdr[8];
     uint32_t kind, top, nh, maxlen, tree_len, t1, hs, bitlen, take, co, seqpos, seqhdr_len;
@@ -79,19 +88,29 @@ __device__ uint32_t writers_scan(uint32_t v, uint32_t *wsum, uint32_t *total) {
     return before + x - v;
 }
 
-// One column's table (t = 0 LL, 1 OF, 2 ML) over n >= 1 sequences: mode, description, accuracy log and encoder form.
-__device__ void ent_table(EntShared &s, int t, uint32_t n) {
-    const int nsym = t == 0 ? 36 : t == 1 ? 32 : 53;
-    const int cap = t == 0 ? ENT_LL_MAXLOG : t == 1 ? ENT_OF_MAXLOG : ENT_ML_MAXLOG;
-    const uint32_t *cnt = s.chist[t];
-    int16_t *norm = s.norm[t];
-    uint8_t *d = s.desc[t];
+// Where ent_table puts a table: the normalised counts, the description (at most dcap bytes of it are stored; desc_len
+// counts them all), the encoder form (stab, dnb, dfs; spread is scratch) and its mode and accuracy log.
+struct EntTableOut {
+    int16_t *norm;
+    uint8_t *desc;
+    uint32_t dcap;
+    uint16_t *stab;
+    int32_t *dnb, *dfs;
+    uint8_t *spread;
+    uint32_t *desc_len, *log, *mode;
+};
+
+// The table of nsym codes with counts cnt[] over n >= 1 values, accuracy log at most cap: mode, description, accuracy
+// log and encoder form.  Used for the LL / OF / ML columns and for the Huffman weights.
+__device__ void ent_table(const uint32_t *cnt, int nsym, int cap, uint32_t n, const EntTableOut o) {
+    int16_t *norm = o.norm;
+    uint8_t *d = o.desc;
     int distinct = 0, one = 0;
     for (int c = 0; c < nsym; c++) if (cnt[c]) { distinct++; one = c; }
     int log = 0;
     if (distinct == 1) {   // RLE_Mode: the code itself; as a table, one state of accuracy log 0
         for (int c = 0; c < nsym; c++) norm[c] = c == one;
-        s.mode[t] = 1; d[0] = (uint8_t)one; s.desc_len[t] = 1;
+        *o.mode = 1; d[0] = (uint8_t)one; *o.desc_len = 1;
     } else {
         // about 4 sequences per state, within [ENT_MIN_LOG, cap], and at least one state per code present
         log = min(cap, max(ENT_MIN_LOG, 32 - __clz(n) - 2));
@@ -121,7 +140,7 @@ __device__ void ent_table(EntShared &s, int t, uint32_t n) {
         auto put = [&](uint32_t v, uint32_t nb) {
             acc |= (uint64_t)v << na;
             na += nb;
-            while (na >= 8) { if (q < sizeof s.desc[0]) d[q] = (uint8_t)acc; q++; acc >>= 8; na -= 8; }
+            while (na >= 8) { if (q < o.dcap) d[q] = (uint8_t)acc; q++; acc >>= 8; na -= 8; }
         };
         int remaining = size + 1, threshold = size, nbits = log + 1, c = 0;
         bool prev0 = false;
@@ -141,31 +160,82 @@ __device__ void ent_table(EntShared &s, int t, uint32_t n) {
             prev0 = v == 1;
             while (remaining < threshold) { nbits--; threshold >>= 1; }
         }
-        if (na) { if (q < sizeof s.desc[0]) d[q] = (uint8_t)acc; q++; }
-        s.mode[t] = 2; s.desc_len[t] = q;
+        if (na) { if (q < o.dcap) d[q] = (uint8_t)acc; q++; }
+        *o.mode = 2; *o.desc_len = q;
     }
-    s.log[t] = log;
+    *o.log = log;
     // encoder form (zstd's FSE_buildCTable): spread the codes over the states (RFC 8878 4.1.1; no "less than 1"
     // cells), list each code's states in state order, and per code the transform from the next state to the bits to
     // write and the state to be in
     const int size = 1 << log, step = (size >> 1) + (size >> 3) + 3;
     for (int c = 0, pos = 0; c < nsym; c++)
-        for (int k = 0; k < norm[c]; k++) { s.spread[t][pos] = (uint8_t)c; pos = (pos + step) & (size - 1); }
-    int32_t *next = s.dnb[t];   // the next free place of each code in stab, before dnb takes its final value
+        for (int k = 0; k < norm[c]; k++) { o.spread[pos] = (uint8_t)c; pos = (pos + step) & (size - 1); }
+    int32_t *next = o.dnb;   // the next free place of each code in stab, before dnb takes its final value
     for (int c = 0, cum = 0; c < nsym; c++) { next[c] = cum; cum += norm[c]; }
-    for (int u = 0; u < size; u++) s.stab[t][next[s.spread[t][u]]++] = (uint16_t)u;
+    for (int u = 0; u < size; u++) o.stab[next[o.spread[u]]++] = (uint16_t)u;
     for (int c = 0; c < nsym; c++) {
         const int k = norm[c], start = next[c] - k;
-        if (k == 0) { s.dnb[t][c] = 0; s.dfs[t][c] = 0; continue; }
-        if (k == 1) { s.dnb[t][c] = (log << 16) - size; s.dfs[t][c] = start - 1; continue; }
+        if (k == 0) { o.dnb[c] = 0; o.dfs[c] = 0; continue; }
+        if (k == 1) { o.dnb[c] = (log << 16) - size; o.dfs[c] = start - 1; continue; }
         const int out = log - (31 - __clz(k - 1));
-        s.dnb[t][c] = (out << 16) - (k << out);
-        s.dfs[t][c] = start - k;
+        o.dnb[c] = (out << 16) - (k << out);
+        o.dfs[c] = start - k;
     }
 }
 
+// The FSE form of the tree description into s.tree (RFC 8878 4.2.1.2; lane 0 of warp 0): a header byte holding the
+// compressed size, the table description of the weights of symbols 0..top-1 (ent_table, accuracy log at most 6), then
+// their bitstream with two interleaved states.  The decoder reads state 1's start, then state 2's, and takes a weight
+// from state 1, state 2, state 1, ... until a state update reads past the stream's start; so state 1 codes the even
+// positions and state 2 the odd ones, and the encoder runs from the last weight to the first.  Each state starts in
+// the lowest state of its weight (zstd's FSE_initCState2), where that update reads at least one bit: the update after
+// the second-to-last weight must run past the start for the decoder to stop there, and the "no bits written" start of
+// the sequence chain (enc[code][0]) reads none when the weight holds more than half the states, as weight 0 often does.
+// Returns the form's size with its header byte, or 0 when it is not allowed: fewer than 2 weights, one distinct weight,
+// or more than ENT_FSE_TREE_MAX bytes after the header byte.
+__device__ uint32_t ent_fse_tree(EntShared &s, uint32_t top, uint32_t mx) {
+    auto wt = [&](uint32_t x) -> uint32_t { return s.hlen[x] ? mx + 1 - s.hlen[x] : 0; };
+    for (int w = 0; w <= ENT_HUF_MAXBITS; w++) s.whist[w] = 0;
+    for (uint32_t x = 0; x < top; x++) s.whist[wt(x)]++;
+    int distinct = 0;
+    for (int w = 0; w <= ENT_HUF_MAXBITS; w++) distinct += s.whist[w] != 0;
+    if (top < 2 || distinct < 2) return 0;
+    uint32_t mode, dlen, log;
+    ent_table(s.whist, ENT_HUF_MAXBITS + 1, ENT_WEIGHT_MAXLOG, top,
+              EntTableOut{s.wnorm, s.tree + 1, ENT_FSE_TREE_MAX, s.wstab, s.wdnb, s.wdfs, s.wspread, &dlen, &log, &mode});
+    if (dlen > ENT_FSE_TREE_MAX) return 0;
+    const uint32_t size = 1u << log;
+    uint32_t X[2];   // state 1, state 2, kept as 2^log + state
+    for (uint32_t t = 0; t < 2; t++) {
+        const uint32_t c = wt(top - 1 - ((top - 1 - t) & 1));   // the last position of parity t
+        uint32_t first = 0;                                      // stab lists each weight's states in state order
+        for (uint32_t w = 0; w < c; w++) first += s.wnorm[w];
+        X[t] = size + s.wstab[first];
+    }
+    uint8_t *out = s.tree + 1;
+    uint64_t acc = 0;
+    uint32_t na = 0, q = dlen;
+    auto put = [&](uint32_t v, uint32_t nb) {
+        acc |= (uint64_t)v << na;
+        na += nb;
+        while (na >= 8) { if (q < ENT_FSE_TREE_MAX) out[q] = (uint8_t)acc; q++; acc >>= 8; na -= 8; }
+    };
+    for (int k = (int)top - 3; k >= 0; k--) {
+        const uint32_t t = k & 1, c = wt(k);
+        const uint32_t nb = (uint32_t)((int)X[t] + s.wdnb[c]) >> 16;
+        put(X[t] & ((1u << nb) - 1), nb);
+        X[t] = size + s.wstab[(int)(X[t] >> nb) + s.wdfs[c]];
+    }
+    put(X[1] - size, log); put(X[0] - size, log); put(1, 1);
+    if (na) { if (q < ENT_FSE_TREE_MAX) out[q] = (uint8_t)acc; q++; }
+    if (q > ENT_FSE_TREE_MAX) return 0;
+    s.tree[0] = (uint8_t)q;
+    return 1 + q;
+}
+
 // Huffman code of the literals (warp 0): lengths, canonical codes, tree description and the one-stream bit count.
-__device__ void ent_huffman(EntShared &s, uint32_t lane) {
+// `full`: the full-alphabet mode, whose tree description may also take the FSE form.
+__device__ void ent_huffman(EntShared &s, uint32_t lane, bool full) {
     const uint32_t top = s.top, m = s.nh;
     for (uint32_t x = lane; x <= top; x += 32) s.hc[x] = s.lhist[x];
     __syncwarp();
@@ -210,12 +280,20 @@ __device__ void ent_huffman(EntShared &s, uint32_t lane) {
     for (uint32_t len = mx; len >= 1; len--)
         for (uint32_t x = 0; x <= top; x++)
             if (s.hlen[x] == len) { s.hcode[x] = (uint16_t)(nxt >> (mx - len)); nxt += 1u << (mx - len); }
-    // tree description, direct form: 127 + top, then the weights (maxbits + 1 - length, or 0) of symbols 0..top-1, two
-    // per byte, the first in the high nibble; the weight of `top` is implied
-    auto wt = [&](uint32_t x) -> uint32_t { return x < top && s.hlen[x] ? mx + 1 - s.hlen[x] : 0; };
-    s.tree[0] = (uint8_t)(127 + top);
-    for (uint32_t k = 0; k < top; k += 2) s.tree[1 + k / 2] = (uint8_t)(wt(k) << 4 | wt(k + 1));
-    s.tree_len = 1 + (top + 1) / 2;
+    // tree description: the smaller of the allowed forms, the direct one on ties; the literals stay raw when neither is.
+    // Direct form (top <= 128): 127 + top, then the weights (maxbits + 1 - length, or 0) of symbols 0..top-1, two per
+    // byte, the first in the high nibble; the weight of `top` is implied.  The FSE form only in full-alphabet mode.
+    const uint32_t dlen = 1 + (top + 1) / 2, flen = full ? ent_fse_tree(s, top, mx) : 0;
+    if (top <= ENT_HUF_MAXSYMBOL && (flen == 0 || dlen <= flen)) {
+        auto wt = [&](uint32_t x) -> uint32_t { return x < top && s.hlen[x] ? mx + 1 - s.hlen[x] : 0; };
+        s.tree[0] = (uint8_t)(127 + top);
+        for (uint32_t k = 0; k < top; k += 2) s.tree[1 + k / 2] = (uint8_t)(wt(k) << 4 | wt(k + 1));
+        s.tree_len = dlen;
+    } else if (flen) {
+        s.tree_len = flen;
+    } else {
+        s.kind = LIT_RAW;
+    }
     for (uint32_t x = 0; x <= top; x++) t1 += s.lhist[x] * s.hlen[x];
     s.t1 = t1;
 }
@@ -287,6 +365,7 @@ __device__ void ent_literals(EntShared &s, const uint8_t *lit, uint32_t nl, uint
     }
 }
 
+template <bool FULL>
 __global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab, const uint32_t *size, uint64_t first,
                                                             uint8_t *slots, const uint64_t *seqs, const uint32_t *nseq,
                                                             const uint32_t *nlit, uint32_t *info, uint8_t *scratch) {
@@ -319,12 +398,15 @@ __global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab,
         for (uint32_t x = lane; x < 256; x += 32) if (s.lhist[x]) { cnt++; top = x; }
         cnt = __reduce_add_sync(~0u, cnt);
         top = __reduce_max_sync(~0u, top);
-        const uint32_t kind = nl == 0 ? LIT_RAW : cnt == 1 ? LIT_RLE : top > ENT_HUF_MAXSYMBOL ? LIT_RAW : LIT_HUF;
+        const uint32_t kind = nl == 0 ? LIT_RAW : cnt == 1 ? LIT_RLE : !FULL && top > ENT_HUF_MAXSYMBOL ? LIT_RAW : LIT_HUF;
         if (lane == 0) { s.kind = kind; s.top = top; s.nh = cnt; }
         __syncwarp();
-        if (kind == LIT_HUF) ent_huffman(s, lane);
+        if (kind == LIT_HUF) ent_huffman(s, lane, FULL);
     } else if (warp <= 3 && lane == 0 && n) {
-        ent_table(s, warp - 1, n);
+        const int t = warp - 1;   // LL, OF, ML
+        ent_table(s.chist[t], t == 0 ? 36 : t == 1 ? 32 : 53, t == 0 ? ENT_LL_MAXLOG : t == 1 ? ENT_OF_MAXLOG : ENT_ML_MAXLOG,
+                  n, EntTableOut{s.norm[t], s.desc[t], sizeof s.desc[t], s.stab[t], s.dnb[t], s.dfs[t], s.spread[t],
+                                 &s.desc_len[t], &s.log[t], &s.mode[t]});
     }
     __syncthreads();
     if (warp == ENT_WRITERS / 32) {
@@ -396,9 +478,10 @@ __global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab,
 
 cudaError_t launch_ent_encode(const LzTables *tab, const uint32_t *size, uint64_t first, uint32_t nb, uint8_t *slots,
                               const uint64_t *seqs, const uint32_t *nseq, const uint32_t *nlit, uint32_t *info,
-                              uint8_t *scratch, cudaStream_t st) {
+                              uint8_t *scratch, bool full, cudaStream_t st) {
     if (nb == 0) return cudaSuccess;
-    k_ent_encode<<<nb, ENT_THREADS, 0, st>>>(tab, size, first, slots, seqs, nseq, nlit, info, scratch);
+    if (full) k_ent_encode<true><<<nb, ENT_THREADS, 0, st>>>(tab, size, first, slots, seqs, nseq, nlit, info, scratch);
+    else k_ent_encode<false><<<nb, ENT_THREADS, 0, st>>>(tab, size, first, slots, seqs, nseq, nlit, info, scratch);
     return cudaGetLastError();
 }
 

@@ -262,6 +262,12 @@ class Engine:
         -> list of n `bytes` blobs, crc[n]."""
         return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lze, base, off, length)
 
+    def blob_encode_batch_lzh(self, base, off, length):
+        """blob_encode_batch_lze with Huffman literals whatever their largest value (the tree in the direct or the
+        FSE-compressed weight form, the smaller one), so binary data gets entropy-coded literals too; every blob is at
+        most its _lze blob (pbsgpu_blob_encode_batch_lzh) -> list of n `bytes` blobs, crc[n]."""
+        return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lzh, base, off, length)
+
     def _blob_encode_sized(self, fn, base, off, length):
         o, l = self._offlen(off, length)
         sizes = l + np.uint64(12)
@@ -494,7 +500,7 @@ class Stream:
 
     def blob_mode(self, mode: str | None):
         """DataBlobs for the new chunks (pbsgpu_stream_blob_mode), set before the first byte: None (no blobs), "raw",
-        "z", "lz" or "lze" -- the encoders of Engine.blob_encode_batch, _z, _lz and _lze."""
+        "z", "lz", "lze" or "lzh" -- the encoders of Engine.blob_encode_batch, _z, _lz, _lze and _lzh."""
         if mode not in BLOB_MODES:
             raise ValueError(f"blob mode must be one of {list(BLOB_MODES)}, not {mode!r}")
         self._eng._ck(self._eng._L.pbsgpu_stream_blob_mode(self._h, BLOB_MODES[mode]))

@@ -60,7 +60,8 @@ class DedupWriter:
     upload_blob: Callable[[bytes, bytes], None] | None = None
     batch_bytes: int = 1 << 30
     # "z": frames of RLE and raw blocks; "lz": also compressed blocks from the LZ77 match stage (pbsgpu_blob_encode_batch_lz);
-    # "lze": those blocks also through zstd's entropy stage (pbsgpu_blob_encode_batch_lze)
+    # "lze": those blocks also through zstd's entropy stage (pbsgpu_blob_encode_batch_lze); "lzh": with Huffman literals
+    # whatever their largest value, for binary data (pbsgpu_blob_encode_batch_lzh)
     blob_compression: str = "z"
     index: list[IndexRecord] = field(default_factory=list)
     # relPath -> XXH3-64 of the file as uploaded: commitWalkState.backedHashes (commit.go:187, :725), computed on the
@@ -138,8 +139,8 @@ class DedupWriter:
 
 
 def _check_blob_compression(c: str) -> None:
-    if c not in ("z", "lz", "lze"):
-        raise ValueError(f"transfer: blob_compression must be 'z', 'lz' or 'lze', not {c!r}")
+    if c not in ("z", "lz", "lze", "lzh"):
+        raise ValueError(f"transfer: blob_compression must be 'z', 'lz', 'lze' or 'lzh', not {c!r}")
 
 
 # pxar v2 format constants (upstream pxar crate format/mod.rs; restated, UNVERIFIED against the Go module)
@@ -168,7 +169,7 @@ class PayloadStreamWriter:
     index: list[tuple[int, bytes, bool]] = field(default_factory=list)   # (end offset in the NEW stream, digest, known)
     payload_offsets: dict[str, int] = field(default_factory=dict)        # entry path -> offset of its PAYLOAD header
     # (digest, DataBlob) for NEW chunks, encoded on the GPU from the stream's windows (pbsgpu_stream_blob_mode) with the
-    # encoder `blob_compression` names ("z", "lz" or "lze", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
+    # encoder `blob_compression` names ("z", "lz", "lze" or "lzh", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
     upload_blob: Callable[[bytes, bytes], None] | None = None
     blob_compression: str = "z"
     # hash_files: relPath -> XXH3-64 of every file written through WriteEntryReader in backed_hashes

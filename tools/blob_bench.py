@@ -1,6 +1,7 @@
 """f3 microbench: DataBlob assembly for 4 MiB chunks of an 8 GiB device-resident image into PINNED host memory through
-the raw C calls (no Python-side allocation or slicing inside the timed region).  Two images: random bytes with half of
-them zero runs, and a text-like image (tests/zstd_lz_ref.py text_corpus, 32 MiB repeated).  For each: GB/s of input and
+the raw C calls (no Python-side allocation or slicing inside the timed region).  Three images: random bytes with half of
+them zero runs, a text-like image (tests/zstd_lz_ref.py text_corpus, 32 MiB repeated) and a binary-like one
+(tests/zstd_huf_ref.py binary_corpus, 32 MiB repeated).  For each: GB/s of input and
 output / input of every encoder, and for context libzstd level 1 (pyarrow) on a 64 MiB host sample of the same image (8 MiB from each GiB),
 its ratio and single-thread rate on the HOST CPU."""
 import subprocess
@@ -14,6 +15,7 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tests"))
 import pbs_plus_b200 as pg  # noqa: E402
+import zstd_huf_ref as hufref  # noqa: E402
 import zstd_lz_ref as lzref  # noqa: E402
 
 print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -37,13 +39,16 @@ def images():
     del d
     tile = torch.from_numpy(lzref.text_corpus(32 << 20, 1)).cuda()
     yield "text-like", tile.repeat(n // len(tile))
+    del tile
+    tile = torch.from_numpy(hufref.binary_corpus(32 << 20, 1)).cuda()
+    yield "binary-like", tile.repeat(n // len(tile))
 
 
 for label, d in images():
     torch.cuda.synchronize()
     print(f"-- {label} image, {n / 2**30:.0f} GiB")
     for name in ("crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz",
-                 "blob_encode_batch_lze"):
+                 "blob_encode_batch_lze", "blob_encode_batch_lzh"):
         for rep in range(3):
             torch.cuda.synchronize()
             t0 = time.perf_counter()

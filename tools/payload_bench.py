@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """PayloadStreamWriter throughput (one pxar payload stream through pbsgpu_stream_*, default 2 GiB windows) with the
-window products off and on: DataBlobs of the new chunks encoded at collect time (upload_blob, "z" and "lze") and the
+window products off and on: DataBlobs of the new chunks encoded at collect time (upload_blob, "z", "lze" and "lzh") and the
 per-file XXH3-64 (hash_files).  The input is 64 files of 128 MiB of the device corpus (seed 4) copied to pageable host
 memory, read through a reader object as a caller's io.Reader would be.  Prints one line per leg and the card it ran on.
 
@@ -77,5 +77,6 @@ def leg(name, **kw):
 leg("plain")
 leg("blobs z", blob_compression="z")
 leg("blobs lze", blob_compression="lze")
+leg("blobs lzh", blob_compression="lzh")
 leg("hashes", hash_files=True)
 leg("z + hashes", blob_compression="z", hash_files=True)
