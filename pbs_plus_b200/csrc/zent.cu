@@ -8,7 +8,7 @@
 //   sequences  LL, OF, ML columns: RLE_Mode when every sequence has the same code, else FSE_Compressed_Mode with
 //              log = min(cap, max(5, bit_length(n) - 2)), raised until 2^log >= the codes present (caps LL 9, OF 8,
 //              ML 9), and the distribution normalised as in ent_table.  Offsets stay offset + 3, so no Repeat_Mode;
-//              the bitstream is K9b's with these tables, the last sequence starting in state enc[code][0].
+//              the bitstream is seq_bitstream's, as K9b's, with these tables.
 //   literals   RLE_Literals_Block when all have one value; Huffman (Compressed_Literals_Block, direct 4-bit weights) when
 //              there are >= 2 values, none above 128, and that section is smaller than the raw one; else raw.  Code
 //              lengths <= 11 (two-queue Huffman, counts halved until the longest fits), canonical codes.  One stream
@@ -39,8 +39,7 @@ struct EntShared {
     uint8_t spread[3][512];            // the code of every state (one table per warp building it)
     uint8_t desc[3][96];
     uint32_t desc_len[3], log[3], mode[3];
-    uint32_t llbase[36], mlbase[53];
-    uint8_t llbits[36], mlbits[53], llcode[64], mlcode[128];
+    SeqCodes codes;
     // Huffman
     uint32_t hc[256], hw[511];
     uint16_t hparent[511], hcode[256];
@@ -55,17 +54,6 @@ struct EntShared {
     uint32_t wsum[ENT_WRITERS / 32], sbits[4];
     uint8_t seqhdr[8];
     uint32_t kind, top, nh, maxlen, tree_len, t1, hs, bitlen, take, co, seqpos, seqhdr_len;
-};
-
-// LL / ML / OF code, value and Offset_Value of a packed K9a sequence
-struct Seq {
-    uint32_t ll, ml, ov, lc, mc, oc;
-    __device__ Seq(uint64_t v, const EntShared &s) {
-        ll = (uint32_t)(v & 0xFFFFF); ml = (uint32_t)((v >> 20) & 0xFFFFF); ov = (uint32_t)(v >> 40) + 3;
-        lc = ll < 64 ? s.llcode[ll] : 31 - __clz(ll) + 19;
-        mc = ml - 3 < 128 ? s.mlcode[ml - 3] : 31 - __clz(ml - 3) + 36;
-        oc = 31 - __clz(ov);
-    }
 };
 
 __device__ __forceinline__ void writers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(ENT_WRITERS) : "memory"); }
@@ -164,23 +152,7 @@ __device__ void ent_table(const uint32_t *cnt, int nsym, int cap, uint32_t n, co
         *o.mode = 2; *o.desc_len = q;
     }
     *o.log = log;
-    // encoder form (zstd's FSE_buildCTable): spread the codes over the states (RFC 8878 4.1.1; no "less than 1"
-    // cells), list each code's states in state order, and per code the transform from the next state to the bits to
-    // write and the state to be in
-    const int size = 1 << log, step = (size >> 1) + (size >> 3) + 3;
-    for (int c = 0, pos = 0; c < nsym; c++)
-        for (int k = 0; k < norm[c]; k++) { o.spread[pos] = (uint8_t)c; pos = (pos + step) & (size - 1); }
-    int32_t *next = o.dnb;   // the next free place of each code in stab, before dnb takes its final value
-    for (int c = 0, cum = 0; c < nsym; c++) { next[c] = cum; cum += norm[c]; }
-    for (int u = 0; u < size; u++) o.stab[next[o.spread[u]]++] = (uint16_t)u;
-    for (int c = 0; c < nsym; c++) {
-        const int k = norm[c], start = next[c] - k;
-        if (k == 0) { o.dnb[c] = 0; o.dfs[c] = 0; continue; }
-        if (k == 1) { o.dnb[c] = (log << 16) - size; o.dfs[c] = start - 1; continue; }
-        const int out = log - (31 - __clz(k - 1));
-        o.dnb[c] = (out << 16) - (k << out);
-        o.dfs[c] = start - k;
-    }
+    fse_ctable(norm, nsym, log, o.spread, o.stab, o.dnb, o.dfs);   // no "less than 1" cells
 }
 
 // The FSE form of the tree description into s.tree (RFC 8878 4.2.1.2; lane 0 of warp 0): a header byte holding the
@@ -321,7 +293,7 @@ __device__ void ent_literals(EntShared &s, const uint8_t *lit, uint32_t nl, uint
     for (uint32_t k = 0; k < ns; k++) c += s.sbits[k] / 8 + 1;   // + the end mark
     const uint32_t big = max(nl, c);
     const uint32_t sf = ns == 1 ? 0 : big <= 1023 ? 1 : big <= 16383 ? 2 : 3, hl = sf < 2 ? 3 : sf + 2;
-    const uint32_t hs = hl + c, raw = (nl <= 31 ? 1 : nl <= 4095 ? 2 : 3) + nl;
+    const uint32_t hs = hl + c, raw = raw_lit_header_len(nl) + nl;
     if (hs >= raw) {
         if (tid == 0) s.kind = LIT_RAW;
         return;
@@ -380,16 +352,17 @@ __global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab,
 
     for (uint32_t k = tid; k < 256; k += ENT_THREADS) { s.lhist[k] = 0; s.hlen[k] = 0; }
     for (uint32_t k = tid; k < 3 * 64; k += ENT_THREADS) s.chist[k / 64][k % 64] = 0;
+    // field by field: with a copy in 4- or 16-byte words ptxas gives the kernel 48 registers (5 CTAs per SM, not 6)
     for (uint32_t k = tid; k < 128; k += ENT_THREADS) {
-        if (k < 36) { s.llbase[k] = __ldg(&tab->ll_base[k]); s.llbits[k] = __ldg(&tab->ll_bits[k]); }
-        if (k < 53) { s.mlbase[k] = __ldg(&tab->ml_base[k]); s.mlbits[k] = __ldg(&tab->ml_bits[k]); }
-        if (k < 64) s.llcode[k] = __ldg(&tab->ll_code[k]);
-        s.mlcode[k] = __ldg(&tab->ml_code[k]);
+        if (k < 36) { s.codes.ll_base[k] = __ldg(&tab->codes.ll_base[k]); s.codes.ll_bits[k] = __ldg(&tab->codes.ll_bits[k]); }
+        if (k < 53) { s.codes.ml_base[k] = __ldg(&tab->codes.ml_base[k]); s.codes.ml_bits[k] = __ldg(&tab->codes.ml_bits[k]); }
+        if (k < 64) s.codes.ll_code[k] = __ldg(&tab->codes.ll_code[k]);
+        s.codes.ml_code[k] = __ldg(&tab->codes.ml_code[k]);
     }
     __syncthreads();
     for (uint32_t i = tid; i < nl; i += ENT_THREADS) atomicAdd(&s.lhist[lit[i]], 1u);
     for (uint32_t k = tid; k < n; k += ENT_THREADS) {
-        const Seq q(sq[k], s);
+        const Seq q(sq[k], s.codes);
         atomicAdd(&s.chist[0][q.lc], 1u); atomicAdd(&s.chist[1][q.oc], 1u); atomicAdd(&s.chist[2][q.mc], 1u);
     }
     __syncthreads();
@@ -411,32 +384,10 @@ __global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab,
     __syncthreads();
     if (warp == ENT_WRITERS / 32) {
         if (lane == 0 && n) {
-            // the FSE chain, as K9b's with the block's tables; a state is kept as 2^log + state (zstd's CState)
             LzBits w{B, 0};
-            uint32_t X[3] = {0, 0, 0}, sz[3];
-#pragma unroll
-            for (int t = 0; t < 3; t++) sz[t] = 1u << s.log[t];
-            auto step = [&](int t, uint32_t c) {
-                const uint32_t nb = (uint32_t)((int)X[t] + s.dnb[t][c]) >> 16;
-                w.add(X[t] & ((1u << nb) - 1), nb);
-                X[t] = sz[t] + s.stab[t][(int)(X[t] >> nb) + s.dfs[t][c]];
-            };
-            for (uint32_t k = n; k-- > 0;) {
-                const Seq q(sq[k], s);
-                if (k + 1 == n) {   // enc[code][0]: the state from which the decoder goes to state 0
-                    X[0] = sz[0]; X[1] = sz[1]; X[2] = sz[2];
-                    const LzBits keep = w;
-                    step(0, q.lc); step(1, q.oc); step(2, q.mc);
-                    w = keep;
-                } else {
-                    step(1, q.oc); step(2, q.mc); step(0, q.lc);
-                }
-                w.add(q.ll - s.llbase[q.lc], s.llbits[q.lc]);
-                w.add(q.ml - s.mlbase[q.mc], s.mlbits[q.mc]);
-                w.add(q.ov - (1u << q.oc), q.oc);
-            }
-            w.add(X[2] - sz[2], s.log[2]); w.add(X[1] - sz[1], s.log[1]); w.add(X[0] - sz[0], s.log[0]); w.add(1, 1);
-            if (w.n) w.byte((uint32_t)w.acc);
+            const FseCTable t[3] = {{s.stab[0], s.dnb[0], s.dfs[0], s.log[0]}, {s.stab[1], s.dnb[1], s.dfs[1], s.log[1]},
+                                    {s.stab[2], s.dnb[2], s.dfs[2], s.log[2]}};
+            seq_bitstream(sq, n, s.codes, t, w);
             s.bitlen = w.q;
         }
     } else if (s.kind == LIT_HUF) {
@@ -444,14 +395,10 @@ __global__ void __launch_bounds__(ENT_THREADS) k_ent_encode(const LzTables *tab,
     }
     __syncthreads();
     if (tid == 0) {
-        const uint32_t hl = nl <= 31 ? 1 : nl <= 4095 ? 2 : 3, kind = s.kind;
+        const uint32_t hl = raw_lit_header_len(nl), kind = s.kind;
         const uint32_t litlen = kind == LIT_HUF ? s.hs : kind == LIT_RLE ? hl + 1 : hl + nl;
-        uint32_t q = 0, seqlen = 1;
-        if (n == 0) s.seqhdr[q++] = 0;
-        else {
-            if (n < 128) s.seqhdr[q++] = (uint8_t)n;
-            else if (n < 0x7F00) { s.seqhdr[q++] = (uint8_t)((n >> 8) + 0x80); s.seqhdr[q++] = (uint8_t)n; }
-            else { s.seqhdr[q++] = 0xFF; s.seqhdr[q++] = (uint8_t)(n - 0x7F00); s.seqhdr[q++] = (uint8_t)((n - 0x7F00) >> 8); }
+        uint32_t q = seq_count_header(n, s.seqhdr), seqlen = 1;
+        if (n) {
             s.seqhdr[q++] = (uint8_t)(s.mode[0] << 6 | s.mode[1] << 4 | s.mode[2] << 2);   // LL, OF, ML
             seqlen = q + s.desc_len[0] + s.desc_len[1] + s.desc_len[2] + s.bitlen;
         }

@@ -18,8 +18,8 @@
 //                     match is extended 32 bytes per step.  Shared memory is the 32 KiB hash table + 1 KiB of cand, so
 //                     six blocks are parsed at once per SM.  Sequences go to a per-pass scratch as packed u64.
 //   K9b k_lz_encode : one THREAD per block (the backward FSE bitstream is serial by construction): literals header in
-//                     front of the literals, the sequences header, the modes byte and the bitstream, behind them in the
-//                     slot.  The tables sit in shared memory; the 32 blocks of a warp run in step.
+//                     front of the literals, the sequences header, the modes byte and the bitstream (seq_bitstream),
+//                     behind them in the slot.  The tables sit in shared memory; the 32 blocks of a warp run in step.
 #include "internal.cuh"
 
 #include <cstring>
@@ -113,40 +113,18 @@ __global__ void __launch_bounds__(128) k_lz_encode(const LzTables *tab, uint64_t
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
     const uint64_t g = first + b;
-    const uint32_t n = nseq[g], nl = nlit[g];
-    const uint32_t hl = nl <= 31 ? 1 : nl <= 4095 ? 2 : 3;   // Raw_Literals_Block header, Size_Format 00 / 01 / 11
+    const uint32_t n = nseq[g], nl = nlit[g], hl = raw_lit_header_len(nl);
     LzBits w{slots + g * LZ_SLOT, 3 - hl};
     if (hl == 1) w.byte(nl << 3);
     else if (hl == 2) { w.byte((nl << 4) | 0x4); w.byte(nl >> 4); }
     else { w.byte((nl << 4) | 0xC); w.byte(nl >> 4); w.byte(nl >> 12); }
     w.q = 3 + nl;
-    if (n == 0) w.byte(0);
-    else {
-        if (n < 128) w.byte(n);
-        else if (n < 0x7F00) { w.byte((n >> 8) + 0x80); w.byte(n & 0xFF); }
-        else { w.byte(0xFF); w.byte((n - 0x7F00) & 0xFF); w.byte((n - 0x7F00) >> 8); }
+    w.q += seq_count_header(n, w.slot + w.q);   // within the slot: 3 + nl + 3 <= LZ_SLOT
+    if (n) {
         w.byte(0);   // Symbol_Compression_Modes: all Predefined_Mode
-        const uint64_t *sq = seqs + (uint64_t)b * LZ_MAX_SEQ;
-        uint32_t sLL = 0, sML = 0, sOF = 0;
-        for (uint32_t k = n; k-- > 0;) {   // last sequence first
-            const uint64_t s = sq[k];
-            const uint32_t ll = (uint32_t)(s & 0xFFFFF), ml = (uint32_t)((s >> 20) & 0xFFFFF), ov = (uint32_t)(s >> 40) + 3;
-            const uint32_t lc = ll < 64 ? T.ll_code[ll] : 31 - __clz(ll) + 19;
-            const uint32_t mc = ml - 3 < 128 ? T.ml_code[ml - 3] : 31 - __clz(ml - 3) + 36;
-            const uint32_t oc = 31 - __clz(ov);
-            if (k + 1 == n) {
-                sLL = T.ll_enc[lc][0] & 63; sML = T.ml_enc[mc][0] & 63; sOF = T.of_enc[oc][0] & 63;
-            } else {   // the states from which the decoder reads this sequence's codes and then goes to the next one's
-                uint32_t e = T.of_enc[oc][sOF]; w.add(e >> 9, (e >> 6) & 7); sOF = e & 63;
-                e = T.ml_enc[mc][sML]; w.add(e >> 9, (e >> 6) & 7); sML = e & 63;
-                e = T.ll_enc[lc][sLL]; w.add(e >> 9, (e >> 6) & 7); sLL = e & 63;
-            }
-            w.add(ll - T.ll_base[lc], T.ll_bits[lc]);
-            w.add(ml - T.ml_base[mc], T.ml_bits[mc]);
-            w.add(ov - (1u << oc), oc);
-        }
-        w.add(sML, 6); w.add(sOF, 5); w.add(sLL, 6); w.add(1, 1);
-        if (w.n) w.byte((uint32_t)w.acc);
+        const FseCTable t[3] = {{T.ll_stab, T.ll_dnb, T.ll_dfs, 6}, {T.of_stab, T.of_dnb, T.of_dfs, 5},
+                                {T.ml_stab, T.ml_dnb, T.ml_dfs, 6}};
+        seq_bitstream(seqs + (uint64_t)b * LZ_MAX_SEQ, n, T.codes, t, w);
     }
     info[g] = (w.q - (3 - hl)) | (3 - hl) << 30;
 }
@@ -159,11 +137,12 @@ cudaError_t launch_lz_encode(const LzTables *tab, uint64_t first, uint32_t nb, u
 }
 
 // ---- host: the predefined tables (RFC 8878 3.1.1.3.2.2 distributions, 4.1.1 table construction) ----------------------
-static const int LL_NORM[36] = {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1, 1, 1,
-                                -1, -1, -1, -1};
-static const int ML_NORM[53] = {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1,
-                                1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1};
-static const int OF_NORM[29] = {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1};
+static const int16_t LL_NORM[36] = {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1,
+                                    1, 1, -1, -1, -1, -1};
+static const int16_t ML_NORM[53] = {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1,
+                                    1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1};
+static const int16_t OF_NORM[29] = {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1,
+                                    -1};
 static const uint32_t LL_BASE[36] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 20, 22, 24, 28, 32, 40,
                                      48, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536};
 static const uint8_t LL_BITS[36] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 3, 3, 4, 6, 7, 8, 9,
@@ -172,42 +151,21 @@ static const uint32_t ML_BASE_HI[21] = {35, 37, 39, 41, 43, 47, 51, 59, 67, 83, 
                                         16387, 32771, 65539};
 static const uint8_t ML_BITS_HI[21] = {1, 1, 1, 1, 2, 2, 3, 3, 4, 4, 5, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16};
 
-// enc[s * size + x] for a distribution norm[n] of accuracy log `log`
-static void fse_enc(const int *norm, int n, int log, uint16_t *enc) {
-    const int size = 1 << log;
-    int sym[64], high = size - 1;
-    for (int s = 0; s < n; s++) if (norm[s] == -1) sym[high--] = s;
-    const int step = (size >> 1) + (size >> 3) + 3;
-    for (int s = 0, pos = 0; s < n; s++)
-        for (int k = 0; k < norm[s]; k++) {
-            sym[pos] = s;
-            do pos = (pos + step) & (size - 1); while (pos > high);
-        }
-    int next[64];
-    for (int s = 0; s < n; s++) next[s] = norm[s] == -1 ? 1 : norm[s];
-    for (int u = 0; u < size; u++) {
-        const int x = next[sym[u]]++;
-        int hb = 0;
-        while ((x >> (hb + 1)) != 0) hb++;
-        const int nb = log - hb, baseline = (x << nb) - size;
-        for (int y = baseline; y < baseline + (1 << nb); y++)
-            enc[sym[u] * size + y] = (uint16_t)(u | nb << 6 | (y - baseline) << 9);
-    }
-}
-
 void lz_fill_tables_host(void *dst) {
     LzTables t;
     memset(&t, 0, sizeof t);
-    fse_enc(LL_NORM, 36, 6, &t.ll_enc[0][0]);
-    fse_enc(ML_NORM, 53, 6, &t.ml_enc[0][0]);
-    fse_enc(OF_NORM, 29, 5, &t.of_enc[0][0]);
-    for (int c = 0; c < 36; c++) { t.ll_base[c] = LL_BASE[c]; t.ll_bits[c] = LL_BITS[c]; }
+    uint8_t spread[64];
+    fse_ctable(LL_NORM, 36, 6, spread, t.ll_stab, t.ll_dnb, t.ll_dfs);
+    fse_ctable(OF_NORM, 29, 5, spread, t.of_stab, t.of_dnb, t.of_dfs);
+    fse_ctable(ML_NORM, 53, 6, spread, t.ml_stab, t.ml_dnb, t.ml_dfs);
+    SeqCodes &s = t.codes;
+    for (int c = 0; c < 36; c++) { s.ll_base[c] = LL_BASE[c]; s.ll_bits[c] = LL_BITS[c]; }
     for (int c = 0; c < 53; c++) {
-        t.ml_base[c] = c < 32 ? c + 3 : ML_BASE_HI[c - 32];
-        t.ml_bits[c] = c < 32 ? 0 : ML_BITS_HI[c - 32];
+        s.ml_base[c] = c < 32 ? c + 3 : ML_BASE_HI[c - 32];
+        s.ml_bits[c] = c < 32 ? 0 : ML_BITS_HI[c - 32];
     }
-    for (uint32_t v = 0, c = 0; v < 64; v++) { while (c + 1 < 36 && LL_BASE[c + 1] <= v) c++; t.ll_code[v] = (uint8_t)c; }
-    for (uint32_t v = 0, c = 0; v < 128; v++) { while (c + 1 < 53 && t.ml_base[c + 1] <= v + 3) c++; t.ml_code[v] = (uint8_t)c; }
+    for (uint32_t v = 0, c = 0; v < 64; v++) { while (c + 1 < 36 && LL_BASE[c + 1] <= v) c++; s.ll_code[v] = (uint8_t)c; }
+    for (uint32_t v = 0, c = 0; v < 128; v++) { while (c + 1 < 53 && s.ml_base[c + 1] <= v + 3) c++; s.ml_code[v] = (uint8_t)c; }
     memcpy(dst, &t, sizeof t);
 }
 
