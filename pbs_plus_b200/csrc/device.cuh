@@ -1,5 +1,5 @@
 // pbs_plus_b200/csrc/device.cuh -- device-only primitives shared by the kernels: shared-memory mbarriers, TMA copies,
-// the warp's TMA staging rule and the "which range owns work unit g" search.
+// the warp's TMA staging rule, the "which range owns work unit g" search and the device-count clamp.
 // Included by the kernel .cu files only (not by internal.cuh / host.hpp), so the C ABI units see no inline asm.
 #pragma once
 #include <cuda.h>   // CUtensorMap
@@ -17,6 +17,10 @@ __device__ __forceinline__ uint32_t owner_of(const uint64_t *first, uint32_t n, 
     }
     return lo;
 }
+
+// A count the device wrote (`n`, read from device memory), bounded by `cap`: the capacity a launch was sized for, or
+// an enclosing count.
+__device__ __forceinline__ unsigned long long live_count(unsigned long long n, unsigned long long cap) { return n < cap ? n : cap; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

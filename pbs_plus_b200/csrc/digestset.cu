@@ -20,6 +20,7 @@
 
 #include <algorithm>
 
+#include "device.cuh"
 #include "internal.cuh"
 
 namespace pbsgpu {
@@ -37,15 +38,11 @@ __device__ __forceinline__ bool eq32(const uint64_t *a, const uint64_t *b) {
 // device) and `cap` otherwise; `cap` bounds every launch.  Entries at index >= n get the all-ones tag and sort behind the
 // real ones (a real digest whose first 8 bytes are all ones still works: the sort is stable, so it stays in front of the
 // padding and padding threads return at once).
-__device__ __forceinline__ uint64_t count_of(const unsigned long long *n_dev, uint64_t cap) {
-    const uint64_t n = n_dev ? *n_dev : cap;
-    return n < cap ? n : cap;
-}
 
 __global__ void k_set_make_keys(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= cap) return;
-    tag[i] = i < count_of(n_dev, cap) ? tag_of((const uint64_t *)(d32 + i * 32)) : ~0ull;
+    tag[i] = i < live_count(n_dev ? *n_dev : cap, cap) ? tag_of((const uint64_t *)(d32 + i * 32)) : ~0ull;
     idx[i] = (uint32_t)i;
 }
 cudaError_t launch_set_make_keys(const uint8_t *d32, const unsigned long long *n_dev, uint64_t cap, uint64_t *tag, uint32_t *idx,
@@ -63,7 +60,7 @@ __global__ void k_set_process(SetTable t, const uint8_t *d32, const uint64_t *ta
                               const unsigned long long *n_dev, uint64_t cap, const unsigned long long *guard, uint64_t guard_max,
                               int do_insert, uint8_t *hit, uint8_t *is_rep_miss, unsigned long long *n_new) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= count_of(n_dev, cap)) return;   // the n real entries are the first n after the stable sort
+    if (j >= live_count(n_dev ? *n_dev : cap, cap)) return;   // the n real entries are the first n after the stable sort
     if (guard && *guard > guard_max) { if (PHASE == 0 && hit) hit[idx_sorted[j]] = 0; return; }
     const uint32_t i = idx_sorted[j];
     const uint64_t *d = (const uint64_t *)(d32 + (uint64_t)i * 32);

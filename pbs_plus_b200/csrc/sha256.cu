@@ -104,16 +104,71 @@ __device__ __forceinline__ void load_block_be(const uint8_t *p, uint32_t (&w)[16
     for (int i = 0; i < 16; i++) w[i] = __byte_perm(x[i], x[i + 1], sel);
 }
 
+// ---------------------------------------------------------------------------
+// The full blocks of one hash as 16-byte aligned LDG.128 loads (5 per 64 B block instead of 17 LDG.32: the L1/tex path
+// is charged per distinct line per instruction, so wide loads matter even though the kernels are ALU bound), the next
+// block prefetched while the current one is compressed; the per-lane word misalignment is undone by a 2-stage SEL
+// network and the byte misalignment + endian swap by ONE PRMT per word.  A hash of `len` bytes at p reads the vec_count
+// aligned vectors from first_vec(p) and no others (the blocks here, the tail in sha_finish); the arena copies just these.
+// ---------------------------------------------------------------------------
+struct BlockStream {
+    static __device__ __forceinline__ const uint4 *first_vec(const uint8_t *p) { return (const uint4 *)(p - ((uintptr_t)p & 15)); }
+    // bytes from first_vec(p) to the end of the input; vec_count rounds it up to whole vectors
+    static __device__ __forceinline__ uint64_t vec_span(const uint8_t *p, uint32_t len) { return ((uintptr_t)p & 15) + (uint64_t)len; }
+    static __device__ __forceinline__ uint64_t vec_count(const uint8_t *p, uint32_t len) { return (vec_span(p, len) + 15) >> 4; }
+
+    uint4 v4, v3, v2, v1, v0;   // declared first and in this order, they keep k_sha_tuned's SASS that of an inline loader
+    const uint4 *q;
+    uint32_t nblk, sel;
+    bool need5, d1, d2;
+
+    // `nblk` full blocks at p; issues the loads of block 0
+    __device__ __forceinline__ BlockStream(const uint8_t *p, uint32_t nblk_) : nblk(nblk_) {
+        const uint32_t delta = (uint32_t)((uintptr_t)p & 15), dw = delta >> 2, sh = delta & 3;
+        q = (const uint4 *)(p - delta);
+        sel = (sh + 3) | ((sh + 2) << 4) | ((sh + 1) << 8) | (sh << 12);
+        need5 = delta != 0;     // never touch the vector past the block when the chunk is 16 B aligned
+        d1 = dw & 1; d2 = dw & 2;
+        v4 = make_uint4(0, 0, 0, 0);
+        if (nblk) {
+            v0 = __ldg(q); v1 = __ldg(q + 1); v2 = __ldg(q + 2); v3 = __ldg(q + 3);
+            if (need5) v4 = __ldg(q + 4);
+        }
+    }
+    // block b's 16 big-endian words; issues the loads of block b + 1
+    __device__ __forceinline__ void next(uint32_t b, uint32_t (&w)[16]) {
+        uint32_t x[20] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w, v2.x, v2.y, v2.z, v2.w,
+                          v3.x, v3.y, v3.z, v3.w, v4.x, v4.y, v4.z, v4.w};
+        if (b + 1 < nblk) {                     // v4 of this block == v0 of the next
+            const uint4 *qn = q + (uint64_t)(b + 1) * 4;
+            v0 = need5 ? v4 : __ldg(qn);
+            v1 = __ldg(qn + 1); v2 = __ldg(qn + 2); v3 = __ldg(qn + 3);
+            if (need5) v4 = __ldg(qn + 4);
+        }
+        uint32_t y[18];
+#pragma unroll
+        for (int i = 0; i < 18; i++) y[i] = d2 ? x[i + 2] : x[i];
+#pragma unroll
+        for (int i = 0; i < 17; i++) y[i] = d1 ? y[i + 1] : y[i];
+#pragma unroll
+        for (int i = 0; i < 16; i++) w[i] = __byte_perm(y[i], y[i + 1], sel);
+    }
+};
+
+// The chunk at position t of `order`: its id (which indexes its digest) and ChunkRef; returns its first byte in the source.
+__device__ __forceinline__ const uint8_t *sha_chunk(const ShaArgs &a, uint64_t t, uint32_t &id, ChunkRef &c) {
+    id = a.order ? a.order[t] : (uint32_t)t;
+    c = a.chunks[id];
+    return a.base + (a.off ? a.off[c.stream] : 0) + c.start;
+}
+
 // position in `order` handled by logical thread t of a launch, honouring the hybrid split
 __device__ __forceinline__ bool sha_slot(const ShaArgs &a, uint64_t t, uint64_t &pos) {
-    unsigned long long n = *a.n_chunks;
-    if (n > a.chunk_cap) n = a.chunk_cap;
-    unsigned long long head = a.part ? *a.n_head : 0ull;
-    if (head > n) head = n;
+    const unsigned long long n = live_count(*a.n_chunks, a.chunk_cap);
+    const unsigned long long head = live_count(a.part ? *a.n_head : 0ull, n);
     if (a.part == 1) { pos = t; return t < head; }
     if (a.part >= 3) {
-        unsigned long long mid = *a.n_mid;
-        if (mid > n) mid = n;
+        unsigned long long mid = live_count(*a.n_mid, n);
         if (mid < head) mid = head;
         if (a.part == 3) { pos = t + head; return pos < mid; }
         pos = t + mid;
@@ -129,9 +184,8 @@ __device__ __forceinline__ bool sha_slot(const ShaArgs &a, uint64_t t, uint64_t 
 __global__ void __launch_bounds__(64) k_sha_simple(ShaArgs a) {
     uint64_t t;
     if (!sha_slot(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, t)) return;
-    uint32_t id = a.order ? a.order[t] : (uint32_t)t;
-    ChunkRef c = a.chunks[id];
-    const uint8_t *p = a.base + (a.off ? a.off[c.stream] : 0) + c.start;
+    uint32_t id; ChunkRef c;
+    const uint8_t *p = sha_chunk(a, t, id, c);
     Sha256State s;
     sha_init(s);
     uint32_t nblk = c.len >> 6;
@@ -151,19 +205,11 @@ cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------
-// Tuned kernel.  Same one-lane-per-chunk mapping, but:
-//   * 16-byte aligned LDG.128 loads (5 per 64 B block instead of 17 LDG.32: the L1/tex
-//     path is charged per distinct line per instruction, so wide loads matter even
-//     though the kernel is ALU bound), next block prefetched while the current one is
-//     compressed; the per-lane word misalignment is undone by a 2-stage SEL network and
-//     the byte misalignment + endian swap by ONE PRMT per word;
-//   * pipe balancing: the SM's integer work splits over the ALU pipe (LOP3/SHF/PRMT/IADD3)
-//     and the FMA pipe (IMAD), 64 lanes/clk/SM each.  ptxas puts almost all of SHA-256 on
-//     the ALU pipe.  Multiplying by constants the compiler cannot see (kernel arguments
-//     1, 2^29, 2^22, 2^7) forces the additions (a*1+b), the two logical shifts of the
-//     message schedule (mul.hi by 2^(32-n)) and one rotation per round (mul.lo + mad.hi)
-//     onto IMAD / IMAD.HI, taking the ALU pipe from ~1280 to ~880 instructions per block
-//     with ~870 on the FMA pipe.  MODE bit0: adds, bit1: shifts, bit2: rotr25.
+// Pipe balancing: the SM's integer work splits over the ALU pipe (LOP3/SHF/PRMT/IADD3) and the FMA pipe (IMAD), 64
+// lanes/clk/SM each.  ptxas puts almost all of SHA-256 on the ALU pipe.  Multiplying by constants the compiler cannot
+// see (kernel arguments 1, 2^29, 2^22, 2^7) forces the additions (a*1+b), the two logical shifts of the message
+// schedule (mul.hi by 2^(32-n)) and one rotation per round (mul.lo + mad.hi) onto IMAD / IMAD.HI, taking the ALU pipe
+// from ~1280 to ~880 instructions per block with ~870 on the FMA pipe.  MODE bit0: adds, bit1: shifts, bit2: rotr25.
 // ---------------------------------------------------------------------------
 struct Opq { uint32_t one, p29, p22, p7; };
 
@@ -191,6 +237,20 @@ template <int MODE> struct Ops {
     }
 };
 
+// Message schedule step of round i on the 16-word ring w (FIPS 180-4 6.2.2 step 1): expands W[i] in place when
+// i >= 16 and returns W[i] + K[i].
+template <class P>
+__device__ __forceinline__ uint32_t sched(uint32_t (&w)[16], int i, const Opq &o) {
+    constexpr uint32_t K[64] = {K256_LIST};
+    if (i >= 16) {
+        uint32_t w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
+        uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ P::shr3(w15, o);
+        uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ P::shr10(w2, o);
+        w[i & 15] = P::add(P::add(w[i & 15], s0, o), P::add(w[(i + 9) & 15], s1, o), o);
+    }
+    return P::add(w[i & 15], K[i], o);
+}
+
 template <int MODE>
 __device__ __forceinline__ void sha_compress_t(Sha256State &s, uint32_t (&w)[16], const Opq &o) {
     constexpr uint32_t K[64] = {K256_LIST};
@@ -198,6 +258,7 @@ __device__ __forceinline__ void sha_compress_t(Sha256State &s, uint32_t (&w)[16]
     uint32_t a = s.h[0], b = s.h[1], c = s.h[2], d = s.h[3], e = s.h[4], f = s.h[5], g = s.h[6], h = s.h[7];
 #pragma unroll
     for (int i = 0; i < 64; i++) {
+        // the schedule stays inline: sched() puts W+K ahead of S1/ch, and ptxas then picks another pipe mix for this loop
         if (i >= 16) {
             uint32_t w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
             uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ P::shr3(w15, o);
@@ -216,44 +277,20 @@ __device__ __forceinline__ void sha_compress_t(Sha256State &s, uint32_t (&w)[16]
     s.h[0] += a; s.h[1] += b; s.h[2] += c; s.h[3] += d; s.h[4] += e; s.h[5] += f; s.h[6] += g; s.h[7] += h;
 }
 
-__device__ __forceinline__ uint4 ldg128(const uint4 *p) { return __ldg(p); }
-
+// Tuned kernel.  Same one-lane-per-chunk mapping, but BlockStream's loads and the pipe-balanced compression above.
 template <int MODE>
 __global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o) {
     uint64_t t;
     if (!sha_slot(a, (uint64_t)blockIdx.x * 32 + threadIdx.x, t)) return;
-    const uint32_t id = a.order ? a.order[t] : (uint32_t)t;
-    const ChunkRef c = a.chunks[id];
-    const uint8_t *p = a.base + (a.off ? a.off[c.stream] : 0) + c.start;
+    uint32_t id; ChunkRef c;
+    const uint8_t *p = sha_chunk(a, t, id, c);
     Sha256State s;
     sha_init(s);
     const uint32_t nblk = c.len >> 6;
-    const uint32_t delta = (uint32_t)((uintptr_t)p & 15), dw = delta >> 2, sh = delta & 3;
-    const uint4 *q = (const uint4 *)(p - delta);
-    const uint32_t sel = (sh + 3) | ((sh + 2) << 4) | ((sh + 1) << 8) | (sh << 12);
-    const bool need5 = delta != 0;     // never touch the vector past the block when the chunk is 16 B aligned
-    const bool d1 = dw & 1, d2 = dw & 2;
-    uint4 v0, v1, v2, v3, v4 = make_uint4(0, 0, 0, 0);
-    if (nblk) {
-        v0 = ldg128(q); v1 = ldg128(q + 1); v2 = ldg128(q + 2); v3 = ldg128(q + 3);
-        if (need5) v4 = ldg128(q + 4);
-    }
+    BlockStream in(p, nblk);
     for (uint32_t b = 0; b < nblk; b++) {
-        uint32_t x[20] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w, v2.x, v2.y, v2.z, v2.w,
-                          v3.x, v3.y, v3.z, v3.w, v4.x, v4.y, v4.z, v4.w};
-        if (b + 1 < nblk) {                     // prefetch the next block (v4 of this block == v0 of the next)
-            const uint4 *qn = q + (uint64_t)(b + 1) * 4;
-            v0 = need5 ? v4 : ldg128(qn);
-            v1 = ldg128(qn + 1); v2 = ldg128(qn + 2); v3 = ldg128(qn + 3);
-            if (need5) v4 = ldg128(qn + 4);
-        }
-        uint32_t y[18], w[16];
-#pragma unroll
-        for (int i = 0; i < 18; i++) y[i] = d2 ? x[i + 2] : x[i];
-#pragma unroll
-        for (int i = 0; i < 17; i++) y[i] = d1 ? y[i + 1] : y[i];
-#pragma unroll
-        for (int i = 0; i < 16; i++) w[i] = __byte_perm(y[i], y[i + 1], sel);
+        uint32_t w[16];
+        in.next(b, w);
         sha_compress_t<MODE>(s, w, o);
     }
     sha_finish(s, p + (uint64_t)nblk * 64, c.len & 63, c.len, a.digests + (uint64_t)id * 32);
@@ -325,8 +362,8 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o) {
     const bool active = sha_slot(a, (uint64_t)blockIdx.x * 32 + lane, t);
     uint32_t id = 0;
     ChunkRef c; c.stream = 0; c.len = 0; c.start = 0;
-    if (active) { id = a.order ? a.order[t] : (uint32_t)t; c = a.chunks[id]; }
-    const uint8_t *p = a.base + ((a.off && active) ? a.off[c.stream] : 0) + c.start;
+    const uint8_t *p = a.base;
+    if (active) p = sha_chunk(a, t, id, c);
     if (a.arena && active) p = a.arena + a.arena_off[t] + ((uintptr_t)p & 15);   // the gathered copy (same alignment mod 16)
     const uint32_t nblk = c.len >> 6;
     const uint32_t nblk_max = __reduce_max_sync(0xffffffffu, nblk);
@@ -342,46 +379,16 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o) {
 
     if (warp == 0) {
         // ------------------------------ producer ------------------------------
-        constexpr uint32_t K[64] = {K256_LIST};
-        typedef Ops<PMODE> P;
-        const uint32_t delta = (uint32_t)((uintptr_t)p & 15), dw = delta >> 2, sh = delta & 3;
-        const uint4 *q = (const uint4 *)(p - delta);
-        const uint32_t sel = (sh + 3) | ((sh + 2) << 4) | ((sh + 1) << 8) | (sh << 12);
-        const bool need5 = delta != 0, d1 = dw & 1, d2 = dw & 2;
-        uint4 v0 = make_uint4(0, 0, 0, 0), v1 = v0, v2 = v0, v3 = v0, v4 = v0;
-        if (nblk) {
-            v0 = ldg128(q); v1 = ldg128(q + 1); v2 = ldg128(q + 2); v3 = ldg128(q + 3);
-            if (need5) v4 = ldg128(q + 4);
-        }
+        BlockStream in(p, nblk);
         uint32_t stage = 0, phase = 0;
         for (uint32_t b = 0; b < nblk_max; b++) {
             mbar_wait(empty[stage], phase ^ 1);
             if (b < nblk) {
-                uint32_t x[20] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w, v2.x, v2.y, v2.z, v2.w,
-                                  v3.x, v3.y, v3.z, v3.w, v4.x, v4.y, v4.z, v4.w};
-                if (b + 1 < nblk) {
-                    const uint4 *qn = q + (uint64_t)(b + 1) * 4;
-                    v0 = need5 ? v4 : ldg128(qn);
-                    v1 = ldg128(qn + 1); v2 = ldg128(qn + 2); v3 = ldg128(qn + 3);
-                    if (need5) v4 = ldg128(qn + 4);
-                }
-                uint32_t y[18], w[16];
-#pragma unroll
-                for (int i = 0; i < 18; i++) y[i] = d2 ? x[i + 2] : x[i];
-#pragma unroll
-                for (int i = 0; i < 17; i++) y[i] = d1 ? y[i + 1] : y[i];
-#pragma unroll
-                for (int i = 0; i < 16; i++) w[i] = __byte_perm(y[i], y[i + 1], sel);
-                uint32_t kw[4];
+                uint32_t w[16], kw[4];
+                in.next(b, w);
 #pragma unroll
                 for (int i = 0; i < 64; i++) {
-                    if (i >= 16) {
-                        uint32_t w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
-                        uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ P::shr3(w15, o);
-                        uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ P::shr10(w2, o);
-                        w[i & 15] = P::add(P::add(w[i & 15], s0, o), P::add(w[(i + 9) & 15], s1, o), o);
-                    }
-                    kw[i & 3] = P::add(w[i & 15], K[i], o);
+                    kw[i & 3] = sched<Ops<PMODE>>(w, i, o);
                     if ((i & 3) == 3) ring[stage][i >> 2][lane] = make_uint4(kw[0], kw[1], kw[2], kw[3]);
                 }
             }
@@ -463,8 +470,7 @@ cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t
 __global__ void k_split_point(const uint32_t *len_sorted_desc, const unsigned long long *n_chunks, uint64_t cap,
                               uint32_t threshold, unsigned long long max_head, unsigned long long *n_head,
                               uint32_t threshold_mid, unsigned long long *n_mid) {
-    unsigned long long n = *n_chunks;
-    if (n > cap) n = cap;
+    const unsigned long long n = live_count(*n_chunks, cap);
     auto first_le = [&](uint32_t thr) {     // first index with len <= thr (lengths sorted descending)
         unsigned long long lo = 0, hi = n;
         while (lo < hi) {
@@ -496,19 +502,16 @@ cudaError_t launch_split_point(const uint32_t *len_sorted_desc, const unsigned l
 // (the ~11 % of the bytes that take the latency kernel) are copied aside first, the latency kernel reads the copy, and
 // the caller gets its buffer back as soon as the bulk pass and this copy are done.
 // Placement: slot t starts 128 B aligned and keeps the source's misalignment mod 16, so the gather is a plain uint4 copy
-// of the 16-byte vectors that cover the chunk (the same vectors the producer warp would have loaded in place).
+// of the 16-byte vectors a hash of the chunk reads (BlockStream::first_vec / vec_count).
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t arena_slot_bytes(const uint8_t *p, uint32_t len) {
-    return (((uintptr_t)p & 15) + (uint64_t)len + 127) & ~127ull;
+    return (BlockStream::vec_span(p, len) + 127) & ~127ull;
 }
 __global__ void __launch_bounds__(1024) k_arena_plan(ShaArgs a, unsigned long long *n_head, uint64_t arena_cap, uint64_t *arena_off) {
     __shared__ uint64_t warp_sum[32];
     __shared__ uint64_t carry_s;
     __shared__ unsigned long long fit_s;
-    unsigned long long n = *a.n_chunks;
-    if (n > a.chunk_cap) n = a.chunk_cap;
-    unsigned long long head = *n_head;
-    if (head > n) head = n;
+    const unsigned long long head = live_count(*n_head, live_count(*a.n_chunks, a.chunk_cap));
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) { carry_s = 0; fit_s = head; }
     __syncthreads();
@@ -516,9 +519,8 @@ __global__ void __launch_bounds__(1024) k_arena_plan(ShaArgs a, unsigned long lo
         const unsigned long long t = t0 + threadIdx.x;
         uint64_t need = 0;
         if (t < head) {
-            const uint32_t id = a.order ? a.order[t] : (uint32_t)t;
-            const ChunkRef c = a.chunks[id];
-            need = arena_slot_bytes(a.base + (a.off ? a.off[c.stream] : 0) + c.start, c.len);
+            uint32_t id; ChunkRef c;
+            need = arena_slot_bytes(sha_chunk(a, t, id, c), c.len);
         }
         uint64_t v = need;   // inclusive scan over the block
 #pragma unroll
@@ -549,19 +551,14 @@ cudaError_t launch_arena_plan(const ShaArgs &a, unsigned long long *n_head, uint
     return cudaGetLastError();
 }
 __global__ void __launch_bounds__(256) k_arena_gather(ShaArgs a, uint8_t *arena, const uint64_t *arena_off) {
-    unsigned long long n = *a.n_chunks;
-    if (n > a.chunk_cap) n = a.chunk_cap;
-    unsigned long long head = *a.n_head;
-    if (head > n) head = n;
+    const unsigned long long head = live_count(*a.n_head, live_count(*a.n_chunks, a.chunk_cap));
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x, tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     for (unsigned long long t = 0; t < head; t++) {
-        const uint32_t id = a.order ? a.order[t] : (uint32_t)t;
-        const ChunkRef c = a.chunks[id];
-        const uint8_t *p = a.base + (a.off ? a.off[c.stream] : 0) + c.start;
-        const uint32_t delta = (uint32_t)((uintptr_t)p & 15);
-        const uint4 *src = (const uint4 *)(p - delta);
+        uint32_t id; ChunkRef c;
+        const uint8_t *p = sha_chunk(a, t, id, c);
+        const uint4 *src = BlockStream::first_vec(p);
         uint4 *dst = (uint4 *)(arena + arena_off[t]);
-        const uint64_t nvec = ((uint64_t)delta + c.len + 15) >> 4;
+        const uint64_t nvec = BlockStream::vec_count(p, c.len);
         uint64_t v = tid;
         for (; v + 3 * stride < nvec; v += 4 * stride) {
             const uint4 x0 = __ldcs(src + v), x1 = __ldcs(src + v + stride), x2 = __ldcs(src + v + 2 * stride), x3 = __ldcs(src + v + 3 * stride);
@@ -597,9 +594,7 @@ cudaError_t launch_len_keys(const ChunkRef *chunks, const unsigned long long *n_
 __global__ void k_pack_chunks(const ChunkRef *chunks, const uint8_t *digests, const uint8_t *hit,
                               const unsigned long long *n_chunks, uint64_t cap, pbsgpu_chunk *out) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned long long n = *n_chunks;
-    if (n > cap) n = cap;
-    if (i >= n) return;
+    if (i >= live_count(*n_chunks, cap)) return;
     ChunkRef c = chunks[i];
     // pbsgpu_chunk = 6 x u64: {stream|flags<<32, end_off, digest[4]}
     uint64_t *o = (uint64_t *)(out + i);

@@ -16,7 +16,7 @@
 #include <string.h>
 #include <vector>
 
-#include "../pbs_plus_b200/csrc/sha256.cu"   // product kernels (k_sha_tuned<M>, k_sha_split<P,C>) for side-by-side timing
+#include "../pbs_plus_b200/csrc/sha256.cu"   // product kernels (k_sha_tuned<M>, k_sha_split<P,C>) for side-by-side timing, and their loader
 using pbsgpu::ChunkRef;
 using pbsgpu::ShaArgs;
 
@@ -103,7 +103,7 @@ __device__ __noinline__ void finish(uint32_t (&s)[8], const uint8_t *tail, uint3
     }
 }
 
-// one lane per range; same load path as the product's k_sha_tuned (LDG.128 + prefetch + SEL/PRMT realign)
+// one lane per range; the product's load path (pbsgpu::BlockStream, as in k_sha_tuned)
 template <int V, int THREADS, int MINB>
 __global__ void __launch_bounds__(THREADS, MINB) k_lab(const uint8_t *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                                        uint8_t *digests, Opq o) {
@@ -114,28 +114,10 @@ __global__ void __launch_bounds__(THREADS, MINB) k_lab(const uint8_t *base, cons
     uint32_t s[8];
     sha_init(s);
     const uint32_t nblk = (uint32_t)(L >> 6);
-    const uint32_t delta = (uint32_t)((uintptr_t)p & 15), dw = delta >> 2, sh = delta & 3;
-    const uint4 *q = (const uint4 *)(p - delta);
-    const uint32_t sel = (sh + 3) | ((sh + 2) << 4) | ((sh + 1) << 8) | (sh << 12);
-    const bool need5 = delta != 0, d1 = dw & 1, d2 = dw & 2;
-    uint4 v0, v1, v2, v3, v4 = make_uint4(0, 0, 0, 0);
-    if (nblk) { v0 = __ldg(q); v1 = __ldg(q + 1); v2 = __ldg(q + 2); v3 = __ldg(q + 3); if (need5) v4 = __ldg(q + 4); }
+    pbsgpu::BlockStream in(p, nblk);
     for (uint32_t b = 0; b < nblk; b++) {
-        uint32_t x[20] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w, v2.x, v2.y, v2.z, v2.w,
-                          v3.x, v3.y, v3.z, v3.w, v4.x, v4.y, v4.z, v4.w};
-        if (b + 1 < nblk) {
-            const uint4 *qn = q + (uint64_t)(b + 1) * 4;
-            v0 = need5 ? v4 : __ldg(qn);
-            v1 = __ldg(qn + 1); v2 = __ldg(qn + 2); v3 = __ldg(qn + 3);
-            if (need5) v4 = __ldg(qn + 4);
-        }
-        uint32_t y[18], w[16];
-#pragma unroll
-        for (int i = 0; i < 18; i++) y[i] = d2 ? x[i + 2] : x[i];
-#pragma unroll
-        for (int i = 0; i < 17; i++) y[i] = d1 ? y[i + 1] : y[i];
-#pragma unroll
-        for (int i = 0; i < 16; i++) w[i] = __byte_perm(y[i], y[i + 1], sel);
+        uint32_t w[16];
+        in.next(b, w);
         compress<V>(s, w, o);
     }
     finish(s, p + (uint64_t)nblk * 64, (uint32_t)(L & 63), L, digests + (uint64_t)t * 32);
