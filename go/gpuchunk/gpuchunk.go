@@ -25,6 +25,7 @@ package gpuchunk
 import "C"
 
 import (
+	"crypto/rand"
 	"errors"
 	"fmt"
 	"io"
@@ -461,6 +462,7 @@ type PayloadOptions struct {
 	BlobMode   int
 	UploadBlob func(digest Digest, blob []byte) error
 	HashFiles  bool
+	Crypt      *Crypt // encrypt mode: keyed digests, encrypted blobs (nil: CryptModeNone)
 }
 
 const (
@@ -488,6 +490,12 @@ func (e *Engine) NewPayloadWriterOpts(cfg Config, known *KnownSet, opt PayloadOp
 		return nil, err
 	}
 	w := &PayloadWriter{st: st, opt: opt, BackedHashes: map[string]uint64{}}
+	if opt.Crypt != nil {
+		if err := st.SetCrypt(opt.Crypt); err != nil {
+			st.Close()
+			return nil, err
+		}
+	}
 	if opt.BlobMode != BlobNone {
 		if opt.UploadBlob == nil {
 			st.Close()
@@ -497,7 +505,7 @@ func (e *Engine) NewPayloadWriterOpts(cfg Config, known *KnownSet, opt PayloadOp
 			st.Close()
 			return nil, err
 		}
-		w.blobBuf = make([]byte, uint64(C.pbsgpu_blob_size(cfg.c.max))+16<<20)
+		w.blobBuf = make([]byte, uint64(C.pbsgpu_blob_size_enc(cfg.c.max))+16<<20)
 	}
 	_, err = st.Write(header(pxarPayloadStartMarker, 16))
 	return w, err
@@ -722,6 +730,57 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]b
 	default:
 		rc = C.pbsgpu_blob_encode_batch_z(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	}
+	if err := b.e.err(rc); err != nil {
+		return nil, err
+	}
+	res := make([][]byte, n)
+	for i := range off {
+		res[i] = out[uint64(oo[i]) : uint64(oo[i])+uint64(ol[i])]
+	}
+	return res, nil
+}
+
+// Crypt is one 32-byte client key of encrypt mode (BackupConfig's CryptMode, commit.go:314) on the engine's device.
+type Crypt struct{ c *C.pbsgpu_crypt }
+
+func (e *Engine) NewCrypt(key [32]byte) (*Crypt, error) {
+	var c *C.pbsgpu_crypt
+	if err := e.err(C.pbsgpu_crypt_create(e.ctx, (*C.uint8_t)(unsafe.Pointer(&key[0])), &c)); err != nil {
+		return nil, err
+	}
+	return &Crypt{c}, nil
+}
+
+// Close zeroes the key material on the host and the device.
+func (c *Crypt) Close() { C.pbsgpu_crypt_destroy(c.c) }
+
+// SetCrypt puts the stream in encrypt mode (before the first byte): keyed digests, and encrypted blobs whose IVs the
+// library draws from the OS CSPRNG.
+func (st *Stream) SetCrypt(c *Crypt) error { return st.e.err(C.pbsgpu_stream_crypt(st.s, c.c, nil)) }
+
+// BlobEncodeEnc returns encrypted DataBlobs of the ranges: mode (BlobRaw .. BlobLZH) picks the compressor whose frame
+// is encrypted when smaller.  Every blob gets a fresh IV from crypto/rand; an IV must never repeat under one key.
+func (b *Batch) BlobEncodeEnc(c *Crypt, mode int, off, length []uint64) ([][]byte, error) {
+	n := len(off)
+	if n == 0 {
+		return nil, nil
+	}
+	iv := make([]byte, 16*n)
+	if _, err := rand.Read(iv); err != nil {
+		return nil, err
+	}
+	o := make([]C.uint64_t, n)
+	l := make([]C.uint64_t, n)
+	oo := make([]C.uint64_t, n)
+	ol := make([]C.uint64_t, n)
+	var total uint64
+	for i := range off {
+		o[i], l[i], oo[i] = C.uint64_t(off[i]), C.uint64_t(length[i]), C.uint64_t(total)
+		total += uint64(C.pbsgpu_blob_size_enc(C.uint64_t(length[i])))
+	}
+	out := make([]byte, total+1)
+	rc := C.pbsgpu_blob_encode_batch_enc(b.e.ctx, c.c, C.int(mode), b.buf, &o[0], &l[0], C.uint32_t(n),
+		(*C.uint8_t)(unsafe.Pointer(&iv[0])), (*C.uint8_t)(unsafe.Pointer(&out[0])), &oo[0], &ol[0], nil)
 	if err := b.e.err(rc); err != nil {
 		return nil, err
 	}

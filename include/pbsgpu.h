@@ -147,7 +147,9 @@ int pbsgpu_batch_wait(pbsgpu_job *job, pbsgpu_chunk *out, uint64_t cap, uint64_t
  *  - a digest set for the asynchronous form too: the probe + insert runs as kernels on the job's stream
  *    (jobs that share a set are ordered in submission order), flags come back with the records.
  *  - stream_xxh3[n] (may be NULL): as pbsgpu_chunk_digest_batch_xxh3 (synchronous form only).
- * `size` must be sizeof(pbsgpu_batch_opts) (forward compatibility). */
+ *  - crypt (may be NULL): keyed digests of encrypt mode (see pbsgpu_crypt_create).
+ * `size` must be sizeof(pbsgpu_batch_opts) (forward compatibility; the size without `crypt` is accepted too). */
+typedef struct pbsgpu_crypt pbsgpu_crypt;
 typedef struct pbsgpu_batch_opts {
     uint32_t size, flags;
     pbsgpu_set *set;
@@ -155,6 +157,10 @@ typedef struct pbsgpu_batch_opts {
     const uint64_t *forced_off;
     uint64_t n_forced;
     uint64_t *stream_xxh3;
+    /* encrypt mode (may be NULL): record digests are keyed, SHA-256(chunk || id_key) as upstream
+     * CryptConfig::compute_digest, and the set's probe + insert sees the keyed digests.  A caller built against the
+     * header without this field passes that layout's size (offsetof(pbsgpu_batch_opts, crypt)) and gets plain digests. */
+    const pbsgpu_crypt *crypt;
 } pbsgpu_batch_opts;
 int pbsgpu_chunk_digest_batch_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base, const uint64_t *off,
                                  const uint64_t *len, uint32_t n, const pbsgpu_batch_opts *opts, pbsgpu_chunk *out,
@@ -187,6 +193,10 @@ int pbsgpu_scan_batch(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base, 
 /* Digest only (a3): SHA-256 of n arbitrary byte ranges; digests = n*32 bytes (host). */
 int pbsgpu_sha256_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                         uint8_t *digests);
+/* The keyed digests of encrypt mode: SHA-256(range || id_key of crypt) of n byte ranges (upstream
+ * CryptConfig::compute_digest). */
+int pbsgpu_sha256_keyed_batch(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off,
+                              const uint64_t *len, uint32_t n, uint8_t *digests);
 
 /* ---- streaming form -----------------------------------------------------------
  * Mirrors how the reference feeds ONE io.Reader of known size through the chunker
@@ -222,6 +232,14 @@ enum { PBSGPU_BLOB_NONE = 0, PBSGPU_BLOB_RAW = 1, PBSGPU_BLOB_Z = 2, PBSGPU_BLOB
 int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode);
 int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
                              uint64_t *n_out);
+/* Encrypt mode for the stream, set before the first byte (PBSGPU_ESTATE after that): its records carry keyed digests
+ * (as pbsgpu_batch_opts.crypt) and poll_blobs returns encrypted blobs (pbsgpu_blob_encode_batch_enc) in the stream's
+ * blob mode, so out_cap must be at least pbsgpu_blob_size_enc(cfg.max).  The stream draws one IV per blob from the OS
+ * CSPRNG (getrandom) when the blob is encoded -- no IV travels through the caller, and none is ever reused.  iv_seed
+ * (32 bytes, or NULL) makes the IVs a function of the seed instead, IV_k = SHA-256(iv_seed || k as u64 LE)[0, 16) for the
+ * k-th blob of the stream: for tests that compare blobs byte for byte.  A seed must never be used for two streams under
+ * one key. */
+int pbsgpu_stream_crypt(pbsgpu_stream *s, const pbsgpu_crypt *crypt, const uint8_t *iv_seed);
 /* XXH3-64 (seed 0) of the stream bytes [offset, offset + len), registered before they are written: offset at or after
  * pbsgpu_stream_position, ranges ascending and not overlapping (PBSGPU_EINVAL otherwise).  The payload writer registers
  * every file's content.  Each byte is hashed once on the device, in the window that holds it.  poll_hashes returns the
@@ -320,6 +338,30 @@ int pbsgpu_blob_encode_batch_lze(pbsgpu_ctx *ctx, const void *base, const uint64
  * of the chunk bytes. */
 int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                  uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+
+/* ---- f3, encrypt mode (BackupConfig's CryptMode, commit.go:314): encrypted DataBlobs ------------------------------
+ * A crypt handle holds one 32-byte AES-256 key (the caller hands over the raw key bytes; key files are not read here).
+ * create expands the key and uploads its tables to the context's device once; destroy zeroes the key material on the
+ * host and on the device.  The handle is used with the context it was created on.
+ * An encrypted blob is { magic[8], crc32 LE, iv[16], tag[16], ciphertext } (44-byte header; upstream pbs-datastore
+ * data_blob.rs / file_formats.rs, restated, UNVERIFIED against the Go module): the payload -- the zstd frame of `mode`'s
+ * encoder when that is smaller than the chunk, else the raw chunk -- is encrypted with AES-256-GCM under the key with the
+ * blob's 16-byte IV and no AAD, and the CRC covers the ciphertext.  The magic is the encrypted-compressed one
+ * (e6 59 1b bf 0b bf d8 0b) for a frame, the encrypted one (7b 67 85 be 22 2d 4c f0) otherwise.
+ * IVs: iv holds n x 16 bytes, one per blob, supplied by the caller, so the output is a pure function of the inputs.
+ * GCM's security rests on never using one IV twice under one key: draw every IV from a CSPRNG (upstream draws them at
+ * random) and never reuse one.  The library never generates or stores IVs.
+ * mode: PBSGPU_BLOB_RAW (encrypt every chunk uncompressed) or PBSGPU_BLOB_Z .. PBSGPU_BLOB_LZH (the compressor whose frame
+ * is used when smaller).  Blob i goes to out + out_off[i] (HOST memory), which must hold pbsgpu_blob_size_enc(len[i])
+ * bytes; out_len[i] receives its size.  base is HOST or DEVICE; ranges < 2^36 bytes.  crc_out may be NULL. */
+/* create also derives the id_key of keyed digests: PBKDF2-HMAC-SHA256(password = key, salt = "_id_key", 10 iterations,
+ * 32 bytes), as upstream CryptConfig::new. */
+int pbsgpu_crypt_create(pbsgpu_ctx *ctx, const uint8_t key[32], pbsgpu_crypt **out);
+void pbsgpu_crypt_destroy(pbsgpu_crypt *crypt);
+uint64_t pbsgpu_blob_size_enc(uint64_t payload_len);
+int pbsgpu_blob_encode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, const void *base, const uint64_t *off,
+                                 const uint64_t *len, uint32_t n, const uint8_t *iv, uint8_t *out, const uint64_t *out_off,
+                                 uint64_t *out_len, uint32_t *crc_out);
 
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------
  * emitBackedFile tees every new file through `xxh3.New()` and keeps `h.Sum64()` (reference

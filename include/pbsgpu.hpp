@@ -71,6 +71,20 @@ class KnownSet {   // the session's known-chunk set (PreviousBackupRef, commit.g
     pbsgpu_set *s_ = nullptr;
 };
 
+// Encrypt mode (BackupConfig's CryptMode, commit.go:314): one 32-byte client key on the engine's device.  The writers
+// below take it to produce keyed digests and, for the payload stream, encrypted blobs.
+class CryptConfig {
+  public:
+    CryptConfig(Engine &e, const uint8_t key[32]) { e.check(pbsgpu_crypt_create(e.ctx(), key, &c_)); }
+    ~CryptConfig() { pbsgpu_crypt_destroy(c_); }   // zeroes the key material
+    CryptConfig(const CryptConfig &) = delete;
+    CryptConfig &operator=(const CryptConfig &) = delete;
+    const pbsgpu_crypt *handle() const { return c_; }
+
+  private:
+    pbsgpu_crypt *c_ = nullptr;
+};
+
 namespace transfer {
 
 struct Entry { std::string Path; uint64_t FileSize; };   // the fields of pxar.Entry the hot path reads
@@ -80,8 +94,10 @@ using Reader = std::function<size_t(uint8_t *buf, size_t n)>;
 
 class DedupWriter {
   public:
-    DedupWriter(Engine &e, const buzhash::Config &cfg, KnownSet *known, uint64_t staging_bytes = 1ull << 30)
-        : e_(e), cfg_(cfg), known_(known), cap_(staging_bytes) {
+    // crypt (may be NULL): the index holds keyed digests
+    DedupWriter(Engine &e, const buzhash::Config &cfg, KnownSet *known, uint64_t staging_bytes = 1ull << 30,
+                const CryptConfig *crypt = nullptr)
+        : e_(e), cfg_(cfg), known_(known), crypt_(crypt), cap_(staging_bytes) {
         buf_ = (uint8_t *)pbsgpu_host_alloc(e.ctx(), cap_);
         if (!buf_) throw Error(PBSGPU_ENOMEM, "pbsgpu: pinned staging allocation failed");
     }
@@ -109,8 +125,10 @@ class DedupWriter {
         std::vector<pbsgpu_chunk> out(cap + 1);
         std::vector<uint64_t> xxh(entries_.size());
         uint64_t n = 0;
-        e_.check(pbsgpu_chunk_digest_batch_xxh3(e_.ctx(), &cfg_, buf_, off_.data(), len_.data(), (uint32_t)entries_.size(),
-                                                known_ ? known_->handle() : nullptr, out.data(), out.size(), &n, xxh.data()));
+        pbsgpu_batch_opts o = {sizeof(pbsgpu_batch_opts), 0, known_ ? known_->handle() : nullptr, nullptr, nullptr, 0,
+                               xxh.data(), crypt_ ? crypt_->handle() : nullptr};
+        e_.check(pbsgpu_chunk_digest_batch_ex(e_.ctx(), &cfg_, buf_, off_.data(), len_.data(), (uint32_t)entries_.size(), &o,
+                                              out.data(), out.size(), &n));
         for (size_t i = 0; i < entries_.size(); i++) backed_hashes_[entries_[i].Path] = xxh[i];
         for (uint64_t i = 0; i < n; i++) {
             IndexRecord r;
@@ -128,6 +146,7 @@ class DedupWriter {
     Engine &e_;
     buzhash::Config cfg_;
     KnownSet *known_;
+    const CryptConfig *crypt_;
     uint8_t *buf_ = nullptr;
     uint64_t cap_, fill_ = 0;
     bool finished_ = false;
@@ -143,20 +162,23 @@ class DedupWriter {
 // library's pinned ring.  WriteEntryReader (commit.go:720) returns the entry's payload offset.
 // Optional: `blob_mode` (PBSGPU_BLOB_RAW .. _LZH) hands the DataBlob of every new chunk to `upload_blob(digest, blob,
 // len)`, encoded on the GPU from the stream's windows; `hash_files` records every file's XXH3-64 in BackedHashes()
-// (commitWalkState.backedHashes, commit.go:725).
+// (commitWalkState.backedHashes, commit.go:725); `crypt` gives keyed digests and encrypted blobs, their IVs drawn from the
+// OS CSPRNG by the stream.
 struct PayloadChunk { uint64_t end_off; uint8_t digest[32]; bool known; };
 using UploadBlob = std::function<void(const uint8_t digest[32], const uint8_t *blob, uint64_t len)>;
 
 class PayloadStreamWriter {
   public:
     PayloadStreamWriter(Engine &e, const buzhash::Config &cfg, KnownSet *known, bool suggest = true,
-                        int blob_mode = PBSGPU_BLOB_NONE, UploadBlob upload_blob = nullptr, bool hash_files = false)
+                        int blob_mode = PBSGPU_BLOB_NONE, UploadBlob upload_blob = nullptr, bool hash_files = false,
+                        const CryptConfig *crypt = nullptr)
         : e_(e), suggest_(suggest), upload_(std::move(upload_blob)), hash_(hash_files) {
         if ((blob_mode != PBSGPU_BLOB_NONE) != (upload_ != nullptr))
             throw Error(PBSGPU_EINVAL, "transfer: a blob mode and an upload_blob callback go together");
-        if (upload_) blob_buf_.resize(pbsgpu_blob_size(cfg.max) + (16u << 20));
+        if (upload_) blob_buf_.resize(pbsgpu_blob_size_enc(cfg.max) + (16u << 20));
         e.check(pbsgpu_stream_open(e.ctx(), &cfg, known ? known->handle() : nullptr, &s_));
         try {   // the destructor does not run for a constructor that throws
+            if (crypt) e.check(pbsgpu_stream_crypt(s_, crypt->handle(), nullptr));
             if (upload_) e.check(pbsgpu_stream_blob_mode(s_, blob_mode));
             raw(header(0x834c68c2194a4ed2ull, 16));                 // PXAR_PAYLOAD_START_MARKER
         } catch (...) {

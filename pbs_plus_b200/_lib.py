@@ -58,9 +58,9 @@ class Timing(C.Structure):
 
 
 class BatchOpts(C.Structure):
-    """pbsgpu_batch_opts: digest set, suggested boundaries, per-stream XXH3 output."""
+    """pbsgpu_batch_opts: digest set, suggested boundaries, per-stream XXH3 output, encrypt mode's keyed digests."""
     _fields_ = [("size", C.c_uint32), ("flags", C.c_uint32), ("set", C.c_void_p), ("forced_stream", C.c_void_p),
-                ("forced_off", C.c_void_p), ("n_forced", C.c_uint64), ("stream_xxh3", C.c_void_p)]
+                ("forced_off", C.c_void_p), ("n_forced", C.c_uint64), ("stream_xxh3", C.c_void_p), ("crypt", C.c_void_p)]
 
 
 class Corpus(C.Structure):
@@ -75,7 +75,7 @@ SYMBOLS = [
     "pbsgpu_set_profiling", "pbsgpu_partition_info", "pbsgpu_scan_partition_sms", "pbsgpu_set_kernel_variant", "pbsgpu_config", "pbsgpu_config_kib",
     "pbsgpu_default_table", "pbsgpu_chunk_digest_batch", "pbsgpu_batch_submit", "pbsgpu_batch_wait",
     "pbsgpu_chunk_digest_batch_ex", "pbsgpu_batch_submit_ex", "pbsgpu_batch_free", "pbsgpu_batch_wait_input", "pbsgpu_batch_input_done",
-    "pbsgpu_scan_batch", "pbsgpu_sha256_batch", "pbsgpu_stream_open", "pbsgpu_stream_write",
+    "pbsgpu_scan_batch", "pbsgpu_sha256_batch", "pbsgpu_sha256_keyed_batch", "pbsgpu_stream_crypt", "pbsgpu_stream_open", "pbsgpu_stream_write",
     "pbsgpu_stream_poll", "pbsgpu_stream_finish", "pbsgpu_stream_close", "pbsgpu_stream_reserve", "pbsgpu_stream_commit",
     "pbsgpu_stream_slot_bytes", "pbsgpu_stream_suggest", "pbsgpu_stream_position", "pbsgpu_stream_blob_mode",
     "pbsgpu_stream_poll_blobs", "pbsgpu_stream_hash_range", "pbsgpu_stream_poll_hashes", "pbsgpu_set_create",
@@ -83,7 +83,8 @@ SYMBOLS = [
     "pbsgpu_set_allgather", "pbsgpu_nccl_unique_id", "pbsgpu_nccl_comm_create", "pbsgpu_nccl_comm_destroy",
     "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
-    "pbsgpu_blob_encode_batch_lzh",
+    "pbsgpu_blob_encode_batch_lzh", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
+    "pbsgpu_blob_encode_batch_enc",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
 ]
@@ -127,6 +128,8 @@ def lib() -> C.CDLL:
     L.pbsgpu_batch_free.restype = None
     L.pbsgpu_scan_batch.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, u64p]
     L.pbsgpu_sha256_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
+    L.pbsgpu_sha256_keyed_batch.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, vp]
+    L.pbsgpu_stream_crypt.argtypes = [vp, vp, vp]
     L.pbsgpu_stream_open.argtypes = [vp, C.POINTER(Cfg), vp, C.POINTER(vp)]
     L.pbsgpu_stream_write.argtypes = [vp, vp, C.c_uint64]
     L.pbsgpu_stream_poll.argtypes = [vp, vp, C.c_uint64, u64p]
@@ -156,6 +159,12 @@ def lib() -> C.CDLL:
     L.pbsgpu_blob_encode_batch_lz.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lze.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lzh.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
+    L.pbsgpu_crypt_destroy.argtypes = [vp]
+    L.pbsgpu_crypt_destroy.restype = None
+    L.pbsgpu_blob_size_enc.argtypes = [C.c_uint64]
+    L.pbsgpu_blob_size_enc.restype = C.c_uint64
+    L.pbsgpu_blob_encode_batch_enc.argtypes = [vp, vp, C.c_int, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp]
     L.pbsgpu_set_create.argtypes = [vp, C.c_uint64, C.POINTER(vp)]
     L.pbsgpu_set_destroy.argtypes = [vp]
     L.pbsgpu_set_destroy.restype = None

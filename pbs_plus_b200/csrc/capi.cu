@@ -655,8 +655,8 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
         ha.base = j->base; ha.off = j->d_off; ha.chunks = j->d_chunks; ha.order = j->d_vals2;
         ha.n_chunks = &j->d_counters[CTR_CHUNKS]; ha.chunk_cap = j->chunk_cap; ha.digests = j->d_digests;
         ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
-        if (j->variant == 1) CK(launch_sha_simple(ha, st));
-        else if (!hybrid_for(ctx)) CK(launch_sha_tuned(ha, ctx->tune, st));
+        if (j->variant == 1) CK(launch_sha_simple(ha, st, j->sha_suffix));
+        else if (!hybrid_for(ctx)) CK(launch_sha_tuned(ha, ctx->tune, st, j->sha_suffix));
         else {
             // hybrid: chunks longer than 2.5 x avg (their serial chains bound the batch's makespan) run on
             // the latency-optimised split kernel on a forked stream, concurrently with the rest
@@ -684,18 +684,18 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
             CK(cudaEventRecord(j->ev[EV_FORK], st));
             if (!serial) CK(cudaStreamWaitEvent(side, j->ev[EV_FORK], 0));
             ha.n_mid = use_mid ? &j->d_counters[CTR_MID] : nullptr;
-            ha.part = 1; CK(launch_sha_split(ha, ctx->tune, side));
+            ha.part = 1; CK(launch_sha_split(ha, ctx->tune, side, j->sha_suffix));
             ha.arena = nullptr; ha.arena_off = nullptr;
             CK(cudaEventRecord(j->ev[EV_JOIN], side));
             if (early) CK(cudaEventRecord(ctx->arena_recs.back().ev, side));   // the region may be reused after this
             if (use_mid) {   // the longer bulk chunks of every job in flight start first (high-priority stream), the short ones fill in
                 CK(cudaStreamWaitEvent(j->st3, j->ev[EV_FORK], 0));
-                ha.part = 3; CK(launch_sha_tuned(ha, ctx->tune, j->st3));
+                ha.part = 3; CK(launch_sha_tuned(ha, ctx->tune, j->st3, j->sha_suffix));
                 CK(cudaEventRecord(j->ev[EV_MID], j->st3));
-                ha.part = 4; CK(launch_sha_tuned(ha, ctx->tune, st));
+                ha.part = 4; CK(launch_sha_tuned(ha, ctx->tune, st, j->sha_suffix));
                 CK(cudaStreamWaitEvent(st, j->ev[EV_MID], 0));
             } else {
-                ha.part = 2; CK(launch_sha_tuned(ha, ctx->tune, st));
+                ha.part = 2; CK(launch_sha_tuned(ha, ctx->tune, st, j->sha_suffix));
             }
             CK(cudaEventRecord(j->ev[EV_BULK], st));
             if (early) {
@@ -804,10 +804,17 @@ int pbsgpu_job_finish(pbsgpu_job *j) {
     return PBSGPU_OK;
 }
 
-static const pbsgpu_batch_opts NO_OPTS = {sizeof(pbsgpu_batch_opts), 0, nullptr, nullptr, nullptr, 0, nullptr};
-static int opts_ok(pbsgpu_ctx *ctx, const pbsgpu_batch_opts *o) {
-    if (o && o->size != sizeof(pbsgpu_batch_opts)) return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.size = %u, expected %zu", o->size, sizeof(pbsgpu_batch_opts));
-    if (o && (o->flags & ~(uint32_t)PBSGPU_BATCH_EARLY_INPUT)) return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.flags = 0x%x: unknown bits", o->flags);
+static const pbsgpu_batch_opts NO_OPTS = {sizeof(pbsgpu_batch_opts), 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr};
+// The caller's options in the current layout.  A caller built against the header before `crypt` passes that layout's
+// size (the offset of `crypt`) and gets plain digests.
+static int opts_read(pbsgpu_ctx *ctx, const pbsgpu_batch_opts *o, pbsgpu_batch_opts *out) {
+    *out = NO_OPTS;
+    if (!o) return PBSGPU_OK;
+    if (o->size != sizeof(pbsgpu_batch_opts) && o->size != offsetof(pbsgpu_batch_opts, crypt))
+        return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.size = %u, expected %zu", o->size, sizeof(pbsgpu_batch_opts));
+    memcpy(out, o, o->size);
+    if (out->flags & ~(uint32_t)PBSGPU_BATCH_EARLY_INPUT) return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.flags = 0x%x: unknown bits", out->flags);
+    if (out->crypt && out->crypt->ctx != ctx) return fail(ctx, PBSGPU_EINVAL, "crypt belongs to another context");
     return PBSGPU_OK;
 }
 
@@ -816,15 +823,16 @@ extern "C" int pbsgpu_batch_submit_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, co
     if (!ctx || !job || (n && (!off || !len))) return PBSGPU_EINVAL;
     Guard g(ctx);
     *job = nullptr;
-    int rc = opts_ok(ctx, opts);
+    pbsgpu_batch_opts o;
+    int rc = opts_read(ctx, opts, &o);
     if (rc) return rc;
-    const pbsgpu_batch_opts &o = opts ? *opts : NO_OPTS;
     if (o.stream_xxh3) return fail(ctx, PBSGPU_EINVAL, "stream_xxh3 is a synchronous-form option");
     if (n && !pbsgpu_is_device_ptr(base_dev)) return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_submit needs a device pointer");
     pbsgpu_job *j = nullptr;
     rc = pbsgpu_job_create(ctx, cfg, base_dev, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j);
     if (rc) return rc;
     j->early = (o.flags & PBSGPU_BATCH_EARLY_INPUT) != 0;
+    j->sha_suffix = pbsgpu_crypt_id_key(o.crypt);
     rc = pbsgpu_job_enqueue(j);
     if (rc) { pbsgpu_job_release(j); return rc; }
     *job = j;
@@ -984,6 +992,7 @@ static int batch_host(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const uint8_t *bas
         rc = pbsgpu_job_create(ctx, cfg, buf, goff.data(), glen.data(), g.count, 1, 1, o.set, fs.data(), o.forced_off + g.f_lo,
                                g.f_hi - g.f_lo, &j);
         if (rc) break;
+        j->sha_suffix = pbsgpu_crypt_id_key(o.crypt);
         cudaStreamWaitEvent(j->ss, copied[gi], 0);
         rc = pbsgpu_job_enqueue(j);
         if (rc == PBSGPU_OK && o.stream_xxh3) rc = pbsgpu_xxh3_enqueue(ctx, buf, goff.data(), glen.data(), g.count, j->st, &xruns[gi]);
@@ -1003,9 +1012,9 @@ extern "C" int pbsgpu_chunk_digest_batch_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *c
                                             uint64_t cap, uint64_t *n_out) {
     if (!ctx || (n && (!off || !len || !base)) || (cap && !out)) return PBSGPU_EINVAL;
     Guard g(ctx);
-    int rc = opts_ok(ctx, opts);
+    pbsgpu_batch_opts o;
+    int rc = opts_read(ctx, opts, &o);
     if (rc) return rc;
-    const pbsgpu_batch_opts &o = opts ? *opts : NO_OPTS;
     if (o.set && o.set->ctx != ctx) return fail(ctx, PBSGPU_EINVAL, "set belongs to another context");
     if (!pbsgpu_cfg_ok(cfg)) return fail(ctx, PBSGPU_EINVAL, "invalid pbsgpu_cfg (use pbsgpu_config)");
     uint64_t produced = 0;
@@ -1014,6 +1023,7 @@ extern "C" int pbsgpu_chunk_digest_batch_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *c
         pbsgpu_job *j = nullptr;
         rc = pbsgpu_job_create(ctx, cfg, base, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j);
         if (rc) return rc;
+        j->sha_suffix = pbsgpu_crypt_id_key(o.crypt);
         XxhRun xr;
         rc = pbsgpu_job_enqueue(j);
         if (rc == PBSGPU_OK && o.stream_xxh3) rc = pbsgpu_xxh3_enqueue(ctx, (const uint8_t *)base, off, len, n, j->st, &xr);

@@ -71,6 +71,11 @@ struct pbsgpu_stream {
     // DataBlobs of new chunks
     int blob_mode = PBSGPU_BLOB_NONE;
     std::deque<BlobWindow> blobs;
+    // encrypt mode (pbsgpu_stream_crypt): keyed digests, encrypted blobs with one IV per blob
+    const pbsgpu_crypt *crypt = nullptr;
+    bool iv_seeded = false;
+    uint8_t iv_seed[32];
+    uint64_t n_blobs = 0;             // blobs encoded so far (index of the next blob's IV)
     // XXH3-64 of registered ranges; hr[k] has registration index hr_base + k
     std::deque<HashRange> hr;
     uint64_t hr_base = 0;
@@ -147,16 +152,26 @@ static int collect_blobs(pbsgpu_stream *s, const pbsgpu_job *j, const uint8_t *b
         const uint64_t end = j->h_out[k].end_off;
         if (!(j->h_out[k].flags & PBSGPU_CHUNK_KNOWN)) {
             off.push_back(prev); len.push_back(end - prev); out_off.push_back(bytes);
-            bytes += pbsgpu_blob_size(end - prev);
+            bytes += s->crypt ? pbsgpu_blob_size_enc(end - prev) : pbsgpu_blob_size(end - prev);
         }
         prev = end;
     }
     if (off.empty()) return PBSGPU_OK;
     BlobWindow bw{(uint8_t *)ctx->pin.get(bytes), std::move(out_off), std::vector<uint64_t>(off.size()), 0};
     if (!bw.host) return fail(ctx, PBSGPU_ENOMEM, "pinned blob arena of %llu bytes failed", (unsigned long long)bytes);
-    const int rc = pbsgpu_blob_encode_mode(ctx, buf, off.data(), len.data(), (uint32_t)off.size(), s->blob_mode, bw.host,
-                                           bw.off.data(), bw.len.data());
+    const uint32_t nb = (uint32_t)off.size();
+    int rc;
+    if (s->crypt) {
+        std::vector<uint8_t> iv(16ull * nb);
+        rc = pbsgpu_stream_ivs(ctx, s->iv_seeded ? s->iv_seed : nullptr, s->n_blobs, nb, iv.data());
+        if (rc == PBSGPU_OK)
+            rc = pbsgpu_blob_encode_batch_enc(ctx, s->crypt, s->blob_mode, buf, off.data(), len.data(), nb, iv.data(), bw.host,
+                                              bw.off.data(), bw.len.data(), nullptr);
+    } else {
+        rc = pbsgpu_blob_encode_mode(ctx, buf, off.data(), len.data(), nb, s->blob_mode, bw.host, bw.off.data(), bw.len.data());
+    }
     if (rc) { ctx->pin.put(bw.host); return rc; }
+    s->n_blobs += nb;
     s->blobs.push_back(std::move(bw));
     return PBSGPU_OK;
 }
@@ -295,6 +310,7 @@ static int stream_process(pbsgpu_stream *s, int eof) {
     pbsgpu_job *j = nullptr;
     int rc = pbsgpu_job_create(ctx, &s->cfg, s->buf[s->cur], &off0, &len0, 1, eof, 1, s->set, fstream.data(), foff.data(), foff.size(), &j);
     if (rc) return rc;
+    j->sha_suffix = pbsgpu_crypt_id_key(s->crypt);
     CK(cudaStreamWaitEvent(j->ss, s->copied, 0));       // every byte of the window has arrived before K1 reads it
     // front half now: the cut points decide what has to be carried over.  On a candidate overflow only the front half is
     // rerun: the back half is enqueued once the carry is known.
@@ -463,14 +479,26 @@ extern "C" int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode) {
     return PBSGPU_OK;
 }
 
+extern "C" int pbsgpu_stream_crypt(pbsgpu_stream *s, const pbsgpu_crypt *crypt, const uint8_t *iv_seed) {
+    if (!s || !crypt) return PBSGPU_EINVAL;
+    Guard g(s->ctx);
+    if (crypt->ctx != s->ctx) return fail(s->ctx, PBSGPU_EINVAL, "crypt belongs to another context");
+    if (s->started || s->finished) return fail(s->ctx, PBSGPU_ESTATE, "encrypt mode is set before the first byte");
+    s->crypt = crypt;
+    s->iv_seeded = iv_seed != nullptr;
+    if (iv_seed) memcpy(s->iv_seed, iv_seed, 32);
+    return PBSGPU_OK;
+}
+
 extern "C" int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
                                         uint64_t *n_out) {
     if (!s || !n_out || (cap && (!out || !blob_len))) return PBSGPU_EINVAL;
     pbsgpu_ctx *ctx = s->ctx;
     Guard g(ctx);
-    if (out_cap < pbsgpu_blob_size(s->cfg.max))
+    const uint64_t largest = s->crypt ? pbsgpu_blob_size_enc(s->cfg.max) : pbsgpu_blob_size(s->cfg.max);
+    if (out_cap < largest)
         return fail(ctx, PBSGPU_EINVAL, "blob buffer of %llu bytes is smaller than one blob of the largest chunk (%llu)",
-                    (unsigned long long)out_cap, (unsigned long long)pbsgpu_blob_size(s->cfg.max));
+                    (unsigned long long)out_cap, (unsigned long long)largest);
     int rc = stream_collect(s, false);
     if (rc) return rc;
     uint64_t k = 0, used = 0;

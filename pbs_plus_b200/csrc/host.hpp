@@ -194,6 +194,7 @@ struct pbsgpu_job {
     int eof = 1, want_digests = 1, variant = 0;
     bool scan_lanes = false;
     pbsgpu_set *set = nullptr;      // fused probe + insert (NULL: none)
+    const uint8_t *sha_suffix = nullptr;   // encrypt mode: the crypt's device id_key, K3 computes keyed digests
     // device
     uint64_t *d_off = nullptr, *d_len = nullptr, *d_tile_first = nullptr, *d_cand = nullptr, *d_cand_sorted = nullptr, *d_forced = nullptr;
     unsigned long long *d_counters = nullptr;   // [CTR_DEVICE], indexed by CTR_*
@@ -252,6 +253,20 @@ int pbsgpu_xxh3_table(pbsgpu_ctx *ctx, const void **tab);   // K7's device table
 // out_len[i] bytes.  Device ranges are encoded in place.
 int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len);
+
+// ---------------------------------------------------------------------------
+// encrypt mode (capi_crypt.cu): one AES-256 key, its K11 tables on the host (J0, E_K(J0)) and on the device
+// ---------------------------------------------------------------------------
+struct pbsgpu_crypt {
+    pbsgpu_ctx *ctx;
+    std::vector<uint8_t> tab;   // pbsgpu::GcmTables, then the 32-byte id_key of keyed digests
+    uint8_t *d_tab = nullptr;   // device copy of tab
+};
+// IVs of blobs first .. first + n - 1 of a stream (16 bytes each): from the OS CSPRNG (getrandom), or, with a 32-byte seed,
+// IV_k = SHA-256(seed || k as u64 LE)[0, 16)
+int pbsgpu_stream_ivs(pbsgpu_ctx *ctx, const uint8_t *seed, uint64_t first, uint32_t n, uint8_t *iv);
+// the crypt's device id_key (K3's keyed suffix), NULL for NULL
+inline const uint8_t *pbsgpu_crypt_id_key(const pbsgpu_crypt *c) { return c ? c->d_tab + pbsgpu::gcm_tables_bytes() : nullptr; }
 
 template <typename T> static T pbsgpu_driver_ep(const char *name) {
     void *p = nullptr;

@@ -102,9 +102,11 @@ struct ShaTune {
     int mid_x10 = 0;      // PBSGPU_BULK_MID_X10: > 0: bulk chunks longer than mid_x10/10 x avg are launched on a HIGH-PRIORITY bulk
                           // stream of their own, so the longer chains of every job in flight start before the short ones
 };
-cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st);
-cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t st);   // throughput kernel
-cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t st);   // latency kernel
+// suffix (device, 32 bytes; encrypt mode's id_key): the digests are SHA-256(chunk || suffix), from the keyed kernels;
+// NULL = plain digests
+cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st, const uint8_t *suffix = nullptr);
+cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix = nullptr);   // throughput kernel
+cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix = nullptr);   // latency kernel
 cudaError_t launch_split_point(const uint32_t *len_sorted_desc, const unsigned long long *n_chunks, uint64_t cap,
                                uint32_t threshold, unsigned long long max_head, unsigned long long *n_head,
                                uint32_t threshold_mid, unsigned long long *n_mid, cudaStream_t st);
@@ -174,6 +176,22 @@ cudaError_t launch_xxh3_pieces(const uint8_t *base, const uint64_t *off, const u
 uint64_t xxh3_empty_host();
 void crc_fill_tables_host(void *dst);
 uint64_t crc_wb_bytes();
+
+// ---- AES-256-GCM (K11, encrypted DataBlobs) ---------------------------------------------------
+constexpr uint32_t GCM_SEG_BLOCKS = 1024;   // 16-byte blocks per warp segment (32 per lane)
+struct GcmMsg {          // one message: plaintext at device address src (any alignment), ciphertext to dst (16 B aligned,
+    uint64_t src, dst;   // whole blocks), len bytes; J0 and E_K(J0) as big-endian words
+    uint64_t len;
+    uint32_t j0[4], ej0[4];
+};
+size_t gcm_tables_bytes();
+void gcm_fill_tables_host(const uint8_t key[32], void *tables);
+void gcm_encrypt_block_host(const void *tables, const uint32_t in[4], uint32_t out[4]);
+void gcm_j0_host(const void *tables, const uint8_t iv[16], uint32_t j0[4]);
+uint64_t gcm_segments(uint64_t len);
+// seg_first[n+1]: prefix of gcm_segments(len); part: 16 B per segment; tags: 16 B per message (device)
+cudaError_t launch_gcm(const GcmMsg *msg, const uint64_t *seg_first, uint32_t n, uint64_t total_segs, const void *tables,
+                       void *part, uint8_t *tags, int sm_count, cudaStream_t st);
 
 // ---- corpus (K5) ------------------------------------------------------------------
 cudaError_t launch_corpus_fill(const pbsgpu_corpus &c, uint64_t first_file, uint32_t n_files, uint8_t *dst,

@@ -89,6 +89,44 @@ __device__ __noinline__ void sha_finish(Sha256State &s, const uint8_t *tail, uin
     }
 }
 
+// sha_finish of the keyed message (chunk || suffix[32]) of encrypt mode: the 32 suffix bytes follow the tail, so only
+// these final one or two blocks differ from the plain digest's.  A function of its own, so sha_finish and the kernels that
+// call it keep their code.
+__device__ __noinline__ void sha_finish_keyed(Sha256State &s, const uint8_t *tail, uint32_t rem, uint64_t len,
+                                              const uint8_t *suffix, uint8_t *out) {
+    const uint64_t bits = (len + 32) * 8;
+    const uint32_t end = rem + 32;
+    const int nblk = end < 56 ? 1 : 2;
+    for (int blk = 0; blk < nblk; blk++) {
+        uint32_t w[16];
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            uint32_t v = 0;
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                uint32_t idx = blk * 64 + i * 4 + k;
+                uint32_t byte = idx < rem ? tail[idx] : idx < end ? suffix[idx - rem] : (idx == end ? 0x80u : 0u);
+                v = (v << 8) | byte;
+            }
+            w[i] = v;
+        }
+        if (blk == nblk - 1) { w[14] = (uint32_t)(bits >> 32); w[15] = (uint32_t)bits; }
+        sha_compress(s, w);
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        out[4 * i] = (uint8_t)(s.h[i] >> 24); out[4 * i + 1] = (uint8_t)(s.h[i] >> 16);
+        out[4 * i + 2] = (uint8_t)(s.h[i] >> 8); out[4 * i + 3] = (uint8_t)s.h[i];
+    }
+}
+// the digest of a hash whose full blocks are done: plain, or keyed with `suffix`
+template <bool KEYED>
+__device__ __forceinline__ void sha_done(const ShaArgs &a, const uint8_t *suffix, Sha256State &s, const uint8_t *tail,
+                                         const ChunkRef &c, uint32_t id) {
+    if (KEYED) sha_finish_keyed(s, tail, c.len & 63, c.len, suffix, a.digests + (uint64_t)id * 32);
+    else sha_finish(s, tail, c.len & 63, c.len, a.digests + (uint64_t)id * 32);
+}
+
 // 64 message bytes at arbitrary alignment -> 16 big-endian words.
 // Loads 4-byte aligned words; ONE PRMT per word does the realignment and the byte swap.
 __device__ __forceinline__ void load_block_be(const uint8_t *p, uint32_t (&w)[16]) {
@@ -181,7 +219,8 @@ __device__ __forceinline__ bool sha_slot(const ShaArgs &a, uint64_t t, uint64_t 
 // ---------------------------------------------------------------------------
 // Cross-check / v0 kernel: one thread per chunk, chunks in `order` (longest first).
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(64) k_sha_simple(ShaArgs a) {
+template <bool KEYED>
+__device__ __forceinline__ void sha_simple_body(const ShaArgs &a, const uint8_t *suffix) {
     uint64_t t;
     if (!sha_slot(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, t)) return;
     uint32_t id; ChunkRef c;
@@ -194,13 +233,16 @@ __global__ void __launch_bounds__(64) k_sha_simple(ShaArgs a) {
         load_block_be(p + (uint64_t)b * 64, w);
         sha_compress(s, w);
     }
-    sha_finish(s, p + (uint64_t)nblk * 64, c.len & 63, c.len, a.digests + (uint64_t)id * 32);
+    sha_done<KEYED>(a, suffix, s, p + (uint64_t)nblk * 64, c, id);
 }
+__global__ void __launch_bounds__(64) k_sha_simple(ShaArgs a) { sha_simple_body<false>(a, nullptr); }
+__global__ void __launch_bounds__(64) k_sha_simple_keyed(ShaArgs a, const uint8_t *suffix) { sha_simple_body<true>(a, suffix); }
 
-cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st) {
+cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st, const uint8_t *suffix) {
     if (a.chunk_cap == 0) return cudaSuccess;
     uint64_t blocks = (a.chunk_cap + 63) / 64;
-    k_sha_simple<<<(unsigned)blocks, 64, 0, st>>>(a);
+    if (suffix) k_sha_simple_keyed<<<(unsigned)blocks, 64, 0, st>>>(a, suffix);
+    else k_sha_simple<<<(unsigned)blocks, 64, 0, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -278,8 +320,9 @@ __device__ __forceinline__ void sha_compress_t(Sha256State &s, uint32_t (&w)[16]
 }
 
 // Tuned kernel.  Same one-lane-per-chunk mapping, but BlockStream's loads and the pipe-balanced compression above.
-template <int MODE>
-__global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o) {
+// KEYED: encrypt mode's digest SHA-256(chunk || suffix); the plain instantiations ignore `suffix`
+template <int MODE, bool KEYED>
+__global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o, const uint8_t *suffix) {
     uint64_t t;
     if (!sha_slot(a, (uint64_t)blockIdx.x * 32 + threadIdx.x, t)) return;
     uint32_t id; ChunkRef c;
@@ -293,7 +336,7 @@ __global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o) {
         in.next(b, w);
         sha_compress_t<MODE>(s, w, o);
     }
-    sha_finish(s, p + (uint64_t)nblk * 64, c.len & 63, c.len, a.digests + (uint64_t)id * 32);
+    sha_done<KEYED>(a, suffix, s, p + (uint64_t)nblk * 64, c, id);
 }
 
 // ---------------------------------------------------------------------------
@@ -351,8 +394,8 @@ __device__ __forceinline__ void sha_rounds(Sha256State &s, const uint4 (&kwv)[16
     s.h[0] += a; s.h[1] += b; s.h[2] += c; s.h[3] += d; s.h[4] += e; s.h[5] += f; s.h[6] += g; s.h[7] += h;
 }
 
-template <int PMODE, int CMODE>
-__global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o) {
+template <int PMODE, int CMODE, bool KEYED>
+__global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o, const uint8_t *suffix) {
     __shared__ __align__(16) uint4 ring[SPLIT_STAGES][16][32];   // [stage][4 rounds][lane] = W+K
     __shared__ __align__(8) uint64_t bars[2 * SPLIT_STAGES];
     uint64_t t0;
@@ -411,24 +454,31 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o) {
             mbar_arrive(empty[stage]);
             if (++stage == SPLIT_STAGES) { stage = 0; phase ^= 1; }
         }
-        if (active) sha_finish(s, p + (uint64_t)nblk * 64, c.len & 63, c.len, a.digests + (uint64_t)id * 32);
+        if (active) sha_done<KEYED>(a, suffix, s, p + (uint64_t)nblk * 64, c, id);
     }
 }
 
 // throughput kernel (mode 0: the compiler's own pipe choice; 2: + schedule shifts on the FMA pipe;
 // 1/3/7: more aggressive offloads -- see DESIGN.md and tools/sha_lab.cu).  `mode` comes from the context
 // (PBSGPU_SHA_MODE read once per pbsgpu_open), never from process-wide state.
-cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t st) {
+cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix) {
     if (a.chunk_cap == 0) return cudaSuccess;
-    if (tune.mode >= 10 && a.part == 0) return launch_sha_split(a, tune, st);
+    if (tune.mode >= 10 && a.part == 0) return launch_sha_split(a, tune, st, suffix);
     Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
     unsigned blocks = (unsigned)((a.chunk_cap + 31) / 32);
-    switch (tune.mode) {
-        case 0: k_sha_tuned<0><<<blocks, 32, 0, st>>>(a, o); break;
-        case 1: k_sha_tuned<1><<<blocks, 32, 0, st>>>(a, o); break;
-        case 3: k_sha_tuned<3><<<blocks, 32, 0, st>>>(a, o); break;
-        case 7: k_sha_tuned<7><<<blocks, 32, 0, st>>>(a, o); break;
-        default: k_sha_tuned<2><<<blocks, 32, 0, st>>>(a, o); break;
+    if (suffix) switch (tune.mode) {
+        case 0: k_sha_tuned<0, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
+        case 1: k_sha_tuned<1, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
+        case 3: k_sha_tuned<3, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
+        case 7: k_sha_tuned<7, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
+        default: k_sha_tuned<2, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
+    }
+    else switch (tune.mode) {
+        case 0: k_sha_tuned<0, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
+        case 1: k_sha_tuned<1, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
+        case 3: k_sha_tuned<3, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
+        case 7: k_sha_tuned<7, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
+        default: k_sha_tuned<2, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
     }
     return cudaGetLastError();
 }
@@ -440,26 +490,29 @@ cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t
 // CTAs per SM (30 -> 4, 85 -> 2, 112 -> 1) and forces the spread; the throughput kernel uses no shared
 // memory and still co-resides.
 template <int PM, int CM>
-static cudaError_t launch_split_t(const ShaArgs &a, const Opq &o, unsigned blocks, int spread_kb, cudaStream_t st) {
+static cudaError_t launch_split_t(const ShaArgs &a, const Opq &o, unsigned blocks, int spread_kb, cudaStream_t st,
+                                  const uint8_t *suffix) {
     size_t dyn = 0;
     if (a.part == 1 && spread_kb > 0) {
         dyn = (size_t)spread_kb * 1024;
-        cudaError_t e = cudaFuncSetAttribute(k_sha_split<PM, CM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+        cudaError_t e = cudaFuncSetAttribute(suffix ? k_sha_split<PM, CM, true> : k_sha_split<PM, CM, false>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
         if (e != cudaSuccess) return e;
     }
-    k_sha_split<PM, CM><<<blocks, 64, dyn, st>>>(a, o);
+    if (suffix) k_sha_split<PM, CM, true><<<blocks, 64, dyn, st>>>(a, o, suffix);
+    else k_sha_split<PM, CM, false><<<blocks, 64, dyn, st>>>(a, o, nullptr);
     return cudaGetLastError();
 }
-cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t st) {
+cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix) {
     if (a.chunk_cap == 0) return cudaSuccess;
     Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
     unsigned blocks = (unsigned)((a.chunk_cap + 31) / 32);
     switch (tune.mode) {
-        case 10: return launch_split_t<0, 0>(a, o, blocks, tune.spread_kb, st);
-        case 12: return launch_split_t<0, 1>(a, o, blocks, tune.spread_kb, st);
-        case 13: return launch_split_t<3, 1>(a, o, blocks, tune.spread_kb, st);
-        case 14: return launch_split_t<3, 2>(a, o, blocks, tune.spread_kb, st);
-        default: return launch_split_t<3, 0>(a, o, blocks, tune.spread_kb, st);   // producer balanced, consumer IADD3
+        case 10: return launch_split_t<0, 0>(a, o, blocks, tune.spread_kb, st, suffix);
+        case 12: return launch_split_t<0, 1>(a, o, blocks, tune.spread_kb, st, suffix);
+        case 13: return launch_split_t<3, 1>(a, o, blocks, tune.spread_kb, st, suffix);
+        case 14: return launch_split_t<3, 2>(a, o, blocks, tune.spread_kb, st, suffix);
+        default: return launch_split_t<3, 0>(a, o, blocks, tune.spread_kb, st, suffix);   // producer balanced, consumer IADD3
     }
 }
 

@@ -122,11 +122,13 @@ class Engine:
         return int((l // np.uint64(m)).sum()) + len(l) + 1
 
     @staticmethod
-    def _opts(digest_set, forced, xxh3=None):
-        """pbsgpu_batch_opts; `forced` = (stream u32[], offset u64[]) suggested boundaries sorted by (stream, offset)."""
+    def _opts(digest_set, forced, xxh3=None, crypt=None):
+        """pbsgpu_batch_opts; `forced` = (stream u32[], offset u64[]) suggested boundaries sorted by (stream, offset);
+        `crypt` (a Crypt) = keyed digests of encrypt mode."""
         o = BatchOpts()
         o.size = C.sizeof(BatchOpts)
         o.set = digest_set._h if digest_set is not None else None
+        o.crypt = crypt._h if crypt is not None else None
         keep = []
         if forced is not None:
             fs = np.ascontiguousarray(forced[0], dtype=np.uint32)
@@ -140,22 +142,24 @@ class Engine:
         return o, keep
 
     def chunk_digest_batch(self, cfg: Cfg, base, off, length, digest_set: "DigestSet | None" = None,
-                           forced=None) -> np.ndarray:
+                           forced=None, crypt: "Crypt | None" = None) -> np.ndarray:
         """stream -> chunks -> digests for n streams; `base` device (tensor/int) or host (numpy).
         Replaces n calls of writer.WriteEntryReader (reference commit.go:720).  `forced` = optional suggested
-        boundaries (stream[], offset[]): file starts of a pxar payload stream (pxarfs.go:408-411)."""
+        boundaries (stream[], offset[]): file starts of a pxar payload stream (pxarfs.go:408-411).  `crypt`: keyed
+        digests SHA-256(chunk || id_key) of encrypt mode, also for the set's probe + insert."""
         o, l = self._offlen(off, length)
         cap = self._chunk_cap(cfg, l) + (len(forced[0]) if forced is not None else 0)
         out = np.zeros(cap, dtype=CHUNK_DTYPE)
         n_out = C.c_uint64()
         keep = base  # keep the buffer alive for the duration of the call
-        opts, _k = self._opts(digest_set, forced)
+        opts, _k = self._opts(digest_set, forced, crypt=crypt)
         self._ck(self._L.pbsgpu_chunk_digest_batch_ex(
             self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o), C.byref(opts), out.ctypes.data, cap,
             C.byref(n_out)))
         return out[: n_out.value]
 
-    def chunk_digest_batch_xxh3(self, cfg: Cfg, base, off, length, digest_set: "DigestSet | None" = None):
+    def chunk_digest_batch_xxh3(self, cfg: Cfg, base, off, length, digest_set: "DigestSet | None" = None,
+                                crypt: "Crypt | None" = None):
         """chunk_digest_batch plus the XXH3-64 of every stream from the same staged bytes (f2: the per-file
         hash of emitBackedFile, reference commit.go:717-725).  Returns (chunks, xxh3[n] uint64)."""
         o, l = self._offlen(off, length)
@@ -164,9 +168,15 @@ class Engine:
         hashes = np.zeros(len(o), dtype=np.uint64)
         n_out = C.c_uint64()
         keep = base
-        self._ck(self._L.pbsgpu_chunk_digest_batch_xxh3(
-            self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o),
-            digest_set._h if digest_set is not None else None, out.ctypes.data, cap, C.byref(n_out), hashes.ctypes.data))
+        if crypt is None:
+            self._ck(self._L.pbsgpu_chunk_digest_batch_xxh3(
+                self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o),
+                digest_set._h if digest_set is not None else None, out.ctypes.data, cap, C.byref(n_out), hashes.ctypes.data))
+        else:
+            opts, _k = self._opts(digest_set, None, hashes, crypt)
+            self._ck(self._L.pbsgpu_chunk_digest_batch_ex(
+                self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o), C.byref(opts), out.ctypes.data,
+                cap, C.byref(n_out)))
         return out[: n_out.value], hashes
 
     def chunk_digest_streams(self, cfg: Cfg, streams: Iterable[np.ndarray], digest_set=None) -> np.ndarray:
@@ -184,14 +194,14 @@ class Engine:
         return self.chunk_digest_batch(cfg, buf, offs, lens, digest_set)
 
     def submit(self, cfg: Cfg, base_dev, off, length, digest_set: "DigestSet | None" = None, forced=None,
-               early_input: bool = False) -> "Job":
+               early_input: bool = False, crypt: "Crypt | None" = None) -> "Job":
         """Asynchronous form; with `digest_set` the probe + insert runs as kernels on the job's stream (jobs sharing a
         set are ordered in submission order) and the KNOWN flags come back with the records.  `early_input`
         (PBSGPU_BATCH_EARLY_INPUT): the long chunks are copied aside so that Job.wait_input() gives the buffer back
-        long before the records are ready."""
+        long before the records are ready.  `crypt`: keyed digests (as chunk_digest_batch)."""
         o, l = self._offlen(off, length)
         h = C.c_void_p()
-        opts, _k = self._opts(digest_set, forced)
+        opts, _k = self._opts(digest_set, forced, crypt=crypt)
         if early_input:
             opts.flags |= _lib.BATCH_EARLY_INPUT
         self._ck(self._L.pbsgpu_batch_submit_ex(self._h, C.byref(cfg), _ptr(base_dev), o.ctypes.data, l.ctypes.data,
@@ -215,6 +225,14 @@ class Engine:
         out = np.zeros((len(o), 32), dtype=np.uint8)
         self._ck(self._L.pbsgpu_sha256_batch(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o),
                                              out.ctypes.data))
+        return out
+
+    def sha256_keyed_batch(self, crypt: "Crypt", base, off, length) -> np.ndarray:
+        """Encrypt mode's keyed digests SHA-256(range || id_key) of n byte ranges; returns (n, 32) uint8."""
+        o, l = self._offlen(off, length)
+        out = np.zeros((len(o), 32), dtype=np.uint8)
+        self._ck(self._L.pbsgpu_sha256_keyed_batch(self._h, crypt._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o),
+                                                   out.ctypes.data))
         return out
 
     # -- f2: per-file content hash of the commit walk ---------------------------------------------
@@ -278,6 +296,33 @@ class Engine:
         crc = np.zeros(len(o), dtype=np.uint32)
         self._ck(fn(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o), out.ctypes.data, boff.ctypes.data,
                     blen.ctypes.data, crc.ctypes.data))
+        return [out[int(boff[i]): int(boff[i]) + int(blen[i])].tobytes() for i in range(len(o))], crc
+
+    # -- f3, encrypt mode -----------------------------------------------------------------------
+    def crypt(self, key: bytes) -> "Crypt":
+        """Handle for one 32-byte AES-256 key (pbsgpu_crypt_create); close() zeroes its key material."""
+        return Crypt(self, key)
+
+    def blob_encode_batch_enc(self, crypt: "Crypt", mode: str, base, off, length, iv: bytes):
+        """Encrypted DataBlobs (AES-256-GCM, pbsgpu_blob_encode_batch_enc) of n ranges: the payload is `mode`'s zstd
+        frame ("z", "lz", "lze", "lzh") where smaller, else the raw chunk ("raw": always).  `iv` holds n x 16 bytes, one
+        IV per blob; an IV must never be used twice under one key (draw them with os.urandom).
+        -> list of n `bytes` blobs, crc[n]."""
+        o, l = self._offlen(off, length)
+        ivs = np.frombuffer(bytes(iv), dtype=np.uint8)
+        if len(ivs) != 16 * len(o):
+            raise ValueError("iv must hold 16 bytes per range")
+        if mode not in BLOB_MODES or mode is None:
+            raise ValueError(f"unknown blob mode {mode!r}")
+        sizes = l + np.uint64(44)
+        boff = np.zeros(len(o) + 1, dtype=np.uint64)
+        np.cumsum(sizes, out=boff[1:])
+        out = np.zeros(max(1, int(boff[-1])), dtype=np.uint8)
+        blen = np.zeros(len(o), dtype=np.uint64)
+        crc = np.zeros(len(o), dtype=np.uint32)
+        self._ck(self._L.pbsgpu_blob_encode_batch_enc(self._h, crypt._h, BLOB_MODES[mode], _ptr(base), o.ctypes.data,
+                                                      l.ctypes.data, len(o), ivs.ctypes.data, out.ctypes.data,
+                                                      boff.ctypes.data, blen.ctypes.data, crc.ctypes.data))
         return [out[int(boff[i]): int(boff[i]) + int(blen[i])].tobytes() for i in range(len(o))], crc
 
     def blob_header(self, crc: int) -> bytes:
@@ -377,6 +422,36 @@ class Job:
         if self._h is not None:
             self._eng._L.pbsgpu_batch_free(self._h)
             self._h, self._keep = None, None
+
+
+class Crypt:
+    """One AES-256 key of encrypt mode on the engine's device (pbsgpu_crypt_create / _destroy)."""
+
+    def __init__(self, eng: Engine, key: bytes):
+        k = np.frombuffer(bytes(key), dtype=np.uint8)
+        if len(k) != 32:
+            raise ValueError("the key must be 32 bytes")
+        self._eng = eng
+        h = C.c_void_p()
+        eng._ck(eng._L.pbsgpu_crypt_create(eng._h, k.ctypes.data, C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None) and self._eng._h:
+            self._eng._L.pbsgpu_crypt_destroy(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
 
 
 class DigestSet:
@@ -505,10 +580,21 @@ class Stream:
             raise ValueError(f"blob mode must be one of {list(BLOB_MODES)}, not {mode!r}")
         self._eng._ck(self._eng._L.pbsgpu_stream_blob_mode(self._h, BLOB_MODES[mode]))
 
+    def crypt(self, crypt: "Crypt", iv_seed: bytes | None = None):
+        """Encrypt mode (pbsgpu_stream_crypt), set before the first byte: keyed digests, and encrypted blobs whose IVs
+        come from the OS CSPRNG -- or, with a 32-byte `iv_seed` (tests), IV_k = SHA-256(iv_seed || k u64 LE)[:16]."""
+        seed = None
+        if iv_seed is not None:
+            seed = np.frombuffer(bytes(iv_seed), dtype=np.uint8)
+            if len(seed) != 32:
+                raise ValueError("iv_seed must be 32 bytes")
+        self._crypt = crypt   # the handle must outlive the stream
+        self._eng._ck(self._eng._L.pbsgpu_stream_crypt(self._h, crypt._h, seed.ctypes.data if seed is not None else None))
+
     def poll_blobs(self, out_cap: int = 0) -> list[bytes]:
         """Every blob available now, in order: blob k belongs to the k-th record without CHUNK_KNOWN."""
         L = self._eng._L
-        want = max(int(out_cap), int(L.pbsgpu_blob_size(self._max)), 1 << 24)
+        want = max(int(out_cap), int(L.pbsgpu_blob_size_enc(self._max)), 1 << 24)
         if getattr(self, "_blob_buf", None) is None or len(self._blob_buf) < want:
             self._blob_buf = np.empty(want, dtype=np.uint8)
         out = self._blob_buf

@@ -23,6 +23,7 @@ Two writers:
 from __future__ import annotations
 
 import io
+import os
 from collections import deque
 from dataclasses import dataclass, field
 from typing import BinaryIO, Callable
@@ -63,6 +64,9 @@ class DedupWriter:
     # "lze": those blocks also through zstd's entropy stage (pbsgpu_blob_encode_batch_lze); "lzh": with Huffman literals
     # whatever their largest value, for binary data (pbsgpu_blob_encode_batch_lzh)
     blob_compression: str = "z"
+    # encrypt mode (CryptMode encrypt, commit.go:314): the 32-byte client key.  Digests become keyed (SHA-256(chunk ||
+    # id_key)) and upload_blob receives encrypted blobs (pbsgpu_blob_encode_batch_enc, IVs from os.urandom)
+    crypt_key: bytes | None = None
     index: list[IndexRecord] = field(default_factory=list)
     # relPath -> XXH3-64 of the file as uploaded: commitWalkState.backedHashes (commit.go:187, :725), computed on the
     # GPU from the same staged bytes instead of through an io.TeeReader on the host
@@ -70,9 +74,12 @@ class DedupWriter:
     _pending: list[tuple[Entry, np.ndarray]] = field(default_factory=list)
     _pending_bytes: int = 0
     _finished: bool = False
+    _crypt: object = None
 
     def __post_init__(self):
         _check_blob_compression(self.blob_compression)
+        if self.crypt_key is not None:
+            self._crypt = self.engine.crypt(self.crypt_key)
 
     def WriteEntryReader(self, entry: Entry, reader: BinaryIO, size: int) -> None:
         """Pulls exactly `size` bytes from `reader` (error if it yields fewer, like io.ReadFull)."""
@@ -94,7 +101,8 @@ class DedupWriter:
             return
         entries, arrs = zip(*self._pending)
         buf, offs, lens = self._pack(arrs)
-        rec, hashes = self.engine.chunk_digest_batch_xxh3(self.config, buf, offs, lens, self.known)
+        keyed = {"crypt": self._crypt} if self._crypt is not None else {}
+        rec, hashes = self.engine.chunk_digest_batch_xxh3(self.config, buf, offs, lens, self.known, **keyed)
         for e, h in zip(entries, hashes):
             self.backed_hashes[e.Path] = int(h)
         new_chunks = []                                   # (digest, stream, start, end) of the chunks the server lacks
@@ -113,8 +121,12 @@ class DedupWriter:
         if self.upload_blob is not None and new_chunks:
             boff = np.array([int(offs[i]) + s0 for _, i, s0, _ in new_chunks], dtype=np.uint64)
             blen = np.array([e0 - s0 for _, _, s0, e0 in new_chunks], dtype=np.uint64)
-            encode = getattr(self.engine, "blob_encode_batch_" + self.blob_compression)
-            blobs, _crc = encode(buf, boff, blen)
+            if self._crypt is not None:
+                blobs, _crc = self.engine.blob_encode_batch_enc(self._crypt, self.blob_compression, buf, boff, blen,
+                                                                os.urandom(16 * len(boff)))
+            else:
+                encode = getattr(self.engine, "blob_encode_batch_" + self.blob_compression)
+                blobs, _crc = encode(buf, boff, blen)
             for (d, _i, _s, _e), blob in zip(new_chunks, blobs):
                 self.upload_blob(d, blob)
         self._pending, self._pending_bytes = [], 0
@@ -177,6 +189,9 @@ class PayloadStreamWriter:
     # (pbsgpu_stream_hash_range).  Off by default: a stream with no hash ranges does no hashing work.
     hash_files: bool = False
     backed_hashes: dict[str, int] = field(default_factory=dict)
+    # encrypt mode: the 32-byte client key (as DedupWriter.crypt_key); the stream draws the blobs' IVs from the OS CSPRNG
+    crypt_key: bytes | None = None
+    _crypt: object = None
     _stream: object = None
     _seg_base: int = 0               # offset in the new stream at which the current pbsgpu stream starts
     _last_ref: int = -1
@@ -187,12 +202,16 @@ class PayloadStreamWriter:
 
     def __post_init__(self):
         _check_blob_compression(self.blob_compression)
+        if self.crypt_key is not None:
+            self._crypt = self.engine.crypt(self.crypt_key)
         self._open()
         self._raw(PXAR_PAYLOAD_START_MARKER.to_bytes(8, "little") + (16).to_bytes(8, "little"))
 
     # -- plumbing ---------------------------------------------------------------------------------------------
     def _open(self):
         self._stream = self.engine.stream(self.config, self.known)
+        if self._crypt is not None:
+            self._stream.crypt(self._crypt)
         if self.upload_blob is not None:
             self._stream.blob_mode(self.blob_compression)
 

@@ -170,11 +170,11 @@ static ShaArgs sha_args(const Work &w) {
 }
 template <int M> static void prod_tuned(const Work &w) {
     pbsgpu::Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
-    pbsgpu::k_sha_tuned<M><<<(w.n + 31) / 32, 32>>>(sha_args(w), o);
+    pbsgpu::k_sha_tuned<M, false><<<(w.n + 31) / 32, 32>>>(sha_args(w), o, nullptr);
 }
 template <int P, int C> static void prod_split(const Work &w) {
     pbsgpu::Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
-    pbsgpu::k_sha_split<P, C><<<(w.n + 31) / 32, 64>>>(sha_args(w), o);
+    pbsgpu::k_sha_split<P, C, false><<<(w.n + 31) / 32, 64>>>(sha_args(w), o, nullptr);
 }
 
 static const Variant VS[] = {
