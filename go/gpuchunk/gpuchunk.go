@@ -376,8 +376,8 @@ func (st *Stream) Finish() ([]Chunk, error) {
 
 func (st *Stream) Close() { C.pbsgpu_stream_close(st.s) }
 
-// Blob modes of SetBlobMode: the encoders of Batch.BlobEncode, BlobEncodeZ, BlobEncodeLZ, BlobEncodeLZE and
-// BlobEncodeLZH.
+// Blob modes of SetBlobMode: the encoders of Batch.BlobEncode, BlobEncodeZ, BlobEncodeLZ, BlobEncodeLZE,
+// BlobEncodeLZH and BlobEncodeLZL (its value is 7; 6 is not assigned).
 const (
 	BlobNone = C.PBSGPU_BLOB_NONE
 	BlobRaw  = C.PBSGPU_BLOB_RAW
@@ -385,6 +385,7 @@ const (
 	BlobLZ   = C.PBSGPU_BLOB_LZ
 	BlobLZE  = C.PBSGPU_BLOB_LZE
 	BlobLZH  = C.PBSGPU_BLOB_LZH
+	BlobLZL  = C.PBSGPU_BLOB_LZL
 )
 
 // SetBlobMode makes the stream encode a DataBlob for every new chunk on the GPU (before the first byte).
@@ -693,6 +694,14 @@ func (b *Batch) BlobEncodeLZH(off, length []uint64) ([][]byte, error) {
 	return b.blobEncodeCompressed(off, length, blobLZH)
 }
 
+// BlobEncodeLZL is BlobEncodeLZH plus long-distance matches: repeats anywhere earlier in the same chunk (a copy of a
+// file inside one chunk, repeated pages of an image) become long matches of the blocks they cross, where that makes the
+// block smaller.  Each blob is at most the size of its BlobEncodeLZH blob.  Like the rest of this shim, it has not been
+// compiled against a Go toolchain.
+func (b *Batch) BlobEncodeLZL(off, length []uint64) ([][]byte, error) {
+	return b.blobEncodeCompressed(off, length, blobLZL)
+}
+
 // which compressed DataBlob encoder blobEncodeCompressed calls
 type blobMode int
 
@@ -701,6 +710,7 @@ const (
 	blobLZ
 	blobLZE
 	blobLZH
+	blobLZL
 )
 
 func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]byte, error) {
@@ -721,6 +731,8 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]b
 	dst := (*C.uint8_t)(unsafe.Pointer(&out[0]))
 	var rc C.int
 	switch mode {
+	case blobLZL:
+		rc = C.pbsgpu_blob_encode_batch_lzl(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	case blobLZH:
 		rc = C.pbsgpu_blob_encode_batch_lzh(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	case blobLZE:
@@ -758,7 +770,7 @@ func (c *Crypt) Close() { C.pbsgpu_crypt_destroy(c.c) }
 // library draws from the OS CSPRNG.
 func (st *Stream) SetCrypt(c *Crypt) error { return st.e.err(C.pbsgpu_stream_crypt(st.s, c.c, nil)) }
 
-// BlobEncodeEnc returns encrypted DataBlobs of the ranges: mode (BlobRaw .. BlobLZH) picks the compressor whose frame
+// BlobEncodeEnc returns encrypted DataBlobs of the ranges: mode (BlobRaw .. BlobLZH, BlobLZL) picks the compressor whose frame
 // is encrypted when smaller.  Every blob gets a fresh IV from crypto/rand; an IV must never repeat under one key.
 func (b *Batch) BlobEncodeEnc(c *Crypt, mode int, off, length []uint64) ([][]byte, error) {
 	n := len(off)

@@ -222,13 +222,13 @@ int pbsgpu_stream_suggest(pbsgpu_stream *s, uint64_t offset);
 /* Bytes written so far (= the payload offset the next entry will get in the mpxar PAYLOAD_REF). */
 uint64_t pbsgpu_stream_position(const pbsgpu_stream *s);
 /* DataBlobs of the stream's NEW chunks, encoded on the device from the window that holds them.  The mode is set before
- * the first byte (PBSGPU_ESTATE after that) and has the meaning of pbsgpu_blob_encode_batch (RAW), _z, _lz, _lze and _lzh;
- * NONE, the default, encodes nothing.  Blob k belongs to the k-th record without PBSGPU_CHUNK_KNOWN in poll() order, so
+ * the first byte (PBSGPU_ESTATE after that) and has the meaning of pbsgpu_blob_encode_batch (RAW), _z, _lz, _lze, _lzh
+ * and _lzl (LZL = 7; the value 6 is not assigned and is rejected); NONE, the default, encodes nothing.  Blob k belongs to the k-th record without PBSGPU_CHUNK_KNOWN in poll() order, so
  * with a digest set every new digest gets exactly one blob.  A window's blobs become available when its records do, all
  * of them after finish().  poll_blobs copies whole blobs back to back into out[0, out_cap) and their lengths into
  * blob_len[0, cap); out_cap must be at least pbsgpu_blob_size(cfg.max), so every call makes progress. */
 enum { PBSGPU_BLOB_NONE = 0, PBSGPU_BLOB_RAW = 1, PBSGPU_BLOB_Z = 2, PBSGPU_BLOB_LZ = 3, PBSGPU_BLOB_LZE = 4,
-       PBSGPU_BLOB_LZH = 5 };
+       PBSGPU_BLOB_LZH = 5, PBSGPU_BLOB_LZL = 7 };
 int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode);
 int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
                              uint64_t *n_out);
@@ -338,6 +338,15 @@ int pbsgpu_blob_encode_batch_lze(pbsgpu_ctx *ctx, const void *base, const uint64
  * of the chunk bytes. */
 int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                  uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+/* pbsgpu_blob_encode_batch_lzh plus long-distance matches: repeats anywhere earlier in the same chunk (up to 2^24 - 4
+ * bytes back), such as copies of a file inside one chunk or repeated pages of an image, which the block-local parse of
+ * _lzh cannot see.  Anchors of a content-defined 64-byte hash are paired with the latest earlier anchor of the same
+ * hash, verified and extended; the kept matches (>= 64 bytes, no overlap) become long spans of the blocks they cross,
+ * and a block with spans is parsed again around them.  Each Compressed_Block is the smaller of the _lzh content and the
+ * span parse's (_lzh on ties), and no block refers to another's state, so each blob is at most the size of its _lzh
+ * blob.  Same arguments, limits and errors as _lzh.  The output is a deterministic function of the chunk bytes. */
+int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                 uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 
 /* ---- f3, encrypt mode (BackupConfig's CryptMode, commit.go:314): encrypted DataBlobs ------------------------------
  * A crypt handle holds one 32-byte AES-256 key (the caller hands over the raw key bytes; key files are not read here).
@@ -351,8 +360,8 @@ int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64
  * IVs: iv holds n x 16 bytes, one per blob, supplied by the caller, so the output is a pure function of the inputs.
  * GCM's security rests on never using one IV twice under one key: draw every IV from a CSPRNG (upstream draws them at
  * random) and never reuse one.  The library never generates or stores IVs.
- * mode: PBSGPU_BLOB_RAW (encrypt every chunk uncompressed) or PBSGPU_BLOB_Z .. PBSGPU_BLOB_LZH (the compressor whose frame
- * is used when smaller).  Blob i goes to out + out_off[i] (HOST memory), which must hold pbsgpu_blob_size_enc(len[i])
+ * mode: PBSGPU_BLOB_RAW (encrypt every chunk uncompressed) or PBSGPU_BLOB_Z .. PBSGPU_BLOB_LZH, PBSGPU_BLOB_LZL (the
+ * compressor whose frame is used when smaller).  Blob i goes to out + out_off[i] (HOST memory), which must hold pbsgpu_blob_size_enc(len[i])
  * bytes; out_len[i] receives its size.  base is HOST or DEVICE; ranges < 2^36 bytes.  crc_out may be NULL. */
 /* create also derives the id_key of keyed digests: PBKDF2-HMAC-SHA256(password = key, salt = "_id_key", 10 iterations,
  * 32 bytes), as upstream CryptConfig::new. */

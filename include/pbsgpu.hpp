@@ -160,7 +160,7 @@ class DedupWriter {
 // Start marker, then per file a 16-byte PAYLOAD header + content (reference internal/pxarmount/pxarfs.go:408-411),
 // chunker state carried across files, a suggested boundary at every file start, bytes read straight into the
 // library's pinned ring.  WriteEntryReader (commit.go:720) returns the entry's payload offset.
-// Optional: `blob_mode` (PBSGPU_BLOB_RAW .. _LZH) hands the DataBlob of every new chunk to `upload_blob(digest, blob,
+// Optional: `blob_mode` (PBSGPU_BLOB_RAW .. _LZH, _LZL) hands the DataBlob of every new chunk to `upload_blob(digest, blob,
 // len)`, encoded on the GPU from the stream's windows; `hash_files` records every file's XXH3-64 in BackedHashes()
 // (commitWalkState.backedHashes, commit.go:725); `crypt` gives keyed digests and encrypted blobs, their IVs drawn from the
 // OS CSPRNG by the stream.

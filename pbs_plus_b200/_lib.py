@@ -37,7 +37,7 @@ CHUNK_DTYPE = np.dtype([("stream", "<u4"), ("flags", "<u4"), ("end_off", "<u8"),
 assert CHUNK_DTYPE.itemsize == C.sizeof(Chunk) == 48
 CHUNK_KNOWN = 1
 # pbsgpu_stream_blob_mode: the DataBlob encoder of a stream's new chunks (None = no blobs)
-BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5}
+BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5, "lzl": 7}   # 6 is not assigned
 
 
 class DevInfo(C.Structure):
@@ -83,7 +83,7 @@ SYMBOLS = [
     "pbsgpu_set_allgather", "pbsgpu_nccl_unique_id", "pbsgpu_nccl_comm_create", "pbsgpu_nccl_comm_destroy",
     "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
-    "pbsgpu_blob_encode_batch_lzh", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
+    "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
     "pbsgpu_blob_encode_batch_enc",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
@@ -159,6 +159,7 @@ def lib() -> C.CDLL:
     L.pbsgpu_blob_encode_batch_lz.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lze.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lzh.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.pbsgpu_blob_encode_batch_lzl.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
     L.pbsgpu_crypt_destroy.argtypes = [vp]
     L.pbsgpu_crypt_destroy.restype = None

@@ -211,8 +211,90 @@ static int crc_where(pbsgpu_ctx *ctx, const std::vector<uint8_t> &comp, uint8_t 
 }
 
 // Which DataBlob encoder a call is: uncompressed only, RLE / raw frames (_z), with the match stage (_lz), with the match
-// and entropy stages (_lze), and with Huffman literals over every byte value (_lzh).
-enum class BlobMode { raw, z, lz, lze, lzh };
+// and entropy stages (_lze), with Huffman literals over every byte value (_lzh), and _lzh with long-distance matches
+// across the whole chunk (_lzl).
+enum class BlobMode { raw, z, lz, lze, lzh, lzl };
+// the encoders by their PBSGPU_BLOB_* value (PBSGPU_BLOB_RAW ..); value 6 is not assigned
+static bool blob_mode_of(int mode, BlobMode *m) {
+    static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze, BlobMode::lzh};
+    if (mode >= PBSGPU_BLOB_RAW && mode <= PBSGPU_BLOB_LZH) { *m = modes[mode - PBSGPU_BLOB_RAW]; return true; }
+    if (mode == PBSGPU_BLOB_LZL) { *m = BlobMode::lzl; return true; }
+    return false;
+}
+
+// K12: the long spans of the blocks that are not constant (z = their index in the match stage's list), in order: span
+// block y is block span_z[y], with the spans spans[span_first[y] .. span_first[y + 1]) (zlz.cuh's packing).  The kept
+// long matches come per pass of whole chunks (LDM_PASS_BYTES, or one longer chunk); each is split at the block edges,
+// and pieces in constant blocks or shorter than LZ_MINMATCH are dropped.
+static int ldm_spans_of(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n,
+                        const std::vector<uint64_t> &blk_first, const std::vector<int64_t> &zof, std::vector<uint32_t> &span_z,
+                        std::vector<uint32_t> &span_first, std::vector<uint64_t> &spans) {
+    pbsgpu_ctx *ctx = b.ctx;
+    std::vector<uint64_t> sfirst(n + 1), vfirst(n + 1);
+    std::vector<uint32_t> pass_c0;
+    for (uint32_t i = 0; i < n; i++) {
+        sfirst[i + 1] = sfirst[i] + ldm_spans(len[i]);
+        vfirst[i + 1] = vfirst[i] + len[i];
+    }
+    for (uint32_t i = 0; i < n; i++)
+        if (pass_c0.empty() || vfirst[i + 1] - vfirst[pass_c0.back()] > LDM_PASS_BYTES || i - pass_c0.back() >= LDM_PASS_CHUNKS)
+            pass_c0.push_back(i);
+    pass_c0.push_back(n);
+    const uint32_t np = (uint32_t)pass_c0.size() - 1;
+    if (sfirst[n] == 0) return PBSGPU_OK;
+    uint64_t *d_sfirst = b.upload(sfirst.data(), n + 1), *d_vfirst = b.upload(vfirst.data(), n + 1);
+    uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n);
+    unsigned long long *d_tot = b.get<unsigned long long>(np);
+    if (!d_sfirst || !d_vfirst || !d_off || !d_len || !d_tot) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    auto pass = [&](uint32_t p) {
+        const uint32_t c0 = pass_c0[p], c1 = pass_c0[p + 1];
+        return LdmArgs{dbase, d_off, d_len, d_sfirst, d_vfirst, c0, c1, sfirst[c0], sfirst[c1]};
+    };
+    // K12a over every pass: the anchor counts size the scratch
+    std::vector<unsigned long long> tot(np);
+    if (b.ok()) b.e = cudaMemsetAsync(d_tot, 0, np * sizeof(unsigned long long), b.st);
+    for (uint32_t p = 0; b.ok() && p < np; p++) b.e = launch_ldm_count(pass(p), d_tot + p, b.st);
+    if (b.ok()) b.e = cudaMemcpyAsync(tot.data(), d_tot, np * sizeof(unsigned long long), cudaMemcpyDeviceToHost, b.st);
+    if (int rc = b.finish("ldm anchor count")) return rc;
+    size_t scratch_bytes = 0;
+    for (uint32_t p = 0; p < np; p++) {
+        if (tot[p] >= (1ull << 31)) return fail(ctx, PBSGPU_EINVAL, "more than 2^31 long-match anchors in one chunk");
+        scratch_bytes = std::max(scratch_bytes, ldm_scratch_bytes(pass(p).s1 - pass(p).s0, tot[p]));
+    }
+    uint8_t *scratch = b.get<uint8_t>(scratch_bytes);
+    if (!scratch) return fail(ctx, PBSGPU_ENOMEM, "long-match scratch of %llu bytes failed", (unsigned long long)scratch_bytes);
+    // K12 per pass; the kept matches as (chunk, start, end, offset)
+    struct Kept { uint64_t chunk, s, e, d; };
+    std::vector<Kept> kept;
+    std::vector<uint64_t> hk, hv;
+    for (uint32_t p = 0; p < np; p++) {
+        if (tot[p] < 2) continue;
+        uint64_t *dk, *dv;
+        uint32_t *dn, nk = 0;
+        b.e = launch_ldm_matches(pass(p), tot[p], scratch, &dk, &dv, &dn, b.st);
+        if (b.ok()) b.e = cudaMemcpyAsync(&nk, dn, 4, cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("ldm matches")) return rc;
+        hk.resize(nk); hv.resize(nk);
+        if (nk && b.ok()) b.e = cudaMemcpyAsync(hk.data(), dk, nk * 8ull, cudaMemcpyDeviceToHost, b.st);
+        if (nk && b.ok()) b.e = cudaMemcpyAsync(hv.data(), dv, nk * 8ull, cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("ldm matches")) return rc;
+        for (uint32_t k = 0; k < nk; k++)
+            kept.push_back({pass_c0[p] + (hk[k] >> 40), hk[k] & LDM_M40, hv[k] & LDM_M40, hv[k] >> 40});
+    }
+    std::sort(kept.begin(), kept.end(), [](const Kept &x, const Kept &y) { return x.chunk != y.chunk ? x.chunk < y.chunk : x.s < y.s; });
+    span_first.assign(1, 0);
+    for (const Kept &m : kept) {
+        for (uint64_t k = m.s / ZFRAME_BLOCK; k <= (m.e - 1) / ZFRAME_BLOCK; k++) {
+            const uint64_t ps = std::max<uint64_t>(m.s, k * ZFRAME_BLOCK), pe = std::min<uint64_t>(m.e, (k + 1) * ZFRAME_BLOCK);
+            const int64_t z = zof[blk_first[m.chunk] + k];
+            if (z < 0 || pe - ps < LZ_MINMATCH) continue;
+            if (span_z.empty() || span_z.back() != (uint32_t)z) { span_z.push_back((uint32_t)z); span_first.push_back(span_first.back()); }
+            spans.push_back((ps - k * ZFRAME_BLOCK) | (pe - ps) << 20 | m.d << 40);
+            span_first.back()++;
+        }
+    }
+    return PBSGPU_OK;
+}
 
 // Compressed form: a blob's payload is a zstd frame when that is smaller than the raw bytes (upstream
 // `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device (zframe.cu, zlz.cu,
@@ -238,39 +320,68 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
     if (b.ok() && n_blocks) b.e = cudaMemcpyAsync(flags.data(), d_flags, n_blocks * 4, cudaMemcpyDeviceToHost, b.st);
     if (int rc = b.finish("zstd block scan")) return rc;
     auto block_size = [&](uint32_t i, uint64_t k) { return (uint32_t)std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK); };
-    // K9 (+ K10): the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS
-    const bool ent = mode == BlobMode::lze || mode == BlobMode::lzh, lz = mode == BlobMode::lz || ent;
+    // K9 (+ K10): the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS.  With
+    // lzl, K12 first finds the long spans; the blocks that hold one are parsed again with them (K9a's span parse, K9b,
+    // K10) into slots nz + y, and each such block keeps the smaller content, K9's on ties.
+    const bool ent = mode == BlobMode::lze || mode == BlobMode::lzh || mode == BlobMode::lzl, lz = mode == BlobMode::lz || ent;
+    const bool full = mode == BlobMode::lzh || mode == BlobMode::lzl;
     std::vector<uint32_t> info;
+    std::vector<uint64_t> slot_of;   // the slot of block z's content
     const uint8_t *slots = nullptr;
     if (lz) {
         std::vector<uint64_t> zsrc;
         std::vector<uint32_t> zsize;
+        std::vector<int64_t> zof(n_blocks, -1);
         for (uint32_t i = 0; i < n; i++)
             for (uint64_t k = 0; k < blk_first[i + 1] - blk_first[i]; k++)
-                if (!(flags[blk_first[i] + k] & 0x100u)) { zsrc.push_back(off[i] + k * ZFRAME_BLOCK); zsize.push_back(block_size(i, k)); }
+                if (!(flags[blk_first[i] + k] & 0x100u)) {
+                    zof[blk_first[i] + k] = (int64_t)zsrc.size();
+                    zsrc.push_back(off[i] + k * ZFRAME_BLOCK); zsize.push_back(block_size(i, k));
+                }
         const uint64_t nz = zsrc.size();
+        std::vector<uint32_t> span_z, span_first;
+        std::vector<uint64_t> spans;
+        if (mode == BlobMode::lzl && nz)
+            if (int rc = ldm_spans_of(b, dbase, off, len, n, blk_first, zof, span_z, span_first, spans)) return rc;
+        const uint64_t ny = span_z.size();
+        for (uint64_t y = 0; y < ny; y++) { zsrc.push_back(zsrc[span_z[y]]); zsize.push_back(zsize[span_z[y]]); }
         if (nz) {
             if (int rc = upload_table_once(ctx, &ctx->d_lz_tab, sizeof(LzTables), lz_fill_tables_host)) return rc;
-            uint64_t *d_zsrc = b.upload(zsrc.data(), nz);
-            uint32_t *d_zsize = b.upload(zsize.data(), nz);
-            uint8_t *d_slots = b.get<uint8_t>(nz * LZ_SLOT);
-            uint64_t *d_seqs = b.get<uint64_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * LZ_MAX_SEQ);
-            uint32_t *d_nseq = b.get<uint32_t>(nz), *d_nlit = b.get<uint32_t>(nz), *d_info = b.get<uint32_t>(nz);
-            uint8_t *d_ent = ent ? b.get<uint8_t>(std::min<uint64_t>(nz, LZ_PASS_BLOCKS) * ENT_SCRATCH) : nullptr;
-            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info || (ent && !d_ent))
+            const uint64_t nall = nz + ny;
+            uint64_t *d_zsrc = b.upload(zsrc.data(), nall);
+            uint32_t *d_zsize = b.upload(zsize.data(), nall);
+            uint8_t *d_slots = b.get<uint8_t>(nall * LZ_SLOT);
+            uint64_t *d_seqs = b.get<uint64_t>(std::min<uint64_t>(nall, LZ_PASS_BLOCKS) * LZ_MAX_SEQ);
+            uint32_t *d_nseq = b.get<uint32_t>(nall), *d_nlit = b.get<uint32_t>(nall), *d_info = b.get<uint32_t>(nall);
+            uint8_t *d_ent = ent ? b.get<uint8_t>(std::min<uint64_t>(nall, LZ_PASS_BLOCKS) * ENT_SCRATCH) : nullptr;
+            uint64_t *d_spans = ny ? b.upload(spans.data(), spans.size()) : nullptr;
+            uint32_t *d_span_first = ny ? b.upload(span_first.data(), ny + 1) : nullptr;
+            if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info || (ent && !d_ent) ||
+                (ny && (!d_spans || !d_span_first)))
                 return fail(ctx, PBSGPU_ENOMEM, "match stage: device allocation failed");
-            for (uint64_t f = 0; b.ok() && f < nz; f += LZ_PASS_BLOCKS) {
-                const uint32_t pn = (uint32_t)std::min<uint64_t>(LZ_PASS_BLOCKS, nz - f);
-                b.e = launch_lz_parse(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit, b.st);
-                if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
-                if (b.ok() && d_ent)
-                    b.e = launch_ent_encode((const LzTables *)ctx->d_lz_tab, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
-                                            d_info, d_ent, mode == BlobMode::lzh, b.st);
-            }
-            info.resize(nz);
-            if (b.ok()) b.e = cudaMemcpyAsync(info.data(), d_info, nz * 4, cudaMemcpyDeviceToHost, b.st);
+            // the blocks [0, nz), then the span blocks [nz, nz + ny), each list in passes of its own
+            auto passes = [&](uint64_t lo, uint64_t hi, bool span_parse) {
+                for (uint64_t f = lo; b.ok() && f < hi; f += LZ_PASS_BLOCKS) {
+                    const uint32_t pn = (uint32_t)std::min<uint64_t>(LZ_PASS_BLOCKS, hi - f);
+                    b.e = span_parse ? launch_lz_parse_spans(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
+                                                             d_spans, d_span_first, nz, b.st)
+                                     : launch_lz_parse(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit, b.st);
+                    if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
+                    if (b.ok() && d_ent)
+                        b.e = launch_ent_encode((const LzTables *)ctx->d_lz_tab, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
+                                                d_info, d_ent, full, b.st);
+                }
+            };
+            passes(0, nz, false);
+            passes(nz, nall, true);
+            info.resize(nall);
+            if (b.ok()) b.e = cudaMemcpyAsync(info.data(), d_info, nall * 4, cudaMemcpyDeviceToHost, b.st);
             if (int rc = b.finish("zstd match stage")) return rc;
             slots = d_slots;
+            slot_of.resize(nz);
+            for (uint64_t z = 0; z < nz; z++) slot_of[z] = z;
+            for (uint64_t y = 0; y < ny; y++)   // a span block keeps its span parse when that is smaller
+                if ((info[nz + y] & 0x3FFFFFFFu) < (info[span_z[y]] & 0x3FFFFFFFu)) slot_of[span_z[y]] = nz + y;
         }
     }
     // every block's Block_Header (bits 0..23; the RLE byte in 24..31), body size and body source (dbase + src, or
@@ -286,8 +397,9 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
             bsrc[blk] = off[i] + k * ZFRAME_BLOCK;
             if (f & 0x100u) { type = 1; body = 1; }
             else if (lz) {
-                const uint32_t cs = info[z] & 0x3FFFFFFFu;
-                if (cs < size) { type = 2; hsize = body = cs; bsrc[blk] = (uint64_t)z * LZ_SLOT + (info[z] >> 30); }
+                const uint64_t y = slot_of[z];
+                const uint32_t cs = info[y] & 0x3FFFFFFFu;
+                if (cs < size) { type = 2; hsize = body = cs; bsrc[blk] = y * LZ_SLOT + (info[y] >> 30); }
                 z++;
             }
             bhdr[blk] = last | type << 1 | hsize << 3 | (f & 0xFFu) << 24;
@@ -378,11 +490,12 @@ static int blob_encode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, c
     return PBSGPU_OK;
 }
 
-// The stream's blob mode (capi_stream.cu): PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH are the five encoders in order.
+// The stream's blob mode (capi_stream.cu): one of the PBSGPU_BLOB_* encoders.
 int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len) {
-    static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze, BlobMode::lzh};
-    return blob_encode(ctx, base, off, len, n, modes[mode - PBSGPU_BLOB_RAW], out, out_off, out_len, nullptr);
+    BlobMode m;
+    if (!blob_mode_of(mode, &m)) return fail(ctx, PBSGPU_EINVAL, "unknown blob mode %d", mode);
+    return blob_encode(ctx, base, off, len, n, m, out, out_off, out_len, nullptr);
 }
 
 extern "C" int pbsgpu_blob_encode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
@@ -413,6 +526,12 @@ extern "C" int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, c
                                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
     return blob_encode(ctx, base, off, len, n, BlobMode::lzh, out, out_off, out_len, crc_out);
+}
+
+extern "C" int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
+    return blob_encode(ctx, base, off, len, n, BlobMode::lzl, out, out_off, out_len, crc_out);
 }
 
 // ---------------------------------------------------------------------------
@@ -543,22 +662,22 @@ extern "C" uint64_t pbsgpu_blob_size_enc(uint64_t payload_len) { return payload_
 extern "C" int pbsgpu_blob_encode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, const void *base,
                                             const uint64_t *off, const uint64_t *len, uint32_t n, const uint8_t *iv,
                                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
-    if (!ctx || !crypt || crypt->ctx != ctx || mode < PBSGPU_BLOB_RAW || mode > PBSGPU_BLOB_LZH ||
+    BlobMode bm;
+    if (!ctx || !crypt || crypt->ctx != ctx || !blob_mode_of(mode, &bm) ||
         (n && (!off || !len || !iv || !out || !out_off || !out_len || !base)))
         return PBSGPU_EINVAL;
     Guard g(ctx);
     if (n == 0) return PBSGPU_OK;
     for (uint32_t i = 0; i < n; i++)
         if (len[i] >= (1ull << 36)) return fail(ctx, PBSGPU_EINVAL, "blob %u longer than 2^36 bytes", i);
-    static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze, BlobMode::lzh};
     Blocking b(ctx, ctx->streams[0]);
     const uint8_t *dbase, *frames = nullptr;
     if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
     std::vector<uint8_t> comp(n, 0);
     std::vector<uint64_t> frame_off(n), frame_len(n);
     std::vector<uint32_t> crc(n, 0);
-    if (mode != PBSGPU_BLOB_RAW)
-        if (int rc = zstd_frames(b, dbase, off, len, n, modes[mode - PBSGPU_BLOB_RAW], comp, frame_off, frame_len, crc, &frames)) return rc;
+    if (bm != BlobMode::raw)
+        if (int rc = zstd_frames(b, dbase, off, len, n, bm, comp, frame_off, frame_len, crc, &frames)) return rc;
     // K11: payload i -> stage + c_off[i] (16 B aligned), tag i
     std::vector<GcmMsg> msg(n);
     std::vector<uint64_t> seg_first(n + 1), c_off(n), c_len(n);

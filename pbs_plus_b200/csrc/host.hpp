@@ -249,7 +249,7 @@ int pbsgpu_xxh3_enqueue(pbsgpu_ctx *ctx, const uint8_t *dbase, const uint64_t *o
 int pbsgpu_xxh3_collect(pbsgpu_ctx *ctx, XxhRun *r, uint64_t *hash_out, cudaStream_t st);
 void pbsgpu_xxh3_release(pbsgpu_ctx *ctx, XxhRun *r);
 int pbsgpu_xxh3_table(pbsgpu_ctx *ctx, const void **tab);   // K7's device table (uploaded on first use)
-// DataBlobs of n ranges with the encoder of `mode` (PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH): blob i at out + out_off[i],
+// DataBlobs of n ranges with the encoder of `mode` (PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH, PBSGPU_BLOB_LZL): blob i at out + out_off[i],
 // out_len[i] bytes.  Device ranges are encoded in place.
 int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len);

@@ -33,9 +33,14 @@ __device__ __forceinline__ uint32_t lz_key(const uint8_t *p) {
     return (uint32_t)__ldg(p) | (uint32_t)__ldg(p + 1) << 8 | (uint32_t)__ldg(p + 2) << 16 | (uint32_t)__ldg(p + 3) << 24;
 }
 
+// SPANS (the _lzl span parse): block g also has the long spans spans[span_first[g - sbase] .. span_first[g - sbase + 1]),
+// packed start | length << 20 | offset << 40 and in order.  A span is taken where it starts and the parse jumps past
+// it; a match is cut at the next span's start and kept only while it is still >= LZ_MINMATCH long.
+template <bool SPANS>
 __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, const uint64_t *src, const uint32_t *size,
                                                          uint64_t first, uint8_t *slots, uint64_t *seqs, uint32_t *nseq,
-                                                         uint32_t *nlit) {
+                                                         uint32_t *nlit, const uint64_t *spans, const uint32_t *span_first,
+                                                         uint64_t sbase) {
     __shared__ int table[1 << LZ_HBITS];
     __shared__ int cand[LZ_TILE];
     const uint64_t g = first + blockIdx.x;
@@ -49,6 +54,12 @@ __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, co
     __syncthreads();
     const uint32_t nk = S >= 4 ? S - 3 : 0;
     uint32_t pos = 0, run = 0, nl = 0, ns = 0;   // parser state (warp 0, the same in every lane)
+    uint32_t sj = 0, send = 0, ss = ~0u, sl = 0, sd = 0;   // SPANS: the next span (start ss; ~0u: none left)
+    auto next_span = [&] {
+        ss = ~0u;
+        if (sj < send) { const uint64_t v = spans[sj]; ss = v & 0xFFFFF; sl = (v >> 20) & 0xFFFFF; sd = (uint32_t)(v >> 40); }
+    };
+    if (SPANS) { sj = span_first[g - sbase]; send = span_first[g - sbase + 1]; next_span(); }
     for (uint32_t t0 = 0; t0 < nk; t0 += LZ_TILE) {
         const uint32_t tend = min(t0 + LZ_TILE, nk);
         const uint32_t i = t0 + threadIdx.x;
@@ -66,9 +77,18 @@ __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, co
         if (i < tend) atomicMax(&table[h], (int)i);
         if (parser) {
             while (pos < tend) {
+                if (SPANS && pos == ss) {
+                    if (lane == 0) sq[ns] = (uint64_t)(ss - run) | (uint64_t)sl << 20 | (uint64_t)sd << 40;
+                    ns++;
+                    pos = run = ss + sl;
+                    sj++;
+                    next_span();
+                    continue;
+                }
+                const uint32_t lim = SPANS ? min(tend, ss) : tend;
                 const uint32_t q = pos + lane;
-                const uint32_t hits = __ballot_sync(~0u, q < tend && cand[q - t0] >= 0);
-                const uint32_t m = hits ? pos + __ffs(hits) - 1 : min(pos + 32, tend);
+                const uint32_t hits = __ballot_sync(~0u, q < lim && cand[q - t0] >= 0);
+                const uint32_t m = hits ? pos + __ffs(hits) - 1 : min(pos + 32, lim);
                 if (q < m) lit[nl + lane] = __ldg(p + q);
                 nl += m - pos;
                 pos = m;
@@ -80,6 +100,15 @@ __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, co
                     const uint32_t diff = __ballot_sync(~0u, a >= S || __ldg(p + c + L + lane) != __ldg(p + a));
                     if (diff) { L += __ffs(diff) - 1; break; }
                     L += 32;
+                }
+                if (SPANS && ss != ~0u) {
+                    L = min(L, ss - m);
+                    if (L < LZ_MINMATCH) {   // too short once cut: m is a literal
+                        if (lane == 0) lit[nl] = __ldg(p + m);
+                        nl++;
+                        pos = m + 1;
+                        continue;
+                    }
                 }
                 if (lane == 0) sq[ns] = (uint64_t)(m - run) | (uint64_t)L << 20 | (uint64_t)(m - c) << 40;
                 ns++;
@@ -100,7 +129,15 @@ __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, co
 cudaError_t launch_lz_parse(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint64_t first, uint32_t nb,
                             uint8_t *slots, uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, cudaStream_t st) {
     if (nb == 0) return cudaSuccess;
-    k_lz_parse<<<nb, LZ_THREADS, 0, st>>>(base, src, size, first, slots, seqs, nseq, nlit);
+    k_lz_parse<false><<<nb, LZ_THREADS, 0, st>>>(base, src, size, first, slots, seqs, nseq, nlit, nullptr, nullptr, 0);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_lz_parse_spans(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint64_t first, uint32_t nb,
+                                  uint8_t *slots, uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, const uint64_t *spans,
+                                  const uint32_t *span_first, uint64_t sbase, cudaStream_t st) {
+    if (nb == 0) return cudaSuccess;
+    k_lz_parse<true><<<nb, LZ_THREADS, 0, st>>>(base, src, size, first, slots, seqs, nseq, nlit, spans, span_first, sbase);
     return cudaGetLastError();
 }
 

@@ -136,6 +136,11 @@ __device__ __forceinline__ void seq_bitstream(const uint64_t *sq, uint32_t n, co
 // seqs + (g - first) * LZ_MAX_SEQ, counts to nseq[g] / nlit[g].
 cudaError_t launch_lz_parse(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint64_t first, uint32_t nb,
                             uint8_t *slots, uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, cudaStream_t st);
+// K9a with long spans (the _lzl span parse): block g's spans are spans[span_first[g - sbase] .. span_first[g - sbase + 1]),
+// each start | length << 20 | offset << 40 (start and length inside the block, length >= LZ_MINMATCH), in order.
+cudaError_t launch_lz_parse_spans(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint64_t first, uint32_t nb,
+                                  uint8_t *slots, uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, const uint64_t *spans,
+                                  const uint32_t *span_first, uint64_t sbase, cudaStream_t st);
 // K9b: the Block_Content of those blocks in their slots; info[g] = content size | (offset of the content in the slot) << 30.
 // A size >= the block's size means the block stays raw (the slot then holds only its first LZ_SLOT bytes).
 cudaError_t launch_lz_encode(const LzTables *tab, uint64_t first, uint32_t nb, uint8_t *slots, const uint64_t *seqs,

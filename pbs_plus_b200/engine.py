@@ -286,6 +286,12 @@ class Engine:
         most its _lze blob (pbsgpu_blob_encode_batch_lzh) -> list of n `bytes` blobs, crc[n]."""
         return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lzh, base, off, length)
 
+    def blob_encode_batch_lzl(self, base, off, length):
+        """blob_encode_batch_lzh plus long-distance matches: repeats anywhere earlier in the same chunk (copies of a
+        file, repeated pages), found by K12 and taken by the blocks they cross where that is smaller; every blob is at
+        most its _lzh blob (pbsgpu_blob_encode_batch_lzl) -> list of n `bytes` blobs, crc[n]."""
+        return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lzl, base, off, length)
+
     def _blob_encode_sized(self, fn, base, off, length):
         o, l = self._offlen(off, length)
         sizes = l + np.uint64(12)
@@ -305,7 +311,7 @@ class Engine:
 
     def blob_encode_batch_enc(self, crypt: "Crypt", mode: str, base, off, length, iv: bytes):
         """Encrypted DataBlobs (AES-256-GCM, pbsgpu_blob_encode_batch_enc) of n ranges: the payload is `mode`'s zstd
-        frame ("z", "lz", "lze", "lzh") where smaller, else the raw chunk ("raw": always).  `iv` holds n x 16 bytes, one
+        frame ("z", "lz", "lze", "lzh", "lzl") where smaller, else the raw chunk ("raw": always).  `iv` holds n x 16 bytes, one
         IV per blob; an IV must never be used twice under one key (draw them with os.urandom).
         -> list of n `bytes` blobs, crc[n]."""
         o, l = self._offlen(off, length)
@@ -575,7 +581,7 @@ class Stream:
 
     def blob_mode(self, mode: str | None):
         """DataBlobs for the new chunks (pbsgpu_stream_blob_mode), set before the first byte: None (no blobs), "raw",
-        "z", "lz", "lze" or "lzh" -- the encoders of Engine.blob_encode_batch, _z, _lz, _lze and _lzh."""
+        "z", "lz", "lze", "lzh" or "lzl" -- the encoders of Engine.blob_encode_batch, _z, _lz, _lze, _lzh and _lzl."""
         if mode not in BLOB_MODES:
             raise ValueError(f"blob mode must be one of {list(BLOB_MODES)}, not {mode!r}")
         self._eng._ck(self._eng._L.pbsgpu_stream_blob_mode(self._h, BLOB_MODES[mode]))

@@ -62,7 +62,8 @@ class DedupWriter:
     batch_bytes: int = 1 << 30
     # "z": frames of RLE and raw blocks; "lz": also compressed blocks from the LZ77 match stage (pbsgpu_blob_encode_batch_lz);
     # "lze": those blocks also through zstd's entropy stage (pbsgpu_blob_encode_batch_lze); "lzh": with Huffman literals
-    # whatever their largest value, for binary data (pbsgpu_blob_encode_batch_lzh)
+    # whatever their largest value, for binary data (pbsgpu_blob_encode_batch_lzh); "lzl": also long matches anywhere
+    # earlier in the chunk, for repeats beyond one 128 KiB block (pbsgpu_blob_encode_batch_lzl)
     blob_compression: str = "z"
     # encrypt mode (CryptMode encrypt, commit.go:314): the 32-byte client key.  Digests become keyed (SHA-256(chunk ||
     # id_key)) and upload_blob receives encrypted blobs (pbsgpu_blob_encode_batch_enc, IVs from os.urandom)
@@ -151,8 +152,8 @@ class DedupWriter:
 
 
 def _check_blob_compression(c: str) -> None:
-    if c not in ("z", "lz", "lze", "lzh"):
-        raise ValueError(f"transfer: blob_compression must be 'z', 'lz', 'lze' or 'lzh', not {c!r}")
+    if c not in ("z", "lz", "lze", "lzh", "lzl"):
+        raise ValueError(f"transfer: blob_compression must be 'z', 'lz', 'lze', 'lzh' or 'lzl', not {c!r}")
 
 
 # pxar v2 format constants (upstream pxar crate format/mod.rs; restated, UNVERIFIED against the Go module)
@@ -181,7 +182,7 @@ class PayloadStreamWriter:
     index: list[tuple[int, bytes, bool]] = field(default_factory=list)   # (end offset in the NEW stream, digest, known)
     payload_offsets: dict[str, int] = field(default_factory=dict)        # entry path -> offset of its PAYLOAD header
     # (digest, DataBlob) for NEW chunks, encoded on the GPU from the stream's windows (pbsgpu_stream_blob_mode) with the
-    # encoder `blob_compression` names ("z", "lz", "lze" or "lzh", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
+    # encoder `blob_compression` names ("z", "lz", "lze", "lzh" or "lzl", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
     upload_blob: Callable[[bytes, bytes], None] | None = None
     blob_compression: str = "z"
     # hash_files: relPath -> XXH3-64 of every file written through WriteEntryReader in backed_hashes

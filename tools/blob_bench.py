@@ -1,9 +1,12 @@
 """f3 microbench: DataBlob assembly for 4 MiB chunks of an 8 GiB device-resident image into PINNED host memory through
-the raw C calls (no Python-side allocation or slicing inside the timed region).  Three images: random bytes with half of
-them zero runs, a text-like image (tests/zstd_lz_ref.py text_corpus, 32 MiB repeated) and a binary-like one
-(tests/zstd_huf_ref.py binary_corpus, 32 MiB repeated).  For each: GB/s of input and
-output / input of every encoder, and for context libzstd level 1 (pyarrow) on a 64 MiB host sample of the same image (8 MiB from each GiB),
-its ratio and single-thread rate on the HOST CPU."""
+the raw C calls (no Python-side allocation or slicing inside the timed region).  Four images: random bytes with half of
+them zero runs, a text-like image (tests/zstd_lz_ref.py text_corpus, 32 MiB repeated), a binary-like one
+(tests/zstd_huf_ref.py binary_corpus, 32 MiB repeated) and one with repeats far beyond one block (every 4 MiB chunk is
+4 copies of 1 MiB of binary_corpus with 2000 random byte edits, tests/zstd_ldm_ref.py repeated_image).  For each: GB/s
+of input and output / input of every encoder, and for context libzstd level 1 (pyarrow) on a 64 MiB host sample of the
+same image (8 MiB from each GiB), its ratio and single-thread rate on the HOST CPU.
+
+    python tools/blob_bench.py [call ...]     # e.g. blob_encode_batch_lzh blob_encode_batch_lzl; default: every call"""
 import subprocess
 import sys
 import time
@@ -16,6 +19,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tests"))
 import pbs_plus_b200 as pg  # noqa: E402
 import zstd_huf_ref as hufref  # noqa: E402
+import zstd_ldm_ref as ldmref  # noqa: E402
 import zstd_lz_ref as lzref  # noqa: E402
 
 print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -32,6 +36,10 @@ blen = np.zeros(len(off), dtype=np.uint64)
 crc = np.zeros(len(off), dtype=np.uint32)
 
 
+CALLS = sys.argv[1:] or ["crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz",
+                         "blob_encode_batch_lze", "blob_encode_batch_lzh", "blob_encode_batch_lzl"]
+
+
 def images():
     d = torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda")
     d[1 << 30: 5 << 30] = 0
@@ -42,13 +50,15 @@ def images():
     del tile
     tile = torch.from_numpy(hufref.binary_corpus(32 << 20, 1)).cuda()
     yield "binary-like", tile.repeat(n // len(tile))
+    del tile
+    tile = torch.from_numpy(ldmref.repeated_image(hufref.binary_corpus(1 << 20, 1))).cuda()
+    yield "repeated", tile.repeat(n // len(tile))
 
 
 for label, d in images():
     torch.cuda.synchronize()
     print(f"-- {label} image, {n / 2**30:.0f} GiB")
-    for name in ("crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz",
-                 "blob_encode_batch_lze", "blob_encode_batch_lzh"):
+    for name in CALLS:
         for rep in range(3):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
