@@ -752,6 +752,58 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]b
 	return res, nil
 }
 
+// BlobDecode checks, decodes and verifies unencrypted DataBlobs (pbsgpu_blob_decode_batch): what a restore, a mount
+// with --verify-chunks or a verify job does per chunk.  blobs are the blobs as read from the datastore; chunkLen and
+// digests come from the dynamic index (the difference of consecutive end offsets, and each entry's digest; nil digests:
+// no digest check).  wantData false is verify only: no decoded byte leaves the GPU.  Returns one PBSGPU_DEC_* status
+// per blob (0 = OK) and, with wantData, the chunks whose status is OK or BAD_DIGEST.
+func (e *Engine) BlobDecode(blobs [][]byte, chunkLen []uint64, digests [][32]byte, wantData bool) ([]int32, [][]byte, error) {
+	n := len(blobs)
+	if n == 0 {
+		return nil, nil, nil
+	}
+	var total, out uint64
+	o := make([]C.uint64_t, n)
+	l := make([]C.uint64_t, n)
+	cl := make([]C.uint64_t, n)
+	oo := make([]C.uint64_t, n)
+	for i, b := range blobs {
+		o[i], l[i], cl[i], oo[i] = C.uint64_t(total), C.uint64_t(len(b)), C.uint64_t(chunkLen[i]), C.uint64_t(out)
+		total += uint64(len(b))
+		out += chunkLen[i]
+	}
+	src := make([]byte, total+1)
+	for i, b := range blobs {
+		copy(src[uint64(o[i]):], b)
+	}
+	var dig *C.uint8_t
+	if digests != nil {
+		dig = (*C.uint8_t)(unsafe.Pointer(&digests[0][0]))
+	}
+	var dst []byte
+	var dstp *C.uint8_t
+	if wantData {
+		dst = make([]byte, out+1)
+		dstp = (*C.uint8_t)(unsafe.Pointer(&dst[0]))
+	}
+	status := make([]int32, n)
+	rc := C.pbsgpu_blob_decode_batch(e.ctx, unsafe.Pointer(&src[0]), &o[0], &l[0], C.uint32_t(n), &cl[0], dig, dstp, &oo[0],
+		(*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	if err := e.err(rc); err != nil {
+		return nil, nil, err
+	}
+	if !wantData {
+		return status, nil, nil
+	}
+	res := make([][]byte, n)
+	for i := range blobs {
+		if status[i] == int32(C.PBSGPU_DEC_OK) || status[i] == int32(C.PBSGPU_DEC_BAD_DIGEST) {
+			res[i] = dst[uint64(oo[i]) : uint64(oo[i])+chunkLen[i]]
+		}
+	}
+	return status, res, nil
+}
+
 // Crypt is one 32-byte client key of encrypt mode (BackupConfig's CryptMode, commit.go:314) on the engine's device.
 type Crypt struct{ c *C.pbsgpu_crypt }
 

@@ -348,6 +348,35 @@ int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64
 int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                  uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 
+/* ---- f3, read side: decode and verify unencrypted DataBlobs (restore, mount, verify jobs) ------------------------
+ * Blob i is [base + off[i], + len[i]) (HOST or DEVICE); its chunk has chunk_len[i] bytes (the difference of consecutive
+ * end offsets of the index, pbsgpu_didx_parse).  Per blob, the checks run in this order and the first that fails sets
+ * status[i]:
+ *   1. the magic: uncompressed or compressed blob (an encrypted magic gives PBSGPU_DEC_ENCRYPTED, any other BAD_MAGIC;
+ *      so does a blob shorter than its 12-byte header);
+ *   2. the CRC-32 of the payload against the header (BAD_CRC);
+ *   3. the decode (BAD_FRAME): an uncompressed payload is the chunk; a compressed one is one or more zstd frames
+ *      (RFC 8878), skippable frames allowed between them.  Every form of RFC 8878 3.1.1 is read; rejected are a
+ *      non-zero Dictionary_ID, reserved bits or block types, a Window_Descriptor above 2^31 bytes, a block above
+ *      Block_Maximum_Size (a Compressed_Block's content must also stay below 128 KiB), a Frame_Content_Size that
+ *      differs from the content, an offset beyond the frame's decoded bytes, invalid FSE or Huffman descriptions
+ *      (Huffman codes up to 11 bits), bitstreams with bits left over or missing, and trailing bytes;
+ *   4. the decoded size == chunk_len[i] (BAD_SIZE; also when the frames would write beyond chunk_len[i]);
+ *   5. the XXH64 content checksum of every frame that has one (BAD_CHECKSUM);
+ *   6. the SHA-256 of the chunk against digest[i] (BAD_DIGEST), when digest (n x 32 bytes) is not NULL.
+ * digest_out (n x 32, may be NULL) receives the SHA-256 of every blob whose status is OK or BAD_DIGEST.
+ * out (HOST or DEVICE; NULL = verify only, no decoded byte leaves the device): chunk i goes to out + out_off[i],
+ * chunk_len[i] bytes.  It holds the chunk when status[i] is OK or BAD_DIGEST; otherwise its contents are undefined
+ * (a DEVICE out may hold a partial decode, a HOST out is left untouched).
+ * A corrupt blob never fails the call: it only sets its own status.  Returns PBSGPU_EINVAL for bad arguments (NULL
+ * arrays, chunk_len[i] >= 2^32), ENOMEM / ECUDA for the call's own failures, 0 otherwise.  Encrypted blobs are not
+ * decrypted here. */
+enum { PBSGPU_DEC_OK = 0, PBSGPU_DEC_BAD_MAGIC, PBSGPU_DEC_BAD_CRC, PBSGPU_DEC_ENCRYPTED, PBSGPU_DEC_BAD_FRAME,
+       PBSGPU_DEC_BAD_SIZE, PBSGPU_DEC_BAD_CHECKSUM, PBSGPU_DEC_BAD_DIGEST };
+int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                             const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
+                             int32_t *status, uint8_t *digest_out);
+
 /* ---- f3, encrypt mode (BackupConfig's CryptMode, commit.go:314): encrypted DataBlobs ------------------------------
  * A crypt handle holds one 32-byte AES-256 key (the caller hands over the raw key bytes; key files are not read here).
  * create expands the key and uploads its tables to the context's device once; destroy zeroes the key material on the

@@ -38,6 +38,8 @@ assert CHUNK_DTYPE.itemsize == C.sizeof(Chunk) == 48
 CHUNK_KNOWN = 1
 # pbsgpu_stream_blob_mode: the DataBlob encoder of a stream's new chunks (None = no blobs)
 BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5, "lzl": 7}   # 6 is not assigned
+# pbsgpu_blob_decode_batch: per-blob status (PBSGPU_DEC_*)
+DEC_OK, DEC_BAD_MAGIC, DEC_BAD_CRC, DEC_ENCRYPTED, DEC_BAD_FRAME, DEC_BAD_SIZE, DEC_BAD_CHECKSUM, DEC_BAD_DIGEST = range(8)
 
 
 class DevInfo(C.Structure):
@@ -84,7 +86,7 @@ SYMBOLS = [
     "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
     "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
-    "pbsgpu_blob_encode_batch_enc",
+    "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
 ]
@@ -160,6 +162,7 @@ def lib() -> C.CDLL:
     L.pbsgpu_blob_encode_batch_lze.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lzh.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lzl.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.pbsgpu_blob_decode_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
     L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
     L.pbsgpu_crypt_destroy.argtypes = [vp]
     L.pbsgpu_crypt_destroy.restype = None

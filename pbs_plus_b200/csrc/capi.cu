@@ -241,6 +241,7 @@ static void ctx_destroy(pbsgpu_ctx *ctx) {
     if (ctx->d_crc_tables) cudaFree(ctx->d_crc_tables);
     if (ctx->d_xxh_tab) cudaFree(ctx->d_xxh_tab);
     if (ctx->d_lz_tab) cudaFree(ctx->d_lz_tab);
+    if (ctx->d_zdec_tab) cudaFree(ctx->d_zdec_tab);
     for (auto &r : ctx->arena_recs) cudaEventDestroy(r.ev);
     ctx->arena_recs.clear();
     if (ctx->arena) cudaFree(ctx->arena);

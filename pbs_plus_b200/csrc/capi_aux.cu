@@ -161,16 +161,11 @@ static void blob_header(const uint8_t magic[8], uint32_t crc, uint8_t *out) {
 }
 extern "C" void pbsgpu_blob_header(uint32_t crc, uint8_t out[12]) { blob_header(BLOB_MAGIC_UNCOMPRESSED, crc, out); }
 
-extern "C" int pbsgpu_crc32_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
-                                  uint32_t n, uint32_t *crc_out) {
-    if (!ctx || (n && (!off || !len || !crc_out))) return PBSGPU_EINVAL;
-    Guard g(ctx);
-    if (n == 0) return PBSGPU_OK;
+// K6 over the device ranges [dbase + off[i], + len[i]) into d_out[n], enqueued on b's stream
+static int crc32_enqueue(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t *d_out) {
+    pbsgpu_ctx *ctx = b.ctx;
     if (int rc = upload_table_once(ctx, &ctx->d_crc_tables, crc_tables_bytes(), crc_fill_tables_host)) return rc;
     const int crc_variant = ctx->crc_variant;   // 0 = TMA-tiled kernel (default), 1 = simple lane-strided kernel (PBSGPU_CRC_VARIANT at open)
-    Blocking b(ctx, ctx->streams[0]);
-    const uint8_t *dbase;
-    if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
     // work units: 128 KiB warp blocks (simple) or <= 576 KiB regions of the 16 B aligned body (tiled)
     const uint64_t UNIT = crc_variant ? crc_wb_bytes() : crc_region_bytes();
     std::vector<uint64_t> wb_first(n + 1);
@@ -186,11 +181,25 @@ extern "C" int pbsgpu_crc32_batch(pbsgpu_ctx *ctx, const void *base, const uint6
     }
     wb_first[n] = total;
     uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n), *d_first = b.upload(wb_first.data(), n + 1);
-    uint32_t *d_part = b.get<uint32_t>(total + 1), *d_out = b.get<uint32_t>(n);
-    if (!d_off || !d_len || !d_first || !d_part || !d_out) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    uint32_t *d_part = b.get<uint32_t>(total + 1);
+    if (!d_off || !d_len || !d_first || !d_part) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
     if (b.ok())
         b.e = crc_variant ? launch_crc32(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st)
                           : launch_crc32_tiled(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st);
+    return PBSGPU_OK;
+}
+
+extern "C" int pbsgpu_crc32_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
+                                  uint32_t n, uint32_t *crc_out) {
+    if (!ctx || (n && (!off || !len || !crc_out))) return PBSGPU_EINVAL;
+    Guard g(ctx);
+    if (n == 0) return PBSGPU_OK;
+    Blocking b(ctx, ctx->streams[0]);
+    const uint8_t *dbase;
+    if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
+    uint32_t *d_out = b.get<uint32_t>(n);
+    if (!d_out) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (int rc = crc32_enqueue(b, dbase, off, len, n, d_out)) return rc;
     if (b.ok()) b.e = cudaMemcpyAsync(crc_out, d_out, (uint64_t)n * 4, cudaMemcpyDeviceToHost, b.st);
     return b.finish("crc32 batch");
 }
@@ -532,6 +541,111 @@ extern "C" int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, c
                                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len || !base))) return PBSGPU_EINVAL;
     return blob_encode(ctx, base, off, len, n, BlobMode::lzl, out, out_off, out_len, crc_out);
+}
+
+// ---------------------------------------------------------------------------
+// f3, read side: decode and verify unencrypted DataBlobs (K6, K13, K3)
+// ---------------------------------------------------------------------------
+// The blobs are staged once; K6 takes the CRC of every payload.  Then, per pass of whole blobs (at most ZDEC_PASS_BLOBS
+// blobs and ZDEC_PASS_BYTES decoded bytes, or one longer blob), K13 decodes into the caller's device buffer or a pass
+// buffer, K3 hashes the chunks that decoded, and a host `out` receives those chunks from the pass buffer.  The host reads
+// only statuses and digests back; no decoded byte crosses PCIe unless `out` is host memory.
+extern "C" int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                        const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
+                                        int32_t *status, uint8_t *digest_out) {
+    if (!ctx || (n && (!base || !off || !len || !chunk_len || !status || (out && !out_off)))) return PBSGPU_EINVAL;
+    Guard g(ctx);
+    if (n == 0) return PBSGPU_OK;
+    for (uint32_t i = 0; i < n; i++) {
+        if (chunk_len[i] >= (1ull << 32)) return fail(ctx, PBSGPU_EINVAL, "chunk %u: chunk_len >= 2^32", i);
+        if (off[i] + len[i] < off[i]) return fail(ctx, PBSGPU_EINVAL, "blob %u: range wraps around", i);
+    }
+    if (int rc = upload_table_once(ctx, &ctx->d_zdec_tab, sizeof(ZdecTables), zdec_fill_tables_host)) return rc;
+    const bool out_dev = out && pbsgpu_is_device_ptr(out), want_sha = digest || digest_out;
+    Blocking b(ctx, ctx->streams[0]);
+    const uint8_t *dbase;
+    if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
+    // K6 over the payloads (a blob too short for its header gets an empty range; its magic check fails first)
+    std::vector<uint64_t> poff(n), plen(n);
+    for (uint32_t i = 0; i < n; i++) { poff[i] = off[i] + 12; plen[i] = len[i] >= 12 ? len[i] - 12 : 0; }
+    uint32_t *d_crc = b.get<uint32_t>(n);
+    int32_t *d_status = b.get<int32_t>(n);
+    if (!d_crc || !d_status) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (int rc = crc32_enqueue(b, dbase, poff.data(), plen.data(), n, d_crc)) return rc;
+    // passes of whole blobs
+    std::vector<uint32_t> pass_first;
+    uint64_t pass_max = 0, acc = 0, blobs_max = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (pass_first.empty() || acc + chunk_len[i] > ZDEC_PASS_BYTES || i - pass_first.back() >= ZDEC_PASS_BLOBS) {
+            pass_first.push_back(i);
+            acc = 0;
+        }
+        acc += chunk_len[i];
+        pass_max = std::max(pass_max, acc);
+        blobs_max = std::max<uint64_t>(blobs_max, i - pass_first.back() + 1);
+    }
+    pass_first.push_back(n);
+    uint8_t *pbuf = out_dev ? nullptr : b.get<uint8_t>(pass_max + 16);
+    uint8_t *lits = b.get<uint8_t>(blobs_max * ZDEC_LIT_SLOT);
+    ZdecBlob *d_blobs = b.get<ZdecBlob>(blobs_max);
+    ChunkRef *d_refs = want_sha ? b.get<ChunkRef>(blobs_max) : nullptr;
+    unsigned long long *d_nref = want_sha ? b.get<unsigned long long>(1) : nullptr;
+    uint8_t *d_dig = want_sha ? b.get<uint8_t>(blobs_max * 32) : nullptr;
+    if ((!out_dev && !pbuf) || !lits || !d_blobs || (want_sha && (!d_refs || !d_nref || !d_dig)))
+        return fail(ctx, PBSGPU_ENOMEM, "decode pass buffers (%llu bytes) failed", (unsigned long long)pass_max);
+    std::vector<ZdecBlob> zb(blobs_max);
+    std::vector<uint64_t> at(blobs_max);   // chunk k of the pass at pass base + at[k]
+    std::vector<ChunkRef> refs(blobs_max);
+    std::vector<uint32_t> ref_blob(blobs_max);
+    std::vector<uint8_t> dig(blobs_max * 32);
+    for (size_t p = 0; p + 1 < pass_first.size(); p++) {
+        const uint32_t i0 = pass_first[p], pn = pass_first[p + 1] - i0;
+        uint8_t *pbase = out_dev ? out : pbuf;
+        uint64_t cur = 0;
+        for (uint32_t k = 0; k < pn; k++) {   // the caller's places, or back to back in the pass buffer
+            const uint32_t i = i0 + k;
+            at[k] = out_dev ? out_off[i] : cur;
+            cur += chunk_len[i];
+            zb[k] = {off[i], len[i], (uint64_t)(uintptr_t)(pbase + at[k]), chunk_len[i]};
+        }
+        if (b.ok()) b.e = cudaMemcpyAsync(d_blobs, zb.data(), pn * sizeof(ZdecBlob), cudaMemcpyHostToDevice, b.st);
+        if (b.ok()) b.e = launch_zdec(dbase, d_blobs, d_crc + i0, pn, (const ZdecTables *)ctx->d_zdec_tab, lits, d_status + i0, b.st);
+        if (b.ok()) b.e = cudaMemcpyAsync(status + i0, d_status + i0, pn * sizeof(int32_t), cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("blob decode")) return rc;
+        // K3 over the chunks that decoded
+        uint32_t nr = 0;
+        for (uint32_t k = 0; want_sha && k < pn; k++)
+            if (status[i0 + k] == PBSGPU_DEC_OK) {
+                refs[nr].stream = nr; refs[nr].len = (uint32_t)chunk_len[i0 + k]; refs[nr].start = at[k];
+                ref_blob[nr++] = i0 + k;
+            }
+        if (nr) {
+            const unsigned long long hn = nr;
+            ShaArgs ha;
+            ha.base = pbase; ha.off = nullptr; ha.chunks = d_refs; ha.order = nullptr; ha.n_chunks = d_nref;
+            ha.chunk_cap = nr; ha.digests = d_dig; ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
+            if (b.ok()) b.e = cudaMemcpyAsync(d_refs, refs.data(), nr * sizeof(ChunkRef), cudaMemcpyHostToDevice, b.st);
+            if (b.ok()) b.e = cudaMemcpyAsync(d_nref, &hn, sizeof hn, cudaMemcpyHostToDevice, b.st);
+            if (b.ok()) b.e = ctx->variant == 1 ? launch_sha_simple(ha, b.st) : launch_sha_tuned(ha, ctx->tune, b.st);
+            if (b.ok()) b.e = cudaMemcpyAsync(dig.data(), d_dig, nr * 32ull, cudaMemcpyDeviceToHost, b.st);
+            if (int rc = b.finish("blob decode digests")) return rc;
+            for (uint32_t r = 0; r < nr; r++) {
+                const uint32_t i = ref_blob[r];
+                if (digest_out) memcpy(digest_out + 32ull * i, dig.data() + 32ull * r, 32);
+                if (digest && memcmp(digest + 32ull * i, dig.data() + 32ull * r, 32) != 0) status[i] = PBSGPU_DEC_BAD_DIGEST;
+            }
+        }
+        // a host `out` receives the chunks that decoded
+        if (out && !out_dev) {
+            for (uint32_t k = 0; b.ok() && k < pn; k++) {
+                const uint32_t i = i0 + k;
+                if ((status[i] == PBSGPU_DEC_OK || status[i] == PBSGPU_DEC_BAD_DIGEST) && chunk_len[i])
+                    b.e = cudaMemcpyAsync(out + out_off[i], pbuf + at[k], chunk_len[i], cudaMemcpyDeviceToHost, b.st);
+            }
+            if (int rc = b.finish("blob decode copy")) return rc;
+        }
+    }
+    return PBSGPU_OK;
 }
 
 // ---------------------------------------------------------------------------

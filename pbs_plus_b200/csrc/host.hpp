@@ -56,6 +56,7 @@ struct pbsgpu_ctx {
     void *d_crc_tables = nullptr;   // K6 tables, uploaded on first use
     void *d_xxh_tab = nullptr;      // K7 secret words, uploaded on first use
     void *d_lz_tab = nullptr;       // K9 predefined FSE tables, uploaded on first use
+    void *d_zdec_tab = nullptr;     // K13 codes and predefined FSE decoding tables, uploaded on first use
     uint32_t table_cache[256];
     bool table_valid = false;
     cudaEvent_t epoch = nullptr;   // recorded at open; kernel intervals are reported relative to it

@@ -132,6 +132,7 @@ cudaError_t launch_zframe_hdr(uint8_t *stage, const uint64_t *frame_off, const u
 #include "zlz.cuh"   // f3: LZ77 match stage + Predefined_Mode sequences (K9)
 #include "zent.cuh"  // f3: entropy stage: FSE_Compressed_Mode sequences + Huffman literals (K10)
 #include "zldm.cuh"  // f3: long-distance matches of _lzl (K12)
+#include "zdec.cuh"  // f3, read side: the zstd decoder (K13)
 namespace pbsgpu {
 
 // ---- digest set (K4) ----------------------------------------------------------------

@@ -174,12 +174,6 @@ cudaError_t launch_lz_encode(const LzTables *tab, uint64_t first, uint32_t nb, u
 }
 
 // ---- host: the predefined tables (RFC 8878 3.1.1.3.2.2 distributions, 4.1.1 table construction) ----------------------
-static const int16_t LL_NORM[36] = {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1,
-                                    1, 1, -1, -1, -1, -1};
-static const int16_t ML_NORM[53] = {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1,
-                                    1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1};
-static const int16_t OF_NORM[29] = {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1,
-                                    -1};
 static const uint32_t LL_BASE[36] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 20, 22, 24, 28, 32, 40,
                                      48, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536};
 static const uint8_t LL_BITS[36] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 3, 3, 4, 6, 7, 8, 9,
@@ -192,9 +186,9 @@ void lz_fill_tables_host(void *dst) {
     LzTables t;
     memset(&t, 0, sizeof t);
     uint8_t spread[64];
-    fse_ctable(LL_NORM, 36, 6, spread, t.ll_stab, t.ll_dnb, t.ll_dfs);
-    fse_ctable(OF_NORM, 29, 5, spread, t.of_stab, t.of_dnb, t.of_dfs);
-    fse_ctable(ML_NORM, 53, 6, spread, t.ml_stab, t.ml_dnb, t.ml_dfs);
+    fse_ctable(PREDEF_LL_NORM, 36, 6, spread, t.ll_stab, t.ll_dnb, t.ll_dfs);
+    fse_ctable(PREDEF_OF_NORM, 29, 5, spread, t.of_stab, t.of_dnb, t.of_dfs);
+    fse_ctable(PREDEF_ML_NORM, 53, 6, spread, t.ml_stab, t.ml_dnb, t.ml_dfs);
     SeqCodes &s = t.codes;
     for (int c = 0; c < 36; c++) { s.ll_base[c] = LL_BASE[c]; s.ll_bits[c] = LL_BITS[c]; }
     for (int c = 0; c < 53; c++) {

@@ -15,6 +15,14 @@ constexpr uint32_t LZ_SLOT = 128u * 1024u + 16u;         // per-block output slo
 constexpr uint32_t LZ_MAX_SEQ = 128u * 1024u / LZ_MINMATCH;   // every sequence covers >= LZ_MINMATCH bytes of its block
 constexpr uint32_t LZ_PASS_BLOCKS = 4096;                // blocks per pass: 1 GiB of sequence scratch
 
+// The Predefined_Mode distributions of the LL, ML and OF codes (RFC 8878 3.1.1.3.2.2), accuracy logs 6, 6 and 5
+constexpr int16_t PREDEF_LL_NORM[36] = {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1,
+                                        1, 1, -1, -1, -1, -1};
+constexpr int16_t PREDEF_ML_NORM[53] = {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1,
+                                        1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1};
+constexpr int16_t PREDEF_OF_NORM[29] = {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1,
+                                        -1, -1};
+
 // The Literals_Length / Match_Length codes (RFC 8878 3.1.1.3.2.1.1), read by K9b and K10.
 struct SeqCodes {
     uint32_t ll_base[36], ml_base[53];   // Literals_Length / Match_Length baselines (Match_Length in bytes, >= 3)
@@ -37,8 +45,11 @@ void lz_fill_tables_host(void *dst);
 // of the table, and the spread skips those states. stab lists the states of each code in state order, grouped by
 // code. Per code, dnb gives the Number_of_Bits to write from a state X (kept as 2^log + state) and dfs the offset of
 // the next state in stab (zstd's symbolTT); a -1 code has the transform of a code with one state.
-__host__ __device__ inline void fse_ctable(const int16_t *norm, int nsym, int log, uint8_t *spread, uint16_t *stab,
-                                           int32_t *dnb, int32_t *dfs) {
+// The code of every state of the FSE table of norm[0..nsym) at accuracy log `log` (RFC 8878 4.1.1), into spread[0, 2^log):
+// a "less than 1" code (-1) takes one state at the top of the table, and the other codes are spread over the states
+// below them.  The counts must sum to 2^log (the absolute value of a -1), as every valid table description does.  The
+// encoder form (fse_ctable) and the decoder form (fse_dtable, zdec.cuh) are both built from it.
+__host__ __device__ inline void fse_spread(const int16_t *norm, int nsym, int log, uint8_t *spread) {
     const int size = 1 << log, step = (size >> 1) + (size >> 3) + 3;
     int high = size - 1;
     for (int c = 0; c < nsym; c++) if (norm[c] == -1) spread[high--] = (uint8_t)c;
@@ -47,6 +58,12 @@ __host__ __device__ inline void fse_ctable(const int16_t *norm, int nsym, int lo
             spread[pos] = (uint8_t)c;
             do pos = (pos + step) & (size - 1); while (pos > high);
         }
+}
+
+__host__ __device__ inline void fse_ctable(const int16_t *norm, int nsym, int log, uint8_t *spread, uint16_t *stab,
+                                           int32_t *dnb, int32_t *dfs) {
+    const int size = 1 << log;
+    fse_spread(norm, nsym, log, spread);
     int32_t *next = dnb;   // the next free place of each code in stab, before dnb takes its final value
     for (int c = 0, cum = 0; c < nsym; c++) { next[c] = cum; cum += norm[c] == -1 ? 1 : norm[c]; }
     for (int u = 0; u < size; u++) stab[next[spread[u]]++] = (uint16_t)u;

@@ -304,6 +304,58 @@ class Engine:
                     blen.ctypes.data, crc.ctypes.data))
         return [out[int(boff[i]): int(boff[i]) + int(blen[i])].tobytes() for i in range(len(o))], crc
 
+    # -- f3, read side -------------------------------------------------------------------------
+    def blob_decode_batch(self, blobs, chunk_len, digests=None, out: str | None = "host"):
+        """Check, decode and verify unencrypted DataBlobs on the GPU (pbsgpu_blob_decode_batch).  `blobs` is a list of
+        `bytes`, or (base, off[n], len[n]) with a host or device base; chunk_len[n] the expected chunk sizes (from the
+        index); digests (n x 32 bytes, or None) the expected SHA-256s.  out: "host" (numpy), "device" (a torch CUDA
+        tensor) or None (verify only: no decoded byte leaves the GPU).
+        -> (status int32[n] (DEC_STATUS names them), data, digests u8[n, 32]); data is a list of n chunks (`bytes` for
+        "host", tensor views for "device", None for blobs whose status is neither OK nor BAD_DIGEST), or None."""
+        if out not in ("host", "device", None):
+            raise ValueError(f"out must be 'host', 'device' or None, not {out!r}")
+        keep = None
+        if isinstance(blobs, tuple):
+            base, o, l = blobs
+            o, l = self._offlen(o, l)
+        else:
+            sizes = np.array([len(b) for b in blobs], dtype=np.uint64)
+            o = np.zeros(len(blobs), dtype=np.uint64)
+            if len(blobs):
+                o[1:] = np.cumsum(sizes)[:-1]
+            base = np.frombuffer(b"".join(bytes(b) for b in blobs) or b"\0", dtype=np.uint8)
+            l = sizes
+        n = len(o)
+        cl = np.ascontiguousarray(chunk_len, dtype=np.uint64)
+        if cl.shape != (n,):
+            raise ValueError("chunk_len must hold one size per blob")
+        dg = None
+        if digests is not None:
+            dg = np.ascontiguousarray(np.frombuffer(bytes(digests), dtype=np.uint8) if isinstance(digests, (bytes, bytearray))
+                                      else np.asarray(digests, dtype=np.uint8)).reshape(-1)
+            if dg.size != 32 * n:
+                raise ValueError("digests must hold 32 bytes per blob")
+        ooff = np.zeros(n, dtype=np.uint64)
+        if n:
+            ooff[1:] = np.cumsum(cl)[:-1]
+        total = max(1, int(cl.sum()))
+        if out == "host":
+            keep = np.zeros(total, dtype=np.uint8)
+        elif out == "device":
+            import torch
+            keep = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self.device}")
+        status = np.zeros(n, dtype=np.int32)
+        dout = np.zeros((n, 32), dtype=np.uint8)
+        self._ck(self._L.pbsgpu_blob_decode_batch(
+            self._h, _ptr(base), o.ctypes.data, l.ctypes.data, n, cl.ctypes.data, dg.ctypes.data if dg is not None else None,
+            _ptr(keep) if keep is not None else None, ooff.ctypes.data, status.ctypes.data, dout.ctypes.data))
+        data = None
+        if keep is not None:
+            good = (status == _lib.DEC_OK) | (status == _lib.DEC_BAD_DIGEST)
+            data = [(keep[int(ooff[i]): int(ooff[i]) + int(cl[i])].tobytes() if out == "host"
+                     else keep[int(ooff[i]): int(ooff[i]) + int(cl[i])]) if good[i] else None for i in range(n)]
+        return status, data, dout
+
     # -- f3, encrypt mode -----------------------------------------------------------------------
     def crypt(self, key: bytes) -> "Crypt":
         """Handle for one 32-byte AES-256 key (pbsgpu_crypt_create); close() zeroes its key material."""
