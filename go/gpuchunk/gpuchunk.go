@@ -758,6 +758,20 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]b
 // no digest check).  wantData false is verify only: no decoded byte leaves the GPU.  Returns one PBSGPU_DEC_* status
 // per blob (0 = OK) and, with wantData, the chunks whose status is OK or BAD_DIGEST.
 func (e *Engine) BlobDecode(blobs [][]byte, chunkLen []uint64, digests [][32]byte, wantData bool) ([]int32, [][]byte, error) {
+	return e.blobDecode(nil, blobs, chunkLen, digests, wantData)
+}
+
+// BlobDecodeEnc is BlobDecode for a snapshot written in encrypt mode (pbsgpu_blob_decode_batch_enc): encrypted blobs
+// are decrypted with c's key once their AES-256-GCM tag verified (PBSGPU_DEC_BAD_TAG otherwise), and their digests are
+// the keyed ones of the index (SHA-256(chunk || id_key)); unencrypted blobs are read as BlobDecode reads them.
+func (e *Engine) BlobDecodeEnc(c *Crypt, blobs [][]byte, chunkLen []uint64, digests [][32]byte, wantData bool) ([]int32, [][]byte, error) {
+	if c == nil {
+		return nil, nil, fmt.Errorf("pbsgpu: BlobDecodeEnc needs a crypt handle")
+	}
+	return e.blobDecode(c, blobs, chunkLen, digests, wantData)
+}
+
+func (e *Engine) blobDecode(c *Crypt, blobs [][]byte, chunkLen []uint64, digests [][32]byte, wantData bool) ([]int32, [][]byte, error) {
 	n := len(blobs)
 	if n == 0 {
 		return nil, nil, nil
@@ -787,8 +801,14 @@ func (e *Engine) BlobDecode(blobs [][]byte, chunkLen []uint64, digests [][32]byt
 		dstp = (*C.uint8_t)(unsafe.Pointer(&dst[0]))
 	}
 	status := make([]int32, n)
-	rc := C.pbsgpu_blob_decode_batch(e.ctx, unsafe.Pointer(&src[0]), &o[0], &l[0], C.uint32_t(n), &cl[0], dig, dstp, &oo[0],
-		(*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	var rc C.int
+	if c == nil {
+		rc = C.pbsgpu_blob_decode_batch(e.ctx, unsafe.Pointer(&src[0]), &o[0], &l[0], C.uint32_t(n), &cl[0], dig, dstp, &oo[0],
+			(*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	} else {
+		rc = C.pbsgpu_blob_decode_batch_enc(e.ctx, c.c, unsafe.Pointer(&src[0]), &o[0], &l[0], C.uint32_t(n), &cl[0], dig, dstp,
+			&oo[0], (*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	}
 	if err := e.err(rc); err != nil {
 		return nil, nil, err
 	}

@@ -370,7 +370,7 @@ int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, const uint64
  * (a DEVICE out may hold a partial decode, a HOST out is left untouched).
  * A corrupt blob never fails the call: it only sets its own status.  Returns PBSGPU_EINVAL for bad arguments (NULL
  * arrays, chunk_len[i] >= 2^32), ENOMEM / ECUDA for the call's own failures, 0 otherwise.  Encrypted blobs are not
- * decrypted here. */
+ * decrypted here (pbsgpu_blob_decode_batch_enc reads them with their key); BAD_TAG is never returned here. */
 enum { PBSGPU_DEC_OK = 0, PBSGPU_DEC_BAD_MAGIC, PBSGPU_DEC_BAD_CRC, PBSGPU_DEC_ENCRYPTED, PBSGPU_DEC_BAD_FRAME,
        PBSGPU_DEC_BAD_SIZE, PBSGPU_DEC_BAD_CHECKSUM, PBSGPU_DEC_BAD_DIGEST };
 int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
@@ -400,6 +400,23 @@ uint64_t pbsgpu_blob_size_enc(uint64_t payload_len);
 int pbsgpu_blob_encode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, const void *base, const uint64_t *off,
                                  const uint64_t *len, uint32_t n, const uint8_t *iv, uint8_t *out, const uint64_t *out_off,
                                  uint64_t *out_len, uint32_t *crc_out);
+/* Read side of encrypt mode (upstream `DataBlob::decode(Some(crypt_config), Some(digest))`): pbsgpu_blob_decode_batch
+ * for a mix of encrypted and unencrypted blobs, with the same arguments, limits and errors, plus `crypt` (required,
+ * created on ctx; otherwise PBSGPU_EINVAL).  Per blob the first failing check sets status[i]:
+ *   1. the magic: any of the four (BAD_MAGIC otherwise, and for an encrypted blob shorter than its 44-byte header or
+ *      a plain one shorter than 12 bytes); PBSGPU_DEC_ENCRYPTED is never returned here;
+ *   2. the CRC-32 of [12, len) of a plain blob, [44, len) of an encrypted one (BAD_CRC);
+ *   3. the AES-256-GCM tag of an encrypted blob under the key and its IV, no AAD (BAD_TAG; compared in constant time);
+ *   4. decode, size and content checksums as for plain blobs: the plaintext of an encrypted-compressed blob is zstd
+ *      frames, that of an encrypted blob is the chunk (BAD_FRAME, BAD_SIZE, BAD_CHECKSUM);
+ *   5. the digest against digest[i] (BAD_DIGEST): the keyed digest SHA-256(chunk || id_key) for encrypted blobs, the
+ *      plain SHA-256 for the others; digest_out receives the same kind.
+ * No unauthenticated plaintext leaves the library: decryption writes into a library-owned stage, and for a blob whose
+ * status is BAD_MAGIC, BAD_CRC or BAD_TAG no byte of `out` (host or device) is written. */
+enum { PBSGPU_DEC_BAD_TAG = PBSGPU_DEC_BAD_DIGEST + 1 };   /* 8: the statuses continue; only the _enc call returns it */
+int pbsgpu_blob_decode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off,
+                                 const uint64_t *len, uint32_t n, const uint64_t *chunk_len, const uint8_t *digest,
+                                 uint8_t *out, const uint64_t *out_off, int32_t *status, uint8_t *digest_out);
 
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------
  * emitBackedFile tees every new file through `xxh3.New()` and keeps `h.Sum64()` (reference

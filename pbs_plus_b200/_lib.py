@@ -40,6 +40,7 @@ CHUNK_KNOWN = 1
 BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5, "lzl": 7}   # 6 is not assigned
 # pbsgpu_blob_decode_batch: per-blob status (PBSGPU_DEC_*)
 DEC_OK, DEC_BAD_MAGIC, DEC_BAD_CRC, DEC_ENCRYPTED, DEC_BAD_FRAME, DEC_BAD_SIZE, DEC_BAD_CHECKSUM, DEC_BAD_DIGEST = range(8)
+DEC_BAD_TAG = 8   # pbsgpu_blob_decode_batch_enc only: the AES-256-GCM tag did not verify
 
 
 class DevInfo(C.Structure):
@@ -86,7 +87,7 @@ SYMBOLS = [
     "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
     "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
-    "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch",
+    "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch", "pbsgpu_blob_decode_batch_enc",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
 ]
@@ -163,6 +164,7 @@ def lib() -> C.CDLL:
     L.pbsgpu_blob_encode_batch_lzh.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_encode_batch_lzl.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_decode_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
+    L.pbsgpu_blob_decode_batch_enc.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
     L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
     L.pbsgpu_crypt_destroy.argtypes = [vp]
     L.pbsgpu_crypt_destroy.restype = None

@@ -17,6 +17,9 @@
 //  - k_gcm_tag (one thread per message) chains the segments by Horner with H^GCM_SEG_BLOCKS (Shoup table), the last
 //    one with H^k (k < GCM_SEG_BLOCKS, table of powers), appends the length block and XORs E_K(J0): the tag.
 // The counter is inc32: only the low 32-bit word advances, wrapping modulo 2^32 inside a message as GCM specifies.
+// Decryption (k_gcm_ctr_ghash<true>) is the same CTR transform; GHASH then runs over the input blocks before the XOR,
+// with the partial last block masked first (its granule can hold bytes of the next blob), and k_gcm_tag yields the tag
+// the ciphertext should carry, which the caller compares with the blob's.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -170,14 +173,34 @@ constexpr int GCM_SMEM = 256 * 32 * 4 /*T0 per lane*/ + 256 * 16 /*m32*/ + 256 *
 __device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
 __device__ __forceinline__ uint32_t rorr(uint32_t x, int r) { return __funnelshift_r(x, x, r); }
 
+// gf_mul with the word loop unrolled, so x is never indexed at run time and stays in registers: gf_mul's x[i >> 5]
+// puts x on the stack (the 16-byte frame of the encrypt kernel, whose code is kept as it is)
+__device__ __forceinline__ void gf_mul_reg(const uint32_t x[4], const uint32_t y[4], uint32_t z[4]) {
+    uint32_t v0 = y[0], v1 = y[1], v2 = y[2], v3 = y[3], z0 = 0, z1 = 0, z2 = 0, z3 = 0;
+#pragma unroll
+    for (int w = 0; w < 4; w++) {
+        const uint32_t xw = x[w];
+#pragma unroll 1
+        for (int i = 31; i >= 0; i--) {
+            const uint32_t m = 0u - ((xw >> i) & 1u);
+            z0 ^= v0 & m; z1 ^= v1 & m; z2 ^= v2 & m; z3 ^= v3 & m;
+            const uint32_t r = 0u - (v3 & 1u);
+            v3 = (v3 >> 1) | (v2 << 31); v2 = (v2 >> 1) | (v1 << 31); v1 = (v1 >> 1) | (v0 << 31); v0 = (v0 >> 1) ^ (r & 0xE1000000u);
+        }
+    }
+    z[0] = z0; z[1] = z1; z[2] = z2; z[3] = z3;
+}
+
 // Bytes of a block with r valid bytes (r < 16): keep bytes 0 .. r-1 of the big-endian words
 __device__ __forceinline__ uint32_t keep_mask(int r, int word) {
     const int v = r - 4 * word;
     return v >= 4 ? 0xFFFFFFFFu : v <= 0 ? 0u : ~(0xFFFFFFFFu >> (8 * v));
 }
 
-// In place: msg[i] covers dev bytes [src, src + len) (any alignment) and writes the ciphertext to dst (16 B aligned,
-// room for whole blocks); part[seg] = the segment's GHASH relative to its last block.
+// msg[i] covers dev bytes [src, src + len) (any alignment) and writes its CTR transform to dst (16 B aligned, room for
+// whole blocks; bytes past len are zero); part[seg] = the segment's GHASH of the ciphertext relative to its last block.
+// Encrypting, the ciphertext is the output; decrypting (DECRYPT), it is the input, hashed before the XOR.
+template <bool DECRYPT>
 __global__ void __launch_bounds__(GCM_THREADS) k_gcm_ctr_ghash(const GcmMsg *msg, const uint64_t *seg_first, uint32_t n,
                                                                uint64_t total_segs, const GcmTables *tab, uint4 *part) {
     extern __shared__ __align__(16) uint8_t gcm_smem[];
@@ -239,16 +262,22 @@ __global__ void __launch_bounds__(GCM_THREADS) k_gcm_ctr_ghash(const GcmMsg *msg
             const uint32_t k0 = LR(s0, s1, s2, s3) ^ RK[56], k1 = LR(s1, s2, s3, s0) ^ RK[57];
             const uint32_t k2 = LR(s2, s3, s0, s1) ^ RK[58], k3 = LR(s3, s0, s1, s2) ^ RK[59];
 #undef LR
-            uint32_t c0 = bswap32(w0) ^ k0, c1 = bswap32(w1) ^ k1, c2 = bswap32(w2) ^ k2, c3 = bswap32(w3) ^ k3;
+            uint32_t x0 = bswap32(w0), x1 = bswap32(w1), x2 = bswap32(w2), x3 = bswap32(w3);
+            if (DECRYPT && 16 * b + 16 > mm.len) {   // the ciphertext is hashed: drop the bytes past the message (the next blob's)
+                const int rv = (int)(mm.len - 16 * b);
+                x0 &= keep_mask(rv, 0); x1 &= keep_mask(rv, 1); x2 &= keep_mask(rv, 2); x3 &= keep_mask(rv, 3);
+            }
+            uint32_t c0 = x0 ^ k0, c1 = x1 ^ k1, c2 = x2 ^ k2, c3 = x3 ^ k3;
             if (16 * b + 16 > mm.len) {   // partial last block: GHASH pads with zeros
                 const int rv = (int)(mm.len - 16 * b);
                 c0 &= keep_mask(rv, 0); c1 &= keep_mask(rv, 1); c2 &= keep_mask(rv, 2); c3 &= keep_mask(rv, 3);
             }
             dst[b] = make_uint4(bswap32(c0), bswap32(c1), bswap32(c2), bswap32(c3));
-            // lane Horner with the step H^32
+            // lane Horner with the step H^32, over the ciphertext: the output when encrypting, the input when decrypting
             uint32_t y[4] = {y0, y1, y2, y3};
             gf_mul_table(y, [&](uint32_t i) { return M32[i]; }, [&](uint32_t i) { return R8[i]; });
-            y0 = y[0] ^ c0; y1 = y[1] ^ c1; y2 = y[2] ^ c2; y3 = y[3] ^ c3;
+            if (DECRYPT) { y0 = y[0] ^ x0; y1 = y[1] ^ x1; y2 = y[2] ^ x2; y3 = y[3] ^ x3; }
+            else { y0 = y[0] ^ c0; y1 = y[1] ^ c1; y2 = y[2] ^ c2; y3 = y[3] ^ c3; }
             last = b;
         }
         uint32_t q[4] = {0, 0, 0, 0};
@@ -256,7 +285,8 @@ __global__ void __launch_bounds__(GCM_THREADS) k_gcm_ctr_ghash(const GcmMsg *msg
             const uint32_t *hp = tab->hp[e - last];
             const uint32_t h[4] = {__ldg(hp), __ldg(hp + 1), __ldg(hp + 2), __ldg(hp + 3)};
             const uint32_t y[4] = {y0, y1, y2, y3};
-            gf_mul(y, h, q);
+            if (DECRYPT) gf_mul_reg(y, h, q);
+            else gf_mul(y, h, q);
         }
 #pragma unroll
         for (int d = 16; d > 0; d >>= 1)
@@ -305,14 +335,15 @@ __global__ void k_gcm_tag(const GcmMsg *msg, const uint64_t *seg_first, uint32_t
 uint64_t gcm_segments(uint64_t len) { return (((len + 15) >> 4) + GCM_SEG_BLOCKS - 1) / GCM_SEG_BLOCKS; }
 
 cudaError_t launch_gcm(const GcmMsg *msg, const uint64_t *seg_first, uint32_t n, uint64_t total_segs, const void *tables,
-                       void *part, uint8_t *tags, int sm_count, cudaStream_t st) {
+                       void *part, uint8_t *tags, int sm_count, cudaStream_t st, bool decrypt) {
     if (n == 0) return cudaSuccess;
     if (total_segs) {
-        cudaError_t e = cudaFuncSetAttribute(k_gcm_ctr_ghash, cudaFuncAttributeMaxDynamicSharedMemorySize, GCM_SMEM);
+        auto kern = decrypt ? k_gcm_ctr_ghash<true> : k_gcm_ctr_ghash<false>;
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GCM_SMEM);
         if (e != cudaSuccess) return e;
         const uint64_t want = (total_segs + GCM_THREADS / 32 - 1) / (GCM_THREADS / 32);
         const uint64_t cap = (uint64_t)sm_count * 4;
-        k_gcm_ctr_ghash<<<(unsigned)(want < cap ? want : cap), GCM_THREADS, GCM_SMEM, st>>>(
+        kern<<<(unsigned)(want < cap ? want : cap), GCM_THREADS, GCM_SMEM, st>>>(
             msg, seg_first, n, total_segs, (const GcmTables *)tables, (uint4 *)part);
     }
     k_gcm_tag<<<(n + 127) / 128, 128, 0, st>>>(msg, seg_first, n, (const GcmTables *)tables, (const uint4 *)part, tags);

@@ -154,6 +154,8 @@ extern "C" int pbsgpu_sha256_keyed_batch(pbsgpu_ctx *ctx, const pbsgpu_crypt *cr
 // ---------------------------------------------------------------------------
 static const uint8_t BLOB_MAGIC_UNCOMPRESSED[8] = {66, 171, 56, 7, 190, 131, 112, 161};
 static const uint8_t BLOB_MAGIC_COMPRESSED[8] = {49, 185, 88, 66, 111, 182, 163, 127};
+static const uint8_t BLOB_MAGIC_ENCRYPTED[8] = {0x7b, 0x67, 0x85, 0xbe, 0x22, 0x2d, 0x4c, 0xf0};
+static const uint8_t BLOB_MAGIC_ENCR_COMPR[8] = {0xe6, 0x59, 0x1b, 0xbf, 0x0b, 0xbf, 0xd8, 0x0b};
 
 static void blob_header(const uint8_t magic[8], uint32_t crc, uint8_t *out) {
     memcpy(out, magic, 8);
@@ -544,16 +546,22 @@ extern "C" int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, c
 }
 
 // ---------------------------------------------------------------------------
-// f3, read side: decode and verify unencrypted DataBlobs (K6, K13, K3)
+// f3, read side: decode and verify DataBlobs (K6, K11, K13, K3)
 // ---------------------------------------------------------------------------
 // The blobs are staged once; K6 takes the CRC of every payload.  Then, per pass of whole blobs (at most ZDEC_PASS_BLOBS
-// blobs and ZDEC_PASS_BYTES decoded bytes, or one longer blob), K13 decodes into the caller's device buffer or a pass
-// buffer, K3 hashes the chunks that decoded, and a host `out` receives those chunks from the pass buffer.  The host reads
-// only statuses and digests back; no decoded byte crosses PCIe unless `out` is host memory.
-extern "C" int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
-                                        const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
-                                        int32_t *status, uint8_t *digest_out) {
-    if (!ctx || (n && (!base || !off || !len || !chunk_len || !status || (out && !out_off)))) return PBSGPU_EINVAL;
+// blobs, ZDEC_PASS_BYTES decoded bytes and ZDEC_PASS_BYTES of ciphertext, or one longer blob), K13 decodes into the
+// caller's device buffer or a pass buffer, K3 hashes the chunks that decoded, and a host `out` receives those chunks
+// from the pass buffer.  The host reads only statuses and digests back; no decoded byte crosses PCIe unless `out` is
+// host memory.
+// With crypt, the host first reads every blob's header and sorts the blobs by magic.  Bad magics and encrypted blobs
+// whose CRC (K6 over the ciphertext) differs stop there.  Per pass, K11 decrypts the other encrypted payloads into a
+// plaintext stage, laid out as plain blobs (zdec.cuh), and the host compares their tags; K13 then decodes the plain
+// blobs from the input and the authenticated ones from the stage, so no unauthenticated byte reaches `out`.  K3 hashes
+// the chunks of encrypted blobs keyed with the crypt's id_key, the others plain (upstream `DataBlob::decode` with a
+// config).  Without crypt nothing is read on the host and every blob goes to K13 from the input.
+static int blob_decode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off, const uint64_t *len,
+                       uint32_t n, const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
+                       int32_t *status, uint8_t *digest_out) {
     Guard g(ctx);
     if (n == 0) return PBSGPU_OK;
     for (uint32_t i = 0; i < n; i++) {
@@ -565,68 +573,202 @@ extern "C" int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const
     Blocking b(ctx, ctx->streams[0]);
     const uint8_t *dbase;
     if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
-    // K6 over the payloads (a blob too short for its header gets an empty range; its magic check fails first)
-    std::vector<uint64_t> poff(n), plen(n);
-    for (uint32_t i = 0; i < n; i++) { poff[i] = off[i] + 12; plen[i] = len[i] >= 12 ? len[i] - 12 : 0; }
+    // kind[i]: the magic's index in BLOB_MAGICS (K13's order), -1 for an unknown magic or a blob shorter than its header;
+    // without crypt every blob is left to K13 (0).  heads: the first ZDEC_HEAD bytes of every blob.
+    static const uint8_t *const BLOB_MAGICS[4] = {BLOB_MAGIC_UNCOMPRESSED, BLOB_MAGIC_COMPRESSED, BLOB_MAGIC_ENCRYPTED,
+                                                  BLOB_MAGIC_ENCR_COMPR};
+    std::vector<int8_t> kind(n, 0);
+    std::vector<uint8_t> heads;
+    if (crypt) {
+        heads.assign((size_t)n * ZDEC_HEAD, 0);
+        if (!pbsgpu_is_device_ptr(base)) {   // host base: read in place
+            for (uint32_t i = 0; i < n; i++)
+                memcpy(heads.data() + (size_t)ZDEC_HEAD * i, (const uint8_t *)base + off[i], std::min<uint64_t>(len[i], ZDEC_HEAD));
+        } else {
+            uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n);
+            uint8_t *d_heads = b.get<uint8_t>((uint64_t)n * ZDEC_HEAD);
+            if (!d_off || !d_len || !d_heads) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+            if (b.ok()) b.e = launch_blob_heads(dbase, d_off, d_len, n, d_heads, b.st);
+            if (b.ok()) b.e = cudaMemcpyAsync(heads.data(), d_heads, heads.size(), cudaMemcpyDeviceToHost, b.st);
+            if (int rc = b.finish("blob headers")) return rc;
+        }
+        for (uint32_t i = 0; i < n; i++) {
+            kind[i] = -1;
+            for (int m = 0; m < 4 && kind[i] < 0; m++)
+                if (memcmp(heads.data() + (size_t)ZDEC_HEAD * i, BLOB_MAGICS[m], 8) == 0) kind[i] = (int8_t)m;
+            if (kind[i] >= 0 && len[i] < (kind[i] >= 2 ? ZDEC_HEAD : 12)) kind[i] = -1;
+        }
+    }
+    // K6 over the payloads: [12, len) of a plain blob, [44, len) of an encrypted one (a blob too short for its header
+    // gets an empty range; its magic check fails first).  ct[i]: the ciphertext bytes of an encrypted blob.
+    std::vector<uint64_t> poff(n), plen(n), ct(n, 0);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t hs = kind[i] >= 2 ? ZDEC_HEAD : 12;
+        poff[i] = off[i] + hs; plen[i] = len[i] >= hs ? len[i] - hs : 0;
+        if (kind[i] >= 2) ct[i] = plen[i];
+    }
     uint32_t *d_crc = b.get<uint32_t>(n);
-    int32_t *d_status = b.get<int32_t>(n);
-    if (!d_crc || !d_status) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
+    if (!d_crc) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
     if (int rc = crc32_enqueue(b, dbase, poff.data(), plen.data(), n, d_crc)) return rc;
+    std::vector<uint32_t> crc;
+    if (crypt) {   // the host checks the magics and the CRCs of encrypted blobs; K13 those of plain blobs
+        crc.resize(n);
+        if (b.ok()) b.e = cudaMemcpyAsync(crc.data(), d_crc, n * 4ull, cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("blob crc")) return rc;
+        for (uint32_t i = 0; i < n; i++) {
+            const uint8_t *h = heads.data() + (size_t)ZDEC_HEAD * i;
+            const uint32_t hc = (uint32_t)h[8] | (uint32_t)h[9] << 8 | (uint32_t)h[10] << 16 | (uint32_t)h[11] << 24;
+            status[i] = kind[i] < 0 ? PBSGPU_DEC_BAD_MAGIC : kind[i] >= 2 && hc != crc[i] ? PBSGPU_DEC_BAD_CRC : PBSGPU_DEC_OK;
+        }
+    }
     // passes of whole blobs
     std::vector<uint32_t> pass_first;
-    uint64_t pass_max = 0, acc = 0, blobs_max = 0;
+    uint64_t pass_max = 0, acc = 0, acc_c = 0, blobs_max = 0, stage_max = 0, stage_acc = 0, segs_max = 0, segs_acc = 0;
     for (uint32_t i = 0; i < n; i++) {
-        if (pass_first.empty() || acc + chunk_len[i] > ZDEC_PASS_BYTES || i - pass_first.back() >= ZDEC_PASS_BLOBS) {
+        if (pass_first.empty() || acc + chunk_len[i] > ZDEC_PASS_BYTES || acc_c + ct[i] > ZDEC_PASS_BYTES ||
+            i - pass_first.back() >= ZDEC_PASS_BLOBS) {
             pass_first.push_back(i);
-            acc = 0;
+            acc = acc_c = stage_acc = segs_acc = 0;
         }
         acc += chunk_len[i];
+        acc_c += ct[i];
+        if (kind[i] >= 2) { stage_acc += 16 + ((ct[i] + 15) & ~15ull); segs_acc += gcm_segments(ct[i]); }
         pass_max = std::max(pass_max, acc);
+        stage_max = std::max(stage_max, stage_acc);
+        segs_max = std::max(segs_max, segs_acc);
         blobs_max = std::max<uint64_t>(blobs_max, i - pass_first.back() + 1);
     }
     pass_first.push_back(n);
     uint8_t *pbuf = out_dev ? nullptr : b.get<uint8_t>(pass_max + 16);
     uint8_t *lits = b.get<uint8_t>(blobs_max * ZDEC_LIT_SLOT);
     ZdecBlob *d_blobs = b.get<ZdecBlob>(blobs_max);
+    int32_t *d_status = b.get<int32_t>(blobs_max);
     ChunkRef *d_refs = want_sha ? b.get<ChunkRef>(blobs_max) : nullptr;
     unsigned long long *d_nref = want_sha ? b.get<unsigned long long>(1) : nullptr;
     uint8_t *d_dig = want_sha ? b.get<uint8_t>(blobs_max * 32) : nullptr;
-    if ((!out_dev && !pbuf) || !lits || !d_blobs || (want_sha && (!d_refs || !d_nref || !d_dig)))
+    if ((!out_dev && !pbuf) || !lits || !d_blobs || !d_status || (want_sha && (!d_refs || !d_nref || !d_dig)))
         return fail(ctx, PBSGPU_ENOMEM, "decode pass buffers (%llu bytes) failed", (unsigned long long)pass_max);
+    // encrypt mode: the plaintext stage and K11's buffers, per pass
+    uint8_t *stage = nullptr, *d_part = nullptr, *d_tags = nullptr, *d_shead = nullptr;
+    GcmMsg *d_msg = nullptr;
+    uint64_t *d_first = nullptr, *d_sat = nullptr;
+    uint32_t *d_csub = nullptr;
+    if (crypt) {
+        stage = b.get<uint8_t>(stage_max + 16); d_part = b.get<uint8_t>(segs_max * 16 + 16);
+        d_tags = b.get<uint8_t>(blobs_max * 16); d_shead = b.get<uint8_t>(blobs_max * 16);
+        d_msg = b.get<GcmMsg>(blobs_max); d_first = b.get<uint64_t>(blobs_max + 1); d_sat = b.get<uint64_t>(blobs_max);
+        d_csub = b.get<uint32_t>(blobs_max);
+        if (!stage || !d_part || !d_tags || !d_shead || !d_msg || !d_first || !d_sat || !d_csub)
+            return fail(ctx, PBSGPU_ENOMEM, "decryption stage (%llu bytes) failed", (unsigned long long)stage_max);
+    }
     std::vector<ZdecBlob> zb(blobs_max);
-    std::vector<uint64_t> at(blobs_max);   // chunk k of the pass at pass base + at[k]
+    std::vector<uint64_t> at(blobs_max), sat(blobs_max);   // chunk k of the pass at pass base + at[k]; its plaintext blob at stage + sat[k]
     std::vector<ChunkRef> refs(blobs_max);
-    std::vector<uint32_t> ref_blob(blobs_max);
-    std::vector<uint8_t> dig(blobs_max * 32);
+    std::vector<uint32_t> ref_blob(blobs_max), list(blobs_max), csub(blobs_max);
+    std::vector<int32_t> st(blobs_max);
+    std::vector<uint8_t> dig(blobs_max * 32), tags, shead;
+    std::vector<GcmMsg> msg;
+    std::vector<uint64_t> seg_first;
     for (size_t p = 0; p + 1 < pass_first.size(); p++) {
         const uint32_t i0 = pass_first[p], pn = pass_first[p + 1] - i0;
         uint8_t *pbase = out_dev ? out : pbuf;
-        uint64_t cur = 0;
+        uint64_t cur = 0, scur = 0;
         for (uint32_t k = 0; k < pn; k++) {   // the caller's places, or back to back in the pass buffer
             const uint32_t i = i0 + k;
             at[k] = out_dev ? out_off[i] : cur;
             cur += chunk_len[i];
-            zb[k] = {off[i], len[i], (uint64_t)(uintptr_t)(pbase + at[k]), chunk_len[i]};
+            sat[k] = scur;
+            if (kind[i] >= 2) scur += 16 + ((ct[i] + 15) & ~15ull);
         }
-        if (b.ok()) b.e = cudaMemcpyAsync(d_blobs, zb.data(), pn * sizeof(ZdecBlob), cudaMemcpyHostToDevice, b.st);
-        if (b.ok()) b.e = launch_zdec(dbase, d_blobs, d_crc + i0, pn, (const ZdecTables *)ctx->d_zdec_tab, lits, d_status + i0, b.st);
-        if (b.ok()) b.e = cudaMemcpyAsync(status + i0, d_status + i0, pn * sizeof(int32_t), cudaMemcpyDeviceToHost, b.st);
-        if (int rc = b.finish("blob decode")) return rc;
-        // K3 over the chunks that decoded
-        uint32_t nr = 0;
-        for (uint32_t k = 0; want_sha && k < pn; k++)
-            if (status[i0 + k] == PBSGPU_DEC_OK) {
-                refs[nr].stream = nr; refs[nr].len = (uint32_t)chunk_len[i0 + k]; refs[nr].start = at[k];
-                ref_blob[nr++] = i0 + k;
+        // K11: the encrypted payloads whose CRC matched, decrypted into the stage; their tags compared on the host in
+        // constant time (XOR-accumulate)
+        msg.clear(); seg_first.assign(1, 0); list.clear();
+        for (uint32_t k = 0; crypt && k < pn; k++) {
+            const uint32_t i = i0 + k;
+            if (kind[i] < 2 || status[i] != PBSGPU_DEC_OK) continue;
+            GcmMsg m;
+            m.src = (uint64_t)(uintptr_t)(dbase + off[i] + ZDEC_HEAD);
+            m.dst = (uint64_t)(uintptr_t)(stage + sat[k] + 16);
+            m.len = ct[i];
+            gcm_j0_host(crypt->tab.data(), heads.data() + (size_t)ZDEC_HEAD * i + 12, m.j0);
+            gcm_encrypt_block_host(crypt->tab.data(), m.j0, m.ej0);
+            msg.push_back(m);
+            seg_first.push_back(seg_first.back() + gcm_segments(ct[i]));
+            list.push_back(k);
+        }
+        if (!msg.empty()) {
+            const uint32_t ne = (uint32_t)msg.size();
+            tags.resize(16ull * ne);
+            if (b.ok()) b.e = cudaMemcpyAsync(d_msg, msg.data(), ne * sizeof(GcmMsg), cudaMemcpyHostToDevice, b.st);
+            if (b.ok()) b.e = cudaMemcpyAsync(d_first, seg_first.data(), (ne + 1) * 8ull, cudaMemcpyHostToDevice, b.st);
+            if (b.ok()) b.e = launch_gcm(d_msg, d_first, ne, seg_first[ne], crypt->d_tab, d_part, d_tags, ctx->sm_count, b.st, true);
+            if (b.ok()) b.e = cudaMemcpyAsync(tags.data(), d_tags, 16ull * ne, cudaMemcpyDeviceToHost, b.st);
+            if (int rc = b.finish("blob decryption")) return rc;
+            for (uint32_t r = 0; r < ne; r++) {
+                const uint32_t i = i0 + list[r];
+                const uint8_t *want = heads.data() + (size_t)ZDEC_HEAD * i + 28;
+                uint8_t diff = 0;
+                for (int j = 0; j < 16; j++) diff |= (uint8_t)(tags[16ull * r + j] ^ want[j]);
+                if (diff) status[i] = PBSGPU_DEC_BAD_TAG;
             }
-        if (nr) {
+        }
+        // K13, once over the plain blobs against the input and once over the authenticated ones against the stage, each
+        // behind a plain header (the magic of the payload's form, the CRC K13 is given)
+        list.clear(); shead.clear();
+        uint32_t n_plain = 0;
+        for (int from_stage = 0; from_stage < 2; from_stage++)
+            for (uint32_t k = 0; k < pn; k++) {
+                const uint32_t i = i0 + k;
+                if (crypt && (status[i] != PBSGPU_DEC_OK || (kind[i] >= 2) != (from_stage == 1))) continue;
+                if (!crypt && from_stage) break;
+                const uint32_t r = (uint32_t)list.size();
+                list.push_back(k);
+                const uint64_t dst = (uint64_t)(uintptr_t)(pbase + at[k]);
+                if (from_stage) {
+                    zb[r] = {sat[k] + 4, 12 + ct[i], dst, chunk_len[i]};
+                    uint8_t h[16] = {0};
+                    blob_header(BLOB_MAGICS[kind[i] - 2], crc[i], h + 4);
+                    shead.insert(shead.end(), h, h + 16);
+                } else {
+                    zb[r] = {off[i], len[i], dst, chunk_len[i]};
+                    n_plain++;
+                }
+                if (crypt) csub[r] = crc[i];
+            }
+        const uint32_t nl = (uint32_t)list.size(), n_stage = nl - n_plain;
+        const uint32_t *crc_l = crypt ? d_csub : d_crc + i0;
+        if (b.ok() && nl) b.e = cudaMemcpyAsync(d_blobs, zb.data(), nl * sizeof(ZdecBlob), cudaMemcpyHostToDevice, b.st);
+        if (b.ok() && crypt && nl) b.e = cudaMemcpyAsync(d_csub, csub.data(), nl * 4ull, cudaMemcpyHostToDevice, b.st);
+        if (n_stage) {
+            std::vector<uint64_t> sat_l(n_stage);
+            for (uint32_t r = 0; r < n_stage; r++) sat_l[r] = sat[list[n_plain + r]];
+            if (b.ok()) b.e = cudaMemcpyAsync(d_sat, sat_l.data(), n_stage * 8ull, cudaMemcpyHostToDevice, b.st);
+            if (b.ok()) b.e = cudaMemcpyAsync(d_shead, shead.data(), shead.size(), cudaMemcpyHostToDevice, b.st);
+            if (b.ok()) b.e = launch_stage_heads(stage, d_sat, d_shead, n_stage, b.st);
+        }
+        const ZdecTables *ztab = (const ZdecTables *)ctx->d_zdec_tab;
+        if (b.ok()) b.e = launch_zdec(dbase, d_blobs, crc_l, n_plain, ztab, lits, d_status, b.st);
+        if (b.ok()) b.e = launch_zdec(stage, d_blobs + n_plain, crc_l + n_plain, n_stage, ztab, lits, d_status + n_plain, b.st);
+        if (b.ok() && nl) b.e = cudaMemcpyAsync(st.data(), d_status, nl * sizeof(int32_t), cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("blob decode")) return rc;
+        for (uint32_t r = 0; r < nl; r++) status[i0 + list[r]] = st[r];
+        // K3 over the chunks that decoded: plain digests, then keyed ones for the encrypted blobs
+        for (int keyed = 0; want_sha && keyed < 2; keyed++) {
+            uint32_t nr = 0;
+            for (uint32_t k = 0; k < pn; k++)
+                if (status[i0 + k] == PBSGPU_DEC_OK && (kind[i0 + k] >= 2) == (keyed == 1)) {
+                    refs[nr].stream = nr; refs[nr].len = (uint32_t)chunk_len[i0 + k]; refs[nr].start = at[k];
+                    ref_blob[nr++] = i0 + k;
+                }
+            if (nr == 0) continue;
+            const uint8_t *suffix = keyed ? pbsgpu_crypt_id_key(crypt) : nullptr;
             const unsigned long long hn = nr;
             ShaArgs ha;
             ha.base = pbase; ha.off = nullptr; ha.chunks = d_refs; ha.order = nullptr; ha.n_chunks = d_nref;
             ha.chunk_cap = nr; ha.digests = d_dig; ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
             if (b.ok()) b.e = cudaMemcpyAsync(d_refs, refs.data(), nr * sizeof(ChunkRef), cudaMemcpyHostToDevice, b.st);
             if (b.ok()) b.e = cudaMemcpyAsync(d_nref, &hn, sizeof hn, cudaMemcpyHostToDevice, b.st);
-            if (b.ok()) b.e = ctx->variant == 1 ? launch_sha_simple(ha, b.st) : launch_sha_tuned(ha, ctx->tune, b.st);
+            if (b.ok()) b.e = ctx->variant == 1 ? launch_sha_simple(ha, b.st, suffix) : launch_sha_tuned(ha, ctx->tune, b.st, suffix);
             if (b.ok()) b.e = cudaMemcpyAsync(dig.data(), d_dig, nr * 32ull, cudaMemcpyDeviceToHost, b.st);
             if (int rc = b.finish("blob decode digests")) return rc;
             for (uint32_t r = 0; r < nr; r++) {
@@ -648,11 +790,24 @@ extern "C" int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const
     return PBSGPU_OK;
 }
 
+extern "C" int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                        const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
+                                        int32_t *status, uint8_t *digest_out) {
+    if (!ctx || (n && (!base || !off || !len || !chunk_len || !status || (out && !out_off)))) return PBSGPU_EINVAL;
+    return blob_decode(ctx, nullptr, base, off, len, n, chunk_len, digest, out, out_off, status, digest_out);
+}
+
+extern "C" int pbsgpu_blob_decode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off,
+                                            const uint64_t *len, uint32_t n, const uint64_t *chunk_len, const uint8_t *digest,
+                                            uint8_t *out, const uint64_t *out_off, int32_t *status, uint8_t *digest_out) {
+    if (!ctx || !crypt || crypt->ctx != ctx || (n && (!base || !off || !len || !chunk_len || !status || (out && !out_off))))
+        return PBSGPU_EINVAL;
+    return blob_decode(ctx, crypt, base, off, len, n, chunk_len, digest, out, out_off, status, digest_out);
+}
+
 // ---------------------------------------------------------------------------
 // f3, encrypt mode: encrypted DataBlobs (K11)
 // ---------------------------------------------------------------------------
-static const uint8_t BLOB_MAGIC_ENCRYPTED[8] = {0x7b, 0x67, 0x85, 0xbe, 0x22, 0x2d, 0x4c, 0xf0};
-static const uint8_t BLOB_MAGIC_ENCR_COMPR[8] = {0xe6, 0x59, 0x1b, 0xbf, 0x0b, 0xbf, 0xd8, 0x0b};
 
 // Host SHA-256 (FIPS 180-4) for the key derivation: 20 compressions per crypt handle, so no device work
 struct HostSha256 {

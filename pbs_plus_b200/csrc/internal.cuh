@@ -191,9 +191,10 @@ void gcm_fill_tables_host(const uint8_t key[32], void *tables);
 void gcm_encrypt_block_host(const void *tables, const uint32_t in[4], uint32_t out[4]);
 void gcm_j0_host(const void *tables, const uint8_t iv[16], uint32_t j0[4]);
 uint64_t gcm_segments(uint64_t len);
-// seg_first[n+1]: prefix of gcm_segments(len); part: 16 B per segment; tags: 16 B per message (device)
+// seg_first[n+1]: prefix of gcm_segments(len); part: 16 B per segment; tags: 16 B per message (device).  decrypt: src
+// holds the ciphertext and dst receives the plaintext; the tag is the one the ciphertext should carry.
 cudaError_t launch_gcm(const GcmMsg *msg, const uint64_t *seg_first, uint32_t n, uint64_t total_segs, const void *tables,
-                       void *part, uint8_t *tags, int sm_count, cudaStream_t st);
+                       void *part, uint8_t *tags, int sm_count, cudaStream_t st, bool decrypt = false);
 
 // ---- corpus (K5) ------------------------------------------------------------------
 cudaError_t launch_corpus_fill(const pbsgpu_corpus &c, uint64_t first_file, uint32_t n_files, uint8_t *dst,

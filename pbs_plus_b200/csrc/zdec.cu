@@ -556,7 +556,35 @@ __global__ void __launch_bounds__(32) k_zdec(const uint8_t *base, const ZdecBlob
     if (lane == 0) status[k] = st;
 }
 
+// one thread per blob: its first min(len, ZDEC_HEAD) bytes to heads + ZDEC_HEAD * i, zeros after them
+__global__ void k_blob_heads(const uint8_t *base, const uint64_t *off, const uint64_t *len, uint32_t n, uint8_t *heads) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint8_t *p = base + off[i];
+    const uint64_t l = len[i];
+    for (uint32_t j = 0; j < ZDEC_HEAD; j++) heads[(uint64_t)ZDEC_HEAD * i + j] = j < l ? p[j] : 0;
+}
+
+// one thread per entry: the 16 bytes at stage + at[k] (16 B aligned)
+__global__ void k_stage_heads(uint8_t *stage, const uint64_t *at, const uint4 *head, uint32_t n) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) *(uint4 *)(stage + at[k]) = head[k];
+}
+
 }  // namespace
+
+cudaError_t launch_blob_heads(const uint8_t *base, const uint64_t *off, const uint64_t *len, uint32_t n, uint8_t *heads,
+                              cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_blob_heads<<<(n + 127) / 128, 128, 0, st>>>(base, off, len, n, heads);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stage_heads(uint8_t *stage, const uint64_t *at, const void *head, uint32_t n, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_stage_heads<<<(n + 127) / 128, 128, 0, st>>>(stage, at, (const uint4 *)head, n);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_zdec(const uint8_t *base, const ZdecBlob *b, const uint32_t *crc, uint32_t nb, const ZdecTables *tab,
                         uint8_t *lits, int32_t *status, cudaStream_t st) {

@@ -47,4 +47,14 @@ struct ZdecBlob {
 cudaError_t launch_zdec(const uint8_t *base, const ZdecBlob *b, const uint32_t *crc, uint32_t nb, const ZdecTables *tab,
                         uint8_t *lits, int32_t *status, cudaStream_t st);
 
+// Encrypted blobs (pbsgpu_blob_decode_batch_enc).  The host reads each blob's header {magic, crc, iv, tag}: from a
+// device base, launch_blob_heads gathers the first ZDEC_HEAD bytes of blob i (zero-filled past its end) to
+// heads + ZDEC_HEAD * i for one D2H copy.  A decrypted payload is laid out in the plaintext stage as a plain blob K13
+// reads: launch_stage_heads writes head[k] (16 bytes: 4 of padding, the 12-byte plain header) to stage + at[k] (16 B
+// aligned), and the plaintext follows at stage + at[k] + 16.
+constexpr uint32_t ZDEC_HEAD = 44;
+cudaError_t launch_blob_heads(const uint8_t *base, const uint64_t *off, const uint64_t *len, uint32_t n, uint8_t *heads,
+                              cudaStream_t st);
+cudaError_t launch_stage_heads(uint8_t *stage, const uint64_t *at, const void *head, uint32_t n, cudaStream_t st);
+
 }  // namespace pbsgpu

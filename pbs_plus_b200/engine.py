@@ -312,6 +312,16 @@ class Engine:
         tensor) or None (verify only: no decoded byte leaves the GPU).
         -> (status int32[n] (DEC_STATUS names them), data, digests u8[n, 32]); data is a list of n chunks (`bytes` for
         "host", tensor views for "device", None for blobs whose status is neither OK nor BAD_DIGEST), or None."""
+        return self._blob_decode(lambda *a: self._L.pbsgpu_blob_decode_batch(self._h, *a), blobs, chunk_len, digests, out)
+
+    def blob_decode_batch_enc(self, crypt: "Crypt", blobs, chunk_len, digests=None, out: str | None = "host"):
+        """blob_decode_batch for encrypted and unencrypted DataBlobs (pbsgpu_blob_decode_batch_enc): encrypted blobs are
+        decrypted with `crypt`'s key after their GCM tag verified (DEC_BAD_TAG otherwise), and their digests are keyed
+        (SHA-256(chunk || id_key)), as in the index an encrypt-mode writer made; unencrypted blobs get plain digests."""
+        return self._blob_decode(lambda *a: self._L.pbsgpu_blob_decode_batch_enc(self._h, crypt._h if crypt is not None else None, *a), blobs, chunk_len,
+                                 digests, out)
+
+    def _blob_decode(self, call, blobs, chunk_len, digests, out):
         if out not in ("host", "device", None):
             raise ValueError(f"out must be 'host', 'device' or None, not {out!r}")
         keep = None
@@ -346,9 +356,8 @@ class Engine:
             keep = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self.device}")
         status = np.zeros(n, dtype=np.int32)
         dout = np.zeros((n, 32), dtype=np.uint8)
-        self._ck(self._L.pbsgpu_blob_decode_batch(
-            self._h, _ptr(base), o.ctypes.data, l.ctypes.data, n, cl.ctypes.data, dg.ctypes.data if dg is not None else None,
-            _ptr(keep) if keep is not None else None, ooff.ctypes.data, status.ctypes.data, dout.ctypes.data))
+        self._ck(call(_ptr(base), o.ctypes.data, l.ctypes.data, n, cl.ctypes.data, dg.ctypes.data if dg is not None else None,
+                      _ptr(keep) if keep is not None else None, ooff.ctypes.data, status.ctypes.data, dout.ctypes.data))
         data = None
         if keep is not None:
             good = (status == _lib.DEC_OK) | (status == _lib.DEC_BAD_DIGEST)

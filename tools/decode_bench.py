@@ -2,10 +2,12 @@
 tools/blob_bench.py (half-zero random, text-like, binary-like, repeated).  Per image, the blobs of three encoders --
 _lzh and _lzl (this engine) and libzstd level 1 (pyarrow, compressed on the host before any timing) -- lie in device
 memory, and the call runs twice: verify only (out = NULL, expected digests given) and with the chunks copied into
-pinned host memory.  Rates are GB/s of decoded bytes, the best of 3 runs.  For context only: libzstd's single-thread
-decode rate on the HOST CPU over a 64 MiB sample of the level-1 blobs.
+pinned host memory.  A fourth arm, "lzh-enc", decodes encrypted _lzh blobs (pbsgpu_blob_encode_batch_enc) with
+pbsgpu_blob_decode_batch_enc and keyed digests the same two ways.  Rates are GB/s of decoded bytes, the best of 3 runs.
+For context only: libzstd's single-thread decode rate on the HOST CPU over a 64 MiB sample of the level-1 blobs.
 
     python tools/decode_bench.py [GiB per image, default 8]"""
+import os
 import subprocess
 import sys
 import time
@@ -34,13 +36,15 @@ CH = 4 << 20
 nc = n // CH
 off = np.arange(0, n, CH, dtype=np.uint64)
 ln = np.full(nc, CH, dtype=np.uint64)
-boff = np.arange(nc, dtype=np.uint64) * np.uint64(CH + 12)
-blobs_h = e.host_alloc(nc * (CH + 12))
+boff = np.arange(nc, dtype=np.uint64) * np.uint64(CH + 44)
+blobs_h = e.host_alloc(nc * (CH + 44))
 blen = np.zeros(nc, dtype=np.uint64)
 crc = np.zeros(nc, dtype=np.uint32)
 dec_h = e.host_alloc(n)
 status = np.zeros(nc, dtype=np.int32)
 dig_out = np.zeros((nc, 32), dtype=np.uint8)
+KEY = os.urandom(32)
+iv = np.frombuffer(os.urandom(16 * nc), dtype=np.uint8)
 
 
 def images():
@@ -85,10 +89,19 @@ for label, d in images():
     torch.cuda.synchronize()
     want = e.sha256_batch(d, off, ln)
     print(f"-- {label} image, {n / 2**30:.0f} GiB")
-    for enc in ("lzh", "lzl", "libzstd-1"):
+    for enc in ("lzh", "lzh-enc", "lzl", "libzstd-1"):
         host_rate = None
         if enc == "libzstd-1":
             host_rate = libzstd_blobs(d)
+        elif enc == "lzh-enc":
+            # an engine of its own: closing it returns the decryption stage, so the other arms keep their device memory
+            ee = pg.Engine(0)
+            cr = ee.crypt(KEY)
+            want_keyed = ee.sha256_keyed_batch(cr, d, off, ln)
+            rc = L_.pbsgpu_blob_encode_batch_enc(ee._h, cr._h, 5, d.data_ptr(), off.ctypes.data, ln.ctypes.data, nc,
+                                                 iv.ctypes.data, blobs_h.ctypes.data, boff.ctypes.data, blen.ctypes.data,
+                                                 crc.ctypes.data)
+            assert rc == 0, rc
         else:
             rc = getattr(L_, "pbsgpu_blob_encode_batch_" + enc)(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, nc,
                                                                 blobs_h.ctypes.data, boff.ctypes.data, blen.ctypes.data,
@@ -101,13 +114,21 @@ for label, d in images():
             for rep in range(3):
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
-                rc = L_.pbsgpu_blob_decode_batch(e._h, bd.data_ptr(), boff.ctypes.data, blen.ctypes.data, nc, ln.ctypes.data,
-                                                 want.ctypes.data, outp, off.ctypes.data, status.ctypes.data,
-                                                 dig_out.ctypes.data)
+                if enc == "lzh-enc":
+                    rc = L_.pbsgpu_blob_decode_batch_enc(ee._h, cr._h, bd.data_ptr(), boff.ctypes.data, blen.ctypes.data, nc,
+                                                         ln.ctypes.data, want_keyed.ctypes.data, outp, off.ctypes.data,
+                                                         status.ctypes.data, dig_out.ctypes.data)
+                else:
+                    rc = L_.pbsgpu_blob_decode_batch(e._h, bd.data_ptr(), boff.ctypes.data, blen.ctypes.data, nc,
+                                                     ln.ctypes.data, want.ctypes.data, outp, off.ctypes.data,
+                                                     status.ctypes.data, dig_out.ctypes.data)
                 best = min(best, time.perf_counter() - t0)
                 assert rc == 0 and (status == 0).all(), (rc, np.unique(status))
             res[mode] = n / best / 1e9
         del bd
+        if enc == "lzh-enc":
+            cr.close()
+            ee.close()
         torch.cuda.empty_cache()
         ctx = f"; libzstd host decode, one thread: {host_rate:.2f} GB/s" if host_rate else ""
         print(f"{enc}: blobs {blen.sum() / n:.4f} of the input; decode {res['verify only']:.2f} GB/s verify only, "
