@@ -874,3 +874,139 @@ func (b *Batch) BlobEncodeEnc(c *Crypt, mode int, off, length []uint64) ([][]byt
 	}
 	return res, nil
 }
+
+// PayloadReader reads a payload archive through its .ppxar.didx (pbsgpu_reader_*): the replacement for
+// reader.PayloadReaderAt() that PxarFS.readFileContent calls (internal/pxarmount/pxarfs.go:38, :409-412).  Chunks are
+// decoded and verified on the GPU once (CRC, GCM tag with a crypt, zstd, digest against the index) into a device cache
+// of cacheBytes (0 = 256 MiB); reads are copied out of that cache.  source returns a chunk's DataBlob by digest
+// (.chunks/<hex>).  Prefetch: the number of chunks after the last touched one fetched along with a miss.
+type PayloadReader struct {
+	e        *Engine
+	r        *C.pbsgpu_reader
+	source   func([32]byte) ([]byte, error)
+	digests  [][32]byte
+	size     uint64
+	Prefetch int
+}
+
+func (e *Engine) NewPayloadReader(didx []byte, c *Crypt, cacheBytes uint64, source func([32]byte) ([]byte, error)) (*PayloadReader, error) {
+	if len(didx) == 0 {
+		return nil, fmt.Errorf("pbsgpu: empty index image")
+	}
+	var cr *C.pbsgpu_crypt
+	if c != nil {
+		cr = c.c
+	}
+	var r *C.pbsgpu_reader
+	if err := e.err(C.pbsgpu_reader_open(e.ctx, (*C.uint8_t)(unsafe.Pointer(&didx[0])), C.uint64_t(len(didx)), cr,
+		C.uint64_t(cacheBytes), &r)); err != nil {
+		return nil, err
+	}
+	n := (len(didx) - 4096) / 40
+	dg := make([][32]byte, n)
+	for i := range dg {
+		copy(dg[i][:], didx[4096+40*i+8:4096+40*i+40])
+	}
+	return &PayloadReader{e: e, r: r, source: source, digests: dg, size: uint64(C.pbsgpu_reader_size(r))}, nil
+}
+
+func (p *PayloadReader) Close() { C.pbsgpu_reader_close(p.r) }
+
+// read serves ranges (payload: (payload offset, file size) of files) into out at outOff: one plan, one fetch of the
+// missing blobs (plus Prefetch chunks after the last one), one read.
+func (p *PayloadReader) read(off, length []uint64, payload bool, out []byte, outOff []uint64) error {
+	n := len(off)
+	if n == 0 {
+		return nil
+	}
+	var flags C.uint32_t
+	if payload {
+		flags = C.PBSGPU_READ_PAYLOAD
+	}
+	o := (*C.uint64_t)(unsafe.Pointer(&off[0]))
+	l := (*C.uint64_t)(unsafe.Pointer(&length[0]))
+	var k C.uint64_t
+	need := make([]uint64, len(p.digests))
+	var np *C.uint64_t
+	if len(need) > 0 {
+		np = (*C.uint64_t)(unsafe.Pointer(&need[0]))
+	}
+	if err := p.e.err(C.pbsgpu_reader_plan(p.r, o, l, C.uint32_t(n), flags, np, nil, C.uint64_t(len(need)), &k)); err != nil {
+		return err
+	}
+	need = need[:k]
+	if k > 0 {
+		for c := need[k-1] + 1; c < uint64(len(p.digests)) && c <= need[k-1]+uint64(p.Prefetch); c++ {
+			need = append(need, c)
+		}
+	}
+	var blobs []byte
+	bo := make([]uint64, len(need)+1)
+	bl := make([]uint64, len(need)+1)
+	for j, c := range need {
+		b, err := p.source(p.digests[c])
+		if err != nil {
+			return err
+		}
+		bo[j], bl[j] = uint64(len(blobs)), uint64(len(b))
+		blobs = append(blobs, b...)
+	}
+	blobs = append(blobs, 0)
+	need = append(need, 0)
+	status := make([]int32, n)
+	rc := C.pbsgpu_reader_read(p.r, o, l, C.uint32_t(n), flags, unsafe.Pointer(&blobs[0]), (*C.uint64_t)(unsafe.Pointer(&bo[0])),
+		(*C.uint64_t)(unsafe.Pointer(&bl[0])), (*C.uint64_t)(unsafe.Pointer(&need[0])), C.uint32_t(len(need)-1),
+		(*C.uint8_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&outOff[0])), (*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	if err := p.e.err(rc); err != nil {
+		return err
+	}
+	for i, s := range status {
+		if s != int32(C.PBSGPU_DEC_OK) {
+			return fmt.Errorf("pbsgpu: read of %d bytes at %d: status %d", length[i], off[i], s)
+		}
+	}
+	return nil
+}
+
+// ReadAt implements io.ReaderAt over the archive: short with io.EOF at its end.
+func (p *PayloadReader) ReadAt(b []byte, off int64) (int, error) {
+	if off < 0 {
+		return 0, errors.New("pbsgpu: negative offset")
+	}
+	if uint64(off) >= p.size {
+		return 0, io.EOF
+	}
+	want := uint64(len(b))
+	if rest := p.size - uint64(off); want > rest {
+		want = rest
+	}
+	if want == 0 {
+		return 0, nil
+	}
+	if err := p.read([]uint64{uint64(off)}, []uint64{want}, false, b, []uint64{0}); err != nil {
+		return 0, err
+	}
+	if want < uint64(len(b)) {
+		return int(want), io.EOF
+	}
+	return int(want), nil
+}
+
+// ReadFiles returns the contents of files given by payload offset and size (restore): one read for all of them.
+func (p *PayloadReader) ReadFiles(offsets, sizes []uint64) ([][]byte, error) {
+	oo := make([]uint64, len(sizes))
+	var total uint64
+	for i, s := range sizes {
+		oo[i] = total
+		total += s
+	}
+	out := make([]byte, total+1)
+	if err := p.read(offsets, sizes, true, out, oo); err != nil {
+		return nil, err
+	}
+	res := make([][]byte, len(sizes))
+	for i, s := range sizes {
+		res[i] = out[oo[i] : oo[i]+s]
+	}
+	return res, nil
+}

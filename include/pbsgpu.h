@@ -418,6 +418,60 @@ int pbsgpu_blob_decode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, con
                                  const uint64_t *len, uint32_t n, const uint64_t *chunk_len, const uint8_t *digest,
                                  uint8_t *out, const uint64_t *out_off, int32_t *status, uint8_t *digest_out);
 
+/* ---- f3, read side: archives (mount and restore read a payload stream through its index) -------------------------
+ * A reader maps byte ranges of the archive an index describes to its chunks, decodes and verifies each chunk it is
+ * given once (pbsgpu_blob_decode_batch(_enc)'s checks), keeps the verified chunks in a cache in device memory and
+ * serves ranges from that cache (reference PxarFS.readFileContent -> SplitArchiveReader.PayloadReaderAt().ReadAt,
+ * internal/pxarmount/pxarfs.go:38, :409-412; restore, internal/pxar/format.go:113-132).  The chunk files themselves are
+ * read by the caller: plan names the chunks a read needs, read takes their blobs.
+ * open: didx is a .didx image, parsed with pbsgpu_didx_parse's rules; its index_csum is verified on the GPU (EINVAL on a
+ * mismatch, and on a chunk of 2^32 bytes or more).  crypt: NULL, or a handle created on ctx (EINVAL otherwise);
+ * encrypted chunks are then decrypted and their keyed digests checked, as pbsgpu_blob_decode_batch_enc; without it an
+ * encrypted blob gets PBSGPU_DEC_ENCRYPTED.  cache_bytes: device memory for verified chunks; 0 = 256 MiB (pxar-mount's
+ * --cache-size default); raised to the index's largest chunk; allocated here (ENOMEM otherwise).
+ * close: frees the cache; with a crypt the cache is zeroed first.  size: the archive's length (the last end offset).
+ * A reader belongs to its ctx: its calls serialise with every other call on the ctx.
+ * Ranges: range i is the archive bytes [off[i], off[i] + len[i]).  With PBSGPU_READ_PAYLOAD, off[i] is a file's
+ * payload offset and len[i] its size: the 16 bytes at off[i] must be {PXAR_PAYLOAD u64 LE, 16 + len[i] u64 LE} (pxar
+ * v2's PAYLOAD header; restated, UNVERIFIED against the Go module) and the range's output is the content at
+ * off[i] + 16.  The header may straddle a chunk boundary.  A range that ends past pbsgpu_reader_size makes the whole
+ * call EINVAL.  A zero-length plain range touches no chunk and is OK; chunks of length 0 are never touched.
+ * plan: the indices of the chunks the ranges touch that the cache does not hold, ascending and without repeats, into
+ * chunk[cap]; their digests into digest (k x 32 bytes, may be NULL), so the caller can open .chunks/<hex> directly.
+ * *n_out receives the count; PBSGPU_ERANGE when it exceeds cap.
+ * read:
+ *   1. every chunk named in blob_chunk is first dropped from the cache; repeated or out-of-range entries are EINVAL;
+ *   2. blob j is [blob_base + blob_off[j], + blob_len[j]) (HOST or DEVICE), the DataBlob of chunk blob_chunk[j].  It is
+ *      decoded with the reader's crypt (or without one) against the chunk's length and digest from the index, and
+ *      blob_status[j] (may be NULL) receives its PBSGPU_DEC_* status.  Every verified blob is cached, also one whose
+ *      chunk no range touches (prefetch);
+ *   3. ranges are served from the chunks still cached plus the chunks this call verified.  status[i] is OK; or, going
+ *      through the range's chunks in ascending order, the first failure: the failed blob's status, or
+ *      PBSGPU_DEC_MISSING for a chunk that was neither cached nor given; or after those PBSGPU_DEC_BAD_HEADER;
+ *   4. out (HOST or DEVICE) receives range i at out + out_off[i]; those len[i] bytes hold the range when status[i] is
+ *      OK and are undefined otherwise, but no byte of a chunk that failed a check ever reaches out: only verified
+ *      chunks enter the cache, and ranges are copied from the cache alone;
+ *   5. a corrupt blob never fails the call.  EINVAL for bad arguments (NULL arrays, unknown flags), ENOMEM / ECUDA for
+ *      the call's own failures.
+ * Cache: a FIFO ring over cache_bytes with 256-byte aligned slots in insertion order; a hit does not refresh an entry.
+ * When one call supplies more blob bytes than the ring holds, the blobs are decoded in groups that fit: the pieces
+ * (range x chunk intersections) of chunks that were cached already are copied before the first group is decoded, and
+ * each group's pieces right after that group, before the next group can evict it. */
+typedef struct pbsgpu_reader pbsgpu_reader;
+int pbsgpu_reader_open(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t size, const pbsgpu_crypt *crypt,
+                       uint64_t cache_bytes, pbsgpu_reader **out);
+void pbsgpu_reader_close(pbsgpu_reader *r);
+uint64_t pbsgpu_reader_size(const pbsgpu_reader *r);
+#define PBSGPU_READ_PAYLOAD 1u
+int pbsgpu_reader_plan(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
+                       uint64_t *chunk, uint8_t *digest, uint64_t cap, uint64_t *n_out);
+int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
+                       const void *blob_base, const uint64_t *blob_off, const uint64_t *blob_len,
+                       const uint64_t *blob_chunk, uint32_t n_blobs,
+                       uint8_t *out, const uint64_t *out_off, int32_t *status, int32_t *blob_status);
+enum { PBSGPU_DEC_MISSING = PBSGPU_DEC_BAD_TAG + 1,   /* 9: a chunk the range needs was neither cached nor given */
+       PBSGPU_DEC_BAD_HEADER };                        /* 10: READ_PAYLOAD and the 16-byte header does not match */
+
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------
  * emitBackedFile tees every new file through `xxh3.New()` and keeps `h.Sum64()` (reference
  * internal/pxarmount/commit.go:717-725); verifyBackedFileHashes later re-reads every file to recompute

@@ -41,6 +41,9 @@ BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5, "lzl": 7} 
 # pbsgpu_blob_decode_batch: per-blob status (PBSGPU_DEC_*)
 DEC_OK, DEC_BAD_MAGIC, DEC_BAD_CRC, DEC_ENCRYPTED, DEC_BAD_FRAME, DEC_BAD_SIZE, DEC_BAD_CHECKSUM, DEC_BAD_DIGEST = range(8)
 DEC_BAD_TAG = 8   # pbsgpu_blob_decode_batch_enc only: the AES-256-GCM tag did not verify
+# pbsgpu_reader_read: a range's chunk was neither cached nor given; a file's 16-byte PAYLOAD header did not match
+DEC_MISSING, DEC_BAD_HEADER = 9, 10
+READ_PAYLOAD = 1   # pbsgpu_reader_plan / _read flags: ranges are (payload offset, file size)
 
 
 class DevInfo(C.Structure):
@@ -88,6 +91,7 @@ SYMBOLS = [
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
     "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
     "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch", "pbsgpu_blob_decode_batch_enc",
+    "pbsgpu_reader_open", "pbsgpu_reader_close", "pbsgpu_reader_size", "pbsgpu_reader_plan", "pbsgpu_reader_read",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
 ]
@@ -165,6 +169,13 @@ def lib() -> C.CDLL:
     L.pbsgpu_blob_encode_batch_lzl.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_blob_decode_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
     L.pbsgpu_blob_decode_batch_enc.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
+    L.pbsgpu_reader_open.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(vp)]
+    L.pbsgpu_reader_close.argtypes = [vp]
+    L.pbsgpu_reader_close.restype = None
+    L.pbsgpu_reader_size.argtypes = [vp]
+    L.pbsgpu_reader_size.restype = C.c_uint64
+    L.pbsgpu_reader_plan.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, u64p]
+    L.pbsgpu_reader_read.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
     L.pbsgpu_crypt_destroy.argtypes = [vp]
     L.pbsgpu_crypt_destroy.restype = None

@@ -559,7 +559,7 @@ extern "C" int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, c
 // blobs from the input and the authenticated ones from the stage, so no unauthenticated byte reaches `out`.  K3 hashes
 // the chunks of encrypted blobs keyed with the crypt's id_key, the others plain (upstream `DataBlob::decode` with a
 // config).  Without crypt nothing is read on the host and every blob goes to K13 from the input.
-static int blob_decode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off, const uint64_t *len,
+int pbsgpu_blob_decode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off, const uint64_t *len,
                        uint32_t n, const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
                        int32_t *status, uint8_t *digest_out) {
     Guard g(ctx);
@@ -794,7 +794,7 @@ extern "C" int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const
                                         const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
                                         int32_t *status, uint8_t *digest_out) {
     if (!ctx || (n && (!base || !off || !len || !chunk_len || !status || (out && !out_off)))) return PBSGPU_EINVAL;
-    return blob_decode(ctx, nullptr, base, off, len, n, chunk_len, digest, out, out_off, status, digest_out);
+    return pbsgpu_blob_decode(ctx, nullptr, base, off, len, n, chunk_len, digest, out, out_off, status, digest_out);
 }
 
 extern "C" int pbsgpu_blob_decode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off,
@@ -802,7 +802,7 @@ extern "C" int pbsgpu_blob_decode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt 
                                             uint8_t *out, const uint64_t *out_off, int32_t *status, uint8_t *digest_out) {
     if (!ctx || !crypt || crypt->ctx != ctx || (n && (!base || !off || !len || !chunk_len || !status || (out && !out_off))))
         return PBSGPU_EINVAL;
-    return blob_decode(ctx, crypt, base, off, len, n, chunk_len, digest, out, out_off, status, digest_out);
+    return pbsgpu_blob_decode(ctx, crypt, base, off, len, n, chunk_len, digest, out, out_off, status, digest_out);
 }
 
 // ---------------------------------------------------------------------------

@@ -254,6 +254,11 @@ int pbsgpu_xxh3_table(pbsgpu_ctx *ctx, const void **tab);   // K7's device table
 // out_len[i] bytes.  Device ranges are encoded in place.
 int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len);
+// The body of pbsgpu_blob_decode_batch (crypt NULL) and _enc (capi_aux.cu), without the argument checks: the archive
+// reader decodes its blobs through it into its device cache.
+int pbsgpu_blob_decode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off, const uint64_t *len,
+                       uint32_t n, const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,
+                       int32_t *status, uint8_t *digest_out);
 
 // ---------------------------------------------------------------------------
 // encrypt mode (capi_crypt.cu): one AES-256 key, its K11 tables on the host (J0, E_K(J0)) and on the device

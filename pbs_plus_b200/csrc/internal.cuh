@@ -196,6 +196,13 @@ uint64_t gcm_segments(uint64_t len);
 cudaError_t launch_gcm(const GcmMsg *msg, const uint64_t *seg_first, uint32_t n, uint64_t total_segs, const void *tables,
                        void *part, uint8_t *tags, int sm_count, cudaStream_t st, bool decrypt = false);
 
+// ---- archive reader (K14, reader.cu) ------------------------------------------------------------
+constexpr uint32_t READ_TILE = 16384;   // bytes per warp
+struct ReadPiece { uint64_t src, dst, len; };   // device addresses: len bytes from src (the reader's cache) to dst
+// tile_first[n+1]: prefix of ceil(len / READ_TILE) over the pieces
+cudaError_t launch_read_gather(const ReadPiece *pieces, const uint64_t *tile_first, uint32_t n, uint64_t total_tiles,
+                               int sm_count, cudaStream_t st);
+
 // ---- corpus (K5) ------------------------------------------------------------------
 cudaError_t launch_corpus_fill(const pbsgpu_corpus &c, uint64_t first_file, uint32_t n_files, uint8_t *dst,
                                uint64_t stride, cudaStream_t st);

@@ -365,6 +365,13 @@ class Engine:
                      else keep[int(ooff[i]): int(ooff[i]) + int(cl[i])]) if good[i] else None for i in range(n)]
         return status, data, dout
 
+    # -- f3, read side: archives ---------------------------------------------------------------
+    def reader(self, didx: bytes, crypt: "Crypt | None" = None, cache_bytes: int = 0) -> "Reader":
+        """Byte ranges of the archive a .didx image describes, served from a cache of verified chunks in device memory
+        (pbsgpu_reader_open).  `crypt` decrypts encrypted chunks and checks their keyed digests; `cache_bytes` 0 means
+        256 MiB, and the cache always holds at least the largest chunk."""
+        return Reader(self, didx, crypt, cache_bytes)
+
     # -- f3, encrypt mode -----------------------------------------------------------------------
     def crypt(self, key: bytes) -> "Crypt":
         """Handle for one 32-byte AES-256 key (pbsgpu_crypt_create); close() zeroes its key material."""
@@ -506,6 +513,101 @@ class Crypt:
     def close(self):
         if getattr(self, "_h", None) and self._eng._h:
             self._eng._L.pbsgpu_crypt_destroy(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
+class Reader:
+    """An archive reader on the engine's device (pbsgpu_reader_*): plan() names the chunks a read needs that the cache
+    lacks, read() verifies the blobs it is given into the cache and copies the ranges out of it."""
+
+    def __init__(self, eng: Engine, didx: bytes, crypt: "Crypt | None", cache_bytes: int):
+        a = np.frombuffer(bytes(didx), dtype=np.uint8)
+        self._eng, self._crypt = eng, crypt   # the crypt handle must outlive the reader
+        h = C.c_void_p()
+        eng._ck(eng._L.pbsgpu_reader_open(eng._h, a.ctypes.data, len(a), crypt._h if crypt is not None else None,
+                                          int(cache_bytes), C.byref(h)))
+        self._h = h
+
+    @property
+    def size(self) -> int:
+        """The archive's length (the index's last end offset)."""
+        return int(self._eng._L.pbsgpu_reader_size(self._h))
+
+    def plan(self, off, length, payload: bool = False):
+        """The chunks the ranges touch that the cache does not hold -> (chunk indices u64[k] ascending, digests
+        u8[k, 32]).  payload: the ranges are (payload offset, file size) of files, their 16-byte headers included."""
+        o, l = Engine._offlen(off, length)
+        flags = _lib.READ_PAYLOAD if payload else 0
+        n = C.c_uint64()
+        rc = self._eng._L.pbsgpu_reader_plan(self._h, o.ctypes.data, l.ctypes.data, len(o), flags, None, None, 0, C.byref(n))
+        if rc != _lib.ERANGE:
+            self._eng._ck(rc)
+        chunks = np.zeros(n.value, dtype=np.uint64)
+        dig = np.zeros((n.value, 32), dtype=np.uint8)
+        if n.value:
+            self._eng._ck(self._eng._L.pbsgpu_reader_plan(self._h, o.ctypes.data, l.ctypes.data, len(o), flags,
+                                                          chunks.ctypes.data, dig.ctypes.data, n.value, C.byref(n)))
+        return chunks, dig
+
+    def read(self, off, length, blobs, payload: bool = False, out: str = "host"):
+        """Read ranges (pbsgpu_reader_read).  `blobs`: {chunk index: DataBlob bytes}, or (base, off[k], len[k], chunk[k])
+        with a host or device base; their chunks are verified into the cache, then the ranges are copied out of it.
+        out: "host" (numpy) or "device" (a torch CUDA tensor).
+        -> (status int32[n] (DEC_* values), data, blob_status int32[k]); data holds per range `bytes` ("host") or a
+        tensor view ("device"), None where the status is not DEC_OK."""
+        if out not in ("host", "device"):
+            raise ValueError(f"out must be 'host' or 'device', not {out!r}")
+        o, l = Engine._offlen(off, length)
+        if isinstance(blobs, tuple):
+            base, bo, bl, bc = blobs
+            bo, bl = Engine._offlen(bo, bl)
+            bc = np.ascontiguousarray(bc, dtype=np.uint64)
+            if bc.shape != bo.shape:
+                raise ValueError("blob chunks must hold one index per blob")
+        else:
+            items = list(blobs.items())
+            bc = np.array([c for c, _ in items], dtype=np.uint64)
+            bl = np.array([len(b) for _, b in items], dtype=np.uint64)
+            bo = np.zeros(len(items), dtype=np.uint64)
+            if len(items):
+                bo[1:] = np.cumsum(bl)[:-1]
+            base = np.frombuffer(b"".join(bytes(b) for _, b in items) or b"\0", dtype=np.uint8)
+        n, k = len(o), len(bo)
+        ooff = np.zeros(n, dtype=np.uint64)
+        if n:
+            ooff[1:] = np.cumsum(l)[:-1]
+        total = max(1, int(l.sum()))
+        if out == "host":
+            buf = np.zeros(total, dtype=np.uint8)
+        else:
+            import torch
+            buf = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self._eng.device}")
+        status = np.zeros(n, dtype=np.int32)
+        bst = np.zeros(k, dtype=np.int32)
+        self._eng._ck(self._eng._L.pbsgpu_reader_read(
+            self._h, o.ctypes.data, l.ctypes.data, n, _lib.READ_PAYLOAD if payload else 0, _ptr(base), bo.ctypes.data,
+            bl.ctypes.data, bc.ctypes.data, k, _ptr(buf), ooff.ctypes.data, status.ctypes.data, bst.ctypes.data))
+        data = []
+        for i in range(n):
+            a, e = int(ooff[i]), int(ooff[i]) + int(l[i])
+            data.append(None if status[i] != _lib.DEC_OK else buf[a:e].tobytes() if out == "host" else buf[a:e])
+        return status, data, bst
+
+    def close(self):
+        if getattr(self, "_h", None) and self._eng._h:
+            self._eng._L.pbsgpu_reader_close(self._h)
         self._h = None
 
     def __del__(self):

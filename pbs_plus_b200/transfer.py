@@ -11,6 +11,10 @@ only new chunks.  This mirror keeps the names and the pull-from-a-reader contrac
 batches the files: entries are queued and pushed through the GPU engine in one batch on
 Flush()/Finish() (SURVEY.md section 8f item 2).  `upload` is a callback (the HTTP/2 upload is out of scope).
 
+One reader: PayloadReader -- the mirror of SplitArchiveReader.PayloadReaderAt() (pxarfs.go:38, :409-412): byte ranges
+and whole files of a payload stream, served through pbsgpu_reader_* from a cache of verified chunks on the GPU; the
+chunk files come from a `chunk_source` callback (reading the datastore is out of scope).
+
 Two writers:
   * PayloadStreamWriter -- the LAYOUT-FAITHFUL one and the default for a drop-in: it produces the pxar v2 payload
     stream the production chunker sees (PAYLOAD_START marker, then per file a 16-byte PAYLOAD header + content,
@@ -30,6 +34,7 @@ from typing import BinaryIO, Callable
 
 import numpy as np
 
+from . import _lib
 from ._lib import CHUNK_DTYPE, CHUNK_KNOWN, Cfg
 from .engine import DigestSet, Engine
 
@@ -321,6 +326,64 @@ class PayloadStreamWriter:
             rec[i]["digest"] = np.frombuffer(dig, dtype=np.uint8)
             rec[i]["flags"] = CHUNK_KNOWN if known else 0
         return self.engine.didx_build(rec, uuid, ctime)
+
+
+_DEC_NAMES = {getattr(_lib, k): k for k in dir(_lib) if k.startswith("DEC_")}
+
+
+class PayloadReader:
+    """Reads a payload stream (.ppxar.didx) the way SplitArchiveReader.PayloadReaderAt() serves PxarFS.readFileContent
+    (pxarfs.go:409-412) and restore (format.go:113-132).  Every chunk is decoded and verified on the GPU once (CRC, GCM
+    tag with `crypt_key`, zstd, digest against the index) into a device cache of `cache_bytes` (0 = 256 MiB, pxar-mount's
+    --cache-size default); reads are copied out of that cache.  `chunk_source(digest)` returns the DataBlob of a chunk
+    (the bytes of .chunks/<hex>).  Errors raise IOError naming the first bad range and its status."""
+
+    def __init__(self, engine: Engine, ppxar_didx: bytes, chunk_source: Callable[[bytes], bytes],
+                 crypt_key: bytes | None = None, cache_bytes: int = 0):
+        self._crypt = engine.crypt(crypt_key) if crypt_key is not None else None
+        self._reader = engine.reader(ppxar_didx, self._crypt, cache_bytes)
+        self._source = chunk_source
+
+    @property
+    def Size(self) -> int:
+        return self._reader.size
+
+    def _read(self, off: list[int], size: list[int], payload: bool) -> list[bytes]:
+        """One plan, one fetch of the missing blobs by digest, one read."""
+        chunks, digests = self._reader.plan(off, size, payload)
+        blobs = {int(c): self._source(bytes(d)) for c, d in zip(chunks, digests)}
+        status, data, _ = self._reader.read(off, size, blobs, payload)
+        bad = np.flatnonzero(status != _lib.DEC_OK)
+        if len(bad):
+            i = int(bad[0])
+            what = "file at payload offset" if payload else "range at"
+            raise IOError(f"transfer: {what} {off[i]} ({size[i]} bytes): {_DEC_NAMES.get(int(status[i]), int(status[i]))}")
+        return data
+
+    def ReadAt(self, off: int, size: int) -> bytes:
+        """io.ReaderAt: up to `size` bytes at archive offset `off`; short (possibly empty) at the archive's end."""
+        if off < 0 or size < 0:
+            raise ValueError("transfer: negative offset or size")
+        size = max(0, min(size, self.Size - off))
+        return self._read([off], [size], False)[0] if size else b""
+
+    def ReadFileContents(self, files: list[tuple[int, int]]) -> list[bytes]:
+        """The contents of files given as (payload offset, size), each checked against its 16-byte PAYLOAD header."""
+        if not files:
+            return []
+        off, size = zip(*files)
+        return self._read(list(off), list(size), True)
+
+    def Close(self) -> None:
+        self._reader.close()
+        if self._crypt is not None:
+            self._crypt.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.Close()
 
 
 def NewRemoteDedupSplitArchiveWriter(engine: Engine, config: Cfg, known: DigestSet | None = None,
