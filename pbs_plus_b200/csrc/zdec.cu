@@ -25,6 +25,9 @@ namespace {
 
 constexpr uint32_t HUF_MAXLOG = 11;                 // longest Huffman code RFC 8878 allows
 constexpr uint32_t BLOCK_MAX = ZFRAME_BLOCK;        // 128 KiB
+// The largest Window_Size upstream's decoder reads: libzstd's streaming decoder refuses a frame that needs more than
+// 2^windowLogMax + 1 bytes of window, and windowLogMax is 27 by default.  A Single_Segment frame's window is its content.
+constexpr uint64_t WINDOW_MAX = (1ull << 27) + 1;
 __device__ __forceinline__ int tab_maxlog(int c) { return c == 1 ? ENT_OF_MAXLOG : ENT_LL_MAXLOG; }   // LL, OF, ML
 __device__ __forceinline__ int tab_maxsym(int c) { return c == 0 ? 35 : c == 1 ? 31 : 52; }
 
@@ -469,7 +472,6 @@ __device__ __forceinline__ int32_t decode_frames(Shared &sh, const ZdecTables &T
         if (!single) {
             if (q >= n) return ST_FRAME;
             const uint32_t wd = p[q++], wlog = 10 + (wd >> 3);
-            if (wlog > 31) return ST_FRAME;
             window = (1ull << wlog) + ((1ull << wlog) >> 3) * (wd & 7);
         }
         const uint32_t did_size = did_flag == 3 ? 4 : did_flag;
@@ -482,6 +484,7 @@ __device__ __forceinline__ int32_t decode_frames(Shared &sh, const ZdecTables &T
         if (fcs_size == 2) fcs += 256;
         q += fcs_size;
         if (single) window = fcs;
+        if (window > WINDOW_MAX) return ST_FRAME;
         f.bmax = (uint32_t)(window < BLOCK_MAX ? window : BLOCK_MAX);
         f.fstart = f.pos;
         f.rep0 = 1; f.rep1 = 4; f.rep2 = 8;
@@ -503,7 +506,7 @@ __device__ __forceinline__ int32_t decode_frames(Shared &sh, const ZdecTables &T
                 for (uint32_t k = lane; k < bsize; k += 32) out[f.pos + k] = v;
                 q += 1; f.pos += bsize;
             } else {
-                if (bsize >= BLOCK_MAX || bsize > f.bmax || bsize > n - q) return ST_FRAME;
+                if (bsize > f.bmax || bsize > n - q) return ST_FRAME;
                 const int32_t r = decode_block(sh, T, f, p + q, bsize, slot, lane);
                 if (r != ST_OK) return r;
                 q += bsize;

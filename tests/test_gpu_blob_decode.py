@@ -12,6 +12,7 @@ import pytest
 from oracle import pyref
 import zstd_dec_forms as zd
 import zstd_forms as zf
+import zstd_stream_ref
 import pbs_plus_b200 as pg
 from pbs_plus_b200 import _lib
 from test_gpu_zstd_lz import pack, to_dev
@@ -182,15 +183,14 @@ def test_per_blob_statuses(eng, torch):
 
 
 def libzstd_result(payload: bytes, size: int):
-    try:
-        got = pa.decompress(payload, decompressed_size=size, codec="zstd", asbytes=True)
-    except Exception:
-        return None
-    return got if len(got) == size else None
+    """What upstream's streaming libzstd decoder reads from the payload, or None where it fails or reads another size."""
+    got = zstd_stream_ref.stream_decode(payload)
+    return got if isinstance(got, bytes) and len(got) == size else None
 
 
 def test_corrupted_frames_never_pass_where_libzstd_fails(eng, torch):
     """Truncations at every block edge and seeded byte flips, the blob CRC recomputed, each between intact neighbours."""
+    zstd_stream_ref.require()
     cases = zd.fixture_cases()
     text = corpora(400_000, 10)["text"].tobytes()
     srcs = [(cases[k][0], cases[k][1]) for k in ("small_window", "two_frames", "handmade", "nofcs")]

@@ -71,7 +71,7 @@ def normalize(counts, log):
 def fse_description(norm, log) -> bytes:
     """FSE table description (RFC 8878 4.1.1): Accuracy_Log - 5 in 4 bits, then each code's count + 1 in a variable
     number of bits (the low values one bit shorter), a zero count followed by 2-bit repeat flags for the zero counts
-    after it; it stops when the counts reach 2^log."""
+    after it; it stops when the counts reach 2^log.  A count of -1 ("less than 1") takes one cell."""
     w = _Bits()
     w.add(log - MIN_LOG, 4)
     remaining, threshold, nbits = (1 << log) + 1, 1 << log, log + 1
@@ -88,7 +88,7 @@ def fse_description(norm, log) -> bytes:
         c = norm[s]
         s += 1
         mx = 2 * threshold - 1 - remaining
-        remaining -= c
+        remaining -= abs(c)
         c += 1
         if c >= threshold:
             c += mx

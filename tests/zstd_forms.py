@@ -439,3 +439,541 @@ def form_cases():
 
 def form_parts() -> list[np.ndarray]:
     return [p for p, _ in form_cases()]
+
+
+# -- a decoder that names the edges it passes ----------------------------------------------------------------------------
+# decode_payload() reads a blob payload (zstd and skippable frames) as RFC 8878 describes it, with upstream's window
+# limit, and counts in `forms` every edge of the format it passes.  It is the census of tests/zstd_edge_frames.py: the
+# forms are read from the bytes, not claimed by the builder.  Edge names:
+#   rep:1 .. rep:3 | rep:1/ll0 .. rep:3/ll0     a repeat offset code with Literals_Length > 0 / == 0 (rep:3/ll0: rep0 - 1)
+#   rep:3/ll0/twice                            rep0 - 1 in two sequences in a row
+#   rep:across-block | rep:across-raw | rep:reset   a repeat code before any new offset in a block: the history from an
+#                                              earlier block, from before a Raw block, or the reset one of a later frame
+#   off:<k>/overlap (k <= 33) | off:overlap   a match at least 32 bytes longer than its offset k; longer than it
+#   off:all | off:into-raw | off:into-rle      offset == the bytes so far of a frame after the first; a match that starts
+#                                              in an earlier Raw / RLE block and runs past its end
+#   off:raw-to-rle                             such a match that runs from a Raw block into the RLE block after it
+#   ll:code35 | ml:code52 | of:code<k>        codes (OF from 20 on)
+#   seq:wide/ll<b>/ml<b>                       a sequence with >= 15 LL, >= 15 ML and >= 23 OF extra bits
+#   logs:<ll>/<of>/<ml>                        the accuracy logs of a block whose three tables are FSE_Compressed
+#   <col>:log<k> | <col>:rle/max | <col>:maxsym | <col>:X-after-<P|R|F>   a table's accuracy log, its largest code in
+#                                              RLE_Mode or an FSE description, Repeat_Mode after each mode
+#   fse:less1 | fse:zeros+3 | fse:zeros+4+    a "less than 1" count; a zero count with exactly 3 / more than 3 more
+#   lit:<form>:max                             the largest size of a literals header form (raw/1B .. 3B, huf/sf0 .. sf3)
+#   huf:last0 | huf:last1 | huf4:n<6..9>      four streams whose last one holds 0 / 1 symbols; of 6..9 literals
+#   lit:treeless/1x | lit:treeless/4x | huf:maxbits11 | huf:256sym | tree:direct/128   Huffman literals
+#   window:m<0..7> | block:bmax/<raw|rle|compressed> | block:content-128k   Window_Descriptor mantissas; blocks of
+#                                              Block_Maximum_Size under a smaller window; a 128 KiB Compressed_Block content
+#   fcs:2/256 | fcs:2/65791 | frame:empty | checksum:unaligned
+#   reject:<rule>                              the rule a payload breaks (decode_payload raises Reject)
+LL_MAXLOG, OF_MAXLOG, ML_MAXLOG = 9, 8, 9
+HUF_MAXLOG = 11
+WINDOW_MAX = (1 << 27) + 1        # libzstd's default: windowLogMax 27, a Window_Size of at most 2^27 + 1 bytes
+BLOCK_MAX = 128 << 10
+
+
+class Reject(ValueError):
+    """A payload that breaks a rule of the format; `rule` names it."""
+
+    def __init__(self, rule: str):
+        super().__init__(rule)
+        self.rule = rule
+
+
+class _Back:
+    """Backward bitstream (RFC 8878 4.1): the highest set bit of the last byte marks its end.  `bit` counts the bits not
+    read yet; reads past the start give zeros and drive it negative."""
+
+    def __init__(self, data: bytes, what: str):
+        if not data or data[-1] == 0:
+            raise Reject(f"{what}:end-mark")
+        self.v = int.from_bytes(data, "little")
+        self.bit = 8 * (len(data) - 1) + data[-1].bit_length() - 1
+
+    def peek(self, n: int) -> int:
+        lo = self.bit - n
+        return ((self.v >> lo) if lo >= 0 else (self.v << -lo)) & ((1 << n) - 1)
+
+    def read(self, n: int) -> int:
+        v = self.peek(n)
+        self.bit -= n
+        return v
+
+    def end(self, what: str):
+        if self.bit:
+            raise Reject(f"{what}:bits-{'left' if self.bit > 0 else 'missing'}")
+
+
+def xxh64(data: bytes, seed: int = 0) -> int:
+    """XXH64 of `data` (the frame content checksum is its low 32 bits)."""
+    P1, P2, P3, P4, P5 = (0x9E3779B185EBCA87, 0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x85EBCA77C2B2AE63,
+                          0x27D4EB2F165667C5)
+    M = (1 << 64) - 1
+
+    def rotl(x, r):
+        return ((x << r) | (x >> (64 - r))) & M
+
+    def rnd(acc, v):
+        return rotl((acc + v * P2) & M, 31) * P1 & M
+
+    n, i = len(data), 0
+    if n >= 32:
+        v = [(seed + P1 + P2) & M, (seed + P2) & M, seed, (seed - P1) & M]
+        w = np.frombuffer(data[:n // 32 * 32], "<u8").reshape(-1, 4).tolist()
+        for row in w:
+            v = [rnd(v[k], row[k]) for k in range(4)]
+        i = n // 32 * 32
+        h = (rotl(v[0], 1) + rotl(v[1], 7) + rotl(v[2], 12) + rotl(v[3], 18)) & M
+        for x in v:
+            h = ((h ^ rnd(0, x)) * P1 + P4) & M
+    else:
+        h = (seed + P5) & M
+    h = (h + n) & M
+    while i + 8 <= n:
+        h = (rotl(h ^ rnd(0, int.from_bytes(data[i:i + 8], "little")), 27) * P1 + P4) & M
+        i += 8
+    if i + 4 <= n:
+        h = (rotl(h ^ (int.from_bytes(data[i:i + 4], "little") * P1 & M), 23) * P2 + P3) & M
+        i += 4
+    while i < n:
+        h = rotl(h ^ (data[i] * P5 & M), 11) * P1 & M
+        i += 1
+    h ^= h >> 33
+    h = h * P2 & M
+    h ^= h >> 29
+    h = h * P3 & M
+    return h ^ (h >> 32)
+
+
+def huf_weights(body: bytes):
+    """A Huffman_Tree_Description at body[0:] -> (its size, the weights of every symbol, the implied last one included,
+    the table log)."""
+    th = body[0]
+    if th >= 128:
+        nw = th - 127
+        size = 1 + (nw + 1) // 2
+        if len(body) < size:
+            raise Reject("tree:truncated")
+        w = [(body[1 + k // 2] >> (4 if k % 2 == 0 else 0)) & 15 for k in range(nw)]
+    else:
+        size = 1 + th
+        if len(body) < size:
+            raise Reject("tree:truncated")
+        try:
+            log, w = fse_weights_decode(body[1:size])
+        except (ValueError, IndexError):
+            raise Reject("tree:weights") from None
+        if log > 6 or len(w) > 255:
+            raise Reject("tree:weights")
+    if max(w) > HUF_MAXLOG:
+        raise Reject("tree:weights")
+    total = sum(1 << (x - 1) for x in w if x)
+    if total == 0:
+        raise Reject("tree:weights")
+    log = total.bit_length()
+    rest = (1 << log) - total
+    if log > HUF_MAXLOG:
+        raise Reject("tree:maxbits")
+    if rest & (rest - 1):
+        raise Reject("tree:incomplete")
+    return size, w + [rest.bit_length()], log
+
+
+class _Frame:
+    def __init__(self):
+        self.rep = [1, 4, 8]
+        self.huf = None                   # (decoding table, log) of the last tree
+        self.tab = [None, None, None]     # (decoding table, log, mode it was built in) per column
+        self.spans = []                   # (start, end, block type) of the frame's Raw and RLE blocks
+
+
+def _huf_table(w, log):
+    table = []
+    for wt in range(1, log + 1):
+        for s, x in enumerate(w):
+            if x == wt:
+                table += [(s, log + 1 - wt)] * (1 << (wt - 1))
+    return table
+
+
+def _huf_stream(data: bytes, table, log, n: int, what: str = "huf") -> bytes:
+    r = _Back(data, what)
+    out = bytearray(n)
+    for k in range(n):
+        s, nb = table[r.peek(log)]
+        out[k] = s
+        r.bit -= nb
+    r.end(what)
+    return bytes(out)
+
+
+_LIT_MAX = {("raw", 1): 31, ("raw", 2): 4095, ("huf", 0): 1023, ("huf", 1): 1023, ("huf", 2): 16383}
+
+
+def _decode_literals(body: bytes, f: _Frame, bmax: int, forms: Counter):
+    """The Literals_Section at body[0:] -> (literals, its size)."""
+    if not body:
+        raise Reject("lit:truncated")
+    t, sf = body[0] & 3, (body[0] >> 2) & 3
+    if t < 2:
+        h = 1 if sf in (0, 2) else 2 if sf == 1 else 3
+        if len(body) < h:
+            raise Reject("lit:truncated")
+        v = int.from_bytes(body[:h], "little")
+        n = v >> 3 if h == 1 else v >> 4
+        if n > bmax:
+            raise Reject("lit:size")
+        kind = ("raw", "rle")[t]
+        if n == _LIT_MAX.get(("raw", h)) or (h == 3 and n >= BLOCK_MAX - 5):
+            forms[f"lit:{kind}/{h}B:max"] += 1
+        if t == 0:
+            if len(body) < h + n:
+                raise Reject("lit:truncated")
+            return body[h:h + n], h + n
+        if len(body) < h + 1:
+            raise Reject("lit:truncated")
+        return body[h:h + 1] * n, h + 1
+    h, bits = {0: (3, 10), 1: (3, 10), 2: (4, 14), 3: (5, 18)}[sf]
+    if len(body) < h:
+        raise Reject("lit:truncated")
+    v = int.from_bytes(body[:h], "little")
+    regen, csize = (v >> 4) & ((1 << bits) - 1), (v >> (4 + bits)) & ((1 << bits) - 1)
+    four = sf != 0
+    if regen > bmax or h + csize > len(body):
+        raise Reject("lit:size")
+    if four and regen < 6:
+        raise Reject("huf:4x-small")
+    if regen == _LIT_MAX.get(("huf", sf)) or (sf == 3 and regen == BLOCK_MAX):
+        forms[f"lit:huf/sf{sf}:max"] += 1
+    q = body[h:h + csize]
+    if t == 2:
+        size, w, log = huf_weights(q)
+        f.huf = (_huf_table(w, log), log)
+        q = q[size:]
+        if log == 11:
+            forms["huf:maxbits11"] += 1
+        if len(w) == 256:
+            forms["huf:256sym"] += 1
+        if body[h] == 255:
+            forms["tree:direct/128"] += 1
+    elif f.huf is None:
+        raise Reject("lit:treeless-none")
+    table, log = f.huf
+    if t == 3:
+        forms[f"lit:treeless/{'4x' if four else '1x'}"] += 1
+    if four and regen <= 9:
+        forms[f"huf4:n{regen}"] += 1
+    if not four:
+        return _huf_stream(q, table, log, regen), h + csize
+    if len(q) < 6:
+        raise Reject("lit:size")
+    l1, l2, l3 = (int.from_bytes(q[k:k + 2], "little") for k in (0, 2, 4))
+    if l1 + l2 + l3 > len(q) - 6:
+        raise Reject("lit:size")
+    seg = (regen + 3) // 4
+    cuts = [6, 6 + l1, 6 + l1 + l2, 6 + l1 + l2 + l3, len(q)]
+    lits = b"".join(_huf_stream(q[cuts[k]:cuts[k + 1]], table, log, seg if k < 3 else regen - 3 * seg, f"huf4:s{k}")
+                    for k in range(4))
+    if regen - 3 * seg <= 1:
+        forms[f"huf:last{regen - 3 * seg}"] += 1
+    return lits, h + csize
+
+
+_COL_MAXLOG = (LL_MAXLOG, OF_MAXLOG, ML_MAXLOG)
+_PREDEF = {}
+
+
+def _decode_table(sec: bytes, pos: int, c: int, mode: int, f: _Frame, forms: Counter) -> int:
+    name, maxsym = COLUMNS[c]
+    if mode == 3:
+        if f.tab[c] is None:
+            raise Reject("modes:repeat-none")
+        forms[f"{name}:X-after-{MODE_LETTER[f.tab[c][2]]}"] += 1
+        return pos
+    if mode == 0:
+        if not _PREDEF:
+            from zstd_lz_ref import LL_NORM, OF_NORM, ML_NORM
+            for k, (norm, log) in enumerate(((LL_NORM, 6), (OF_NORM, 5), (ML_NORM, 6))):
+                _PREDEF[k] = (fse_decoding_table(norm, log), log)
+        f.tab[c] = (*_PREDEF[c], 0)
+        return pos
+    if mode == 1:
+        if pos >= len(sec) or sec[pos] > maxsym:
+            raise Reject("table:rle-symbol")
+        if sec[pos] == (24 if c == 1 else maxsym):      # OF: 24, the largest code a 16 MiB chunk can use
+            forms[f"{name}:rle/max"] += 1
+        f.tab[c] = ([(sec[pos], 0, 0)], 0, 1)
+        return pos + 1
+    if pos >= len(sec):
+        raise Reject("table:description")
+    if (sec[pos] & 15) + 5 > _COL_MAXLOG[c]:
+        raise Reject("table:log")
+    try:
+        log, counts, end = read_fse_description(sec + bytes(8), pos, maxsym)
+    except (ValueError, IndexError):
+        raise Reject("table:description") from None
+    if end > len(sec):
+        raise Reject("table:description")
+    forms[f"{name}:log{log}"] += 1
+    if len(counts) == maxsym + 1:
+        forms[f"{name}:maxsym"] += 1
+    if -1 in counts:
+        forms["fse:less1"] += 1
+    run = 0
+    for x in counts + [1]:
+        if x == 0:
+            run += 1
+            continue
+        if run == 4:
+            forms["fse:zeros+3"] += 1
+        elif run > 4:
+            forms["fse:zeros+4+"] += 1
+        run = 0
+    f.tab[c] = (fse_decoding_table(counts, log), log, 2)
+    return end
+
+
+def _decode_block(body: bytes, f: _Frame, out: bytearray, fstart: int, bmax: int, first_seq_block: bool,
+                  after_raw: bool, later_frame: bool, forms: Counter) -> bool:
+    """A Compressed_Block's content appended to out; True when it has sequences."""
+    from zstd_lz_ref import LL_BASE, LL_BITS, ML_BASE, ML_BITS
+    lits, used = _decode_literals(body, f, bmax, forms)
+    sec = body[used:]
+    if not sec:
+        raise Reject("seq:truncated")
+    n, k = sec[0], 1
+    if n == 0:
+        if len(sec) != 1:
+            raise Reject("seq:trailing")
+    elif n == 255:
+        if len(sec) < 3:
+            raise Reject("seq:truncated")
+        n, k = sec[1] + (sec[2] << 8) + 0x7F00, 3
+    elif n >= 128:
+        if len(sec) < 2:
+            raise Reject("seq:truncated")
+        n, k = ((n - 128) << 8) + sec[1], 2
+    b0, lpos = len(out), 0
+    if n:
+        if k >= len(sec):
+            raise Reject("seq:truncated")
+        m = sec[k]
+        if m & 3:
+            raise Reject("modes:reserved")
+        pos = k + 1
+        for c in range(3):
+            pos = _decode_table(sec, pos, c, (m >> (6 - 2 * c)) & 3, f, forms)
+        r = _Back(sec[pos:], "seq")
+        (tl, gl, _), (to, go, _), (tm, gm, _) = f.tab
+        if (m >> 2) & 0x3F == 0b101010:
+            forms[f"logs:{gl}/{go}/{gm}"] += 1
+        sl, so, sm = r.read(gl), r.read(go), r.read(gm)
+        new_offset, prev_idx = False, -1
+        for j in range(n):
+            lc, lb, lbase = tl[sl]
+            oc, ob, obase = to[so]
+            mc, mb, mbase = tm[sm]
+            ov = (1 << oc) + r.read(oc)
+            ml = ML_BASE[mc] + r.read(ML_BITS[mc])
+            ll = LL_BASE[lc] + r.read(LL_BITS[lc])
+            if j + 1 < n:
+                sl, sm, so = lbase + r.read(lb), mbase + r.read(mb), obase + r.read(ob)
+            rep = f.rep
+            if ov > 3:
+                off = ov - 3
+                f.rep = [off, rep[0], rep[1]]
+                new_offset, prev_idx = True, -1
+            else:
+                idx = ov - 1 + (ll == 0)
+                forms[f"rep:{ov}" + ("/ll0" if ll == 0 else "")] += 1
+                if idx == 3 and prev_idx == 3:
+                    forms["rep:3/ll0/twice"] += 1
+                prev_idx = idx
+                if not new_offset:
+                    if later_frame and first_seq_block:
+                        forms["rep:reset"] += 1
+                    elif not first_seq_block:
+                        forms["rep:across-raw" if after_raw else "rep:across-block"] += 1
+                off = (rep[0], rep[1], rep[2], rep[0] - 1)[idx]
+                f.rep = ([rep[0], rep[1], rep[2]], [rep[1], rep[0], rep[2]], [rep[2], rep[0], rep[1]],
+                         [rep[0] - 1, rep[0], rep[1]])[idx]
+            if lpos + ll > len(lits):
+                raise Reject("seq:literals-overrun")
+            if len(out) + ll + ml - b0 > bmax:
+                raise Reject("block:decoded-size")
+            here = len(out) + ll
+            if off <= 0:
+                raise Reject("seq:offset-zero")
+            if off > here - fstart:
+                raise Reject("seq:offset-beyond")
+            forms[f"ll:code{lc}"] += lc == 35
+            forms[f"ml:code{mc}"] += mc == 52
+            forms[f"of:code{oc}"] += oc >= 20
+            if LL_BITS[lc] >= 15 and ML_BITS[mc] >= 15 and oc >= 23:
+                forms[f"seq:wide/ll{LL_BITS[lc]}/ml{ML_BITS[mc]}"] += 1
+            if off == here - fstart and fstart:
+                forms["off:all"] += 1
+            for i, (s0, s1, bt) in enumerate(f.spans):
+                if s0 <= here - off < s1 < here - off + ml:
+                    forms[f"off:into-{bt}"] += 1
+                    if i + 1 < len(f.spans) and f.spans[i + 1][0] == s1:
+                        forms[f"off:{bt}-to-{f.spans[i + 1][2]}"] += 1
+            out += lits[lpos:lpos + ll]
+            lpos += ll
+            if off < ml:
+                forms["off:overlap"] += 1
+                if off <= 33 and ml >= off + 32:
+                    forms[f"off:{off}/overlap"] += 1
+                src = out[here - off:here]
+                out += (src * (ml // off + 1))[:ml]
+            else:
+                out += out[here - off:here - off + ml]
+        r.end("seq")
+    if len(out) + len(lits) - lpos - b0 > bmax:
+        raise Reject("block:decoded-size")
+    out += lits[lpos:]
+    return n > 0
+
+
+def decode_payload(payload: bytes, forms: Counter | None = None) -> bytes:
+    """The content of a blob payload: zstd frames with skippable frames between them.  Raises Reject; counts the edges
+    it passes in `forms`."""
+    forms = Counter() if forms is None else forms
+    data, out, q, nframe = bytes(payload), bytearray(), 0, 0
+    while q < len(data):
+        if len(data) - q < 4:
+            raise Reject("frame:truncated")
+        magic = int.from_bytes(data[q:q + 4], "little")
+        if magic & 0xFFFFFFF0 == 0x184D2A50:
+            if len(data) - q < 8:
+                raise Reject("skippable:header")
+            if int.from_bytes(data[q + 4:q + 8], "little") > len(data) - q - 8:
+                raise Reject("skippable:truncated")
+            q += 8 + int.from_bytes(data[q + 4:q + 8], "little")
+            continue
+        if magic != ZSTD_MAGIC:
+            raise Reject("frame:magic")
+        q += 4
+        if q >= len(data):
+            raise Reject("frame:truncated")
+        fhd = data[q]
+        q += 1
+        single, checksum, did = (fhd >> 5) & 1, (fhd >> 2) & 1, fhd & 3
+        if fhd & 8:
+            raise Reject("frame:reserved")
+        window = 0
+        if not single:
+            if q >= len(data):
+                raise Reject("frame:truncated")
+            wd = data[q]
+            q += 1
+            wlog = 10 + (wd >> 3)
+            window = (1 << wlog) + ((1 << wlog) >> 3) * (wd & 7)
+        dsz, fsz = (0, 1, 2, 4)[did], ((1 if single else 0), 2, 4, 8)[fhd >> 6]
+        if len(data) - q < dsz + fsz:
+            raise Reject("frame:truncated")
+        if any(data[q:q + dsz]):
+            raise Reject("frame:dictionary")
+        q += dsz
+        fcs = int.from_bytes(data[q:q + fsz], "little") + (256 if fsz == 2 else 0)
+        q += fsz
+        if fsz == 2 and fcs in (256, 65791):
+            forms[f"fcs:2/{fcs}"] += 1
+        if single:
+            window = fcs
+        if window > WINDOW_MAX:
+            raise Reject("frame:window/" + ("single" if single else f"m{wd & 7}"))
+        if not single:
+            forms[f"window:m{wd & 7}"] += 1
+        bmax = min(window, BLOCK_MAX)
+        f, fstart = _Frame(), len(out)
+        seq_blocks, prev_raw = 0, False
+        while True:
+            if len(data) - q < 3:
+                raise Reject("frame:truncated")
+            bh = int.from_bytes(data[q:q + 3], "little")
+            q += 3
+            bt, bsize = (bh >> 1) & 3, bh >> 3
+            start = len(out)
+            if bt == 3:
+                raise Reject("block:reserved")
+            if bt == 0:
+                if bsize > bmax:
+                    raise Reject("block:size/raw")
+                if bsize > len(data) - q:
+                    raise Reject("frame:truncated")
+                out += data[q:q + bsize]
+                q += bsize
+            elif bt == 1:
+                if bsize > bmax:
+                    raise Reject("block:size/rle")
+                if q >= len(data):
+                    raise Reject("frame:truncated")
+                out += data[q:q + 1] * bsize
+                q += 1
+            else:
+                if bsize == BLOCK_MAX:
+                    forms["block:content-128k"] += 1
+                if bsize > bmax:
+                    raise Reject("block:size/compressed")
+                if bsize > len(data) - q:
+                    raise Reject("frame:truncated")
+                if _decode_block(data[q:q + bsize], f, out, fstart, bmax, seq_blocks == 0, prev_raw, nframe > 0,
+                                 forms):
+                    seq_blocks += 1
+                q += bsize
+            kind = ("raw", "rle", "compressed")[bt]
+            if bt < 2:
+                f.spans.append((start, len(out), kind))
+            prev_raw = bt == 0 and seq_blocks > 0
+            if not single and len(out) - start == bmax and bmax < BLOCK_MAX:
+                forms[f"block:bmax/{kind}"] += 1
+            if bh & 1:
+                break
+        if fsz and len(out) - fstart != fcs:
+            raise Reject("frame:content-size")
+        if len(out) == fstart:
+            forms["frame:empty"] += 1
+        if checksum:
+            if len(data) - q < 4:
+                raise Reject("frame:truncated")
+            if xxh64(bytes(out[fstart:])) & 0xFFFFFFFF != int.from_bytes(data[q:q + 4], "little"):
+                raise Reject("frame:checksum")
+            if fstart % 8 and len(out) - fstart >= 32:
+                forms["checksum:unaligned"] += 1
+            q += 4
+        nframe += 1
+    return bytes(out)
+
+
+# The edges tests/zstd_edge_frames.edge_cases() must reach, read by decode_payload (tests/test_zstd_edges_cpu.py checks
+# the set, and that every case reaches one of them that no other case reaches; the GPU tests decode every case)
+REQUIRED_EDGES = {
+    "rep:1", "rep:2", "rep:3", "rep:1/ll0", "rep:2/ll0", "rep:3/ll0", "rep:3/ll0/twice",
+    "rep:across-block", "rep:across-raw", "rep:reset",
+    *(f"off:{k}/overlap" for k in range(1, 34)), "off:overlap", "off:all", "off:into-raw", "off:into-rle",
+    "off:raw-to-rle",
+    "ll:code35", "ml:code52", "of:code24", "seq:wide/ll16/ml15", "seq:wide/ll15/ml16",
+    *(f"{c}:log{k}" for c in ("LL", "ML") for k in range(5, 10)), *(f"OF:log{k}" for k in range(5, 9)),
+    "logs:5/5/5", "logs:6/6/6", "logs:7/7/7", "logs:8/8/8", "logs:9/8/9",
+    "LL:rle/max", "OF:rle/max", "ML:rle/max", "LL:maxsym", "OF:maxsym", "ML:maxsym",
+    "fse:less1", "fse:zeros+3", "fse:zeros+4+",
+    "LL:X-after-P", "LL:X-after-F", "OF:X-after-P", "OF:X-after-R", "ML:X-after-R", "ML:X-after-F",
+    "lit:raw/1B:max", "lit:raw/2B:max", "lit:raw/3B:max", "lit:rle/3B:max",
+    "lit:huf/sf0:max", "lit:huf/sf1:max", "lit:huf/sf2:max", "lit:huf/sf3:max",
+    "huf:last0", "huf:last1", "huf4:n6", "huf4:n7", "huf4:n8", "huf4:n9", "lit:treeless/1x", "lit:treeless/4x",
+    "huf:maxbits11", "huf:256sym", "tree:direct/128",
+    *(f"window:m{k}" for k in range(8)), "block:bmax/raw", "block:bmax/rle", "block:bmax/compressed",
+    "block:content-128k", "fcs:2/256", "fcs:2/65791", "frame:empty", "checksum:unaligned",
+    # rejections: K13's rules (DESIGN.md K13) and the stream ends
+    "reject:frame:window/m0", "reject:frame:window/m1", "reject:frame:window/single", "reject:frame:reserved",
+    "reject:frame:dictionary", "reject:block:reserved", "reject:block:size/raw", "reject:block:size/rle",
+    "reject:block:size/compressed", "reject:block:decoded-size", "reject:frame:content-size", "reject:frame:checksum",
+    "reject:frame:magic", "reject:skippable:header", "reject:skippable:truncated",
+    "reject:seq:offset-zero", "reject:seq:offset-beyond", "reject:seq:literals-overrun", "reject:seq:trailing",
+    "reject:modes:repeat-none", "reject:modes:reserved", "reject:table:rle-symbol", "reject:table:log",
+    "reject:table:description", "reject:seq:bits-left", "reject:seq:bits-missing", "reject:seq:end-mark",
+    "reject:lit:treeless-none", "reject:lit:size", "reject:huf:4x-small", "reject:huf:bits-left", "reject:huf:bits-missing",
+    *(f"reject:huf4:s{k}:bits-{e}" for k in range(4) for e in ("left", "missing")), "reject:huf:end-mark",
+    "reject:tree:incomplete", "reject:tree:weights",
+}
