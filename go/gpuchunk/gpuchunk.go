@@ -1010,3 +1010,181 @@ func (p *PayloadReader) ReadFiles(offsets, sizes []uint64) ([][]byte, error) {
 	}
 	return res, nil
 }
+
+// SeedFromFidx feeds the previous snapshot's .fidx of the same disk image (pbsgpu_set_seed_fidx), as the upstream
+// client does for fixed indexes: unchanged chunks of the image are not uploaded again.
+func (k *KnownSet) SeedFromFidx(fidx []byte) (uint64, error) {
+	if len(fidx) == 0 {
+		return 0, fmt.Errorf("pbsgpu: empty index image")
+	}
+	var n C.uint64_t
+	rc := C.pbsgpu_set_seed_fidx(k.s, (*C.uint8_t)(unsafe.Pointer(&fidx[0])), C.uint64_t(len(fidx)), &n)
+	return uint64(n), k.e.err(rc)
+}
+
+// ImageWriter backs up a disk image as a fixed index (<name>.img.fidx; a VM disk, or
+// `proxmox-backup-client backup disk.img:/dev/sdX`): the image is cut at every multiple of ChunkSize (upstream writes
+// 4 MiB), read in slices of whole chunks into C-owned pinned staging, and each slice goes through the GPU in one batch
+// call with fixed cuts (pbsgpu_batch_opts.fixed_size): SHA-256 per chunk (keyed with a crypt), probe against the known
+// set, and, with a blob mode, the DataBlob of every new chunk handed to Upload.
+type ImageWriter struct {
+	e         *Engine
+	known     *KnownSet
+	crypt     *Crypt
+	mode      int // BlobRaw .. BlobLZH, BlobLZL; 0 = no blobs
+	chunkSize uint64
+	buf       unsafe.Pointer
+	cap       uint64
+	size      uint64
+	ended     bool
+	digests   []byte
+	Upload    func(digest [32]byte, blob []byte) error
+}
+
+// NewImageWriter: chunkSize a power of two from 4 KiB to 16 MiB; stagingBytes is rounded down to whole chunks (at least
+// one).  known and c may be nil; blobMode 0 encodes no blobs.
+func (e *Engine) NewImageWriter(chunkSize uint32, known *KnownSet, c *Crypt, blobMode int, stagingBytes uint64) (*ImageWriter, error) {
+	cs := uint64(chunkSize)
+	if cs < 4096 || cs > 16<<20 || cs&(cs-1) != 0 {
+		return nil, fmt.Errorf("pbsgpu: chunk size %d is not a power of two from 4 KiB to 16 MiB", cs)
+	}
+	stagingBytes -= stagingBytes % cs
+	if stagingBytes == 0 {
+		stagingBytes = cs
+	}
+	p := C.pbsgpu_host_alloc(e.ctx, C.uint64_t(stagingBytes))
+	if p == nil {
+		return nil, errors.New("pbsgpu: pinned staging allocation failed")
+	}
+	return &ImageWriter{e: e, known: known, crypt: c, mode: blobMode, chunkSize: cs, buf: p, cap: stagingBytes}, nil
+}
+
+// WriteFrom pulls exactly size bytes of the image from r (io.ReadFull semantics).  It may be called again for the
+// bytes that follow as long as every call but the last covers whole chunks.
+func (w *ImageWriter) WriteFrom(r io.Reader, size uint64) error {
+	for size > 0 {
+		if w.ended {
+			return errors.New("pbsgpu: the image's last slice ended inside a chunk")
+		}
+		n := size
+		if n > w.cap {
+			n = w.cap
+		}
+		if _, err := io.ReadFull(r, unsafe.Slice((*byte)(w.buf), n)); err != nil {
+			return fmt.Errorf("read image: %w", err)
+		}
+		if err := w.slice(n); err != nil {
+			return err
+		}
+		size -= n
+	}
+	return nil
+}
+
+func (w *ImageWriter) slice(n uint64) error {
+	cs := w.chunkSize
+	nch := (n + cs - 1) / cs
+	out := make([]C.pbsgpu_chunk, nch)
+	off, ln := []C.uint64_t{0}, []C.uint64_t{C.uint64_t(n)}
+	var o C.pbsgpu_batch_opts
+	o.size = C.uint32_t(C.sizeof_pbsgpu_batch_opts)
+	o.fixed_size = C.uint32_t(cs)
+	if w.known != nil {
+		o.set = w.known.s
+	}
+	if w.crypt != nil {
+		o.crypt = w.crypt.c
+	}
+	var got C.uint64_t
+	rc := C.pbsgpu_chunk_digest_batch_ex(w.e.ctx, nil, w.buf, &off[0], &ln[0], 1, &o, &out[0], C.uint64_t(nch), &got)
+	if err := w.e.err(rc); err != nil {
+		return err
+	}
+	var newOff, newLen []uint64
+	var newDig [][32]byte
+	for i := 0; i < int(got); i++ {
+		var d [32]byte
+		copy(d[:], C.GoBytes(unsafe.Pointer(&out[i].digest[0]), 32))
+		w.digests = append(w.digests, d[:]...)
+		if out[i].flags&C.PBSGPU_CHUNK_KNOWN == 0 {
+			s := uint64(i) * cs
+			l := cs
+			if n-s < l {
+				l = n - s
+			}
+			newOff, newLen, newDig = append(newOff, s), append(newLen, l), append(newDig, d)
+		}
+	}
+	if w.mode != 0 && w.Upload != nil && len(newOff) > 0 {
+		b := &Batch{e: w.e, buf: w.buf, cap: w.cap}
+		var blobs [][]byte
+		var err error
+		switch {
+		case w.crypt != nil:
+			blobs, err = b.BlobEncodeEnc(w.crypt, w.mode, newOff, newLen)
+		case w.mode == int(BlobRaw):
+			blobs, err = b.BlobEncode(newOff, newLen)
+		case w.mode == int(BlobZ):
+			blobs, err = b.BlobEncodeZ(newOff, newLen)
+		case w.mode == int(BlobLZ):
+			blobs, err = b.BlobEncodeLZ(newOff, newLen)
+		case w.mode == int(BlobLZE):
+			blobs, err = b.BlobEncodeLZE(newOff, newLen)
+		case w.mode == int(BlobLZH):
+			blobs, err = b.BlobEncodeLZH(newOff, newLen)
+		default:
+			blobs, err = b.BlobEncodeLZL(newOff, newLen)
+		}
+		if err != nil {
+			return err
+		}
+		for i, blob := range blobs {
+			if err := w.Upload(newDig[i], blob); err != nil {
+				return err
+			}
+		}
+	}
+	w.size += n
+	w.ended = n%cs != 0
+	return nil
+}
+
+// Finish renders the image's .fidx (checksum on the GPU).
+func (w *ImageWriter) Finish(uuid [16]byte, ctime int64) ([]byte, error) {
+	n := uint64(len(w.digests) / 32)
+	out := make([]byte, uint64(C.pbsgpu_fidx_size(C.uint64_t(n))))
+	var dp *C.uint8_t
+	if n > 0 {
+		dp = (*C.uint8_t)(unsafe.Pointer(&w.digests[0]))
+	}
+	rc := C.pbsgpu_fidx_build(w.e.ctx, dp, C.uint64_t(n), C.uint64_t(w.size), C.uint64_t(w.chunkSize),
+		(*C.uint8_t)(unsafe.Pointer(&uuid[0])), C.int64_t(ctime), (*C.uint8_t)(unsafe.Pointer(&out[0])), C.uint64_t(len(out)))
+	if err := w.e.err(rc); err != nil {
+		return nil, err
+	}
+	return out, nil
+}
+
+func (w *ImageWriter) Close() { C.pbsgpu_host_free(w.e.ctx, w.buf) }
+
+// NewImageReader reads a disk image through its .fidx (pbsgpu_reader_open_fidx): the restore or map of a
+// `.img.fidx` archive.  ReadAt serves byte ranges of the image; ReadFiles fails (an image has no pxar headers).
+func (e *Engine) NewImageReader(fidx []byte, c *Crypt, cacheBytes uint64, source func([32]byte) ([]byte, error)) (*PayloadReader, error) {
+	if len(fidx) < 4096 {
+		return nil, fmt.Errorf("pbsgpu: index image too short")
+	}
+	var cr *C.pbsgpu_crypt
+	if c != nil {
+		cr = c.c
+	}
+	var r *C.pbsgpu_reader
+	if err := e.err(C.pbsgpu_reader_open_fidx(e.ctx, (*C.uint8_t)(unsafe.Pointer(&fidx[0])), C.uint64_t(len(fidx)), cr,
+		C.uint64_t(cacheBytes), &r)); err != nil {
+		return nil, err
+	}
+	dg := make([][32]byte, (len(fidx)-4096)/32)
+	for i := range dg {
+		copy(dg[i][:], fidx[4096+32*i:4096+32*i+32])
+	}
+	return &PayloadReader{e: e, r: r, source: source, digests: dg, size: uint64(C.pbsgpu_reader_size(r))}, nil
+}

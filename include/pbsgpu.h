@@ -148,7 +148,13 @@ int pbsgpu_batch_wait(pbsgpu_job *job, pbsgpu_chunk *out, uint64_t cap, uint64_t
  *    (jobs that share a set are ordered in submission order), flags come back with the records.
  *  - stream_xxh3[n] (may be NULL): as pbsgpu_chunk_digest_batch_xxh3 (synchronous form only).
  *  - crypt (may be NULL): keyed digests of encrypt mode (see pbsgpu_crypt_create).
- * `size` must be sizeof(pbsgpu_batch_opts) (forward compatibility; the size without `crypt` is accepted too). */
+ *  - fixed_size (0 = the chunker): cut every stream at fixed offsets instead -- chunk k covers [k * fixed_size,
+ *    min((k + 1) * fixed_size, len)), so only a stream's last chunk is short and an empty stream has no chunk: the chunks
+ *    of a fixed index (.fidx, pbsgpu_fidx_build).  A power of two from 4 KiB to 16 MiB (upstream writes 4 MiB); cfg may
+ *    then be NULL and n_forced must be 0 (PBSGPU_EINVAL otherwise).  No state crosses a chunk boundary, so an image of any
+ *    size can be fed as slices that start at multiples of fixed_size, one call per slice.
+ * `size` must be sizeof(pbsgpu_batch_opts) (forward compatibility; the sizes without `fixed_size` and without `crypt`
+ * are accepted too and give the fields of those layouts). */
 typedef struct pbsgpu_crypt pbsgpu_crypt;
 typedef struct pbsgpu_batch_opts {
     uint32_t size, flags;
@@ -161,6 +167,7 @@ typedef struct pbsgpu_batch_opts {
      * CryptConfig::compute_digest, and the set's probe + insert sees the keyed digests.  A caller built against the
      * header without this field passes that layout's size (offsetof(pbsgpu_batch_opts, crypt)) and gets plain digests. */
     const pbsgpu_crypt *crypt;
+    uint32_t fixed_size;   /* fixed cuts (see above); callers of the layout without it pass offsetof(pbsgpu_batch_opts, fixed_size) */
 } pbsgpu_batch_opts;
 int pbsgpu_chunk_digest_batch_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base, const uint64_t *off,
                                  const uint64_t *len, uint32_t n, const pbsgpu_batch_opts *opts, pbsgpu_chunk *out,
@@ -264,6 +271,9 @@ int pbsgpu_set_count(pbsgpu_set *set, uint64_t *count);
 /* Seed from a PBS dynamic index (.didx) image: 4096-byte header + 40-byte
  * {u64 end_le, digest[32]} entries (what origPayloadIdx holds, commit.go:324-329). */
 int pbsgpu_set_seed_didx(pbsgpu_set *set, const uint8_t *didx, uint64_t size, uint64_t *n_entries);
+/* Seed from a PBS fixed index (.fidx) image, the previous snapshot's index of the same disk image (as the upstream
+ * client does for fixed indexes): its digests, after pbsgpu_fidx_parse's checks without the checksum. */
+int pbsgpu_set_seed_fidx(pbsgpu_set *set, const uint8_t *fidx, uint64_t bytes, uint64_t *n_entries);
 
 /* ---- e: multi-GPU merge of the digest set (SURVEY.md section 8 e / 8 b) -----------------------------------------
  * One process (or thread) per GPU chunks its own shard of the files; the ONE exchange step is an NCCL all-gather of
@@ -293,6 +303,24 @@ int pbsgpu_didx_build(pbsgpu_ctx *ctx, const pbsgpu_chunk *chunks, uint64_t n, c
 /* ends / digests may be NULL to only count; verify != 0 recomputes index_csum (PBSGPU_EINVAL on mismatch). */
 int pbsgpu_didx_parse(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t size, uint64_t *ends, uint8_t *digests,
                       uint64_t cap, uint64_t *n_entries, int verify);
+
+/* ---- PBS fixed index (.fidx) images: disk images (`<name>.img.fidx`; a VM backup, or proxmox-backup-client backup
+ * disk.img:/dev/sdX).  Layout restated from upstream PBS pbs-datastore fixed_index.rs (UNVERIFIED against the Go
+ * module): 4096-byte header { magic[8] = 2f 7f 41 ed 91 fd 0f cd, uuid[16], ctime i64 LE, index_csum[32] = SHA-256 over
+ * the digest table, size u64 LE (image bytes), chunk_size u64 LE, zero padding } followed by n = ceil(size / chunk_size)
+ * digests of 32 bytes; chunk i covers [i * chunk_size, min((i + 1) * chunk_size, size)).  The records of a batch call
+ * with pbsgpu_batch_opts.fixed_size = chunk_size over the image give those digests in order. */
+uint64_t pbsgpu_fidx_size(uint64_t n_chunks);
+/* digests: n x 32 bytes (HOST); n must be ceil(size / chunk_size), chunk_size in [1, 2^32) (PBSGPU_EINVAL otherwise).
+ * The checksum is computed on the GPU. */
+int pbsgpu_fidx_build(pbsgpu_ctx *ctx, const uint8_t *digests, uint64_t n, uint64_t size, uint64_t chunk_size,
+                      const uint8_t uuid[16], int64_t ctime, uint8_t *out, uint64_t cap);
+/* size / chunk_size (may be NULL) receive the header's fields, *n_entries the chunk count; digests (may be NULL to only
+ * count) receives n x 32 bytes (PBSGPU_ERANGE when cap < n).  PBSGPU_EINVAL for a wrong magic, a chunk_size of 0 or of
+ * 2^32 and more, a length other than 4096 + 32 * ceil(size / chunk_size), and with verify != 0 a checksum mismatch
+ * (recomputed on the GPU; ctx may be NULL without verify). */
+int pbsgpu_fidx_parse(pbsgpu_ctx *ctx, const uint8_t *fidx, uint64_t bytes, uint64_t *size, uint64_t *chunk_size,
+                      uint8_t *digests, uint64_t cap, uint64_t *n_entries, int verify);
 
 /* ---- f3 ("next" row): DataBlob checksums for NEW chunks ---------------------------------------
  * A new chunk is uploaded as a PBS DataBlob { magic[8], crc32 LE of the payload, payload } (upstream
@@ -460,6 +488,11 @@ int pbsgpu_blob_decode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, con
 typedef struct pbsgpu_reader pbsgpu_reader;
 int pbsgpu_reader_open(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t size, const pbsgpu_crypt *crypt,
                        uint64_t cache_bytes, pbsgpu_reader **out);
+/* A reader over a disk image's fixed index (.fidx, parsed and verified with pbsgpu_fidx_parse's rules): chunk i ends at
+ * min((i + 1) * chunk_size, size), and plan, read, size and close behave as for a .didx reader.  An image has no pxar
+ * headers: PBSGPU_READ_PAYLOAD on such a reader is PBSGPU_EINVAL. */
+int pbsgpu_reader_open_fidx(pbsgpu_ctx *ctx, const uint8_t *fidx, uint64_t bytes, const pbsgpu_crypt *crypt,
+                            uint64_t cache_bytes, pbsgpu_reader **out);
 void pbsgpu_reader_close(pbsgpu_reader *r);
 uint64_t pbsgpu_reader_size(const pbsgpu_reader *r);
 #define PBSGPU_READ_PAYLOAD 1u

@@ -9,6 +9,9 @@
 //     writer.Finish()                                            :383
 // Go `error` returns become pbsgpu::Error exceptions carrying the same text a Go caller would wrap.
 #pragma once
+#include <sys/random.h>
+
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <deque>
@@ -62,6 +65,11 @@ class KnownSet {   // the session's known-chunk set (PreviousBackupRef, commit.g
     uint64_t SeedFromDidx(const std::vector<uint8_t> &didx) {   // origPayloadIdx, commit.go:324-328
         uint64_t n = 0;
         if (!didx.empty()) e_.check(pbsgpu_set_seed_didx(s_, didx.data(), didx.size(), &n));
+        return n;
+    }
+    uint64_t SeedFromFidx(const std::vector<uint8_t> &fidx) {   // the previous snapshot's index of the same disk image
+        uint64_t n = 0;
+        e_.check(pbsgpu_set_seed_fidx(s_, fidx.data(), fidx.size(), &n));
         return n;
     }
     uint64_t size() const { uint64_t c = 0; pbsgpu_set_count(s_, &c); return c; }
@@ -126,7 +134,7 @@ class DedupWriter {
         std::vector<uint64_t> xxh(entries_.size());
         uint64_t n = 0;
         pbsgpu_batch_opts o = {sizeof(pbsgpu_batch_opts), 0, known_ ? known_->handle() : nullptr, nullptr, nullptr, 0,
-                               xxh.data(), crypt_ ? crypt_->handle() : nullptr};
+                               xxh.data(), crypt_ ? crypt_->handle() : nullptr, 0};
         e_.check(pbsgpu_chunk_digest_batch_ex(e_.ctx(), &cfg_, buf_, off_.data(), len_.data(), (uint32_t)entries_.size(), &o,
                                               out.data(), out.size(), &n));
         for (size_t i = 0; i < entries_.size(); i++) backed_hashes_[entries_[i].Path] = xxh[i];
@@ -274,6 +282,93 @@ class PayloadStreamWriter {
     std::deque<size_t> pending_;          // index_ positions of new chunks whose blob has not come back yet
     std::deque<std::string> hashed_;      // paths whose hash has not come back yet
     std::map<std::string, uint64_t> backed_hashes_;
+};
+
+// ---- disk images: a fixed index (<name>.img.fidx) ---------------------------------------------------------------------
+// The image is cut at every multiple of `chunk_size` (upstream writes 4 MiB).  WriteSlice takes the next bytes of the
+// image (HOST or DEVICE memory); every slice but the last is a multiple of chunk_size.  Each chunk is digested on the
+// GPU (keyed with `crypt`) and probed against `known` (seed it with KnownSet::SeedFromFidx); with a blob mode
+// (PBSGPU_BLOB_RAW .. _LZH, _LZL), every new chunk's DataBlob goes to `upload_blob` (encrypted with `crypt`, IVs from
+// getrandom).  Finish() renders the .fidx.
+class FixedIndexWriter {
+  public:
+    FixedIndexWriter(Engine &e, uint32_t chunk_size, KnownSet *known, int blob_mode = PBSGPU_BLOB_NONE,
+                     UploadBlob upload_blob = nullptr, const CryptConfig *crypt = nullptr)
+        : e_(e), cs_(chunk_size), known_(known), mode_(blob_mode), upload_(std::move(upload_blob)), crypt_(crypt) {
+        if ((mode_ != PBSGPU_BLOB_NONE) != (upload_ != nullptr))
+            throw Error(PBSGPU_EINVAL, "transfer: a blob mode and an upload_blob callback go together");
+    }
+    void WriteSlice(const uint8_t *data, uint64_t len) {
+        if (len == 0) return;
+        if (ended_) throw Error(PBSGPU_EINVAL, "transfer: the image's last slice ended inside a chunk; no slice may follow it");
+        const uint64_t off = 0, n = (len + cs_ - 1) / cs_;
+        std::vector<pbsgpu_chunk> out(n);
+        uint64_t got = 0;
+        pbsgpu_batch_opts o = {sizeof(pbsgpu_batch_opts), 0, known_ ? known_->handle() : nullptr, nullptr, nullptr, 0,
+                               nullptr, crypt_ ? crypt_->handle() : nullptr, cs_};
+        e_.check(pbsgpu_chunk_digest_batch_ex(e_.ctx(), nullptr, data, &off, &len, 1, &o, out.data(), n, &got));
+        std::vector<uint64_t> boff, blen;
+        std::vector<const uint8_t *> bdig;
+        for (uint64_t i = 0; i < got; i++) {
+            digests_.insert(digests_.end(), out[i].digest, out[i].digest + 32);
+            known_flags_.push_back((out[i].flags & PBSGPU_CHUNK_KNOWN) != 0);
+            if (!known_flags_.back()) { boff.push_back(i * cs_); blen.push_back(std::min<uint64_t>(cs_, len - i * cs_)); bdig.push_back(out[i].digest); }
+        }
+        if (upload_ && !boff.empty()) upload(data, boff, blen, bdig);
+        size_ += len;
+        ended_ = len % cs_ != 0;
+    }
+    // The image's .fidx (checksum on the GPU).
+    std::vector<uint8_t> Finish(const uint8_t uuid[16] = nullptr, int64_t ctime = 0) {
+        const uint8_t zero[16] = {};
+        const uint64_t n = digests_.size() / 32;
+        std::vector<uint8_t> img(pbsgpu_fidx_size(n));
+        e_.check(pbsgpu_fidx_build(e_.ctx(), digests_.data(), n, size_, cs_, uuid ? uuid : zero, ctime, img.data(), img.size()));
+        return img;
+    }
+    const std::vector<uint8_t> &Digests() const { return digests_; }   // 32 bytes per chunk, in image order
+    const std::vector<bool> &Known() const { return known_flags_; }
+    uint64_t Size() const { return size_; }
+
+  private:
+    void upload(const uint8_t *data, const std::vector<uint64_t> &off, const std::vector<uint64_t> &len,
+                const std::vector<const uint8_t *> &dig) {
+        const uint32_t n = (uint32_t)off.size();
+        std::vector<uint64_t> out_off(n + 1, 0), out_len(n);
+        for (uint32_t i = 0; i < n; i++)
+            out_off[i + 1] = out_off[i] + (crypt_ ? pbsgpu_blob_size_enc(len[i]) : pbsgpu_blob_size(len[i]));
+        std::vector<uint8_t> buf(out_off[n]);
+        if (crypt_) {
+            std::vector<uint8_t> iv(16ull * n);
+            for (size_t k = 0; k < iv.size();) {
+                const ssize_t r = getrandom(iv.data() + k, iv.size() - k, 0);
+                if (r <= 0) throw Error(PBSGPU_EINVAL, "transfer: getrandom failed");
+                k += (size_t)r;
+            }
+            e_.check(pbsgpu_blob_encode_batch_enc(e_.ctx(), crypt_->handle(), mode_, data, off.data(), len.data(), n, iv.data(),
+                                                  buf.data(), out_off.data(), out_len.data(), nullptr));
+        } else if (mode_ == PBSGPU_BLOB_RAW) {
+            e_.check(pbsgpu_blob_encode_batch(e_.ctx(), data, off.data(), len.data(), n, buf.data(), out_off.data(), nullptr));
+            for (uint32_t i = 0; i < n; i++) out_len[i] = out_off[i + 1] - out_off[i];
+        } else {
+            auto fn = mode_ == PBSGPU_BLOB_Z ? pbsgpu_blob_encode_batch_z : mode_ == PBSGPU_BLOB_LZ ? pbsgpu_blob_encode_batch_lz
+                    : mode_ == PBSGPU_BLOB_LZE ? pbsgpu_blob_encode_batch_lze : mode_ == PBSGPU_BLOB_LZH ? pbsgpu_blob_encode_batch_lzh
+                    : mode_ == PBSGPU_BLOB_LZL ? pbsgpu_blob_encode_batch_lzl : nullptr;
+            if (!fn) throw Error(PBSGPU_EINVAL, "transfer: unknown blob mode " + std::to_string(mode_));
+            e_.check(fn(e_.ctx(), data, off.data(), len.data(), n, buf.data(), out_off.data(), out_len.data(), nullptr));
+        }
+        for (uint32_t i = 0; i < n; i++) upload_(dig[i], buf.data() + out_off[i], out_len[i]);
+    }
+    Engine &e_;
+    uint32_t cs_;
+    KnownSet *known_;
+    int mode_;
+    UploadBlob upload_;
+    const CryptConfig *crypt_;
+    std::vector<uint8_t> digests_;
+    std::vector<bool> known_flags_;
+    uint64_t size_ = 0;
+    bool ended_ = false;
 };
 
 }  // namespace transfer

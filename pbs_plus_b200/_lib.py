@@ -69,6 +69,15 @@ class BatchOpts(C.Structure):
                 ("forced_off", C.c_void_p), ("n_forced", C.c_uint64), ("stream_xxh3", C.c_void_p), ("crypt", C.c_void_p)]
 
 
+class BatchOptsFixed(BatchOpts):
+    """pbsgpu_batch_opts in its current layout: BatchOpts (the layout up to `crypt`, which the library still accepts)
+    plus `fixed_size`, the fixed cuts of a .fidx image (0 = the chunker)."""
+    _fields_ = [("fixed_size", C.c_uint32)]
+
+
+FIDX_MAGIC = bytes([0x2f, 0x7f, 0x41, 0xed, 0x91, 0xfd, 0x0f, 0xcd])   # sha256("Proxmox Backup fixed sized chunk index v1.0")[:8]
+
+
 class Corpus(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("file_len", C.c_uint64), ("block_len", C.c_uint64),
                 ("run_blocks", C.c_uint32), ("dup_permille", C.c_uint32), ("edit_mode", C.c_uint32),
@@ -87,7 +96,8 @@ SYMBOLS = [
     "pbsgpu_stream_poll_blobs", "pbsgpu_stream_hash_range", "pbsgpu_stream_poll_hashes", "pbsgpu_set_create",
     "pbsgpu_set_destroy", "pbsgpu_set_insert", "pbsgpu_set_probe", "pbsgpu_set_count", "pbsgpu_set_seed_didx",
     "pbsgpu_set_allgather", "pbsgpu_nccl_unique_id", "pbsgpu_nccl_comm_create", "pbsgpu_nccl_comm_destroy",
-    "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
+    "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_fidx_size", "pbsgpu_fidx_build", "pbsgpu_fidx_parse",
+    "pbsgpu_set_seed_fidx", "pbsgpu_reader_open_fidx", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
     "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
     "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
     "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch", "pbsgpu_blob_decode_batch_enc",
@@ -193,6 +203,12 @@ def lib() -> C.CDLL:
     L.pbsgpu_didx_size.restype = C.c_uint64
     L.pbsgpu_didx_build.argtypes = [vp, vp, C.c_uint64, vp, C.c_int64, vp, C.c_uint64]
     L.pbsgpu_didx_parse.argtypes = [vp, vp, C.c_uint64, vp, vp, C.c_uint64, u64p, C.c_int]
+    L.pbsgpu_set_seed_fidx.argtypes = [vp, vp, C.c_uint64, u64p]
+    L.pbsgpu_fidx_size.argtypes = [C.c_uint64]
+    L.pbsgpu_fidx_size.restype = C.c_uint64
+    L.pbsgpu_fidx_build.argtypes = [vp, vp, C.c_uint64, C.c_uint64, C.c_uint64, vp, C.c_int64, vp, C.c_uint64]
+    L.pbsgpu_fidx_parse.argtypes = [vp, vp, C.c_uint64, u64p, u64p, vp, C.c_uint64, u64p, C.c_int]
+    L.pbsgpu_reader_open_fidx.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(vp)]
     L.pbsgpu_crc32_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
     L.pbsgpu_xxh3_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
     L.pbsgpu_chunk_digest_batch_xxh3.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, vp, vp, C.c_uint64, u64p, vp]

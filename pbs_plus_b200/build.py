@@ -61,17 +61,19 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
 
 def build_cxx_driver() -> Path:
-    """C++ caller of the C ABI through include/pbsgpu.hpp (stands in for the Go caller)."""
+    """C++ callers of the C ABI through include/pbsgpu.hpp (they stand in for the Go caller): tests/cxx/*.cpp, each
+    to a .bin beside it.  Returns the main driver's path."""
     root = HERE.parent
-    src, out = root / "tests" / "cxx" / "driver.cpp", root / "tests" / "cxx" / "driver.bin"
-    if not src.exists():
-        return out
-    dep = max(src.stat().st_mtime, (root / "include" / "pbsgpu.hpp").stat().st_mtime,
-              (root / "include" / "pbsgpu.h").stat().st_mtime)
-    if not out.exists() or out.stat().st_mtime < dep:
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-o", str(out), str(src), f"-L{HERE}", "-lpbsgpu",
-                               "-Wl,-rpath,$ORIGIN/../../pbs_plus_b200"])
-    return out
+    for name in ("driver", "fidx_driver"):
+        src, out = root / "tests" / "cxx" / f"{name}.cpp", root / "tests" / "cxx" / f"{name}.bin"
+        if not src.exists():
+            continue
+        dep = max(src.stat().st_mtime, (root / "include" / "pbsgpu.hpp").stat().st_mtime,
+                  (root / "include" / "pbsgpu.h").stat().st_mtime)
+        if not out.exists() or out.stat().st_mtime < dep:
+            subprocess.check_call(["g++", "-O2", "-std=c++17", "-o", str(out), str(src), f"-L{HERE}", "-lpbsgpu",
+                                   "-Wl,-rpath,$ORIGIN/../../pbs_plus_b200"])
+    return root / "tests" / "cxx" / "driver.bin"
 
 
 if __name__ == "__main__":

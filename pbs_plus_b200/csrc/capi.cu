@@ -473,9 +473,39 @@ static int job_alloc(pbsgpu_job *j) {
     return PBSGPU_OK;
 }
 
+static int job_place(pbsgpu_job *j, pbsgpu_job **out);
+
+// A job with fixed cuts of `fixed_size` bytes (a power of two, checked by the caller): no chunker table, no candidates.
+// Its cfg is the chunk size in every field the back half reads: avg = max = fixed_size keeps every chunk below the hybrid
+// launch's threshold (thr_x10 / 10 x avg), so the equal-length chunks all take the throughput kernel -- the latency
+// kernel only pays for the few chunks far longer than the rest, and fixed chunks have no such tail.
+static int job_create_fixed(pbsgpu_ctx *ctx, const void *base_dev, const uint64_t *off, const uint64_t *len, uint32_t n,
+                            pbsgpu_set *set, uint64_t n_forced, uint32_t fixed_size, pbsgpu_job **out) {
+    if (n >= (1u << 24)) return fail(ctx, PBSGPU_EINVAL, "too many streams in one batch (%u >= 2^24)", n);
+    if (set && set->ctx != ctx) return fail(ctx, PBSGPU_EINVAL, "set belongs to another context");
+    if (n_forced) return fail(ctx, PBSGPU_EINVAL, "suggested boundaries do not apply to fixed-size chunks");
+    pbsgpu_job *j = new pbsgpu_job();
+    j->ctx = ctx; j->base = (const uint8_t *)base_dev; j->n = n; j->eof = 1;
+    j->want_digests = 1; j->variant = ctx->variant; j->profiling = ctx->profiling; j->set = set;
+    memset(&j->cfg, 0, sizeof j->cfg);
+    j->cfg.avg = j->cfg.min = j->cfg.max = fixed_size;
+    while ((1u << j->fixed_log2) < fixed_size) j->fixed_log2++;
+    j->off.assign(off, off + n); j->len.assign(len, len + n);
+    uint64_t total = 0, chunks = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (len[i] >= (1ull << KEY_POS_BITS)) { delete j; return fail(ctx, PBSGPU_EINVAL, "stream %u longer than 2^40 bytes", i); }
+        total += len[i];
+        chunks += (len[i] + fixed_size - 1) >> j->fixed_log2;
+    }
+    j->total_bytes = total; j->chunk_cap = chunks; j->cand_cap = 0;
+    if (chunks >= (1ull << 31)) { delete j; return fail(ctx, PBSGPU_EINVAL, "batch too large (%llu chunks)", (unsigned long long)chunks); }
+    return job_place(j, out);
+}
+
 int pbsgpu_job_create(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base_dev, const uint64_t *off, const uint64_t *len,
                       uint32_t n, int eof, int want_digests, pbsgpu_set *set, const uint32_t *forced_stream,
-                      const uint64_t *forced_off, uint64_t n_forced, pbsgpu_job **out) {
+                      const uint64_t *forced_off, uint64_t n_forced, pbsgpu_job **out, uint32_t fixed_size) {
+    if (fixed_size) return job_create_fixed(ctx, base_dev, off, len, n, set, n_forced, fixed_size, out);
     if (!pbsgpu_cfg_ok(cfg)) return fail(ctx, PBSGPU_EINVAL, "invalid pbsgpu_cfg (use pbsgpu_config)");
     if (n >= (1u << 24)) return fail(ctx, PBSGPU_EINVAL, "too many streams in one batch (%u >= 2^24)", n);
     if (set && set->ctx != ctx) return fail(ctx, PBSGPU_EINVAL, "set belongs to another context");
@@ -523,6 +553,12 @@ int pbsgpu_job_create(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base_d
     if (chunks >= (1ull << 31)) { delete j; return fail(ctx, PBSGPU_EINVAL, "batch too large (%llu chunk slots)", (unsigned long long)chunks); }
     j->cand_cap = expected_cand_cap(*cfg, total) + n_forced;
     if (j->cand_cap >= (1ull << 31)) { delete j; return fail(ctx, PBSGPU_EINVAL, "batch too large (candidate buffer)"); }
+    return job_place(j, out);
+}
+
+// The job's streams, buffers and events; releases the job on failure.
+static int job_place(pbsgpu_job *j, pbsgpu_job **out) {
+    pbsgpu_ctx *ctx = j->ctx;
     j->st = ctx->streams[ctx->next_stream];
     j->st2 = ctx->streams2[ctx->next_stream];
     j->st3 = ctx->streams3[ctx->next_stream];
@@ -598,6 +634,20 @@ int pbsgpu_job_enqueue_front(pbsgpu_job *j) {
     cudaStream_t st = j->ss;   // the scan partition's stream (= the job's own stream when the GPU has no scan partition)
     const uint32_t n = j->n;
     j->state = JOB_FRONT;
+    if (j->fixed_log2) {   // fixed cuts: one small chain instead of K1 -> sort -> K2
+        if (n) {
+            CK(cudaMemcpyAsync(j->d_off, j->off.data(), n * 8, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(j->d_len, j->len.data(), n * 8, cudaMemcpyHostToDevice, st));
+        }
+        CK(cudaMemsetAsync(j->d_counters, 0, CTR_DEVICE * sizeof(unsigned long long), st));
+        if (j->profiling) CK(cudaEventRecord(j->ev[EV_START], st));
+        CK(cudaEventRecord(j->ev[EV_SCAN], st));
+        if (j->profiling) CK(cudaEventRecord(j->ev[EV_SORT], st));
+        CK(launch_fixed_refs(j->d_len, n, j->fixed_log2, j->d_counts, j->d_chunk_first, &j->d_counters[CTR_CHUNKS], j->chunk_cap,
+                             j->d_chunks, st));
+        CK(cudaEventRecord(j->ev[EV_RESOLVE], st));
+        return PBSGPU_OK;
+    }
     int rc = upload_table(ctx, &j->cfg, st);
     if (rc) return rc;
     if (n) {
@@ -676,7 +726,8 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
             // early input release: the head chunks are copied to the arena and hashed from there
             // (the copy runs HERE, on the job's own stream and the big partition -- a few ms -- not on the side stream,
             // where it would queue behind the 0.3 s latency kernel of the slot's previous job)
-            early = j->early && !serial && !use_mid && arena_reserve(j, st);
+            // (a fixed-cut job has no head chunks: its bulk pass is the whole job, so it takes no arena)
+            early = j->early && !j->fixed_log2 && !serial && !use_mid && arena_reserve(j, st);
             if (early) {
                 CK(launch_arena_plan(ha, &j->d_counters[CTR_HEAD], j->arena_len, j->d_arena_off, st));
                 CK(launch_arena_gather(ha, ctx->arena + j->arena_lo, j->d_arena_off, ctx->sm_count, st));
@@ -781,7 +832,7 @@ int pbsgpu_job_finish(pbsgpu_job *j) {
     j->state = JOB_FINISHED;
     pbsgpu_timing &t = j->timing;
     t.bytes = j->total_bytes; t.chunks = j->h_counters[CTR_CHUNKS]; t.candidates = j->h_counters[CTR_CANDIDATES]; t.reruns = j->reruns;
-    t.scan_launches = 1;
+    t.scan_launches = j->fixed_log2 ? 0 : 1;
     const bool hyb = j->variant == 0 && hybrid_for(ctx);
     t.sha_launches = j->want_digests ? (hyb ? 2 : 1) : 0;
     t.other_launches = 3 + (j->d_forced ? 1 : 0) + (j->want_digests ? 2 + (hyb ? 1 : 0) : 0) + (j->set ? 3 : 0) + (j->early_active ? 2 : 0);
@@ -805,17 +856,22 @@ int pbsgpu_job_finish(pbsgpu_job *j) {
     return PBSGPU_OK;
 }
 
-static const pbsgpu_batch_opts NO_OPTS = {sizeof(pbsgpu_batch_opts), 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr};
-// The caller's options in the current layout.  A caller built against the header before `crypt` passes that layout's
-// size (the offset of `crypt`) and gets plain digests.
+static const pbsgpu_batch_opts NO_OPTS = {sizeof(pbsgpu_batch_opts), 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr, 0};
+// The caller's options in the current layout.  A caller built against an older header passes that layout's size (the
+// offset of `crypt`: plain digests; the offset of `fixed_size`: the chunker) and gets the fields it knows.
 static int opts_read(pbsgpu_ctx *ctx, const pbsgpu_batch_opts *o, pbsgpu_batch_opts *out) {
     *out = NO_OPTS;
     if (!o) return PBSGPU_OK;
-    if (o->size != sizeof(pbsgpu_batch_opts) && o->size != offsetof(pbsgpu_batch_opts, crypt))
+    if (o->size != sizeof(pbsgpu_batch_opts) && o->size != offsetof(pbsgpu_batch_opts, fixed_size) &&
+        o->size != offsetof(pbsgpu_batch_opts, crypt))
         return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.size = %u, expected %zu", o->size, sizeof(pbsgpu_batch_opts));
     memcpy(out, o, o->size);
     if (out->flags & ~(uint32_t)PBSGPU_BATCH_EARLY_INPUT) return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.flags = 0x%x: unknown bits", out->flags);
     if (out->crypt && out->crypt->ctx != ctx) return fail(ctx, PBSGPU_EINVAL, "crypt belongs to another context");
+    const uint32_t fs = out->fixed_size;
+    if (fs && (fs < 4096u || fs > (16u << 20) || (fs & (fs - 1))))
+        return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_opts.fixed_size = %u: a power of two from 4 KiB to 16 MiB", fs);
+    if (fs && out->n_forced) return fail(ctx, PBSGPU_EINVAL, "suggested boundaries do not apply to fixed-size chunks");
     return PBSGPU_OK;
 }
 
@@ -830,7 +886,7 @@ extern "C" int pbsgpu_batch_submit_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, co
     if (o.stream_xxh3) return fail(ctx, PBSGPU_EINVAL, "stream_xxh3 is a synchronous-form option");
     if (n && !pbsgpu_is_device_ptr(base_dev)) return fail(ctx, PBSGPU_EINVAL, "pbsgpu_batch_submit needs a device pointer");
     pbsgpu_job *j = nullptr;
-    rc = pbsgpu_job_create(ctx, cfg, base_dev, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j);
+    rc = pbsgpu_job_create(ctx, cfg, base_dev, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j, o.fixed_size);
     if (rc) return rc;
     j->early = (o.flags & PBSGPU_BATCH_EARLY_INPUT) != 0;
     j->sha_suffix = pbsgpu_crypt_id_key(o.crypt);
@@ -991,7 +1047,7 @@ static int batch_host(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const uint8_t *bas
         for (auto &s : fs) s -= g.first;
         pbsgpu_job *j = nullptr;
         rc = pbsgpu_job_create(ctx, cfg, buf, goff.data(), glen.data(), g.count, 1, 1, o.set, fs.data(), o.forced_off + g.f_lo,
-                               g.f_hi - g.f_lo, &j);
+                               g.f_hi - g.f_lo, &j, o.fixed_size);
         if (rc) break;
         j->sha_suffix = pbsgpu_crypt_id_key(o.crypt);
         cudaStreamWaitEvent(j->ss, copied[gi], 0);
@@ -1017,12 +1073,12 @@ extern "C" int pbsgpu_chunk_digest_batch_ex(pbsgpu_ctx *ctx, const pbsgpu_cfg *c
     int rc = opts_read(ctx, opts, &o);
     if (rc) return rc;
     if (o.set && o.set->ctx != ctx) return fail(ctx, PBSGPU_EINVAL, "set belongs to another context");
-    if (!pbsgpu_cfg_ok(cfg)) return fail(ctx, PBSGPU_EINVAL, "invalid pbsgpu_cfg (use pbsgpu_config)");
+    if (!o.fixed_size && !pbsgpu_cfg_ok(cfg)) return fail(ctx, PBSGPU_EINVAL, "invalid pbsgpu_cfg (use pbsgpu_config)");
     uint64_t produced = 0;
     if (n == 0) { if (n_out) *n_out = 0; return PBSGPU_OK; }
     if (pbsgpu_is_device_ptr(base)) {   // device input: one job over all streams
         pbsgpu_job *j = nullptr;
-        rc = pbsgpu_job_create(ctx, cfg, base, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j);
+        rc = pbsgpu_job_create(ctx, cfg, base, off, len, n, 1, 1, o.set, o.forced_stream, o.forced_off, o.n_forced, &j, o.fixed_size);
         if (rc) return rc;
         j->sha_suffix = pbsgpu_crypt_id_key(o.crypt);
         XxhRun xr;

@@ -113,6 +113,63 @@ extern "C" int pbsgpu_didx_parse(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t 
 }
 
 // ---------------------------------------------------------------------------
+// fixed index images (disk images): header { magic, uuid, ctime, index_csum, size, chunk_size } + the digests
+// ---------------------------------------------------------------------------
+static const uint8_t FIDX_MAGIC[8] = {0x2f, 0x7f, 0x41, 0xed, 0x91, 0xfd, 0x0f, 0xcd};
+
+static void put_u64(uint8_t *p, uint64_t v) { for (int i = 0; i < 8; i++) p[i] = (uint8_t)(v >> (8 * i)); }
+static uint64_t get_u64(const uint8_t *p) { uint64_t v = 0; for (int i = 0; i < 8; i++) v |= (uint64_t)p[i] << (8 * i); return v; }
+
+extern "C" uint64_t pbsgpu_fidx_size(uint64_t n) { return 4096 + n * 32; }
+
+extern "C" int pbsgpu_fidx_build(pbsgpu_ctx *ctx, const uint8_t *digests, uint64_t n, uint64_t size, uint64_t chunk_size,
+                                 const uint8_t uuid[16], int64_t ctime, uint8_t *out, uint64_t cap) {
+    if (!ctx || (n && !digests) || !out || !uuid) return PBSGPU_EINVAL;
+    if (chunk_size == 0 || chunk_size >= (1ull << 32)) return fail(ctx, PBSGPU_EINVAL, "fidx chunk_size %llu not in [1, 2^32)", (unsigned long long)chunk_size);
+    if (n != size / chunk_size + (size % chunk_size != 0))
+        return fail(ctx, PBSGPU_EINVAL, "fidx: %llu digests for %llu bytes in chunks of %llu", (unsigned long long)n,
+                    (unsigned long long)size, (unsigned long long)chunk_size);
+    if (cap < pbsgpu_fidx_size(n)) return fail(ctx, PBSGPU_ERANGE, "fidx buffer too small: %llu < %llu", (unsigned long long)cap, (unsigned long long)pbsgpu_fidx_size(n));
+    memset(out, 0, 4096);
+    memcpy(out, FIDX_MAGIC, 8);
+    memcpy(out + 8, uuid, 16);
+    put_u64(out + 24, (uint64_t)ctime);
+    put_u64(out + 64, size);
+    put_u64(out + 72, chunk_size);
+    if (n) memcpy(out + 4096, digests, n * 32);
+    uint64_t off0 = 0, len0 = n * 32;
+    return pbsgpu_sha256_batch(ctx, out + 4096, &off0, &len0, 1, out + 32);   // index_csum (GPU)
+}
+
+extern "C" int pbsgpu_fidx_parse(pbsgpu_ctx *ctx, const uint8_t *fidx, uint64_t bytes, uint64_t *size, uint64_t *chunk_size,
+                                 uint8_t *digests, uint64_t cap, uint64_t *n_entries, int verify) {
+    if (!fidx || !n_entries) return PBSGPU_EINVAL;
+    if (bytes < 4096 || memcmp(fidx, FIDX_MAGIC, 8) != 0) return fail(ctx, PBSGPU_EINVAL, "not a fixed index image");
+    const uint64_t sz = get_u64(fidx + 64), cs = get_u64(fidx + 72);
+    if (cs == 0 || cs >= (1ull << 32)) return fail(ctx, PBSGPU_EINVAL, "fixed index: chunk_size %llu not in [1, 2^32)", (unsigned long long)cs);
+    const uint64_t n = sz / cs + (sz % cs != 0);
+    if (n > (bytes - 4096) / 32 || bytes - 4096 != n * 32)
+        return fail(ctx, PBSGPU_EINVAL, "fixed index: %llu bytes, but size %llu in chunks of %llu needs %llu digests",
+                    (unsigned long long)bytes, (unsigned long long)sz, (unsigned long long)cs, (unsigned long long)n);
+    *n_entries = n;
+    if (size) *size = sz;
+    if (chunk_size) *chunk_size = cs;
+    if (digests) {
+        if (cap < n) return fail(ctx, PBSGPU_ERANGE, "output capacity %llu < %llu entries", (unsigned long long)cap, (unsigned long long)n);
+        if (n) memcpy(digests, fidx + 4096, n * 32);
+    }
+    if (verify) {
+        if (!ctx) return PBSGPU_EINVAL;
+        uint8_t csum[32];
+        uint64_t off0 = 0, len0 = n * 32;
+        int rc = pbsgpu_sha256_batch(ctx, fidx + 4096, &off0, &len0, 1, csum);
+        if (rc) return rc;
+        if (memcmp(csum, fidx + 32, 32) != 0) return fail(ctx, PBSGPU_EINVAL, "index checksum mismatch");
+    }
+    return PBSGPU_OK;
+}
+
+// ---------------------------------------------------------------------------
 // SHA-256 of n byte ranges (K3 without the chunker)
 // ---------------------------------------------------------------------------
 // suffix: encrypt mode's device id_key (keyed digests), or NULL

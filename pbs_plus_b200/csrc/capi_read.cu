@@ -31,6 +31,7 @@ struct pbsgpu_reader {
     uint64_t cap = 0, cursor = 0, seq = 0, gen = 0;
     std::deque<Slot> ring;
     std::unordered_map<uint64_t, Held> held;
+    bool image = false;   // over a fixed index: no pxar headers, PBSGPU_READ_PAYLOAD is refused
 };
 
 static uint64_t slot_bytes(uint64_t len) { return std::max<uint64_t>(256, (len + 255) & ~255ull); }
@@ -62,16 +63,11 @@ static const pbsgpu_reader::Slot &place(pbsgpu_reader *r, uint64_t chunk, uint64
     return r->ring.back();
 }
 
-extern "C" int pbsgpu_reader_open(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t size, const pbsgpu_crypt *crypt,
-                                  uint64_t cache_bytes, pbsgpu_reader **out) {
-    if (!ctx || !didx || !out || (crypt && crypt->ctx != ctx)) return PBSGPU_EINVAL;
-    Guard g(ctx);
-    uint64_t n = 0;
-    if (int rc = pbsgpu_didx_parse(ctx, didx, size, nullptr, nullptr, 0, &n, 0)) return rc;
-    pbsgpu_reader *r = new pbsgpu_reader{};
-    r->ctx = ctx; r->crypt = crypt;
-    r->ends.resize(n); r->clen.resize(n); r->digests.resize(n * 32);
-    if (int rc = pbsgpu_didx_parse(ctx, didx, size, r->ends.data(), r->digests.data(), n, &n, 1)) { delete r; return rc; }
+// The chunk lengths from r->ends, then the cache; frees r on failure.
+static int reader_start(pbsgpu_reader *r, uint64_t cache_bytes, pbsgpu_reader **out) {
+    pbsgpu_ctx *ctx = r->ctx;
+    const uint64_t n = r->ends.size();
+    r->clen.resize(n);
     uint64_t largest = 0;
     for (uint64_t c = 0; c < n; c++) {
         r->clen[c] = r->ends[c] - (c ? r->ends[c - 1] : 0);
@@ -87,6 +83,35 @@ extern "C" int pbsgpu_reader_open(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t
     }
     *out = r;
     return PBSGPU_OK;
+}
+
+extern "C" int pbsgpu_reader_open(pbsgpu_ctx *ctx, const uint8_t *didx, uint64_t size, const pbsgpu_crypt *crypt,
+                                  uint64_t cache_bytes, pbsgpu_reader **out) {
+    if (!ctx || !didx || !out || (crypt && crypt->ctx != ctx)) return PBSGPU_EINVAL;
+    Guard g(ctx);
+    uint64_t n = 0;
+    if (int rc = pbsgpu_didx_parse(ctx, didx, size, nullptr, nullptr, 0, &n, 0)) return rc;
+    pbsgpu_reader *r = new pbsgpu_reader{};
+    r->ctx = ctx; r->crypt = crypt;
+    r->ends.resize(n); r->digests.resize(n * 32);
+    if (int rc = pbsgpu_didx_parse(ctx, didx, size, r->ends.data(), r->digests.data(), n, &n, 1)) { delete r; return rc; }
+    return reader_start(r, cache_bytes, out);
+}
+
+// The same reader over a fixed index: the end offsets are synthesized, so lookup, cache, decode and gather are shared.
+extern "C" int pbsgpu_reader_open_fidx(pbsgpu_ctx *ctx, const uint8_t *fidx, uint64_t bytes, const pbsgpu_crypt *crypt,
+                                       uint64_t cache_bytes, pbsgpu_reader **out) {
+    if (!ctx || !fidx || !out || (crypt && crypt->ctx != ctx)) return PBSGPU_EINVAL;
+    Guard g(ctx);
+    uint64_t n = 0, size = 0, cs = 0;
+    if (int rc = pbsgpu_fidx_parse(ctx, fidx, bytes, &size, &cs, nullptr, 0, &n, 0)) return rc;
+    pbsgpu_reader *r = new pbsgpu_reader{};
+    r->ctx = ctx; r->crypt = crypt; r->image = true;
+    r->digests.resize(n * 32);
+    if (int rc = pbsgpu_fidx_parse(ctx, fidx, bytes, nullptr, nullptr, r->digests.data(), n, &n, 1)) { delete r; return rc; }
+    r->ends.resize(n);
+    for (uint64_t c = 0; c < n; c++) r->ends[c] = std::min((c + 1) * cs, size);
+    return reader_start(r, cache_bytes, out);
 }
 
 extern "C" void pbsgpu_reader_close(pbsgpu_reader *r) {
@@ -119,6 +144,7 @@ template <typename F> static void for_pieces(const pbsgpu_reader *r, uint64_t lo
 // The arguments every call checks: flags, and every range (with its PAYLOAD header) inside the archive.
 static int check_ranges(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags) {
     if (flags & ~PBSGPU_READ_PAYLOAD) return fail(r->ctx, PBSGPU_EINVAL, "unknown read flags 0x%x", flags);
+    if (r->image && (flags & PBSGPU_READ_PAYLOAD)) return fail(r->ctx, PBSGPU_EINVAL, "an image has no pxar PAYLOAD headers");
     const uint64_t hs = flags & PBSGPU_READ_PAYLOAD ? 16 : 0, size = pbsgpu_reader_size(r);
     for (uint32_t i = 0; i < n; i++)
         if (off[i] > size || len[i] > size - off[i] || hs > size - off[i] - len[i])

@@ -168,6 +168,14 @@ extern "C" int pbsgpu_set_seed_didx(pbsgpu_set *s, const uint8_t *didx, uint64_t
     return set_process(s, dig.data(), n, 1, nullptr);
 }
 
+extern "C" int pbsgpu_set_seed_fidx(pbsgpu_set *s, const uint8_t *fidx, uint64_t bytes, uint64_t *n_entries) {
+    if (!s || !fidx) return PBSGPU_EINVAL;
+    uint64_t n = 0;
+    if (int rc = pbsgpu_fidx_parse(s->ctx, fidx, bytes, nullptr, nullptr, nullptr, 0, &n, 0)) return rc;
+    if (n_entries) *n_entries = n;
+    return set_process(s, fidx + 4096, n, 1, nullptr);   // the digest table is contiguous: n x 32 bytes
+}
+
 // ---------------------------------------------------------------------------
 // e: multi-GPU merge.  NCCL is resolved at run time (dlopen) so that libpbsgpu.so has no link-time dependency on it:
 // single-GPU users never need libnccl, and a host that already loaded one (torch's bundled libnccl.so.2) shares it.

@@ -194,6 +194,7 @@ struct pbsgpu_job {
     uint64_t total_bytes = 0, total_tiles = 0, chunk_cap = 0, cand_cap = 0;
     int eof = 1, want_digests = 1, variant = 0;
     bool scan_lanes = false;
+    uint32_t fixed_log2 = 0;        // > 0: fixed cuts of 2^fixed_log2 bytes (pbsgpu_batch_opts.fixed_size); no candidates
     pbsgpu_set *set = nullptr;      // fused probe + insert (NULL: none)
     const uint8_t *sha_suffix = nullptr;   // encrypt mode: the crypt's device id_key, K3 computes keyed digests
     // device
@@ -227,7 +228,7 @@ struct pbsgpu_job {
 
 int pbsgpu_job_create(pbsgpu_ctx *ctx, const pbsgpu_cfg *cfg, const void *base_dev, const uint64_t *off, const uint64_t *len,
                       uint32_t n, int eof, int want_digests, pbsgpu_set *set, const uint32_t *forced_stream,
-                      const uint64_t *forced_off, uint64_t n_forced, pbsgpu_job **out);
+                      const uint64_t *forced_off, uint64_t n_forced, pbsgpu_job **out, uint32_t fixed_size = 0);
 int pbsgpu_job_enqueue_front(pbsgpu_job *j);
 int pbsgpu_job_enqueue_back(pbsgpu_job *j);
 int pbsgpu_job_enqueue(pbsgpu_job *j);

@@ -70,6 +70,10 @@ struct ResolveArgs {
 cudaError_t launch_resolve(const ResolveArgs &a, cudaStream_t st);   // count + scan + write (3 launches)
 cudaError_t launch_append_keys(const uint64_t *keys, uint64_t n, uint64_t *cand, uint64_t cand_cap, unsigned long long *cand_count,
                                cudaStream_t st);
+// fixed cuts of 2^cs_log2 bytes (replaces K1 + sort + K2): counts[n], chunk_first[n+1] and *n_chunks_dev as launch_resolve
+// writes them, chunks[n_chunks] (n_chunks: the host's count, sum of ceil(len / cs))
+cudaError_t launch_fixed_refs(const uint64_t *len, uint32_t n, uint32_t cs_log2, uint32_t *counts, uint64_t *chunk_first,
+                              unsigned long long *n_chunks_dev, uint64_t n_chunks, ChunkRef *chunks, cudaStream_t st);
 
 // ---- SHA-256 (K3) ----------------------------------------------------------------
 struct ShaArgs {

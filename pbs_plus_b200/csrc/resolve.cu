@@ -109,6 +109,41 @@ cudaError_t launch_append_keys(const uint64_t *keys, uint64_t n, uint64_t *cand,
     return cudaGetLastError();
 }
 
+// Fixed cuts (pbsgpu_batch_opts.fixed_size, the chunking of .fidx images): chunk k of stream s covers
+// [k * cs, min((k + 1) * cs, len[s])), so only a stream's last chunk can be short and a stream of length 0 has none.
+// No state crosses a chunk boundary, so these launches replace K1, the sort and K2; the ChunkRefs they write are what
+// K2 writes for the same cuts, and the back half reads them unchanged.
+__global__ void __launch_bounds__(128) k_fixed_counts(const uint64_t *len, uint32_t n, uint32_t cs_log2, uint32_t *counts) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < n) counts[s] = (uint32_t)((len[s] + (1ull << cs_log2) - 1) >> cs_log2);
+}
+
+// One thread per chunk, in (stream, offset) order: the stream is the last s with chunk_first[s] <= t.
+__global__ void __launch_bounds__(256) k_fixed_refs(const uint64_t *len, const uint64_t *chunk_first, uint32_t n,
+                                                    uint32_t cs_log2, uint64_t n_chunks, ChunkRef *chunks) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_chunks) return;
+    uint32_t lo = 0, hi = n;   // upper_bound over chunk_first[1..n]
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (chunk_first[mid + 1] <= t) lo = mid + 1; else hi = mid;
+    }
+    const uint64_t start = (t - chunk_first[lo]) << cs_log2, l = len[lo] - start;
+    ChunkRef c;
+    c.stream = lo; c.start = start;
+    c.len = (uint32_t)(l < (1ull << cs_log2) ? l : (1ull << cs_log2));
+    chunks[t] = c;
+}
+
+cudaError_t launch_fixed_refs(const uint64_t *len, uint32_t n, uint32_t cs_log2, uint32_t *counts, uint64_t *chunk_first,
+                              unsigned long long *n_chunks_dev, uint64_t n_chunks, ChunkRef *chunks, cudaStream_t st) {
+    if (n == 0) return cudaMemsetAsync(n_chunks_dev, 0, sizeof(unsigned long long), st);
+    k_fixed_counts<<<(n + 127) / 128, 128, 0, st>>>(len, n, cs_log2, counts);
+    k_scan_counts<<<1, 1024, 0, st>>>(counts, n, chunk_first, n_chunks_dev);
+    if (n_chunks) k_fixed_refs<<<(unsigned)((n_chunks + 255) / 256), 256, 0, st>>>(len, chunk_first, n, cs_log2, n_chunks, chunks);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_resolve(const ResolveArgs &a, cudaStream_t st) {
     if (a.n_streams == 0) return cudaMemsetAsync(a.n_chunks, 0, sizeof(unsigned long long), st);
     unsigned blocks = (a.n_streams + 127) / 128;

@@ -13,7 +13,7 @@ from typing import Iterable, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import BLOB_MODES, CHUNK_DTYPE, CHUNK_KNOWN, BatchOpts, Cfg, Corpus, DevInfo, PbsGpuError, Timing
+from ._lib import BLOB_MODES, CHUNK_DTYPE, CHUNK_KNOWN, BatchOptsFixed, Cfg, Corpus, DevInfo, PbsGpuError, Timing
 
 
 def _ptr(x) -> int:
@@ -27,6 +27,10 @@ def _ptr(x) -> int:
     if isinstance(x, (bytes, bytearray, memoryview)):
         return int(np.frombuffer(x, dtype=np.uint8).ctypes.data)
     raise TypeError(f"cannot take the address of {type(x)}")
+
+
+def _cfg_ref(cfg: Cfg | None):
+    return C.byref(cfg) if cfg is not None else None
 
 
 def make_config(avg_bytes: int, table: np.ndarray | None = None) -> Cfg:
@@ -117,18 +121,21 @@ class Engine:
         return o, l
 
     @staticmethod
-    def _chunk_cap(cfg: Cfg, l: np.ndarray) -> int:
+    def _chunk_cap(cfg: Cfg | None, l: np.ndarray, fixed_size: int = 0) -> int:
+        if fixed_size:
+            return int(((l + np.uint64(fixed_size - 1)) // np.uint64(fixed_size)).sum()) + 1
         m = max(int(cfg.min), 65)
         return int((l // np.uint64(m)).sum()) + len(l) + 1
 
     @staticmethod
-    def _opts(digest_set, forced, xxh3=None, crypt=None):
+    def _opts(digest_set, forced, xxh3=None, crypt=None, fixed_size: int = 0):
         """pbsgpu_batch_opts; `forced` = (stream u32[], offset u64[]) suggested boundaries sorted by (stream, offset);
-        `crypt` (a Crypt) = keyed digests of encrypt mode."""
-        o = BatchOpts()
-        o.size = C.sizeof(BatchOpts)
+        `crypt` (a Crypt) = keyed digests of encrypt mode; `fixed_size` = fixed cuts instead of the chunker."""
+        o = BatchOptsFixed()
+        o.size = C.sizeof(BatchOptsFixed)
         o.set = digest_set._h if digest_set is not None else None
         o.crypt = crypt._h if crypt is not None else None
+        o.fixed_size = int(fixed_size)
         keep = []
         if forced is not None:
             fs = np.ascontiguousarray(forced[0], dtype=np.uint32)
@@ -141,20 +148,21 @@ class Engine:
             o.stream_xxh3 = xxh3.ctypes.data
         return o, keep
 
-    def chunk_digest_batch(self, cfg: Cfg, base, off, length, digest_set: "DigestSet | None" = None,
-                           forced=None, crypt: "Crypt | None" = None) -> np.ndarray:
+    def chunk_digest_batch(self, cfg: Cfg | None, base, off, length, digest_set: "DigestSet | None" = None,
+                           forced=None, crypt: "Crypt | None" = None, fixed_size: int = 0) -> np.ndarray:
         """stream -> chunks -> digests for n streams; `base` device (tensor/int) or host (numpy).
         Replaces n calls of writer.WriteEntryReader (reference commit.go:720).  `forced` = optional suggested
         boundaries (stream[], offset[]): file starts of a pxar payload stream (pxarfs.go:408-411).  `crypt`: keyed
-        digests SHA-256(chunk || id_key) of encrypt mode, also for the set's probe + insert."""
+        digests SHA-256(chunk || id_key) of encrypt mode, also for the set's probe + insert.  `fixed_size`: cut every
+        stream at multiples of it instead (the chunks of a .fidx image; cfg may be None)."""
         o, l = self._offlen(off, length)
-        cap = self._chunk_cap(cfg, l) + (len(forced[0]) if forced is not None else 0)
+        cap = self._chunk_cap(cfg, l, fixed_size) + (len(forced[0]) if forced is not None else 0)
         out = np.zeros(cap, dtype=CHUNK_DTYPE)
         n_out = C.c_uint64()
         keep = base  # keep the buffer alive for the duration of the call
-        opts, _k = self._opts(digest_set, forced, crypt=crypt)
+        opts, _k = self._opts(digest_set, forced, crypt=crypt, fixed_size=fixed_size)
         self._ck(self._L.pbsgpu_chunk_digest_batch_ex(
-            self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o), C.byref(opts), out.ctypes.data, cap,
+            self._h, _cfg_ref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o), C.byref(opts), out.ctypes.data, cap,
             C.byref(n_out)))
         return out[: n_out.value]
 
@@ -193,20 +201,20 @@ class Engine:
             buf[int(o): int(o) + len(a)] = a
         return self.chunk_digest_batch(cfg, buf, offs, lens, digest_set)
 
-    def submit(self, cfg: Cfg, base_dev, off, length, digest_set: "DigestSet | None" = None, forced=None,
-               early_input: bool = False, crypt: "Crypt | None" = None) -> "Job":
+    def submit(self, cfg: Cfg | None, base_dev, off, length, digest_set: "DigestSet | None" = None, forced=None,
+               early_input: bool = False, crypt: "Crypt | None" = None, fixed_size: int = 0) -> "Job":
         """Asynchronous form; with `digest_set` the probe + insert runs as kernels on the job's stream (jobs sharing a
         set are ordered in submission order) and the KNOWN flags come back with the records.  `early_input`
         (PBSGPU_BATCH_EARLY_INPUT): the long chunks are copied aside so that Job.wait_input() gives the buffer back
-        long before the records are ready.  `crypt`: keyed digests (as chunk_digest_batch)."""
+        long before the records are ready.  `crypt`, `fixed_size`: as chunk_digest_batch."""
         o, l = self._offlen(off, length)
         h = C.c_void_p()
-        opts, _k = self._opts(digest_set, forced, crypt=crypt)
+        opts, _k = self._opts(digest_set, forced, crypt=crypt, fixed_size=fixed_size)
         if early_input:
             opts.flags |= _lib.BATCH_EARLY_INPUT
-        self._ck(self._L.pbsgpu_batch_submit_ex(self._h, C.byref(cfg), _ptr(base_dev), o.ctypes.data, l.ctypes.data,
+        self._ck(self._L.pbsgpu_batch_submit_ex(self._h, _cfg_ref(cfg), _ptr(base_dev), o.ctypes.data, l.ctypes.data,
                                                 len(o), C.byref(opts), C.byref(h)))
-        return Job(self, h, self._chunk_cap(cfg, l) + (len(forced[0]) if forced is not None else 0), base_dev)
+        return Job(self, h, self._chunk_cap(cfg, l, fixed_size) + (len(forced[0]) if forced is not None else 0), base_dev)
 
     def scan_batch(self, cfg: Cfg, base_dev, off, length):
         """Boundaries only (a2).  Returns (ends, stream_first)."""
@@ -372,6 +380,11 @@ class Engine:
         256 MiB, and the cache always holds at least the largest chunk."""
         return Reader(self, didx, crypt, cache_bytes)
 
+    def reader_fidx(self, fidx: bytes, crypt: "Crypt | None" = None, cache_bytes: int = 0) -> "Reader":
+        """The same reader over a disk image's .fidx (pbsgpu_reader_open_fidx): byte ranges of the image; payload reads
+        are refused, an image has no pxar headers."""
+        return Reader(self, fidx, crypt, cache_bytes, fixed=True)
+
     # -- f3, encrypt mode -----------------------------------------------------------------------
     def crypt(self, key: bytes) -> "Crypt":
         """Handle for one 32-byte AES-256 key (pbsgpu_crypt_create); close() zeroes its key material."""
@@ -425,6 +438,31 @@ class Engine:
         self._ck(self._L.pbsgpu_didx_parse(self._h, a.ctypes.data, len(a), ends.ctypes.data, dig.ctypes.data, n.value,
                                            C.byref(n), 1 if verify else 0))
         return ends, dig
+
+    # -- fixed index images (disk images) ------------------------------------------------------
+    def fidx_build(self, digests, size: int, chunk_size: int, uuid: bytes = b"\0" * 16, ctime: int = 0) -> bytes:
+        """Fixed-index (.fidx) image of an image of `size` bytes in chunks of `chunk_size`: digests (n x 32 bytes, n =
+        ceil(size / chunk_size)) in image order; the checksum is computed on the GPU."""
+        d = np.ascontiguousarray(np.frombuffer(bytes(digests), dtype=np.uint8) if isinstance(digests, (bytes, bytearray))
+                                 else np.asarray(digests, dtype=np.uint8)).reshape(-1)
+        if d.size % 32:
+            raise ValueError("digests must hold 32 bytes each")
+        n = d.size // 32
+        out = np.zeros(int(self._L.pbsgpu_fidx_size(n)), dtype=np.uint8)
+        u = np.frombuffer(bytes(uuid).ljust(16, b"\0")[:16], dtype=np.uint8)
+        self._ck(self._L.pbsgpu_fidx_build(self._h, d.ctypes.data if n else None, n, int(size), int(chunk_size), u.ctypes.data,
+                                           int(ctime), out.ctypes.data, len(out)))
+        return out.tobytes()
+
+    def fidx_parse(self, image: bytes, verify: bool = True):
+        """-> (size, chunk_size, digests u8[n, 32]); verify recomputes the index checksum on the GPU."""
+        a = np.frombuffer(bytes(image), dtype=np.uint8)
+        n, size, cs = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        self._ck(self._L.pbsgpu_fidx_parse(self._h, a.ctypes.data, len(a), None, None, None, 0, C.byref(n), 0))
+        dig = np.zeros((n.value, 32), dtype=np.uint8)
+        self._ck(self._L.pbsgpu_fidx_parse(self._h, a.ctypes.data, len(a), C.byref(size), C.byref(cs), dig.ctypes.data,
+                                           n.value, C.byref(n), 1 if verify else 0))
+        return int(size.value), int(cs.value), dig
 
     # -- misc ---------------------------------------------------------------------------
     def digest_set(self, capacity_hint: int = 1 << 16) -> "DigestSet":
@@ -532,12 +570,12 @@ class Reader:
     """An archive reader on the engine's device (pbsgpu_reader_*): plan() names the chunks a read needs that the cache
     lacks, read() verifies the blobs it is given into the cache and copies the ranges out of it."""
 
-    def __init__(self, eng: Engine, didx: bytes, crypt: "Crypt | None", cache_bytes: int):
-        a = np.frombuffer(bytes(didx), dtype=np.uint8)
+    def __init__(self, eng: Engine, index: bytes, crypt: "Crypt | None", cache_bytes: int, fixed: bool = False):
+        a = np.frombuffer(bytes(index), dtype=np.uint8)
         self._eng, self._crypt = eng, crypt   # the crypt handle must outlive the reader
         h = C.c_void_p()
-        eng._ck(eng._L.pbsgpu_reader_open(eng._h, a.ctypes.data, len(a), crypt._h if crypt is not None else None,
-                                          int(cache_bytes), C.byref(h)))
+        op = eng._L.pbsgpu_reader_open_fidx if fixed else eng._L.pbsgpu_reader_open
+        eng._ck(op(eng._h, a.ctypes.data, len(a), crypt._h if crypt is not None else None, int(cache_bytes), C.byref(h)))
         self._h = h
 
     @property
@@ -674,6 +712,13 @@ class DigestSet:
         a = np.frombuffer(image, dtype=np.uint8)
         n = C.c_uint64()
         self._eng._ck(self._eng._L.pbsgpu_set_seed_didx(self._h, a.ctypes.data, len(a), C.byref(n)))
+        return int(n.value)
+
+    def seed_fidx(self, image: bytes) -> int:
+        """Seed from the previous snapshot's .fidx of the same image (pbsgpu_set_seed_fidx); returns its chunk count."""
+        a = np.frombuffer(bytes(image), dtype=np.uint8)
+        n = C.c_uint64()
+        self._eng._ck(self._eng._L.pbsgpu_set_seed_fidx(self._h, a.ctypes.data, len(a), C.byref(n)))
         return int(n.value)
 
 

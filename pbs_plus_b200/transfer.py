@@ -23,6 +23,8 @@ Two writers:
     supports WriteEntryRef (chunk reuse from the previous .ppxar.didx, commit.go:752, :848-860).
   * DedupWriter -- per-file batching (every file its own stream).  Faster for many small files, but its index does NOT
     describe a ppxar payload stream: use it for dedup statistics / digest computation, not to write .ppxar.didx.
+
+And for disk images (`.img.fidx` archives): FixedIndexWriter -- fixed-size chunks through the batch call, fed in slices.
 """
 from __future__ import annotations
 
@@ -326,6 +328,84 @@ class PayloadStreamWriter:
             rec[i]["digest"] = np.frombuffer(dig, dtype=np.uint8)
             rec[i]["flags"] = CHUNK_KNOWN if known else 0
         return self.engine.didx_build(rec, uuid, ctime)
+
+
+@dataclass
+class FixedIndexWriter:
+    """Backs up a disk image as a fixed index (`<name>.img.fidx`): the image is cut at every multiple of `chunk_size`
+    (upstream writes 4 MiB chunks), and each chunk is digested on the GPU, probed against `known` (seed it from the
+    previous snapshot's index with DigestSet.seed_fidx) and, when new, handed to `upload_blob(digest, blob)` as a
+    DataBlob made by the encoder `blob_compression` names ("z", "lz", "lze", "lzh" or "lzl", as for DedupWriter).  No
+    state crosses a chunk boundary, so the image is fed in slices of any size that are multiples of `chunk_size` -- only
+    the last may end inside a chunk -- one batch call per slice, from host memory or straight from device memory."""
+    engine: Engine
+    chunk_size: int = 4 << 20
+    known: DigestSet | None = None
+    upload_blob: Callable[[bytes, bytes], None] | None = None
+    blob_compression: str = "z"
+    # encrypt mode: the 32-byte client key (as DedupWriter.crypt_key): keyed digests and encrypted blobs
+    crypt_key: bytes | None = None
+    digests: list[bytes] = field(default_factory=list)   # per chunk, in image order
+    known_flags: list[bool] = field(default_factory=list)
+    size: int = 0                                        # image bytes written so far
+    _crypt: object = None
+    _ended: bool = False                                 # a slice ended inside a chunk: it was the last
+
+    def __post_init__(self):
+        _check_blob_compression(self.blob_compression)
+        cs = int(self.chunk_size)
+        if cs < 4096 or cs > 16 << 20 or cs & (cs - 1):
+            raise ValueError(f"transfer: chunk_size must be a power of two from 4 KiB to 16 MiB, not {cs}")
+        if self.crypt_key is not None:
+            self._crypt = self.engine.crypt(self.crypt_key)
+
+    def WriteSlice(self, data) -> None:
+        """The next bytes of the image: a numpy array or bytes on the host, or a 1-D torch CUDA tensor of uint8."""
+        if isinstance(data, (bytes, bytearray, memoryview)):
+            data = np.frombuffer(data, dtype=np.uint8)
+        n = int(data.numel()) if hasattr(data, "numel") else len(data)
+        if n == 0:
+            return
+        if self._ended:
+            raise ValueError("transfer: the image's last slice ended inside a chunk; no slice may follow it")
+        cs = int(self.chunk_size)
+        rec = self.engine.chunk_digest_batch(None, data, [0], [n], self.known, crypt=self._crypt, fixed_size=cs)
+        new = []
+        for k, r in enumerate(rec):
+            known = bool(r["flags"] & CHUNK_KNOWN)
+            self.digests.append(bytes(r["digest"]))
+            self.known_flags.append(known)
+            if not known:
+                new.append(k)
+        if self.upload_blob is not None and new:
+            boff = np.array(new, dtype=np.uint64) * np.uint64(cs)
+            blen = np.minimum(np.uint64(n) - boff, np.uint64(cs))
+            if self._crypt is not None:
+                blobs, _crc = self.engine.blob_encode_batch_enc(self._crypt, self.blob_compression, data, boff, blen,
+                                                                os.urandom(16 * len(boff)))
+            else:
+                blobs, _crc = getattr(self.engine, "blob_encode_batch_" + self.blob_compression)(data, boff, blen)
+            for k, blob in zip(new, blobs):
+                self.upload_blob(bytes(rec[k]["digest"]), blob)
+        self.size += n
+        self._ended = n % cs != 0
+
+    def WriteFrom(self, reader: BinaryIO, size: int, slice_bytes: int = 1 << 30) -> None:
+        """Pulls exactly `size` bytes from `reader` (io.ReadFull semantics) in slices of `slice_bytes` (rounded down to
+        whole chunks)."""
+        step = max(int(self.chunk_size), slice_bytes - slice_bytes % int(self.chunk_size))
+        left = size
+        while left:
+            want = min(left, step)
+            data = reader.read(want)
+            if len(data) != want:
+                raise IOError(f"transfer: short read of the image: got {size - left + len(data)} of {size} bytes (unexpected EOF)")
+            self.WriteSlice(data)
+            left -= want
+
+    def fidx(self, uuid: bytes = b"\0" * 16, ctime: int = 0) -> bytes:
+        """The image's .fidx (checksum on the GPU)."""
+        return self.engine.fidx_build(b"".join(self.digests), self.size, int(self.chunk_size), uuid, ctime)
 
 
 _DEC_NAMES = {getattr(_lib, k): k for k in dir(_lib) if k.startswith("DEC_")}
