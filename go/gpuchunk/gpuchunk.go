@@ -25,11 +25,14 @@ package gpuchunk
 import "C"
 
 import (
+	"bytes"
 	"crypto/rand"
 	"errors"
 	"fmt"
+	"hash/crc32"
 	"io"
 	"runtime"
+	"strings"
 	"unsafe"
 )
 
@@ -912,8 +915,52 @@ func (e *Engine) NewPayloadReader(didx []byte, c *Crypt, cacheBytes uint64, sour
 
 func (p *PayloadReader) Close() { C.pbsgpu_reader_close(p.r) }
 
-// read serves ranges (payload: (payload offset, file size) of files) into out at outOff: one plan, one fetch of the
-// missing blobs (plus Prefetch chunks after the last one), one read.
+// fetch plans ranges (payload: (payload offset, file size) of files) and fetches the missing blobs (plus Prefetch
+// chunks after the last one): the blobs concatenated, their offsets, lengths and chunk indices, each with one
+// trailing element so the slices are never empty.
+func (p *PayloadReader) fetch(off, length []uint64, flags C.uint32_t) (blobs []byte, bo, bl, need []uint64, err error) {
+	o := (*C.uint64_t)(unsafe.Pointer(&off[0]))
+	l := (*C.uint64_t)(unsafe.Pointer(&length[0]))
+	var k C.uint64_t
+	need = make([]uint64, len(p.digests))
+	var np *C.uint64_t
+	if len(need) > 0 {
+		np = (*C.uint64_t)(unsafe.Pointer(&need[0]))
+	}
+	if err = p.e.err(C.pbsgpu_reader_plan(p.r, o, l, C.uint32_t(len(off)), flags, np, nil, C.uint64_t(len(need)), &k)); err != nil {
+		return
+	}
+	need = need[:k]
+	if k > 0 {
+		for c := need[k-1] + 1; c < uint64(len(p.digests)) && c <= need[k-1]+uint64(p.Prefetch); c++ {
+			need = append(need, c)
+		}
+	}
+	bo = make([]uint64, len(need)+1)
+	bl = make([]uint64, len(need)+1)
+	for j, c := range need {
+		b, ferr := p.source(p.digests[c])
+		if ferr != nil {
+			return nil, nil, nil, nil, ferr
+		}
+		bo[j], bl[j] = uint64(len(blobs)), uint64(len(b))
+		blobs = append(blobs, b...)
+	}
+	blobs = append(blobs, 0)
+	need = append(need, 0)
+	return
+}
+
+func (p *PayloadReader) statusErr(off, length []uint64, status []int32) error {
+	for i, s := range status {
+		if s != int32(C.PBSGPU_DEC_OK) {
+			return fmt.Errorf("pbsgpu: read of %d bytes at %d: status %d", length[i], off[i], s)
+		}
+	}
+	return nil
+}
+
+// read serves ranges into out at outOff: one plan, one fetch, one read.
 func (p *PayloadReader) read(off, length []uint64, payload bool, out []byte, outOff []uint64) error {
 	n := len(off)
 	if n == 0 {
@@ -923,49 +970,66 @@ func (p *PayloadReader) read(off, length []uint64, payload bool, out []byte, out
 	if payload {
 		flags = C.PBSGPU_READ_PAYLOAD
 	}
-	o := (*C.uint64_t)(unsafe.Pointer(&off[0]))
-	l := (*C.uint64_t)(unsafe.Pointer(&length[0]))
-	var k C.uint64_t
-	need := make([]uint64, len(p.digests))
-	var np *C.uint64_t
-	if len(need) > 0 {
-		np = (*C.uint64_t)(unsafe.Pointer(&need[0]))
-	}
-	if err := p.e.err(C.pbsgpu_reader_plan(p.r, o, l, C.uint32_t(n), flags, np, nil, C.uint64_t(len(need)), &k)); err != nil {
+	blobs, bo, bl, need, err := p.fetch(off, length, flags)
+	if err != nil {
 		return err
 	}
-	need = need[:k]
-	if k > 0 {
-		for c := need[k-1] + 1; c < uint64(len(p.digests)) && c <= need[k-1]+uint64(p.Prefetch); c++ {
-			need = append(need, c)
-		}
-	}
-	var blobs []byte
-	bo := make([]uint64, len(need)+1)
-	bl := make([]uint64, len(need)+1)
-	for j, c := range need {
-		b, err := p.source(p.digests[c])
-		if err != nil {
-			return err
-		}
-		bo[j], bl[j] = uint64(len(blobs)), uint64(len(b))
-		blobs = append(blobs, b...)
-	}
-	blobs = append(blobs, 0)
-	need = append(need, 0)
 	status := make([]int32, n)
-	rc := C.pbsgpu_reader_read(p.r, o, l, C.uint32_t(n), flags, unsafe.Pointer(&blobs[0]), (*C.uint64_t)(unsafe.Pointer(&bo[0])),
+	rc := C.pbsgpu_reader_read(p.r, (*C.uint64_t)(unsafe.Pointer(&off[0])), (*C.uint64_t)(unsafe.Pointer(&length[0])),
+		C.uint32_t(n), flags, unsafe.Pointer(&blobs[0]), (*C.uint64_t)(unsafe.Pointer(&bo[0])),
 		(*C.uint64_t)(unsafe.Pointer(&bl[0])), (*C.uint64_t)(unsafe.Pointer(&need[0])), C.uint32_t(len(need)-1),
 		(*C.uint8_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&outOff[0])), (*C.int32_t)(unsafe.Pointer(&status[0])), nil)
 	if err := p.e.err(rc); err != nil {
 		return err
 	}
-	for i, s := range status {
-		if s != int32(C.PBSGPU_DEC_OK) {
-			return fmt.Errorf("pbsgpu: read of %d bytes at %d: status %d", length[i], off[i], s)
-		}
+	return p.statusErr(off, length, status)
+}
+
+// readDeflate is read whose outputs are the ranges' raw Deflate streams, compressed on the GPU
+// (pbsgpu_reader_read_deflate); more[i] != 0: a later call continues stream i.  Returns the streams and CRC-32s.
+func (p *PayloadReader) readDeflate(off, length []uint64, payload bool, more []uint8) ([][]byte, []uint32, error) {
+	n := len(off)
+	if n == 0 {
+		return nil, nil, nil
 	}
-	return nil
+	var flags C.uint32_t
+	if payload {
+		flags = C.PBSGPU_READ_PAYLOAD
+	}
+	blobs, bo, bl, need, err := p.fetch(off, length, flags)
+	if err != nil {
+		return nil, nil, err
+	}
+	oo := make([]uint64, n)
+	var total uint64
+	for i, s := range length {
+		oo[i] = total
+		total += uint64(C.pbsgpu_deflate_bound(C.uint64_t(s)))
+	}
+	out := make([]byte, total+1)
+	olen := make([]uint64, n)
+	crc := make([]uint32, n)
+	status := make([]int32, n)
+	var mp *C.uint8_t
+	if more != nil {
+		mp = (*C.uint8_t)(unsafe.Pointer(&more[0]))
+	}
+	rc := C.pbsgpu_reader_read_deflate(p.r, (*C.uint64_t)(unsafe.Pointer(&off[0])), (*C.uint64_t)(unsafe.Pointer(&length[0])),
+		C.uint32_t(n), flags, mp, unsafe.Pointer(&blobs[0]), (*C.uint64_t)(unsafe.Pointer(&bo[0])),
+		(*C.uint64_t)(unsafe.Pointer(&bl[0])), (*C.uint64_t)(unsafe.Pointer(&need[0])), C.uint32_t(len(need)-1),
+		(*C.uint8_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&oo[0])), (*C.uint64_t)(unsafe.Pointer(&olen[0])),
+		(*C.uint32_t)(unsafe.Pointer(&crc[0])), (*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	if err := p.e.err(rc); err != nil {
+		return nil, nil, err
+	}
+	if err := p.statusErr(off, length, status); err != nil {
+		return nil, nil, err
+	}
+	res := make([][]byte, n)
+	for i := range res {
+		res[i] = out[oo[i] : oo[i]+olen[i]]
+	}
+	return res, crc, nil
 }
 
 // ReadAt implements io.ReaderAt over the archive: short with io.EOF at its end.
@@ -1187,4 +1251,190 @@ func (e *Engine) NewImageReader(fidx []byte, c *Crypt, cacheBytes uint64, source
 		copy(dg[i][:], fidx[4096+32*i:4096+32*i+32])
 	}
 	return &PayloadReader{e: e, r: r, source: source, digests: dg, size: uint64(C.pbsgpu_reader_size(r))}, nil
+}
+
+// ZipWriter writes one <name>.zip of a restore (the replacement for zip.NewWriter + io.Copy(rangeReader) in
+// createZipForSource, internal/pxar/zip.go): files are deflated on the GPU from a PayloadReader
+// (pbsgpu_reader_read_deflate) and the container is written by pbsgpu_zip_*.  Every entry but a directory has flag bit
+// 3 and a data descriptor; Close writes the central directory.  Files up to PieceBytes go in batches of about PieceBytes
+// file bytes, one read per batch; a larger file goes in 128 KiB-aligned pieces of plain ranges continued with `more`,
+// after one plain read of its 16-byte PAYLOAD header, and its CRC-32 is combined from the pieces'.
+type ZipWriter struct {
+	pr         *PayloadReader
+	w          io.Writer
+	PieceBytes uint64
+	pos        uint64
+	entries    []C.pbsgpu_zip_entry
+}
+
+// ZipFile is one regular file of AddFiles: its path in the archive, st_mode, mtime and place in the payload stream.
+type ZipFile struct {
+	Path          string
+	Mode          uint32
+	Mtime         int64
+	PayloadOffset uint64
+	Size          uint64
+}
+
+func (e *Engine) NewZipWriter(pr *PayloadReader, w io.Writer) *ZipWriter {
+	return &ZipWriter{pr: pr, w: w, PieceBytes: 1 << 30}
+}
+
+func (z *ZipWriter) write(b []byte) error {
+	_, err := z.w.Write(b)
+	z.pos += uint64(len(b))
+	return err
+}
+
+func zipRecord(f func(out *C.uint8_t, cap C.uint64_t) C.uint64_t) []byte {
+	need := uint64(f(nil, 0))
+	out := make([]byte, need+1)
+	f((*C.uint8_t)(unsafe.Pointer(&out[0])), C.uint64_t(need))
+	return out[:need]
+}
+
+func (z *ZipWriter) entry(name string, mode uint32, mtime int64, method uint32, size uint64) *C.pbsgpu_zip_entry {
+	e := C.pbsgpu_zip_entry{name: (*C.uint8_t)(C.CBytes([]byte(name + "\x00"))), name_len: C.uint32_t(len(name)), mode: C.uint32_t(mode),
+		mtime: C.int64_t(mtime), method: C.uint32_t(method), size: C.uint64_t(size), offset: C.uint64_t(z.pos)}
+	z.entries = append(z.entries, e)
+	return &z.entries[len(z.entries)-1]
+}
+
+func (z *ZipWriter) localHeader(e *C.pbsgpu_zip_entry) error {
+	return z.write(zipRecord(func(o *C.uint8_t, c C.uint64_t) C.uint64_t { return C.pbsgpu_zip_local_header(e, o, c) }))
+}
+
+func (z *ZipWriter) descriptor(e *C.pbsgpu_zip_entry) error {
+	return z.write(zipRecord(func(o *C.uint8_t, c C.uint64_t) C.uint64_t { return C.pbsgpu_zip_data_descriptor(e, o, c) }))
+}
+
+// AddDirectory adds a directory entry (its name gets a trailing '/').
+func (z *ZipWriter) AddDirectory(path string, mode uint32, mtime int64) error {
+	if !strings.HasSuffix(path, "/") {
+		path += "/"
+	}
+	return z.localHeader(z.entry(path, mode, mtime, 0, 0))
+}
+
+// AddSymlink adds a symlink entry: stored, the target as content.
+func (z *ZipWriter) AddSymlink(path, target string, mode uint32, mtime int64) error {
+	e := z.entry(path, mode, mtime, 0, uint64(len(target)))
+	e.crc, e.comp_size = C.uint32_t(crc32.ChecksumIEEE([]byte(target))), C.uint64_t(len(target))
+	if err := z.localHeader(e); err != nil {
+		return err
+	}
+	if err := z.write([]byte(target)); err != nil {
+		return err
+	}
+	return z.descriptor(e)
+}
+
+// AddFiles adds regular files, deflated on the GPU.
+func (z *ZipWriter) AddFiles(files []ZipFile) error {
+	piece := z.PieceBytes / (128 << 10) * (128 << 10)
+	if piece == 0 {
+		piece = 128 << 10
+	}
+	var batch []ZipFile
+	var acc uint64
+	flush := func() error {
+		if len(batch) == 0 {
+			return nil
+		}
+		off, size := make([]uint64, len(batch)), make([]uint64, len(batch))
+		for i, f := range batch {
+			off[i], size[i] = f.PayloadOffset, f.Size
+		}
+		streams, crcs, err := z.pr.readDeflate(off, size, true, nil)
+		if err != nil {
+			return err
+		}
+		for i, f := range batch {
+			e := z.entry(f.Path, f.Mode, f.Mtime, 8, f.Size)
+			e.crc, e.comp_size = C.uint32_t(crcs[i]), C.uint64_t(len(streams[i]))
+			if err := z.localHeader(e); err != nil {
+				return err
+			}
+			if err := z.write(streams[i]); err != nil {
+				return err
+			}
+			if err := z.descriptor(e); err != nil {
+				return err
+			}
+		}
+		batch, acc = batch[:0], 0
+		return nil
+	}
+	for _, f := range files {
+		if f.Size > piece {
+			if err := flush(); err != nil {
+				return err
+			}
+			if err := z.large(f, piece); err != nil {
+				return err
+			}
+			continue
+		}
+		if len(batch) > 0 && acc+f.Size > piece {
+			if err := flush(); err != nil {
+				return err
+			}
+		}
+		batch = append(batch, f)
+		acc += f.Size
+	}
+	return flush()
+}
+
+func (z *ZipWriter) large(f ZipFile, piece uint64) error {
+	hdr := make([]byte, 16)
+	if err := z.pr.read([]uint64{f.PayloadOffset}, []uint64{16}, false, hdr, []uint64{0}); err != nil {
+		return err
+	}
+	if !bytes.Equal(hdr, header(pxarPayload, 16+f.Size)) {
+		return fmt.Errorf("pbsgpu: file at payload offset %d (%d bytes): bad PAYLOAD header", f.PayloadOffset, f.Size)
+	}
+	e := z.entry(f.Path, f.Mode, f.Mtime, 8, f.Size)
+	if err := z.localHeader(e); err != nil {
+		return err
+	}
+	var crc uint32
+	var csize uint64
+	for lo := uint64(0); lo < f.Size; {
+		n := f.Size - lo
+		if n > piece {
+			n = piece
+		}
+		more := []uint8{0}
+		if lo+n < f.Size {
+			more[0] = 1
+		}
+		s, c, err := z.pr.readDeflate([]uint64{f.PayloadOffset + 16 + lo}, []uint64{n}, false, more)
+		if err != nil {
+			return err
+		}
+		crc = uint32(C.pbsgpu_crc32_combine(C.uint32_t(crc), C.uint32_t(c[0]), C.uint64_t(n)))
+		csize += uint64(len(s[0]))
+		if err := z.write(s[0]); err != nil {
+			return err
+		}
+		lo += n
+	}
+	e.crc, e.comp_size = C.uint32_t(crc), C.uint64_t(csize)
+	return z.descriptor(e)
+}
+
+// Close writes the central directory and its end records, and frees the names.
+func (z *ZipWriter) Close() error {
+	var ep *C.pbsgpu_zip_entry
+	if len(z.entries) > 0 {
+		ep = &z.entries[0]
+	}
+	n := C.uint64_t(len(z.entries))
+	err := z.write(zipRecord(func(o *C.uint8_t, c C.uint64_t) C.uint64_t { return C.pbsgpu_zip_directory(ep, n, C.uint64_t(z.pos), o, c) }))
+	for i := range z.entries {
+		C.free(unsafe.Pointer(z.entries[i].name))
+	}
+	z.entries = nil
+	return err
 }

@@ -505,6 +505,67 @@ int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const uint64_t *le
 enum { PBSGPU_DEC_MISSING = PBSGPU_DEC_BAD_TAG + 1,   /* 9: a chunk the range needs was neither cached nor given */
        PBSGPU_DEC_BAD_HEADER };                        /* 10: READ_PAYLOAD and the 16-byte header does not match */
 
+/* ---- f3, read side: zip restore ------------------------------------------------------------------------------------
+ * Restore as zip (reference internal/pxar/zip.go, RestoreModeZip): files are compressed on the GPU into raw Deflate
+ * streams (RFC 1951) and the host writes the zip container around them (APPNOTE 6.3.x, as Go's archive/zip writes it).
+ * Deflate format (tests/deflate_ref.py restates it; DESIGN.md K15): a range is cut into 128 KiB segments coded
+ * independently (no match reaches an earlier segment), each with K9a's greedy parse at distances <= 32768 and matches
+ * <= 258 bytes, as the smallest of: stored blocks of <= 65535 bytes; one fixed-code block; one dynamic-code block
+ * (two-queue Huffman, 15-bit codes, 7-bit code-length code) -- stored, then fixed, on ties.  The stream's last block
+ * has BFINAL; any other segment ends byte-aligned (a fixed or dynamic block is followed by an empty stored block).
+ * The stream of 0 bytes is 03 00.
+ * pbsgpu_deflate_bound(len) = len + 15 * ceil(len / 131072) + 2: every stream of len bytes fits (a segment is never
+ * larger than its stored form, at most 3 stored blocks of 5 header bytes).
+ * pbsgpu_deflate_batch: n raw Deflate streams of [base + off[i], + len[i]) (HOST or DEVICE base) into out + out_off[i]
+ * (HOST or DEVICE, pbsgpu_deflate_bound(len[i]) reserved); out_len[i] = its size, crc_out[i] = the CRC-32 of the range
+ * (crc_out may be NULL).  more (may be NULL): more[i] != 0 means a later call continues stream i -- no BFINAL, a
+ * byte-aligned end, and len[i] must be a multiple of 128 KiB (EINVAL otherwise; a piece of 0 bytes is no bytes).
+ * Concatenating the pieces gives exactly the one-call stream.  Scratch is bounded per pass of 4096 segments, so a call
+ * of any size works.
+ * pbsgpu_crc32_combine: the CRC-32 of A || B from crc1 = CRC-32(A), crc2 = CRC-32(B) and len2 = |B| (host only). */
+uint64_t pbsgpu_deflate_bound(uint64_t len);
+int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                         const uint8_t *more, uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+uint32_t pbsgpu_crc32_combine(uint32_t crc1, uint32_t crc2, uint64_t len2);
+/* The zip container (host only, no ctx).  An entry: its name bytes (a directory's ends in '/'), Unix st_mode, mtime in
+ * seconds since the epoch, method (0 stored, 8 deflate), the CRC-32 and the compressed and uncompressed sizes of its
+ * content, and the offset of its local header in the archive.
+ *  - Entries whose name does not end in '/' (files: method 8; symlinks: method 0, the content is the target) set flag
+ *    bit 3: their local header carries zero CRC and sizes, and a data descriptor (signature, CRC, sizes; 8-byte sizes
+ *    when either size is >= 0xFFFFFFFF) follows the content.  Directories: method 0, sizes 0, no descriptor.
+ *  - "version made by" is Unix; external attributes are st_mode << 16, plus 0x10 for a directory; flag bit 11 is set
+ *    when the name is valid UTF-8 and not ASCII; DOS date and time are UTC, clamped to 1980-2107; an extended timestamp
+ *    (0x5455) is written when 0 <= mtime < 2^32.
+ *  - The central directory's zip64 extra field carries only the fields that overflow (size, compressed size, offset,
+ *    in that order); the zip64 end record and locator are written when the entry count (>= 0xFFFF), the directory's
+ *    offset or its size (>= 0xFFFFFFFF) overflow.
+ * Each call returns the record's size in bytes and writes it to out only when cap is at least that size.
+ * pbsgpu_zip_directory: the central directory of entries e[0..n), starting at archive offset `offset`, with its end
+ * records. */
+typedef struct pbsgpu_zip_entry {
+    const uint8_t *name;
+    uint32_t name_len;
+    uint32_t mode;
+    int64_t mtime;
+    uint32_t method;
+    uint32_t crc;
+    uint64_t comp_size, size;
+    uint64_t offset;
+} pbsgpu_zip_entry;
+/* pbsgpu_reader_read_deflate: pbsgpu_reader_read's arguments and rules (plan, groups, statuses, PBSGPU_READ_PAYLOAD header
+ * check, argument errors), but each range's output is its raw Deflate stream, as pbsgpu_deflate_batch writes it (more,
+ * crc_out as there): out is HOST memory with pbsgpu_deflate_bound(len[i]) reserved at out + out_off[i] (a device out is
+ * EINVAL), out_len[i] is the stream's size, and 0 when status[i] is not OK; no byte of a failed range is written.  The
+ * ranges are read into a device stage of the call's total range bytes and deflated there: file bytes never cross PCIe
+ * uncompressed. */
+int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
+                               const uint8_t *more, const void *blob_base, const uint64_t *blob_off, const uint64_t *blob_len,
+                               const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out, const uint64_t *out_off,
+                               uint64_t *out_len, uint32_t *crc_out, int32_t *status, int32_t *blob_status);
+uint64_t pbsgpu_zip_local_header(const pbsgpu_zip_entry *e, uint8_t *out, uint64_t cap);
+uint64_t pbsgpu_zip_data_descriptor(const pbsgpu_zip_entry *e, uint8_t *out, uint64_t cap);
+uint64_t pbsgpu_zip_directory(const pbsgpu_zip_entry *e, uint64_t n, uint64_t offset, uint8_t *out, uint64_t cap);
+
 /* ---- f2 ("next" row): the commit walk's per-file content hash ----------------------------------
  * emitBackedFile tees every new file through `xxh3.New()` and keeps `h.Sum64()` (reference
  * internal/pxarmount/commit.go:717-725); verifyBackedFileHashes later re-reads every file to recompute

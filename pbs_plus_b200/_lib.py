@@ -84,6 +84,17 @@ class Corpus(C.Structure):
                 ("edit_thresh16", C.c_uint32), ("edit_seed", C.c_uint64)]
 
 
+class ZipEntry(C.Structure):
+    """pbsgpu_zip_entry: one entry of the zip container (name bytes, Unix st_mode, mtime, method, CRC, sizes, the
+    offset of its local header)."""
+    _fields_ = [("name", C.c_void_p), ("name_len", C.c_uint32), ("mode", C.c_uint32), ("mtime", C.c_int64),
+                ("method", C.c_uint32), ("crc", C.c_uint32), ("comp_size", C.c_uint64), ("size", C.c_uint64),
+                ("offset", C.c_uint64)]
+
+
+DEFLATE_SEGMENT = 128 * 1024   # pbsgpu_deflate_batch: a piece that a later call continues is a multiple of this
+
+
 # every symbol include/pbsgpu.h declares (tests assert the .so exports all of them)
 SYMBOLS = [
     "pbsgpu_version", "pbsgpu_open", "pbsgpu_close", "pbsgpu_strerror", "pbsgpu_device_info",
@@ -102,6 +113,8 @@ SYMBOLS = [
     "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
     "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch", "pbsgpu_blob_decode_batch_enc",
     "pbsgpu_reader_open", "pbsgpu_reader_close", "pbsgpu_reader_size", "pbsgpu_reader_plan", "pbsgpu_reader_read",
+    "pbsgpu_deflate_bound", "pbsgpu_deflate_batch", "pbsgpu_crc32_combine", "pbsgpu_reader_read_deflate", "pbsgpu_zip_local_header",
+    "pbsgpu_zip_data_descriptor", "pbsgpu_zip_directory",
     "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
     "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
 ]
@@ -186,6 +199,19 @@ def lib() -> C.CDLL:
     L.pbsgpu_reader_size.restype = C.c_uint64
     L.pbsgpu_reader_plan.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, u64p]
     L.pbsgpu_reader_read.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.pbsgpu_deflate_bound.argtypes = [C.c_uint64]
+    L.pbsgpu_deflate_bound.restype = C.c_uint64
+    L.pbsgpu_deflate_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp]
+    L.pbsgpu_reader_read_deflate.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp,
+                                             vp, vp, vp]
+    L.pbsgpu_crc32_combine.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64]
+    L.pbsgpu_crc32_combine.restype = C.c_uint32
+    L.pbsgpu_zip_local_header.argtypes = [C.POINTER(ZipEntry), vp, C.c_uint64]
+    L.pbsgpu_zip_local_header.restype = C.c_uint64
+    L.pbsgpu_zip_data_descriptor.argtypes = [C.POINTER(ZipEntry), vp, C.c_uint64]
+    L.pbsgpu_zip_data_descriptor.restype = C.c_uint64
+    L.pbsgpu_zip_directory.argtypes = [vp, C.c_uint64, C.c_uint64, vp, C.c_uint64]
+    L.pbsgpu_zip_directory.restype = C.c_uint64
     L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
     L.pbsgpu_crypt_destroy.argtypes = [vp]
     L.pbsgpu_crypt_destroy.restype = None

@@ -220,8 +220,7 @@ static void blob_header(const uint8_t magic[8], uint32_t crc, uint8_t *out) {
 }
 extern "C" void pbsgpu_blob_header(uint32_t crc, uint8_t out[12]) { blob_header(BLOB_MAGIC_UNCOMPRESSED, crc, out); }
 
-// K6 over the device ranges [dbase + off[i], + len[i]) into d_out[n], enqueued on b's stream
-static int crc32_enqueue(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t *d_out) {
+int pbsgpu_crc32_enqueue(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t *d_out) {
     pbsgpu_ctx *ctx = b.ctx;
     if (int rc = upload_table_once(ctx, &ctx->d_crc_tables, crc_tables_bytes(), crc_fill_tables_host)) return rc;
     const int crc_variant = ctx->crc_variant;   // 0 = TMA-tiled kernel (default), 1 = simple lane-strided kernel (PBSGPU_CRC_VARIANT at open)
@@ -258,7 +257,7 @@ extern "C" int pbsgpu_crc32_batch(pbsgpu_ctx *ctx, const void *base, const uint6
     if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
     uint32_t *d_out = b.get<uint32_t>(n);
     if (!d_out) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
-    if (int rc = crc32_enqueue(b, dbase, off, len, n, d_out)) return rc;
+    if (int rc = pbsgpu_crc32_enqueue(b, dbase, off, len, n, d_out)) return rc;
     if (b.ok()) b.e = cudaMemcpyAsync(crc_out, d_out, (uint64_t)n * 4, cudaMemcpyDeviceToHost, b.st);
     return b.finish("crc32 batch");
 }
@@ -666,7 +665,7 @@ int pbsgpu_blob_decode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *b
     }
     uint32_t *d_crc = b.get<uint32_t>(n);
     if (!d_crc) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
-    if (int rc = crc32_enqueue(b, dbase, poff.data(), plen.data(), n, d_crc)) return rc;
+    if (int rc = pbsgpu_crc32_enqueue(b, dbase, poff.data(), plen.data(), n, d_crc)) return rc;
     std::vector<uint32_t> crc;
     if (crypt) {   // the host checks the magics and the CRCs of encrypted blobs; K13 those of plain blobs
         crc.resize(n);

@@ -356,3 +356,53 @@ extern "C" int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const u
     }
     return PBSGPU_OK;
 }
+
+// The zip restore's read: the ranges go through pbsgpu_reader_read into a device stage owned by this call, and only the
+// ranges whose status is OK are deflated from there (pbsgpu_deflate_batch) into the caller's host memory, so file bytes
+// cross PCIe compressed and no byte of a failed range reaches `out`.
+extern "C" int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
+                                          const uint8_t *more, const void *blob_base, const uint64_t *blob_off,
+                                          const uint64_t *blob_len, const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out,
+                                          const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out, int32_t *status,
+                                          int32_t *blob_status) {
+    if (!r || (n && (!off || !len || !out || !out_off || !out_len || !status)) ||
+        (n_blobs && (!blob_base || !blob_off || !blob_len || !blob_chunk)))
+        return PBSGPU_EINVAL;
+    pbsgpu_ctx *ctx = r->ctx;
+    Guard g(ctx);
+    if (n && pbsgpu_is_device_ptr(out)) return fail(ctx, PBSGPU_EINVAL, "read_deflate: out must be host memory");
+    for (uint32_t i = 0; i < n; i++)
+        if (more && more[i] && len[i] % DEFLATE_SEGMENT)
+            return fail(ctx, PBSGPU_EINVAL, "range %u: a piece that a later call continues must be a multiple of 128 KiB", i);
+    if (int rc = check_ranges(r, off, len, n, flags)) return rc;
+    std::vector<uint64_t> soff(n);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n; i++) { soff[i] = total; total += len[i]; }
+    Blocking b(ctx, ctx->streams[0]);
+    uint8_t *stage = b.get<uint8_t>(total + 16);
+    if (!stage) return fail(ctx, PBSGPU_ENOMEM, "read_deflate: device stage of %llu bytes failed", (unsigned long long)total);
+    if (int rc = pbsgpu_reader_read(r, off, len, n, flags, blob_base, blob_off, blob_len, blob_chunk, n_blobs, stage,
+                                    soff.data(), status, blob_status))
+        return rc;
+    std::vector<uint64_t> ko, kl, koo, klen;
+    std::vector<uint8_t> km;
+    std::vector<uint32_t> idx, kcrc;
+    for (uint32_t i = 0; i < n; i++) {
+        out_len[i] = 0;
+        if (crc_out) crc_out[i] = 0;
+        if (status[i] != PBSGPU_DEC_OK) continue;
+        idx.push_back(i); ko.push_back(soff[i]); kl.push_back(len[i]); koo.push_back(out_off[i]);
+        km.push_back(more && more[i]);
+    }
+    const uint32_t k = (uint32_t)idx.size();
+    if (k == 0) return PBSGPU_OK;
+    klen.resize(k); kcrc.resize(k);
+    if (int rc = pbsgpu_deflate_batch(ctx, stage, ko.data(), kl.data(), k, km.data(), out, koo.data(), klen.data(),
+                                      crc_out ? kcrc.data() : nullptr))
+        return rc;
+    for (uint32_t j = 0; j < k; j++) {
+        out_len[idx[j]] = klen[j];
+        if (crc_out) crc_out[idx[j]] = kcrc[j];
+    }
+    return PBSGPU_OK;
+}

@@ -241,6 +241,8 @@ int pbsgpu_job_finish(pbsgpu_job *j);     // blocks; reruns on candidate overflo
 cudaError_t pbsgpu_job_sync(pbsgpu_job *j);
 void pbsgpu_job_release(pbsgpu_job *j);   // waits for what the job still has in flight unless it finished
 
+// K6 (capi_aux.cu) over the device ranges [dbase + off[i], + len[i]) into d_out[n], enqueued on b's stream
+int pbsgpu_crc32_enqueue(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t *d_out);
 // K7 (capi_aux.cu): enqueue-only / collect pair so the fused batch call can put it on a job's stream
 struct XxhRun {
     uint64_t *d_off = nullptr, *d_len = nullptr, *d_first = nullptr, *d_out = nullptr, *d_state = nullptr, *d_S = nullptr;

@@ -208,42 +208,8 @@ __device__ uint32_t ent_fse_tree(EntShared &s, uint32_t top, uint32_t mx) {
 // Huffman code of the literals (warp 0): lengths, canonical codes, tree description and the one-stream bit count.
 // `full`: the full-alphabet mode, whose tree description may also take the FSE form.
 __device__ void ent_huffman(EntShared &s, uint32_t lane, bool full) {
-    const uint32_t top = s.top, m = s.nh;
-    for (uint32_t x = lane; x <= top; x += 32) s.hc[x] = s.lhist[x];
-    __syncwarp();
-    for (;;) {
-        // present symbols in (count, symbol) order
-        for (uint32_t x = lane; x <= top; x += 32) {
-            const uint32_t c = s.hc[x];
-            if (!c) continue;
-            uint32_t r = 0;
-            for (uint32_t y = 0; y <= top; y++) { const uint32_t e = s.hc[y]; r += e && (e < c || (e == c && y < x)); }
-            s.horder[r] = (uint8_t)x;
-        }
-        __syncwarp();
-        if (lane == 0) {
-            // two-queue Huffman: leaves in that order, internal nodes in the order they are made; each step joins the two
-            // smallest fronts, a leaf before a node of equal count.  A parent is made after its children.
-            for (uint32_t k = 0; k < m; k++) s.hw[k] = s.hc[s.horder[k]];
-            uint32_t i = 0, j = m, nxt = m;
-            for (uint32_t k = 0; k + 1 < m; k++, nxt++) {
-                uint32_t a, b;
-                if (i < m && (j >= nxt || s.hw[i] <= s.hw[j])) a = i++; else a = j++;
-                if (i < m && (j >= nxt || s.hw[i] <= s.hw[j])) b = i++; else b = j++;
-                s.hw[nxt] = s.hw[a] + s.hw[b];
-                s.hparent[a] = s.hparent[b] = (uint16_t)nxt;
-            }
-            s.hdepth[2 * m - 2] = 0;
-            for (int k = 2 * (int)m - 3; k >= 0; k--) s.hdepth[k] = s.hdepth[s.hparent[k]] + 1;
-            uint32_t mx = 0;
-            for (uint32_t k = 0; k < m; k++) { s.hlen[s.horder[k]] = s.hdepth[k]; mx = max(mx, (uint32_t)s.hdepth[k]); }
-            s.maxlen = mx;
-        }
-        __syncwarp();
-        if (s.maxlen <= ENT_HUF_MAXBITS) break;
-        for (uint32_t x = lane; x <= top; x += 32) s.hc[x] = (s.hc[x] + 1) >> 1;   // a present symbol stays present
-        __syncwarp();
-    }
+    const uint32_t top = s.top;
+    huf_lengths(s.lhist, top + 1, s.nh, ENT_HUF_MAXBITS, lane, s.hc, s.horder, s.hw, s.hparent, s.hdepth, s.hlen, &s.maxlen);
     if (lane) return;
     // canonical codes (RFC 8878 4.2.1.3): in (length descending, symbol ascending) order, consecutive prefixes in units
     // of 2^(maxbits - length)

@@ -36,7 +36,9 @@ __device__ __forceinline__ uint32_t lz_key(const uint8_t *p) {
 // SPANS (the _lzl span parse): block g also has the long spans spans[span_first[g - sbase] .. span_first[g - sbase + 1]),
 // packed start | length << 20 | offset << 40 and in order.  A span is taken where it starts and the parse jumps past
 // it; a match is cut at the next span's start and kept only while it is still >= LZ_MINMATCH long.
-template <bool SPANS>
+// DEFLATE (K15's parse, deflate.cuh): a candidate counts only at distance <= DEFLATE_WINDOW, and a match is cut at
+// DEFLATE_MAX_MATCH; the parse resumes behind the cut match.
+template <bool SPANS, bool DEFLATE = false>
 __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, const uint64_t *src, const uint32_t *size,
                                                          uint64_t first, uint8_t *slots, uint64_t *seqs, uint32_t *nseq,
                                                          uint32_t *nlit, const uint64_t *spans, const uint32_t *span_first,
@@ -68,7 +70,7 @@ __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, co
             const uint32_t key = lz_key(p + i);
             h = (key * 0x9E3779B1u) >> (32 - LZ_HBITS);
             const int c = table[h];
-            bool m = c >= 0 && lz_key(p + c) == key;
+            bool m = c >= 0 && (!DEFLATE || i - (uint32_t)c <= DEFLATE_WINDOW) && lz_key(p + c) == key;
 #pragma unroll
             for (int e = 4; e < LZ_MINMATCH; e++) m = m && i + e < S && __ldg(p + c + e) == __ldg(p + i + e);
             cand[threadIdx.x] = m ? c : -1;
@@ -100,7 +102,9 @@ __global__ void __launch_bounds__(LZ_THREADS) k_lz_parse(const uint8_t *base, co
                     const uint32_t diff = __ballot_sync(~0u, a >= S || __ldg(p + c + L + lane) != __ldg(p + a));
                     if (diff) { L += __ffs(diff) - 1; break; }
                     L += 32;
+                    if (DEFLATE && L >= DEFLATE_MAX_MATCH) break;
                 }
+                if (DEFLATE) L = min(L, DEFLATE_MAX_MATCH);
                 if (SPANS && ss != ~0u) {
                     L = min(L, ss - m);
                     if (L < LZ_MINMATCH) {   // too short once cut: m is a literal
@@ -138,6 +142,13 @@ cudaError_t launch_lz_parse_spans(const uint8_t *base, const uint64_t *src, cons
                                   const uint32_t *span_first, uint64_t sbase, cudaStream_t st) {
     if (nb == 0) return cudaSuccess;
     k_lz_parse<true><<<nb, LZ_THREADS, 0, st>>>(base, src, size, first, slots, seqs, nseq, nlit, spans, span_first, sbase);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_lz_parse_deflate(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint32_t nb, uint8_t *slots,
+                                    uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, cudaStream_t st) {
+    if (nb == 0) return cudaSuccess;
+    k_lz_parse<false, true><<<nb, LZ_THREADS, 0, st>>>(base, src, size, 0, slots, seqs, nseq, nlit, nullptr, nullptr, 0);
     return cudaGetLastError();
 }
 

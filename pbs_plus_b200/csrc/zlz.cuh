@@ -158,6 +158,10 @@ cudaError_t launch_lz_parse(const uint8_t *base, const uint64_t *src, const uint
 cudaError_t launch_lz_parse_spans(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint64_t first, uint32_t nb,
                                   uint8_t *slots, uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, const uint64_t *spans,
                                   const uint32_t *span_first, uint64_t sbase, cudaStream_t st);
+// K9a with the Deflate limits of deflate.cuh (K15's parse): blocks [0, nb) of (src[], size[]), outputs as launch_lz_parse's
+// with first = 0.
+cudaError_t launch_lz_parse_deflate(const uint8_t *base, const uint64_t *src, const uint32_t *size, uint32_t nb, uint8_t *slots,
+                                    uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, cudaStream_t st);
 // K9b: the Block_Content of those blocks in their slots; info[g] = content size | (offset of the content in the slot) << 30.
 // A size >= the block's size means the block stays raw (the slot then holds only its first LZ_SLOT bytes).
 cudaError_t launch_lz_encode(const LzTables *tab, uint64_t first, uint32_t nb, uint8_t *slots, const uint64_t *seqs,

@@ -52,6 +52,49 @@ def default_table() -> np.ndarray:
     return np.ctypeslib.as_array(_lib.lib().pbsgpu_default_table(), shape=(256,)).copy()
 
 
+def deflate_bound(n: int) -> int:
+    """pbsgpu_deflate_bound: the bytes every raw Deflate stream of n bytes fits in."""
+    return int(_lib.lib().pbsgpu_deflate_bound(n))
+
+
+def crc32_combine(crc1: int, crc2: int, len2: int) -> int:
+    """CRC-32 of A || B from CRC-32(A), CRC-32(B) and len(B) (pbsgpu_crc32_combine, host only)."""
+    return int(_lib.lib().pbsgpu_crc32_combine(crc1, crc2, len2))
+
+
+def zip_entry(name: bytes, mode: int, mtime: int, method: int = 0, crc: int = 0, comp_size: int = 0, size: int = 0,
+              offset: int = 0) -> "_lib.ZipEntry":
+    """A pbsgpu_zip_entry; the returned structure keeps `name` alive."""
+    name = bytes(name)
+    buf = C.create_string_buffer(name, len(name) or 1)
+    e = _lib.ZipEntry(C.cast(buf, C.c_void_p), len(name), mode, mtime, method, crc, comp_size, size, offset)
+    e._keep = buf
+    return e
+
+
+def _zip_record(fn, *args) -> bytes:
+    need = fn(*args, None, 0)
+    out = C.create_string_buffer(max(1, need))
+    assert fn(*args, out, need) == need
+    return out.raw[:need]
+
+
+def zip_local_header(e) -> bytes:
+    """The local file header of an entry (pbsgpu_zip_local_header)."""
+    return _zip_record(_lib.lib().pbsgpu_zip_local_header, C.byref(e))
+
+
+def zip_data_descriptor(e) -> bytes:
+    """The data descriptor behind an entry's content; b"" for a directory (pbsgpu_zip_data_descriptor)."""
+    return _zip_record(_lib.lib().pbsgpu_zip_data_descriptor, C.byref(e))
+
+
+def zip_directory(entries, offset: int) -> bytes:
+    """The central directory of `entries` at archive offset `offset`, with its end records (pbsgpu_zip_directory)."""
+    arr = (_lib.ZipEntry * max(1, len(entries)))(*entries)
+    return _zip_record(_lib.lib().pbsgpu_zip_directory, arr, len(entries), offset)
+
+
 class Engine:
     """One context on one GPU (pbsgpu_open).  Raises if the device or the .so is missing."""
 
@@ -258,6 +301,35 @@ class Engine:
         out = np.zeros(len(o), dtype=np.uint32)
         self._ck(self._L.pbsgpu_crc32_batch(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o), out.ctypes.data))
         return out
+
+    def deflate_batch(self, base, off, length, more=None, out: str = "host"):
+        """Raw Deflate streams (RFC 1951) of n byte ranges (host or device base) on the GPU (pbsgpu_deflate_batch).
+        more: per range, a later call continues the stream (its length a multiple of DEFLATE_SEGMENT).
+        out: "host" -> list of bytes, "device" -> list of torch CUDA tensor views.  -> (streams, crc32 u32[n])"""
+        if out not in ("host", "device"):
+            raise ValueError(f"out must be 'host' or 'device', not {out!r}")
+        o, l = self._offlen(off, length)
+        n = len(o)
+        bound = np.array([deflate_bound(int(x)) for x in l], dtype=np.uint64)
+        ooff = np.zeros(n, dtype=np.uint64)
+        if n:
+            ooff[1:] = np.cumsum(bound)[:-1]
+        total = max(1, int(bound.sum()))
+        if out == "host":
+            buf = np.zeros(total, dtype=np.uint8)
+        else:
+            import torch
+            buf = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self.device}")
+        m = None if more is None else np.ascontiguousarray(more, dtype=np.uint8)
+        if m is not None and m.shape != o.shape:
+            raise ValueError("more must hold one flag per range")
+        olen = np.zeros(n, dtype=np.uint64)
+        crc = np.zeros(n, dtype=np.uint32)
+        self._ck(self._L.pbsgpu_deflate_batch(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, n,
+                                              None if m is None else m.ctypes.data, _ptr(buf), ooff.ctypes.data,
+                                              olen.ctypes.data, crc.ctypes.data))
+        views = [buf[int(a):int(a) + int(b)] for a, b in zip(ooff, olen)]
+        return [v.tobytes() for v in views] if out == "host" else views, crc
 
     def blob_encode_batch(self, base, off, length):
         """Complete uncompressed DataBlobs (magic | crc32 | payload) of n ranges -> (bytes buffer, blob_off[n+1], crc[n])."""
@@ -566,6 +638,25 @@ class Crypt:
         self.close()
 
 
+def _blob_args(blobs):
+    """Reader.read's `blobs` -> (base, blob_off u64[k], blob_len u64[k], blob_chunk u64[k])."""
+    if isinstance(blobs, tuple):
+        base, bo, bl, bc = blobs
+        bo, bl = Engine._offlen(bo, bl)
+        bc = np.ascontiguousarray(bc, dtype=np.uint64)
+        if bc.shape != bo.shape:
+            raise ValueError("blob chunks must hold one index per blob")
+        return base, bo, bl, bc
+    items = list(blobs.items())
+    bc = np.array([c for c, _ in items], dtype=np.uint64)
+    bl = np.array([len(b) for _, b in items], dtype=np.uint64)
+    bo = np.zeros(len(items), dtype=np.uint64)
+    if len(items):
+        bo[1:] = np.cumsum(bl)[:-1]
+    base = np.frombuffer(b"".join(bytes(b) for _, b in items) or b"\0", dtype=np.uint8)
+    return base, bo, bl, bc
+
+
 class Reader:
     """An archive reader on the engine's device (pbsgpu_reader_*): plan() names the chunks a read needs that the cache
     lacks, read() verifies the blobs it is given into the cache and copies the ranges out of it."""
@@ -608,20 +699,7 @@ class Reader:
         if out not in ("host", "device"):
             raise ValueError(f"out must be 'host' or 'device', not {out!r}")
         o, l = Engine._offlen(off, length)
-        if isinstance(blobs, tuple):
-            base, bo, bl, bc = blobs
-            bo, bl = Engine._offlen(bo, bl)
-            bc = np.ascontiguousarray(bc, dtype=np.uint64)
-            if bc.shape != bo.shape:
-                raise ValueError("blob chunks must hold one index per blob")
-        else:
-            items = list(blobs.items())
-            bc = np.array([c for c, _ in items], dtype=np.uint64)
-            bl = np.array([len(b) for _, b in items], dtype=np.uint64)
-            bo = np.zeros(len(items), dtype=np.uint64)
-            if len(items):
-                bo[1:] = np.cumsum(bl)[:-1]
-            base = np.frombuffer(b"".join(bytes(b) for _, b in items) or b"\0", dtype=np.uint8)
+        base, bo, bl, bc = _blob_args(blobs)
         n, k = len(o), len(bo)
         ooff = np.zeros(n, dtype=np.uint64)
         if n:
@@ -642,6 +720,34 @@ class Reader:
             a, e = int(ooff[i]), int(ooff[i]) + int(l[i])
             data.append(None if status[i] != _lib.DEC_OK else buf[a:e].tobytes() if out == "host" else buf[a:e])
         return status, data, bst
+
+    def read_deflate(self, off, length, blobs, payload: bool = False, more=None):
+        """read() whose outputs are the ranges' raw Deflate streams (pbsgpu_reader_read_deflate): the ranges are
+        deflated on the device.  more: per range, a later call continues its stream (length a multiple of
+        DEFLATE_SEGMENT).  `blobs` as in read().  -> (status int32[n], streams (bytes, None where the status is not
+        DEC_OK), crc32 u32[n], blob_status int32[k])"""
+        o, l = Engine._offlen(off, length)
+        base, bo, bl, bc = _blob_args(blobs)
+        n, k = len(o), len(bo)
+        bound = np.array([deflate_bound(int(x)) for x in l], dtype=np.uint64)
+        ooff = np.zeros(n, dtype=np.uint64)
+        if n:
+            ooff[1:] = np.cumsum(bound)[:-1]
+        buf = np.zeros(max(1, int(bound.sum())), dtype=np.uint8)
+        m = None if more is None else np.ascontiguousarray(more, dtype=np.uint8)
+        if m is not None and m.shape != o.shape:
+            raise ValueError("more must hold one flag per range")
+        olen = np.zeros(n, dtype=np.uint64)
+        crc = np.zeros(n, dtype=np.uint32)
+        status = np.zeros(n, dtype=np.int32)
+        bst = np.zeros(k, dtype=np.int32)
+        self._eng._ck(self._eng._L.pbsgpu_reader_read_deflate(
+            self._h, o.ctypes.data, l.ctypes.data, n, _lib.READ_PAYLOAD if payload else 0,
+            None if m is None else m.ctypes.data, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
+            buf.ctypes.data, ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data, status.ctypes.data, bst.ctypes.data))
+        streams = [None if status[i] != _lib.DEC_OK else buf[int(ooff[i]):int(ooff[i]) + int(olen[i])].tobytes()
+                   for i in range(n)]
+        return status, streams, crc, bst
 
     def close(self):
         if getattr(self, "_h", None) and self._eng._h:

@@ -25,11 +25,15 @@ Two writers:
     describe a ppxar payload stream: use it for dedup statistics / digest computation, not to write .ppxar.didx.
 
 And for disk images (`.img.fidx` archives): FixedIndexWriter -- fixed-size chunks through the batch call, fed in slices.
+
+Restore as zip (reference internal/pxar/zip.go): ZipWriter -- files of a PayloadReader deflated on the GPU
+(pbsgpu_reader_read_deflate) inside a zip container written by pbsgpu_zip_*.
 """
 from __future__ import annotations
 
 import io
 import os
+import zlib
 from collections import deque
 from dataclasses import dataclass, field
 from typing import BinaryIO, Callable
@@ -38,6 +42,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import CHUNK_DTYPE, CHUNK_KNOWN, Cfg
+from . import engine as _engine
 from .engine import DigestSet, Engine
 
 
@@ -440,6 +445,18 @@ class PayloadReader:
             raise IOError(f"transfer: {what} {off[i]} ({size[i]} bytes): {_DEC_NAMES.get(int(status[i]), int(status[i]))}")
         return data
 
+    def _read_deflate(self, off: list[int], size: list[int], payload: bool, more=None):
+        """_read whose outputs are raw Deflate streams -> (streams, crc32s)."""
+        chunks, digests = self._reader.plan(off, size, payload)
+        blobs = {int(c): self._source(bytes(d)) for c, d in zip(chunks, digests)}
+        status, streams, crc, _ = self._reader.read_deflate(off, size, blobs, payload, more)
+        bad = np.flatnonzero(status != _lib.DEC_OK)
+        if len(bad):
+            i = int(bad[0])
+            what = "file at payload offset" if payload else "range at"
+            raise IOError(f"transfer: {what} {off[i]} ({size[i]} bytes): {_DEC_NAMES.get(int(status[i]), int(status[i]))}")
+        return streams, [int(c) for c in crc]
+
     def ReadAt(self, off: int, size: int) -> bytes:
         """io.ReaderAt: up to `size` bytes at archive offset `off`; short (possibly empty) at the archive's end."""
         if off < 0 or size < 0:
@@ -464,6 +481,84 @@ class PayloadReader:
 
     def __exit__(self, *a):
         self.Close()
+
+
+class ZipWriter:
+    """One `<name>.zip` of a restore (reference createZipForSource, internal/pxar/zip.go), written to `w`: directories,
+    symlinks (stored, the target as content) and files deflated on the GPU from a PayloadReader.  Every entry but a
+    directory has flag bit 3 and a data descriptor; Close writes the central directory.
+
+    AddFiles takes (path, st_mode, mtime, payload offset, size) tuples.  Files up to `piece_bytes` go in batches of
+    about `piece_bytes` file bytes, one plan / fetch / read_deflate per batch; a larger file goes in 128 KiB-aligned
+    pieces of plain ranges continued with `more`, after one plain read of its 16-byte PAYLOAD header, and its CRC-32 is
+    combined from the pieces'."""
+
+    def __init__(self, reader: PayloadReader, w: BinaryIO, piece_bytes: int = 1 << 30):
+        self._r, self._w = reader, w
+        self._piece = max(_lib.DEFLATE_SEGMENT, piece_bytes // _lib.DEFLATE_SEGMENT * _lib.DEFLATE_SEGMENT)
+        self._pos, self._entries = 0, []
+
+    def _write(self, b: bytes) -> None:
+        self._w.write(b)
+        self._pos += len(b)
+
+    def _entry(self, name: str, mode: int, mtime: int, method: int, body, crc: int, csize: int, size: int) -> None:
+        e = _engine.zip_entry(name.encode(), mode, int(mtime), method, crc, csize, size, self._pos)
+        self._write(_engine.zip_local_header(e))
+        for part in body:
+            self._write(part)
+        self._write(_engine.zip_data_descriptor(e))
+        self._entries.append(e)
+
+    def AddDirectory(self, path: str, mode: int, mtime: int) -> None:
+        name = path if path.endswith("/") else path + "/"
+        self._entry(name, mode, mtime, 0, [], 0, 0, 0)
+
+    def AddSymlink(self, path: str, target: str, mode: int, mtime: int) -> None:
+        t = target.encode()
+        self._entry(path, mode, mtime, 0, [t], zlib.crc32(t), len(t), len(t))
+
+    def AddFiles(self, files: list[tuple[str, int, int, int, int]]) -> None:
+        batch, acc = [], 0
+        for f in files:
+            if f[4] > self._piece:
+                self._flush(batch)
+                batch, acc = [], 0
+                self._large(*f)
+                continue
+            if batch and acc + f[4] > self._piece:
+                self._flush(batch)
+                batch, acc = [], 0
+            batch.append(f)
+            acc += f[4]
+        self._flush(batch)
+
+    def _flush(self, batch) -> None:
+        if not batch:
+            return
+        streams, crcs = self._r._read_deflate([f[3] for f in batch], [f[4] for f in batch], True)
+        for (path, mode, mtime, _, size), s, c in zip(batch, streams, crcs):
+            self._entry(path, mode, mtime, 8, [s], c, len(s), size)
+
+    def _large(self, path: str, mode: int, mtime: int, payload_offset: int, size: int) -> None:
+        if self._r.ReadAt(payload_offset, 16) != payload_header(size):
+            raise IOError(f"transfer: file at payload offset {payload_offset} ({size} bytes): DEC_BAD_HEADER")
+
+        # the local header carries no CRC or sizes (flag bit 3): the pieces stream out, then the descriptor
+        e = _engine.zip_entry(path.encode(), mode, int(mtime), 8, 0, 0, size, self._pos)
+        self._write(_engine.zip_local_header(e))
+        lo, crc, csize = 0, 0, 0
+        while lo < size:
+            n = min(self._piece, size - lo)
+            (s,), (c,) = self._r._read_deflate([payload_offset + 16 + lo], [n], False, [int(lo + n < size)])
+            crc, csize, lo = _engine.crc32_combine(crc, c, n), csize + len(s), lo + n
+            self._write(s)
+        e.crc, e.comp_size = crc, csize
+        self._write(_engine.zip_data_descriptor(e))
+        self._entries.append(e)
+
+    def Close(self) -> None:
+        self._write(_engine.zip_directory(self._entries, self._pos))
 
 
 def NewRemoteDedupSplitArchiveWriter(engine: Engine, config: Cfg, known: DigestSet | None = None,
