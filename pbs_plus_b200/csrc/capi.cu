@@ -6,7 +6,8 @@
 // runtime; no torch types.  There is no CPU fallback anywhere in this file: every data
 // path launches the kernels in scan.cu / resolve.cu / sha256.cu / digestset.cu.
 // Sibling translation units: capi_set.cu (digest set, NCCL merge), capi_stream.cu (streaming form),
-// capi_aux.cu (dynamic index and the blocking byte-range calls: SHA-256, CRC-32, DataBlob, XXH3).
+// capi_aux.cu (index images and the blocking byte-range calls: SHA-256, CRC-32, XXH3), capi_blob.cu (DataBlobs) and
+// capi_crypt.cu (encrypt mode's key handle).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>

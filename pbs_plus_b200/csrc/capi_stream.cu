@@ -15,7 +15,7 @@
 //
 // Two optional products of a window, made before its buffer is released:
 //  - DataBlobs of its new chunks (pbsgpu_stream_blob_mode): at collect time the window's chunks without
-//    PBSGPU_CHUNK_KNOWN are encoded in place by the batch encoders (capi_aux.cu) into a pinned arena of the stream.
+//    PBSGPU_CHUNK_KNOWN are encoded in place by the batch encoder (capi_blob.cu) into a pinned arena of the stream.
 //  - XXH3-64 of registered byte ranges (pbsgpu_stream_hash_range): each window hashes the blocks, tails and short ranges
 //    that lie in its CONSUMED part [base_off, base_off + consumed) with K7's piece form, on the stream's own CUDA stream
 //    (window k+1 continues window k's chain).  Ranges do not overlap, so at most one range crosses a window end; the
@@ -160,16 +160,11 @@ static int collect_blobs(pbsgpu_stream *s, const pbsgpu_job *j, const uint8_t *b
     BlobWindow bw{(uint8_t *)ctx->pin.get(bytes), std::move(out_off), std::vector<uint64_t>(off.size()), 0};
     if (!bw.host) return fail(ctx, PBSGPU_ENOMEM, "pinned blob arena of %llu bytes failed", (unsigned long long)bytes);
     const uint32_t nb = (uint32_t)off.size();
-    int rc;
-    if (s->crypt) {
-        std::vector<uint8_t> iv(16ull * nb);
-        rc = pbsgpu_stream_ivs(ctx, s->iv_seeded ? s->iv_seed : nullptr, s->n_blobs, nb, iv.data());
-        if (rc == PBSGPU_OK)
-            rc = pbsgpu_blob_encode_batch_enc(ctx, s->crypt, s->blob_mode, buf, off.data(), len.data(), nb, iv.data(), bw.host,
-                                              bw.off.data(), bw.len.data(), nullptr);
-    } else {
-        rc = pbsgpu_blob_encode_mode(ctx, buf, off.data(), len.data(), nb, s->blob_mode, bw.host, bw.off.data(), bw.len.data());
-    }
+    std::vector<uint8_t> iv(s->crypt ? 16ull * nb : 0);
+    int rc = s->crypt ? pbsgpu_stream_ivs(ctx, s->iv_seeded ? s->iv_seed : nullptr, s->n_blobs, nb, iv.data()) : PBSGPU_OK;
+    if (rc == PBSGPU_OK)
+        rc = pbsgpu_blob_encode(ctx, s->crypt, s->blob_mode, iv.data(), buf, off.data(), len.data(), nb, bw.host, bw.off.data(),
+                                bw.len.data(), nullptr);
     if (rc) { ctx->pin.put(bw.host); return rc; }
     s->n_blobs += nb;
     s->blobs.push_back(std::move(bw));

@@ -117,11 +117,11 @@ bool pbsgpu_is_pinned_ptr(const void *p);
 bool pbsgpu_cfg_ok(const pbsgpu_cfg *c);
 
 // ---------------------------------------------------------------------------
-// Blocking calls (capi_aux.cu, capi_set.cu): the device work is a chain of enqueues on one stream and the call returns
-// once it is done.  pbsgpu_finish always synchronises `st`, then maps the chain's first error `e` (or the sync's) to
-// PBSGPU_ECUDA "what: ...".  A Blocking keeps that first error (enqueue only while ok()) and the call's pool blocks;
-// they go back to the pool in the destructor after one more synchronisation, so on every exit path no kernel still uses
-// a block the pool can hand out again.
+// Blocking calls (capi_aux.cu, capi_blob.cu, capi_set.cu): the device work is a chain of enqueues on one stream and the
+// call returns once it is done.  pbsgpu_finish always synchronises `st`, then maps the chain's first error `e` (or the
+// sync's) to PBSGPU_ECUDA "what: ...".  A Blocking keeps that first error (enqueue only while ok()) and the call's pool
+// blocks; they go back to the pool in the destructor after one more synchronisation, so on every exit path no kernel
+// still uses a block the pool can hand out again.
 // ---------------------------------------------------------------------------
 int pbsgpu_finish(pbsgpu_ctx *ctx, cudaStream_t st, cudaError_t e, const char *what);
 struct Blocking {
@@ -150,6 +150,9 @@ struct Blocking {
     int stage(const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, const uint8_t **dbase);
     int finish(const char *what) { return pbsgpu_finish(ctx, st, e, what); }
 };
+// A constant table of a kernel (K6, K7, K9, K13): built on the host by `fill` and uploaded to *d on the context's first
+// use (freed with the context)
+int pbsgpu_upload_table_once(pbsgpu_ctx *ctx, void **d, size_t bytes, void (*fill)(void *));
 
 // ---------------------------------------------------------------------------
 // digest set (capi_set.cu)
@@ -243,6 +246,10 @@ void pbsgpu_job_release(pbsgpu_job *j);   // waits for what the job still has in
 
 // K6 (capi_aux.cu) over the device ranges [dbase + off[i], + len[i]) into d_out[n], enqueued on b's stream
 int pbsgpu_crc32_enqueue(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t *d_out);
+// K3 (capi_aux.cu) over the device chunks d_refs[0, *d_n) of `base` (n bounds the launch) into d_dig[32 n], keyed with the
+// device `suffix` (a crypt's id_key) or plain, enqueued on b's stream with the context's kernel variant
+void pbsgpu_sha256_enqueue(Blocking &b, const uint8_t *base, const pbsgpu::ChunkRef *d_refs, const unsigned long long *d_n,
+                           uint32_t n, const uint8_t *suffix, uint8_t *d_dig);
 // K7 (capi_aux.cu): enqueue-only / collect pair so the fused batch call can put it on a job's stream
 struct XxhRun {
     uint64_t *d_off = nullptr, *d_len = nullptr, *d_first = nullptr, *d_out = nullptr, *d_state = nullptr, *d_S = nullptr;
@@ -253,11 +260,13 @@ int pbsgpu_xxh3_enqueue(pbsgpu_ctx *ctx, const uint8_t *dbase, const uint64_t *o
 int pbsgpu_xxh3_collect(pbsgpu_ctx *ctx, XxhRun *r, uint64_t *hash_out, cudaStream_t st);
 void pbsgpu_xxh3_release(pbsgpu_ctx *ctx, XxhRun *r);
 int pbsgpu_xxh3_table(pbsgpu_ctx *ctx, const void **tab);   // K7's device table (uploaded on first use)
-// DataBlobs of n ranges with the encoder of `mode` (PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH, PBSGPU_BLOB_LZL): blob i at out + out_off[i],
-// out_len[i] bytes.  Device ranges are encoded in place.
-int pbsgpu_blob_encode_mode(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n, int mode,
-                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len);
-// The body of pbsgpu_blob_decode_batch (crypt NULL) and _enc (capi_aux.cu), without the argument checks: the archive
+// DataBlobs (capi_blob.cu) of n ranges with the encoder of `mode` (PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH, PBSGPU_BLOB_LZL),
+// encrypted with crypt and the IVs iv[16 n] or plain (crypt NULL): blob i at out + out_off[i], out_len[i] bytes (out_len
+// and crc_out may be NULL).  Device ranges are encoded in place.  The body of every pbsgpu_blob_encode_batch* call.
+int pbsgpu_blob_encode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, const uint8_t *iv, const void *base,
+                       const uint64_t *off, const uint64_t *len, uint32_t n, uint8_t *out, const uint64_t *out_off,
+                       uint64_t *out_len, uint32_t *crc_out);
+// The body of pbsgpu_blob_decode_batch (crypt NULL) and _enc (capi_blob.cu), without the argument checks: the archive
 // reader decodes its blobs through it into its device cache.
 int pbsgpu_blob_decode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, const void *base, const uint64_t *off, const uint64_t *len,
                        uint32_t n, const uint64_t *chunk_len, const uint8_t *digest, uint8_t *out, const uint64_t *out_off,

@@ -2,7 +2,7 @@
 //
 // _lzl is _lzh plus long matches that reach anywhere earlier in the same chunk.  K12 finds them per pass of whole chunks
 // (LDM_PASS_BYTES; tests/zstd_ldm_ref.py states every rule below); the host splits the kept ones at the 128 KiB block
-// edges into long spans, and K9a's span parse, K9b and K10 encode the blocks that hold one (capi_aux.cu, zstd_frames).
+// edges into long spans, and K9a's span parse, K9b and K10 encode the blocks that hold one (capi_blob.cu, zstd_frames).
 //
 //   anchor    position i >= 63 of a chunk whose gear hash h = sum_k G[byte i-k] << k (k < 64) has its top LDM_RATE bits
 //             zero; the fingerprint is h.  G is splitmix64 from LDM_SEED.

@@ -2,7 +2,7 @@
 //
 // Every 128 KiB block of a chunk that is not one repeated byte (K8a decides that) becomes a zstd Compressed_Block
 // (RFC 8878 3.1.1.3): a greedy LZ77 parse inside the block, Raw_Literals and a sequences section whose three FSE tables
-// are the predefined ones.  The host (capi_aux.cu, zstd_frames) keeps that block when it is smaller than the raw one.
+// are the predefined ones.  The host (capi_blob.cu, zstd_frames) keeps that block when it is smaller than the raw one.
 // The output is a pure function of the block's bytes; tests/zstd_lz_ref.py (zstd_frame_lz) states it.
 //
 //   cand(i)   for i <= S-4: the largest j in an EARLIER tile of LZ_TILE positions with h(j) == h(i), where

@@ -334,11 +334,7 @@ class Engine:
     def blob_encode_batch(self, base, off, length):
         """Complete uncompressed DataBlobs (magic | crc32 | payload) of n ranges -> (bytes buffer, blob_off[n+1], crc[n])."""
         o, l = self._offlen(off, length)
-        sizes = l + np.uint64(12)
-        boff = np.zeros(len(o) + 1, dtype=np.uint64)
-        np.cumsum(sizes, out=boff[1:])
-        out = np.zeros(int(boff[-1]), dtype=np.uint8)
-        crc = np.zeros(len(o), dtype=np.uint32)
+        out, boff, crc = self._blob_layout(l, 12)
         self._ck(self._L.pbsgpu_blob_encode_batch(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o),
                                                   out.ctypes.data if len(out) else None, boff.ctypes.data, crc.ctypes.data))
         return out, boff, crc
@@ -372,14 +368,18 @@ class Engine:
         most its _lzh blob (pbsgpu_blob_encode_batch_lzl) -> list of n `bytes` blobs, crc[n]."""
         return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lzl, base, off, length)
 
+    @staticmethod
+    def _blob_layout(l, head: int):
+        """Room for n blobs back to back, each its uncompressed payload behind a `head`-byte header (12, or 44 encrypted)
+        -> (out buffer, blob_off[n+1], crc[n])."""
+        boff = np.zeros(len(l) + 1, dtype=np.uint64)
+        np.cumsum(l + np.uint64(head), out=boff[1:])
+        return np.zeros(int(boff[-1]), dtype=np.uint8), boff, np.zeros(len(l), dtype=np.uint32)
+
     def _blob_encode_sized(self, fn, base, off, length):
         o, l = self._offlen(off, length)
-        sizes = l + np.uint64(12)
-        boff = np.zeros(len(o) + 1, dtype=np.uint64)
-        np.cumsum(sizes, out=boff[1:])
-        out = np.zeros(max(1, int(boff[-1])), dtype=np.uint8)
+        out, boff, crc = self._blob_layout(l, 12)
         blen = np.zeros(len(o), dtype=np.uint64)
-        crc = np.zeros(len(o), dtype=np.uint32)
         self._ck(fn(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o), out.ctypes.data, boff.ctypes.data,
                     blen.ctypes.data, crc.ctypes.data))
         return [out[int(boff[i]): int(boff[i]) + int(blen[i])].tobytes() for i in range(len(o))], crc
@@ -473,12 +473,8 @@ class Engine:
             raise ValueError("iv must hold 16 bytes per range")
         if mode not in BLOB_MODES or mode is None:
             raise ValueError(f"unknown blob mode {mode!r}")
-        sizes = l + np.uint64(44)
-        boff = np.zeros(len(o) + 1, dtype=np.uint64)
-        np.cumsum(sizes, out=boff[1:])
-        out = np.zeros(max(1, int(boff[-1])), dtype=np.uint8)
+        out, boff, crc = self._blob_layout(l, 44)
         blen = np.zeros(len(o), dtype=np.uint64)
-        crc = np.zeros(len(o), dtype=np.uint32)
         self._ck(self._L.pbsgpu_blob_encode_batch_enc(self._h, crypt._h, BLOB_MODES[mode], _ptr(base), o.ctypes.data,
                                                       l.ctypes.data, len(o), ivs.ctypes.data, out.ctypes.data,
                                                       boff.ctypes.data, blen.ctypes.data, crc.ctypes.data))
