@@ -95,29 +95,101 @@ class ZipEntry(C.Structure):
 DEFLATE_SEGMENT = 128 * 1024   # pbsgpu_deflate_batch: a piece that a later call continues is a multiple of this
 
 
-# every symbol include/pbsgpu.h declares (tests assert the .so exports all of them)
-SYMBOLS = [
-    "pbsgpu_version", "pbsgpu_open", "pbsgpu_close", "pbsgpu_strerror", "pbsgpu_device_info",
-    "pbsgpu_set_profiling", "pbsgpu_partition_info", "pbsgpu_scan_partition_sms", "pbsgpu_set_kernel_variant", "pbsgpu_config", "pbsgpu_config_kib",
-    "pbsgpu_default_table", "pbsgpu_chunk_digest_batch", "pbsgpu_batch_submit", "pbsgpu_batch_wait",
-    "pbsgpu_chunk_digest_batch_ex", "pbsgpu_batch_submit_ex", "pbsgpu_batch_free", "pbsgpu_batch_wait_input", "pbsgpu_batch_input_done",
-    "pbsgpu_scan_batch", "pbsgpu_sha256_batch", "pbsgpu_sha256_keyed_batch", "pbsgpu_stream_crypt", "pbsgpu_stream_open", "pbsgpu_stream_write",
-    "pbsgpu_stream_poll", "pbsgpu_stream_finish", "pbsgpu_stream_close", "pbsgpu_stream_reserve", "pbsgpu_stream_commit",
-    "pbsgpu_stream_slot_bytes", "pbsgpu_stream_suggest", "pbsgpu_stream_position", "pbsgpu_stream_blob_mode",
-    "pbsgpu_stream_poll_blobs", "pbsgpu_stream_hash_range", "pbsgpu_stream_poll_hashes", "pbsgpu_set_create",
-    "pbsgpu_set_destroy", "pbsgpu_set_insert", "pbsgpu_set_probe", "pbsgpu_set_count", "pbsgpu_set_seed_didx",
-    "pbsgpu_set_allgather", "pbsgpu_nccl_unique_id", "pbsgpu_nccl_comm_create", "pbsgpu_nccl_comm_destroy",
-    "pbsgpu_didx_size", "pbsgpu_didx_build", "pbsgpu_didx_parse", "pbsgpu_fidx_size", "pbsgpu_fidx_build", "pbsgpu_fidx_parse",
-    "pbsgpu_set_seed_fidx", "pbsgpu_reader_open_fidx", "pbsgpu_crc32_batch", "pbsgpu_blob_header",
-    "pbsgpu_blob_size", "pbsgpu_blob_encode_batch", "pbsgpu_blob_encode_batch_z", "pbsgpu_blob_encode_batch_lz", "pbsgpu_blob_encode_batch_lze",
-    "pbsgpu_blob_encode_batch_lzh", "pbsgpu_blob_encode_batch_lzl", "pbsgpu_crypt_create", "pbsgpu_crypt_destroy", "pbsgpu_blob_size_enc",
-    "pbsgpu_blob_encode_batch_enc", "pbsgpu_blob_decode_batch", "pbsgpu_blob_decode_batch_enc",
-    "pbsgpu_reader_open", "pbsgpu_reader_close", "pbsgpu_reader_size", "pbsgpu_reader_plan", "pbsgpu_reader_read",
-    "pbsgpu_deflate_bound", "pbsgpu_deflate_batch", "pbsgpu_crc32_combine", "pbsgpu_reader_read_deflate", "pbsgpu_zip_local_header",
-    "pbsgpu_zip_data_descriptor", "pbsgpu_zip_directory",
-    "pbsgpu_xxh3_batch", "pbsgpu_chunk_digest_batch_xxh3",
-    "pbsgpu_host_alloc", "pbsgpu_host_free", "pbsgpu_corpus_fill",
-]
+# Every symbol include/pbsgpu.h declares (tests assert the .so exports all of them) and its ctypes signature: the
+# argument types, or (argument types, result type) where the result is not int.
+_vp, _u32p, _u64p = C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)
+_SIGNATURES = {
+    "pbsgpu_version": [],
+    "pbsgpu_open": [C.c_int, C.POINTER(_vp)],
+    "pbsgpu_close": ([_vp], None),
+    "pbsgpu_strerror": ([_vp], C.c_char_p),
+    "pbsgpu_device_info": [_vp, C.POINTER(DevInfo)],
+    "pbsgpu_set_profiling": [_vp, C.c_int],
+    "pbsgpu_partition_info": [_vp, C.POINTER(C.c_int), C.POINTER(C.c_int)],
+    "pbsgpu_scan_partition_sms": [_vp],
+    "pbsgpu_set_kernel_variant": [_vp, C.c_int],
+    "pbsgpu_config": [C.c_uint32, _u32p, C.POINTER(Cfg)],
+    "pbsgpu_config_kib": [C.c_uint32, _u32p, C.POINTER(Cfg)],
+    "pbsgpu_default_table": ([], _u32p),
+    "pbsgpu_chunk_digest_batch": [_vp, C.POINTER(Cfg), _vp, _vp, _vp, C.c_uint32, _vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_batch_submit": [_vp, C.POINTER(Cfg), _vp, _vp, _vp, C.c_uint32, C.POINTER(_vp)],
+    "pbsgpu_batch_wait": [_vp, _vp, C.c_uint64, _u64p, C.POINTER(Timing)],
+    "pbsgpu_chunk_digest_batch_ex": [_vp, C.POINTER(Cfg), _vp, _vp, _vp, C.c_uint32, C.POINTER(BatchOpts), _vp, C.c_uint64, _u64p],
+    "pbsgpu_batch_submit_ex": [_vp, C.POINTER(Cfg), _vp, _vp, _vp, C.c_uint32, C.POINTER(BatchOpts), C.POINTER(_vp)],
+    "pbsgpu_batch_free": ([_vp], None),
+    "pbsgpu_batch_wait_input": [_vp],
+    "pbsgpu_batch_input_done": [_vp],
+    "pbsgpu_scan_batch": [_vp, C.POINTER(Cfg), _vp, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _vp, _u64p],
+    "pbsgpu_sha256_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp],
+    "pbsgpu_sha256_keyed_batch": [_vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp],
+    "pbsgpu_stream_crypt": [_vp, _vp, _vp],
+    "pbsgpu_stream_open": [_vp, C.POINTER(Cfg), _vp, C.POINTER(_vp)],
+    "pbsgpu_stream_write": [_vp, _vp, C.c_uint64],
+    "pbsgpu_stream_poll": [_vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_stream_finish": [_vp],
+    "pbsgpu_stream_close": ([_vp], None),
+    "pbsgpu_stream_reserve": [_vp, C.POINTER(_vp)],
+    "pbsgpu_stream_commit": [_vp, C.c_uint64],
+    "pbsgpu_stream_slot_bytes": ([_vp], C.c_uint64),
+    "pbsgpu_stream_suggest": [_vp, C.c_uint64],
+    "pbsgpu_stream_position": ([_vp], C.c_uint64),
+    "pbsgpu_stream_blob_mode": [_vp, C.c_int],
+    "pbsgpu_stream_poll_blobs": [_vp, _vp, C.c_uint64, _vp, C.c_uint64, _u64p],
+    "pbsgpu_stream_hash_range": [_vp, C.c_uint64, C.c_uint64],
+    "pbsgpu_stream_poll_hashes": [_vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_set_create": [_vp, C.c_uint64, C.POINTER(_vp)],
+    "pbsgpu_set_destroy": ([_vp], None),
+    "pbsgpu_set_insert": [_vp, _vp, C.c_uint64, _vp],
+    "pbsgpu_set_probe": [_vp, _vp, C.c_uint64, _vp],
+    "pbsgpu_set_count": [_vp, _u64p],
+    "pbsgpu_set_seed_didx": [_vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_set_allgather": [_vp, _vp, _vp, C.c_uint64, _vp],
+    "pbsgpu_nccl_unique_id": [_vp],
+    "pbsgpu_nccl_comm_create": [_vp, _vp, C.c_int, C.c_int, C.POINTER(_vp)],
+    "pbsgpu_nccl_comm_destroy": ([_vp], None),
+    "pbsgpu_didx_size": ([C.c_uint64], C.c_uint64),
+    "pbsgpu_didx_build": [_vp, _vp, C.c_uint64, _vp, C.c_int64, _vp, C.c_uint64],
+    "pbsgpu_didx_parse": [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _u64p, C.c_int],
+    "pbsgpu_fidx_size": ([C.c_uint64], C.c_uint64),
+    "pbsgpu_fidx_build": [_vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _vp, C.c_int64, _vp, C.c_uint64],
+    "pbsgpu_fidx_parse": [_vp, _vp, C.c_uint64, _u64p, _u64p, _vp, C.c_uint64, _u64p, C.c_int],
+    "pbsgpu_set_seed_fidx": [_vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_reader_open_fidx": [_vp, _vp, C.c_uint64, _vp, C.c_uint64, C.POINTER(_vp)],
+    "pbsgpu_crc32_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp],
+    "pbsgpu_blob_header": ([C.c_uint32, _vp], None),
+    "pbsgpu_blob_size": ([C.c_uint64], C.c_uint64),
+    "pbsgpu_blob_encode_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp],
+    "pbsgpu_blob_encode_batch_z": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_encode_batch_lz": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_encode_batch_lze": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_encode_batch_lzh": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_encode_batch_lzl": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_crypt_create": [_vp, _vp, C.POINTER(_vp)],
+    "pbsgpu_crypt_destroy": ([_vp], None),
+    "pbsgpu_blob_size_enc": ([C.c_uint64], C.c_uint64),
+    "pbsgpu_blob_encode_batch_enc": [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_decode_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_decode_batch_enc": [_vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pbsgpu_reader_open": [_vp, _vp, C.c_uint64, _vp, C.c_uint64, C.POINTER(_vp)],
+    "pbsgpu_reader_close": ([_vp], None),
+    "pbsgpu_reader_size": ([_vp], C.c_uint64),
+    "pbsgpu_reader_plan": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_reader_read": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_deflate_bound": ([C.c_uint64], C.c_uint64),
+    "pbsgpu_deflate_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp],
+    "pbsgpu_crc32_combine": ([C.c_uint32, C.c_uint32, C.c_uint64], C.c_uint32),
+    "pbsgpu_reader_read_deflate": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
+                                   _vp, _vp],
+    "pbsgpu_zip_local_header": ([C.POINTER(ZipEntry), _vp, C.c_uint64], C.c_uint64),
+    "pbsgpu_zip_data_descriptor": ([C.POINTER(ZipEntry), _vp, C.c_uint64], C.c_uint64),
+    "pbsgpu_zip_directory": ([_vp, C.c_uint64, C.c_uint64, _vp, C.c_uint64], C.c_uint64),
+    "pbsgpu_xxh3_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp],
+    "pbsgpu_chunk_digest_batch_xxh3": [_vp, C.POINTER(Cfg), _vp, _vp, _vp, C.c_uint32, _vp, _vp, C.c_uint64, _u64p, _vp],
+    "pbsgpu_host_alloc": ([_vp, C.c_uint64], _vp),
+    "pbsgpu_host_free": ([_vp, _vp], None),
+    "pbsgpu_corpus_fill": [_vp, C.POINTER(Corpus), C.c_uint64, C.c_uint32, _vp, C.c_uint64],
+}
+SYMBOLS = list(_SIGNATURES)
 
 _lib = None
 
@@ -132,118 +204,8 @@ def lib() -> C.CDLL:
             f"{LIB_PATH} not found: the CUDA extension is the product and there is no fallback. "
             "Build it with `python -m pbs_plus_b200.build` (or __graft_entry__.build()).")
     L = C.CDLL(str(LIB_PATH))
-    vp, u32p, u64p = C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)
-    L.pbsgpu_version.restype = C.c_int
-    L.pbsgpu_open.argtypes = [C.c_int, C.POINTER(vp)]
-    L.pbsgpu_close.argtypes = [vp]
-    L.pbsgpu_close.restype = None
-    L.pbsgpu_strerror.argtypes = [vp]
-    L.pbsgpu_strerror.restype = C.c_char_p
-    L.pbsgpu_device_info.argtypes = [vp, C.POINTER(DevInfo)]
-    L.pbsgpu_set_profiling.argtypes = [vp, C.c_int]
-    L.pbsgpu_partition_info.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.pbsgpu_scan_partition_sms.argtypes = [vp]
-    L.pbsgpu_set_kernel_variant.argtypes = [vp, C.c_int]
-    L.pbsgpu_config.argtypes = [C.c_uint32, u32p, C.POINTER(Cfg)]
-    L.pbsgpu_config_kib.argtypes = [C.c_uint32, u32p, C.POINTER(Cfg)]
-    L.pbsgpu_default_table.restype = u32p
-    L.pbsgpu_chunk_digest_batch.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, vp, vp, C.c_uint64, u64p]
-    L.pbsgpu_batch_submit.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, C.POINTER(vp)]
-    L.pbsgpu_batch_wait.argtypes = [vp, vp, C.c_uint64, u64p, C.POINTER(Timing)]
-    L.pbsgpu_chunk_digest_batch_ex.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, C.POINTER(BatchOpts), vp, C.c_uint64, u64p]
-    L.pbsgpu_batch_submit_ex.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, C.POINTER(BatchOpts), C.POINTER(vp)]
-    L.pbsgpu_batch_free.argtypes = [vp]
-    L.pbsgpu_batch_wait_input.argtypes = [vp]
-    L.pbsgpu_batch_input_done.argtypes = [vp]
-    L.pbsgpu_batch_free.restype = None
-    L.pbsgpu_scan_batch.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, u64p]
-    L.pbsgpu_sha256_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
-    L.pbsgpu_sha256_keyed_batch.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, vp]
-    L.pbsgpu_stream_crypt.argtypes = [vp, vp, vp]
-    L.pbsgpu_stream_open.argtypes = [vp, C.POINTER(Cfg), vp, C.POINTER(vp)]
-    L.pbsgpu_stream_write.argtypes = [vp, vp, C.c_uint64]
-    L.pbsgpu_stream_poll.argtypes = [vp, vp, C.c_uint64, u64p]
-    L.pbsgpu_stream_finish.argtypes = [vp]
-    L.pbsgpu_stream_close.argtypes = [vp]
-    L.pbsgpu_stream_close.restype = None
-    L.pbsgpu_stream_reserve.argtypes = [vp, C.POINTER(vp)]
-    L.pbsgpu_stream_commit.argtypes = [vp, C.c_uint64]
-    L.pbsgpu_stream_slot_bytes.argtypes = [vp]
-    L.pbsgpu_stream_slot_bytes.restype = C.c_uint64
-    L.pbsgpu_stream_suggest.argtypes = [vp, C.c_uint64]
-    L.pbsgpu_stream_position.argtypes = [vp]
-    L.pbsgpu_stream_position.restype = C.c_uint64
-    L.pbsgpu_stream_blob_mode.argtypes = [vp, C.c_int]
-    L.pbsgpu_stream_poll_blobs.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, u64p]
-    L.pbsgpu_stream_hash_range.argtypes = [vp, C.c_uint64, C.c_uint64]
-    L.pbsgpu_stream_poll_hashes.argtypes = [vp, vp, C.c_uint64, u64p]
-    L.pbsgpu_set_allgather.argtypes = [vp, vp, vp, C.c_uint64, vp]
-    L.pbsgpu_nccl_unique_id.argtypes = [vp]
-    L.pbsgpu_nccl_comm_create.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(vp)]
-    L.pbsgpu_nccl_comm_destroy.argtypes = [vp]
-    L.pbsgpu_nccl_comm_destroy.restype = None
-    L.pbsgpu_blob_size.argtypes = [C.c_uint64]
-    L.pbsgpu_blob_size.restype = C.c_uint64
-    L.pbsgpu_blob_encode_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp]
-    L.pbsgpu_blob_encode_batch_z.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
-    L.pbsgpu_blob_encode_batch_lz.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
-    L.pbsgpu_blob_encode_batch_lze.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
-    L.pbsgpu_blob_encode_batch_lzh.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
-    L.pbsgpu_blob_encode_batch_lzl.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
-    L.pbsgpu_blob_decode_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
-    L.pbsgpu_blob_decode_batch_enc.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
-    L.pbsgpu_reader_open.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(vp)]
-    L.pbsgpu_reader_close.argtypes = [vp]
-    L.pbsgpu_reader_close.restype = None
-    L.pbsgpu_reader_size.argtypes = [vp]
-    L.pbsgpu_reader_size.restype = C.c_uint64
-    L.pbsgpu_reader_plan.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, u64p]
-    L.pbsgpu_reader_read.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
-    L.pbsgpu_deflate_bound.argtypes = [C.c_uint64]
-    L.pbsgpu_deflate_bound.restype = C.c_uint64
-    L.pbsgpu_deflate_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp]
-    L.pbsgpu_reader_read_deflate.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp,
-                                             vp, vp, vp]
-    L.pbsgpu_crc32_combine.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64]
-    L.pbsgpu_crc32_combine.restype = C.c_uint32
-    L.pbsgpu_zip_local_header.argtypes = [C.POINTER(ZipEntry), vp, C.c_uint64]
-    L.pbsgpu_zip_local_header.restype = C.c_uint64
-    L.pbsgpu_zip_data_descriptor.argtypes = [C.POINTER(ZipEntry), vp, C.c_uint64]
-    L.pbsgpu_zip_data_descriptor.restype = C.c_uint64
-    L.pbsgpu_zip_directory.argtypes = [vp, C.c_uint64, C.c_uint64, vp, C.c_uint64]
-    L.pbsgpu_zip_directory.restype = C.c_uint64
-    L.pbsgpu_crypt_create.argtypes = [vp, vp, C.POINTER(vp)]
-    L.pbsgpu_crypt_destroy.argtypes = [vp]
-    L.pbsgpu_crypt_destroy.restype = None
-    L.pbsgpu_blob_size_enc.argtypes = [C.c_uint64]
-    L.pbsgpu_blob_size_enc.restype = C.c_uint64
-    L.pbsgpu_blob_encode_batch_enc.argtypes = [vp, vp, C.c_int, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp]
-    L.pbsgpu_set_create.argtypes = [vp, C.c_uint64, C.POINTER(vp)]
-    L.pbsgpu_set_destroy.argtypes = [vp]
-    L.pbsgpu_set_destroy.restype = None
-    L.pbsgpu_set_insert.argtypes = [vp, vp, C.c_uint64, vp]
-    L.pbsgpu_set_probe.argtypes = [vp, vp, C.c_uint64, vp]
-    L.pbsgpu_set_count.argtypes = [vp, u64p]
-    L.pbsgpu_set_seed_didx.argtypes = [vp, vp, C.c_uint64, u64p]
-    L.pbsgpu_didx_size.argtypes = [C.c_uint64]
-    L.pbsgpu_didx_size.restype = C.c_uint64
-    L.pbsgpu_didx_build.argtypes = [vp, vp, C.c_uint64, vp, C.c_int64, vp, C.c_uint64]
-    L.pbsgpu_didx_parse.argtypes = [vp, vp, C.c_uint64, vp, vp, C.c_uint64, u64p, C.c_int]
-    L.pbsgpu_set_seed_fidx.argtypes = [vp, vp, C.c_uint64, u64p]
-    L.pbsgpu_fidx_size.argtypes = [C.c_uint64]
-    L.pbsgpu_fidx_size.restype = C.c_uint64
-    L.pbsgpu_fidx_build.argtypes = [vp, vp, C.c_uint64, C.c_uint64, C.c_uint64, vp, C.c_int64, vp, C.c_uint64]
-    L.pbsgpu_fidx_parse.argtypes = [vp, vp, C.c_uint64, u64p, u64p, vp, C.c_uint64, u64p, C.c_int]
-    L.pbsgpu_reader_open_fidx.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(vp)]
-    L.pbsgpu_crc32_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
-    L.pbsgpu_xxh3_batch.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
-    L.pbsgpu_chunk_digest_batch_xxh3.argtypes = [vp, C.POINTER(Cfg), vp, vp, vp, C.c_uint32, vp, vp, C.c_uint64, u64p, vp]
-    L.pbsgpu_blob_header.argtypes = [C.c_uint32, vp]
-    L.pbsgpu_blob_header.restype = None
-    L.pbsgpu_host_alloc.argtypes = [vp, C.c_uint64]
-    L.pbsgpu_host_alloc.restype = vp
-    L.pbsgpu_host_free.argtypes = [vp, vp]
-    L.pbsgpu_host_free.restype = None
-    L.pbsgpu_corpus_fill.argtypes = [vp, C.POINTER(Corpus), C.c_uint64, C.c_uint32, vp, C.c_uint64]
+    for name, sig in _SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.argtypes, fn.restype = sig if isinstance(sig, tuple) else (sig, C.c_int)
     _lib = L
     return L

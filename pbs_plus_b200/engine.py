@@ -33,6 +33,59 @@ def _cfg_ref(cfg: Cfg | None):
     return C.byref(cfg) if cfg is not None else None
 
 
+def _offsets(sizes) -> tuple[np.ndarray, int]:
+    """Ranges of `sizes` laid back to back -> (exclusive offsets u64[n], total)."""
+    sizes = np.asarray(sizes, dtype=np.uint64)
+    off = np.zeros(len(sizes), dtype=np.uint64)
+    if len(sizes):
+        off[1:] = np.cumsum(sizes)[:-1]
+    return off, int(sizes.sum())
+
+
+def _pack(arrays) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Host streams in one buffer, each starting 256-byte aligned -> (buf, off u64[n], len u64[n])."""
+    arrs = [np.ascontiguousarray(a, dtype=np.uint8) for a in arrays]
+    off, total = _offsets([(len(a) + 255) & ~255 for a in arrs])
+    buf = np.zeros(max(total, 1), dtype=np.uint8)
+    for a, o in zip(arrs, off):
+        buf[int(o): int(o) + len(a)] = a
+    return buf, off, np.array([len(a) for a in arrs], dtype=np.uint64)
+
+
+def _join(items) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """`bytes`-like items back to back, unpadded -> (base, off u64[n], len u64[n]); the base of no items is b"\\0"."""
+    lens = np.array([len(b) for b in items], dtype=np.uint64)
+    off, _ = _offsets(lens)
+    return np.frombuffer(b"".join(bytes(b) for b in items) or b"\0", dtype=np.uint8), off, lens
+
+
+def _split(buf, off, length, keep=None) -> list:
+    """buf[off[i]:off[i] + length[i]] per range: `bytes` from a numpy buffer, a view of a tensor; None where keep[i] is
+    false."""
+    views = [buf[int(a): int(a) + int(n)] if keep is None or keep[i] else None
+             for i, (a, n) in enumerate(zip(off, length))]
+    return [v.tobytes() if isinstance(v, np.ndarray) else v for v in views]
+
+
+def _deflate_layout(l: np.ndarray, more):
+    """Output room of n raw Deflate streams -> (out_off u64[n] spaced by deflate_bound, total bytes, more u8[n] or
+    None)."""
+    off, total = _offsets([deflate_bound(int(x)) for x in l])
+    m = None if more is None else np.ascontiguousarray(more, dtype=np.uint8)
+    if m is not None and m.shape != l.shape:
+        raise ValueError("more must hold one flag per range")
+    return off, total, m
+
+
+def _digests(digests, per: str, n: int | None = None) -> np.ndarray:
+    """Digests as `bytes` or an array, 32 bytes per item (n items, or any number) -> flat u8; `per` ends the error."""
+    d = np.ascontiguousarray(np.frombuffer(bytes(digests), dtype=np.uint8) if isinstance(digests, (bytes, bytearray))
+                             else np.asarray(digests, dtype=np.uint8)).reshape(-1)
+    if d.size != 32 * (d.size // 32 if n is None else n):
+        raise ValueError(f"digests must hold 32 bytes {per}")
+    return d
+
+
 def make_config(avg_bytes: int, table: np.ndarray | None = None) -> Cfg:
     """Chunker parameters; replaces buzhash.NewConfig (reference commit.go:302-305). avg in BYTES."""
     cfg = Cfg()
@@ -131,6 +184,16 @@ class Engine:
     def __exit__(self, *a):
         self.close()
 
+    def _alloc(self, nbytes: int, out: str | None):
+        """The output buffer of a call (at least one byte): numpy for "host", a torch CUDA tensor on this engine's
+        device for "device", None for None."""
+        if out == "host":
+            return np.zeros(max(1, nbytes), dtype=np.uint8)
+        if out == "device":
+            import torch
+            return torch.empty(max(1, nbytes), dtype=torch.uint8, device=f"cuda:{self.device}")
+        return None
+
     def device_info(self) -> dict:
         d = DevInfo()
         self._ck(self._L.pbsgpu_device_info(self._h, C.byref(d)))
@@ -164,11 +227,12 @@ class Engine:
         return o, l
 
     @staticmethod
-    def _chunk_cap(cfg: Cfg | None, l: np.ndarray, fixed_size: int = 0) -> int:
+    def _chunk_cap(cfg: Cfg | None, l: np.ndarray, fixed_size: int = 0, forced=None) -> int:
+        extra = 1 + (len(forced[0]) if forced is not None else 0)
         if fixed_size:
-            return int(((l + np.uint64(fixed_size - 1)) // np.uint64(fixed_size)).sum()) + 1
+            return int(((l + np.uint64(fixed_size - 1)) // np.uint64(fixed_size)).sum()) + extra
         m = max(int(cfg.min), 65)
-        return int((l // np.uint64(m)).sum()) + len(l) + 1
+        return int((l // np.uint64(m)).sum()) + len(l) + extra
 
     @staticmethod
     def _opts(digest_set, forced, xxh3=None, crypt=None, fixed_size: int = 0):
@@ -199,7 +263,7 @@ class Engine:
         digests SHA-256(chunk || id_key) of encrypt mode, also for the set's probe + insert.  `fixed_size`: cut every
         stream at multiples of it instead (the chunks of a .fidx image; cfg may be None)."""
         o, l = self._offlen(off, length)
-        cap = self._chunk_cap(cfg, l, fixed_size) + (len(forced[0]) if forced is not None else 0)
+        cap = self._chunk_cap(cfg, l, fixed_size, forced)
         out = np.zeros(cap, dtype=CHUNK_DTYPE)
         n_out = C.c_uint64()
         keep = base  # keep the buffer alive for the duration of the call
@@ -218,30 +282,15 @@ class Engine:
         out = np.zeros(cap, dtype=CHUNK_DTYPE)
         hashes = np.zeros(len(o), dtype=np.uint64)
         n_out = C.c_uint64()
-        keep = base
-        if crypt is None:
-            self._ck(self._L.pbsgpu_chunk_digest_batch_xxh3(
-                self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o),
-                digest_set._h if digest_set is not None else None, out.ctypes.data, cap, C.byref(n_out), hashes.ctypes.data))
-        else:
-            opts, _k = self._opts(digest_set, None, hashes, crypt)
-            self._ck(self._L.pbsgpu_chunk_digest_batch_ex(
-                self._h, C.byref(cfg), _ptr(keep), o.ctypes.data, l.ctypes.data, len(o), C.byref(opts), out.ctypes.data,
-                cap, C.byref(n_out)))
+        opts, _k = self._opts(digest_set, None, hashes, crypt)
+        self._ck(self._L.pbsgpu_chunk_digest_batch_ex(
+            self._h, C.byref(cfg), _ptr(base), o.ctypes.data, l.ctypes.data, len(o), C.byref(opts), out.ctypes.data,
+            cap, C.byref(n_out)))
         return out[: n_out.value], hashes
 
     def chunk_digest_streams(self, cfg: Cfg, streams: Iterable[np.ndarray], digest_set=None) -> np.ndarray:
         """Convenience for host streams that are separate arrays: packs them and calls the batch ABI."""
-        arrs = [np.ascontiguousarray(s, dtype=np.uint8) for s in streams]
-        lens = np.array([len(a) for a in arrs], dtype=np.uint64)
-        offs = np.zeros(len(arrs), dtype=np.uint64)
-        pos = 0
-        for i, a in enumerate(arrs):
-            offs[i] = pos
-            pos += (len(a) + 255) & ~255
-        buf = np.zeros(max(pos, 1), dtype=np.uint8)
-        for a, o in zip(arrs, offs):
-            buf[int(o): int(o) + len(a)] = a
+        buf, offs, lens = _pack(streams)
         return self.chunk_digest_batch(cfg, buf, offs, lens, digest_set)
 
     def submit(self, cfg: Cfg | None, base_dev, off, length, digest_set: "DigestSet | None" = None, forced=None,
@@ -257,7 +306,7 @@ class Engine:
             opts.flags |= _lib.BATCH_EARLY_INPUT
         self._ck(self._L.pbsgpu_batch_submit_ex(self._h, _cfg_ref(cfg), _ptr(base_dev), o.ctypes.data, l.ctypes.data,
                                                 len(o), C.byref(opts), C.byref(h)))
-        return Job(self, h, self._chunk_cap(cfg, l, fixed_size) + (len(forced[0]) if forced is not None else 0), base_dev)
+        return Job(self, h, self._chunk_cap(cfg, l, fixed_size, forced), base_dev)
 
     def scan_batch(self, cfg: Cfg, base_dev, off, length):
         """Boundaries only (a2).  Returns (ends, stream_first)."""
@@ -310,26 +359,14 @@ class Engine:
             raise ValueError(f"out must be 'host' or 'device', not {out!r}")
         o, l = self._offlen(off, length)
         n = len(o)
-        bound = np.array([deflate_bound(int(x)) for x in l], dtype=np.uint64)
-        ooff = np.zeros(n, dtype=np.uint64)
-        if n:
-            ooff[1:] = np.cumsum(bound)[:-1]
-        total = max(1, int(bound.sum()))
-        if out == "host":
-            buf = np.zeros(total, dtype=np.uint8)
-        else:
-            import torch
-            buf = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self.device}")
-        m = None if more is None else np.ascontiguousarray(more, dtype=np.uint8)
-        if m is not None and m.shape != o.shape:
-            raise ValueError("more must hold one flag per range")
+        ooff, total, m = _deflate_layout(l, more)
+        buf = self._alloc(total, out)
         olen = np.zeros(n, dtype=np.uint64)
         crc = np.zeros(n, dtype=np.uint32)
         self._ck(self._L.pbsgpu_deflate_batch(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, n,
                                               None if m is None else m.ctypes.data, _ptr(buf), ooff.ctypes.data,
                                               olen.ctypes.data, crc.ctypes.data))
-        views = [buf[int(a):int(a) + int(b)] for a, b in zip(ooff, olen)]
-        return [v.tobytes() for v in views] if out == "host" else views, crc
+        return _split(buf, ooff, olen), crc
 
     def blob_encode_batch(self, base, off, length):
         """Complete uncompressed DataBlobs (magic | crc32 | payload) of n ranges -> (bytes buffer, blob_off[n+1], crc[n])."""
@@ -372,17 +409,18 @@ class Engine:
     def _blob_layout(l, head: int):
         """Room for n blobs back to back, each its uncompressed payload behind a `head`-byte header (12, or 44 encrypted)
         -> (out buffer, blob_off[n+1], crc[n])."""
-        boff = np.zeros(len(l) + 1, dtype=np.uint64)
-        np.cumsum(l + np.uint64(head), out=boff[1:])
-        return np.zeros(int(boff[-1]), dtype=np.uint8), boff, np.zeros(len(l), dtype=np.uint32)
+        off, total = _offsets(l + np.uint64(head))
+        return np.zeros(total, dtype=np.uint8), np.append(off, np.uint64(total)), np.zeros(len(l), dtype=np.uint32)
 
-    def _blob_encode_sized(self, fn, base, off, length):
+    def _blob_encode_sized(self, fn, base, off, length, head: int = 12):
+        """Blobs whose sizes the encoder reports: fn(ctx, base, off, len, n, out, blob_off, blob_len, crc) -> list of n
+        `bytes` blobs, crc[n]."""
         o, l = self._offlen(off, length)
-        out, boff, crc = self._blob_layout(l, 12)
+        out, boff, crc = self._blob_layout(l, head)
         blen = np.zeros(len(o), dtype=np.uint64)
         self._ck(fn(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, len(o), out.ctypes.data, boff.ctypes.data,
                     blen.ctypes.data, crc.ctypes.data))
-        return [out[int(boff[i]): int(boff[i]) + int(blen[i])].tobytes() for i in range(len(o))], crc
+        return _split(out, boff, blen), crc
 
     # -- f3, read side -------------------------------------------------------------------------
     def blob_decode_batch(self, blobs, chunk_len, digests=None, out: str | None = "host"):
@@ -404,46 +442,24 @@ class Engine:
     def _blob_decode(self, call, blobs, chunk_len, digests, out):
         if out not in ("host", "device", None):
             raise ValueError(f"out must be 'host', 'device' or None, not {out!r}")
-        keep = None
         if isinstance(blobs, tuple):
             base, o, l = blobs
             o, l = self._offlen(o, l)
         else:
-            sizes = np.array([len(b) for b in blobs], dtype=np.uint64)
-            o = np.zeros(len(blobs), dtype=np.uint64)
-            if len(blobs):
-                o[1:] = np.cumsum(sizes)[:-1]
-            base = np.frombuffer(b"".join(bytes(b) for b in blobs) or b"\0", dtype=np.uint8)
-            l = sizes
+            base, o, l = _join(blobs)
         n = len(o)
         cl = np.ascontiguousarray(chunk_len, dtype=np.uint64)
         if cl.shape != (n,):
             raise ValueError("chunk_len must hold one size per blob")
-        dg = None
-        if digests is not None:
-            dg = np.ascontiguousarray(np.frombuffer(bytes(digests), dtype=np.uint8) if isinstance(digests, (bytes, bytearray))
-                                      else np.asarray(digests, dtype=np.uint8)).reshape(-1)
-            if dg.size != 32 * n:
-                raise ValueError("digests must hold 32 bytes per blob")
-        ooff = np.zeros(n, dtype=np.uint64)
-        if n:
-            ooff[1:] = np.cumsum(cl)[:-1]
-        total = max(1, int(cl.sum()))
-        if out == "host":
-            keep = np.zeros(total, dtype=np.uint8)
-        elif out == "device":
-            import torch
-            keep = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self.device}")
+        dg = None if digests is None else _digests(digests, "per blob", n)
+        ooff, total = _offsets(cl)
+        buf = self._alloc(total, out)
         status = np.zeros(n, dtype=np.int32)
         dout = np.zeros((n, 32), dtype=np.uint8)
         self._ck(call(_ptr(base), o.ctypes.data, l.ctypes.data, n, cl.ctypes.data, dg.ctypes.data if dg is not None else None,
-                      _ptr(keep) if keep is not None else None, ooff.ctypes.data, status.ctypes.data, dout.ctypes.data))
-        data = None
-        if keep is not None:
-            good = (status == _lib.DEC_OK) | (status == _lib.DEC_BAD_DIGEST)
-            data = [(keep[int(ooff[i]): int(ooff[i]) + int(cl[i])].tobytes() if out == "host"
-                     else keep[int(ooff[i]): int(ooff[i]) + int(cl[i])]) if good[i] else None for i in range(n)]
-        return status, data, dout
+                      _ptr(buf) if buf is not None else None, ooff.ctypes.data, status.ctypes.data, dout.ctypes.data))
+        good = (status == _lib.DEC_OK) | (status == _lib.DEC_BAD_DIGEST)
+        return status, None if buf is None else _split(buf, ooff, cl, good), dout
 
     # -- f3, read side: archives ---------------------------------------------------------------
     def reader(self, didx: bytes, crypt: "Crypt | None" = None, cache_bytes: int = 0) -> "Reader":
@@ -467,18 +483,15 @@ class Engine:
         frame ("z", "lz", "lze", "lzh", "lzl") where smaller, else the raw chunk ("raw": always).  `iv` holds n x 16 bytes, one
         IV per blob; an IV must never be used twice under one key (draw them with os.urandom).
         -> list of n `bytes` blobs, crc[n]."""
-        o, l = self._offlen(off, length)
-        ivs = np.frombuffer(bytes(iv), dtype=np.uint8)
-        if len(ivs) != 16 * len(o):
-            raise ValueError("iv must hold 16 bytes per range")
-        if mode not in BLOB_MODES or mode is None:
-            raise ValueError(f"unknown blob mode {mode!r}")
-        out, boff, crc = self._blob_layout(l, 44)
-        blen = np.zeros(len(o), dtype=np.uint64)
-        self._ck(self._L.pbsgpu_blob_encode_batch_enc(self._h, crypt._h, BLOB_MODES[mode], _ptr(base), o.ctypes.data,
-                                                      l.ctypes.data, len(o), ivs.ctypes.data, out.ctypes.data,
-                                                      boff.ctypes.data, blen.ctypes.data, crc.ctypes.data))
-        return [out[int(boff[i]): int(boff[i]) + int(blen[i])].tobytes() for i in range(len(o))], crc
+        def enc(h, base, o, l, n, *outputs):
+            ivs = np.frombuffer(bytes(iv), dtype=np.uint8)
+            if len(ivs) != 16 * n:
+                raise ValueError("iv must hold 16 bytes per range")
+            if mode not in BLOB_MODES or mode is None:
+                raise ValueError(f"unknown blob mode {mode!r}")
+            return self._L.pbsgpu_blob_encode_batch_enc(h, crypt._h, BLOB_MODES[mode], base, o, l, n, ivs.ctypes.data,
+                                                        *outputs)
+        return self._blob_encode_sized(enc, base, off, length, 44)
 
     def blob_header(self, crc: int) -> bytes:
         out = np.zeros(12, dtype=np.uint8)
@@ -511,10 +524,7 @@ class Engine:
     def fidx_build(self, digests, size: int, chunk_size: int, uuid: bytes = b"\0" * 16, ctime: int = 0) -> bytes:
         """Fixed-index (.fidx) image of an image of `size` bytes in chunks of `chunk_size`: digests (n x 32 bytes, n =
         ceil(size / chunk_size)) in image order; the checksum is computed on the GPU."""
-        d = np.ascontiguousarray(np.frombuffer(bytes(digests), dtype=np.uint8) if isinstance(digests, (bytes, bytearray))
-                                 else np.asarray(digests, dtype=np.uint8)).reshape(-1)
-        if d.size % 32:
-            raise ValueError("digests must hold 32 bytes each")
+        d = _digests(digests, "each")
         n = d.size // 32
         out = np.zeros(int(self._L.pbsgpu_fidx_size(n)), dtype=np.uint8)
         u = np.frombuffer(bytes(uuid).ljust(16, b"\0")[:16], dtype=np.uint8)
@@ -604,21 +614,15 @@ class Job:
             self._h, self._keep = None, None
 
 
-class Crypt:
-    """One AES-256 key of encrypt mode on the engine's device (pbsgpu_crypt_create / _destroy)."""
-
-    def __init__(self, eng: Engine, key: bytes):
-        k = np.frombuffer(bytes(key), dtype=np.uint8)
-        if len(k) != 32:
-            raise ValueError("the key must be 32 bytes")
-        self._eng = eng
-        h = C.c_void_p()
-        eng._ck(eng._L.pbsgpu_crypt_create(eng._h, k.ctypes.data, C.byref(h)))
-        self._h = h
+class _Handle:
+    """A library object that lives inside an Engine's context: close() calls the C function `_destroy` names once, and
+    only while the engine is still open (closing the engine frees everything in its context)."""
+    _destroy = ""
+    _h = None
 
     def close(self):
-        if getattr(self, "_h", None) and self._eng._h:
-            self._eng._L.pbsgpu_crypt_destroy(self._h)
+        if self._h and self._eng._h:
+            getattr(self._eng._L, self._destroy)(self._h)
         self._h = None
 
     def __del__(self):
@@ -634,6 +638,20 @@ class Crypt:
         self.close()
 
 
+class Crypt(_Handle):
+    """One AES-256 key of encrypt mode on the engine's device (pbsgpu_crypt_create / _destroy)."""
+    _destroy = "pbsgpu_crypt_destroy"
+
+    def __init__(self, eng: Engine, key: bytes):
+        k = np.frombuffer(bytes(key), dtype=np.uint8)
+        if len(k) != 32:
+            raise ValueError("the key must be 32 bytes")
+        self._eng = eng
+        h = C.c_void_p()
+        eng._ck(eng._L.pbsgpu_crypt_create(eng._h, k.ctypes.data, C.byref(h)))
+        self._h = h
+
+
 def _blob_args(blobs):
     """Reader.read's `blobs` -> (base, blob_off u64[k], blob_len u64[k], blob_chunk u64[k])."""
     if isinstance(blobs, tuple):
@@ -644,18 +662,14 @@ def _blob_args(blobs):
             raise ValueError("blob chunks must hold one index per blob")
         return base, bo, bl, bc
     items = list(blobs.items())
-    bc = np.array([c for c, _ in items], dtype=np.uint64)
-    bl = np.array([len(b) for _, b in items], dtype=np.uint64)
-    bo = np.zeros(len(items), dtype=np.uint64)
-    if len(items):
-        bo[1:] = np.cumsum(bl)[:-1]
-    base = np.frombuffer(b"".join(bytes(b) for _, b in items) or b"\0", dtype=np.uint8)
-    return base, bo, bl, bc
+    base, bo, bl = _join([b for _, b in items])
+    return base, bo, bl, np.array([c for c, _ in items], dtype=np.uint64)
 
 
-class Reader:
+class Reader(_Handle):
     """An archive reader on the engine's device (pbsgpu_reader_*): plan() names the chunks a read needs that the cache
     lacks, read() verifies the blobs it is given into the cache and copies the ranges out of it."""
+    _destroy = "pbsgpu_reader_close"
 
     def __init__(self, eng: Engine, index: bytes, crypt: "Crypt | None", cache_bytes: int, fixed: bool = False):
         a = np.frombuffer(bytes(index), dtype=np.uint8)
@@ -697,25 +711,14 @@ class Reader:
         o, l = Engine._offlen(off, length)
         base, bo, bl, bc = _blob_args(blobs)
         n, k = len(o), len(bo)
-        ooff = np.zeros(n, dtype=np.uint64)
-        if n:
-            ooff[1:] = np.cumsum(l)[:-1]
-        total = max(1, int(l.sum()))
-        if out == "host":
-            buf = np.zeros(total, dtype=np.uint8)
-        else:
-            import torch
-            buf = torch.empty(total, dtype=torch.uint8, device=f"cuda:{self._eng.device}")
+        ooff, total = _offsets(l)
+        buf = self._eng._alloc(total, out)
         status = np.zeros(n, dtype=np.int32)
         bst = np.zeros(k, dtype=np.int32)
         self._eng._ck(self._eng._L.pbsgpu_reader_read(
             self._h, o.ctypes.data, l.ctypes.data, n, _lib.READ_PAYLOAD if payload else 0, _ptr(base), bo.ctypes.data,
             bl.ctypes.data, bc.ctypes.data, k, _ptr(buf), ooff.ctypes.data, status.ctypes.data, bst.ctypes.data))
-        data = []
-        for i in range(n):
-            a, e = int(ooff[i]), int(ooff[i]) + int(l[i])
-            data.append(None if status[i] != _lib.DEC_OK else buf[a:e].tobytes() if out == "host" else buf[a:e])
-        return status, data, bst
+        return status, _split(buf, ooff, l, status == _lib.DEC_OK), bst
 
     def read_deflate(self, off, length, blobs, payload: bool = False, more=None):
         """read() whose outputs are the ranges' raw Deflate streams (pbsgpu_reader_read_deflate): the ranges are
@@ -725,14 +728,8 @@ class Reader:
         o, l = Engine._offlen(off, length)
         base, bo, bl, bc = _blob_args(blobs)
         n, k = len(o), len(bo)
-        bound = np.array([deflate_bound(int(x)) for x in l], dtype=np.uint64)
-        ooff = np.zeros(n, dtype=np.uint64)
-        if n:
-            ooff[1:] = np.cumsum(bound)[:-1]
-        buf = np.zeros(max(1, int(bound.sum())), dtype=np.uint8)
-        m = None if more is None else np.ascontiguousarray(more, dtype=np.uint8)
-        if m is not None and m.shape != o.shape:
-            raise ValueError("more must hold one flag per range")
+        ooff, total, m = _deflate_layout(l, more)
+        buf = self._eng._alloc(total, "host")
         olen = np.zeros(n, dtype=np.uint64)
         crc = np.zeros(n, dtype=np.uint32)
         status = np.zeros(n, dtype=np.int32)
@@ -741,47 +738,18 @@ class Reader:
             self._h, o.ctypes.data, l.ctypes.data, n, _lib.READ_PAYLOAD if payload else 0,
             None if m is None else m.ctypes.data, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
             buf.ctypes.data, ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data, status.ctypes.data, bst.ctypes.data))
-        streams = [None if status[i] != _lib.DEC_OK else buf[int(ooff[i]):int(ooff[i]) + int(olen[i])].tobytes()
-                   for i in range(n)]
-        return status, streams, crc, bst
-
-    def close(self):
-        if getattr(self, "_h", None) and self._eng._h:
-            self._eng._L.pbsgpu_reader_close(self._h)
-        self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
+        return status, _split(buf, ooff, olen, status == _lib.DEC_OK), crc, bst
 
 
-class DigestSet:
+class DigestSet(_Handle):
     """Known-digest set on the device (reference: dedup seed, commit.go:286-294, :324-329)."""
+    _destroy = "pbsgpu_set_destroy"
 
     def __init__(self, eng: Engine, capacity_hint: int):
         self._eng = eng
         h = C.c_void_p()
         eng._ck(eng._L.pbsgpu_set_create(eng._h, capacity_hint, C.byref(h)))
         self._h = h
-
-    def close(self):
-        if getattr(self, "_h", None) and self._eng._h:
-            self._eng._L.pbsgpu_set_destroy(self._h)
-        self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def __len__(self):
         c = C.c_uint64()
@@ -804,24 +772,20 @@ class DigestSet:
     def allgather(self, comm: "NcclComm", digests) -> np.ndarray:
         """The ONE multi-GPU exchange step (pbsgpu_set_allgather): every rank contributes its digests, every replica
         inserts all of them in global (rank, index) order; returns this rank's flags."""
-        d = np.ascontiguousarray(digests, dtype=np.uint8).reshape(-1, 32)
-        hit = np.zeros(len(d), dtype=np.uint8)
-        self._eng._ck(self._eng._L.pbsgpu_set_allgather(self._h, comm._h, d.ctypes.data if len(d) else None, len(d),
-                                                         hit.ctypes.data if len(d) else None))
-        return hit
+        return self._run(lambda h, *a: self._eng._L.pbsgpu_set_allgather(h, comm._h, *a), digests)
+
+    def _seed(self, fn, image) -> int:
+        a = np.frombuffer(bytes(image), dtype=np.uint8)
+        n = C.c_uint64()
+        self._eng._ck(fn(self._h, a.ctypes.data, len(a), C.byref(n)))
+        return int(n.value)
 
     def seed_didx(self, image: bytes) -> int:
-        a = np.frombuffer(image, dtype=np.uint8)
-        n = C.c_uint64()
-        self._eng._ck(self._eng._L.pbsgpu_set_seed_didx(self._h, a.ctypes.data, len(a), C.byref(n)))
-        return int(n.value)
+        return self._seed(self._eng._L.pbsgpu_set_seed_didx, image)
 
     def seed_fidx(self, image: bytes) -> int:
         """Seed from the previous snapshot's .fidx of the same image (pbsgpu_set_seed_fidx); returns its chunk count."""
-        a = np.frombuffer(bytes(image), dtype=np.uint8)
-        n = C.c_uint64()
-        self._eng._ck(self._eng._L.pbsgpu_set_seed_fidx(self._h, a.ctypes.data, len(a), C.byref(n)))
-        return int(n.value)
+        return self._seed(self._eng._L.pbsgpu_set_seed_fidx, image)
 
 
 class NcclComm:
@@ -851,8 +815,9 @@ class NcclComm:
             self._h = None
 
 
-class Stream:
+class Stream(_Handle):
     """Streaming form: one io.Reader-like byte stream, state carried across writes."""
+    _destroy = "pbsgpu_stream_close"
 
     def __init__(self, eng: Engine, cfg: Cfg, digest_set: DigestSet | None):
         self._eng = eng
@@ -934,33 +899,23 @@ class Stream:
         """Every XXH3-64 of the registered ranges available now, in registration order (`cap` per C call)."""
         out = np.zeros(cap, dtype=np.uint64)
         n = C.c_uint64()
-        parts = []
-        while True:
+
+        def poll():
             self._eng._ck(self._eng._L.pbsgpu_stream_poll_hashes(self._h, out.ctypes.data, cap, C.byref(n)))
-            if n.value == 0:
-                return np.concatenate(parts) if parts else np.zeros(0, dtype=np.uint64)
-            parts.append(out[: n.value].copy())
+            return out[: n.value].copy()
+        return self._drain(poll, np.uint64)
 
     def finish(self) -> np.ndarray:
         self._eng._ck(self._eng._L.pbsgpu_stream_finish(self._h))
+        return self._drain(self.poll, CHUNK_DTYPE)
+
+    @staticmethod
+    def _drain(poll, dtype) -> np.ndarray:
+        """Everything `poll` returns until it returns nothing, concatenated."""
         parts = []
-        while True:
-            p = self.poll()
-            if len(p) == 0:
-                break
+        while len(p := poll()):
             parts.append(p)
-        return np.concatenate(parts) if parts else np.zeros(0, dtype=CHUNK_DTYPE)
-
-    def close(self):
-        if getattr(self, "_h", None) and self._eng._h:
-            self._eng._L.pbsgpu_stream_close(self._h)
-        self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        return np.concatenate(parts) if parts else np.zeros(0, dtype=dtype)
 
 
 def corpus(seed: int, file_len: int, block_len: int = 4 << 20, run_blocks: int = 8, dup_permille: int = 0,

@@ -113,7 +113,7 @@ class DedupWriter:
         if not self._pending:
             return
         entries, arrs = zip(*self._pending)
-        buf, offs, lens = self._pack(arrs)
+        buf, offs, lens = _engine._pack(arrs)
         keyed = {"crypt": self._crypt} if self._crypt is not None else {}
         rec, hashes = self.engine.chunk_digest_batch_xxh3(self.config, buf, offs, lens, self.known, **keyed)
         for e, h in zip(entries, hashes):
@@ -134,28 +134,10 @@ class DedupWriter:
         if self.upload_blob is not None and new_chunks:
             boff = np.array([int(offs[i]) + s0 for _, i, s0, _ in new_chunks], dtype=np.uint64)
             blen = np.array([e0 - s0 for _, _, s0, e0 in new_chunks], dtype=np.uint64)
-            if self._crypt is not None:
-                blobs, _crc = self.engine.blob_encode_batch_enc(self._crypt, self.blob_compression, buf, boff, blen,
-                                                                os.urandom(16 * len(boff)))
-            else:
-                encode = getattr(self.engine, "blob_encode_batch_" + self.blob_compression)
-                blobs, _crc = encode(buf, boff, blen)
+            blobs = _encode_new(self.engine, self._crypt, self.blob_compression, buf, boff, blen)
             for (d, _i, _s, _e), blob in zip(new_chunks, blobs):
                 self.upload_blob(d, blob)
         self._pending, self._pending_bytes = [], 0
-
-    @staticmethod
-    def _pack(arrs):
-        lens = np.array([len(a) for a in arrs], dtype=np.uint64)
-        offs = np.zeros(len(arrs), dtype=np.uint64)
-        pos = 0
-        for i, a in enumerate(arrs):
-            offs[i] = pos
-            pos += (len(a) + 255) & ~255
-        buf = np.zeros(max(pos, 1), dtype=np.uint8)
-        for a, o in zip(arrs, offs):
-            buf[int(o): int(o) + len(a)] = a
-        return buf, offs, lens
 
     def Finish(self) -> list[IndexRecord]:
         self.Flush()
@@ -164,8 +146,19 @@ class DedupWriter:
 
 
 def _check_blob_compression(c: str) -> None:
-    if c not in ("z", "lz", "lze", "lzh", "lzl"):
-        raise ValueError(f"transfer: blob_compression must be 'z', 'lz', 'lze', 'lzh' or 'lzl', not {c!r}")
+    names = [m for m in _lib.BLOB_MODES if m not in (None, "raw")]
+    if c not in names:
+        raise ValueError(f"transfer: blob_compression must be {', '.join(map(repr, names[:-1]))} or {names[-1]!r}, "
+                         f"not {c!r}")
+
+
+def _encode_new(engine: Engine, crypt, mode: str, base, off, length) -> list[bytes]:
+    """The DataBlobs of new chunks: encrypted with `crypt` under fresh random IVs, else plain by `mode`'s encoder."""
+    if crypt is not None:
+        blobs, _crc = engine.blob_encode_batch_enc(crypt, mode, base, off, length, os.urandom(16 * len(off)))
+    else:
+        blobs, _crc = getattr(engine, "blob_encode_batch_" + mode)(base, off, length)
+    return blobs
 
 
 # pxar v2 format constants (upstream pxar crate format/mod.rs; restated, UNVERIFIED against the Go module)
@@ -385,12 +378,7 @@ class FixedIndexWriter:
         if self.upload_blob is not None and new:
             boff = np.array(new, dtype=np.uint64) * np.uint64(cs)
             blen = np.minimum(np.uint64(n) - boff, np.uint64(cs))
-            if self._crypt is not None:
-                blobs, _crc = self.engine.blob_encode_batch_enc(self._crypt, self.blob_compression, data, boff, blen,
-                                                                os.urandom(16 * len(boff)))
-            else:
-                blobs, _crc = getattr(self.engine, "blob_encode_batch_" + self.blob_compression)(data, boff, blen)
-            for k, blob in zip(new, blobs):
+            for k, blob in zip(new, _encode_new(self.engine, self._crypt, self.blob_compression, data, boff, blen)):
                 self.upload_blob(bytes(rec[k]["digest"]), blob)
         self.size += n
         self._ended = n % cs != 0
@@ -433,28 +421,29 @@ class PayloadReader:
     def Size(self) -> int:
         return self._reader.size
 
-    def _read(self, off: list[int], size: list[int], payload: bool) -> list[bytes]:
-        """One plan, one fetch of the missing blobs by digest, one read."""
+    def _fetch(self, off: list[int], size: list[int], payload: bool) -> dict[int, bytes]:
+        """One plan, one fetch of the missing blobs by digest."""
         chunks, digests = self._reader.plan(off, size, payload)
-        blobs = {int(c): self._source(bytes(d)) for c, d in zip(chunks, digests)}
-        status, data, _ = self._reader.read(off, size, blobs, payload)
+        return {int(c): self._source(bytes(d)) for c, d in zip(chunks, digests)}
+
+    @staticmethod
+    def _check(status, off: list[int], size: list[int], payload: bool) -> None:
         bad = np.flatnonzero(status != _lib.DEC_OK)
         if len(bad):
             i = int(bad[0])
             what = "file at payload offset" if payload else "range at"
             raise IOError(f"transfer: {what} {off[i]} ({size[i]} bytes): {_DEC_NAMES.get(int(status[i]), int(status[i]))}")
+
+    def _read(self, off: list[int], size: list[int], payload: bool) -> list[bytes]:
+        """One plan, one fetch, one read."""
+        status, data, _ = self._reader.read(off, size, self._fetch(off, size, payload), payload)
+        self._check(status, off, size, payload)
         return data
 
     def _read_deflate(self, off: list[int], size: list[int], payload: bool, more=None):
         """_read whose outputs are raw Deflate streams -> (streams, crc32s)."""
-        chunks, digests = self._reader.plan(off, size, payload)
-        blobs = {int(c): self._source(bytes(d)) for c, d in zip(chunks, digests)}
-        status, streams, crc, _ = self._reader.read_deflate(off, size, blobs, payload, more)
-        bad = np.flatnonzero(status != _lib.DEC_OK)
-        if len(bad):
-            i = int(bad[0])
-            what = "file at payload offset" if payload else "range at"
-            raise IOError(f"transfer: {what} {off[i]} ({size[i]} bytes): {_DEC_NAMES.get(int(status[i]), int(status[i]))}")
+        status, streams, crc, _ = self._reader.read_deflate(off, size, self._fetch(off, size, payload), payload, more)
+        self._check(status, off, size, payload)
         return streams, [int(c) for c in crc]
 
     def ReadAt(self, off: int, size: int) -> bytes:
@@ -587,16 +576,7 @@ def verifyBackedFileHashes(engine: Engine, open_file: Callable[[str], BinaryIO],
         nonlocal names, arrs, held
         if not names:
             return
-        lens = np.array([len(a) for a in arrs], dtype=np.uint64)
-        offs = np.zeros(len(arrs), dtype=np.uint64)
-        pos = 0
-        for i, a in enumerate(arrs):
-            offs[i] = pos
-            pos += (len(a) + 255) & ~255
-        buf = np.zeros(max(pos, 1), dtype=np.uint8)
-        for a, o in zip(arrs, offs):
-            buf[int(o): int(o) + len(a)] = a
-        got = engine.xxh3_batch(buf, offs, lens)
+        got = engine.xxh3_batch(*_engine._pack(arrs))
         for name, h in zip(names, got):
             if int(h) != hashes[name]:
                 raise IOError(f'backed file "{name}" content hash differs')
