@@ -380,7 +380,7 @@ func (st *Stream) Finish() ([]Chunk, error) {
 func (st *Stream) Close() { C.pbsgpu_stream_close(st.s) }
 
 // Blob modes of SetBlobMode: the encoders of Batch.BlobEncode, BlobEncodeZ, BlobEncodeLZ, BlobEncodeLZE,
-// BlobEncodeLZH and BlobEncodeLZL (its value is 7; 6 is not assigned).
+// BlobEncodeLZH, BlobEncodeLZL (its value is 7) and BlobEncodeLZC (10; 6, 8 and 9 are not assigned).
 const (
 	BlobNone = C.PBSGPU_BLOB_NONE
 	BlobRaw  = C.PBSGPU_BLOB_RAW
@@ -389,6 +389,7 @@ const (
 	BlobLZE  = C.PBSGPU_BLOB_LZE
 	BlobLZH  = C.PBSGPU_BLOB_LZH
 	BlobLZL  = C.PBSGPU_BLOB_LZL
+	BlobLZC  = C.PBSGPU_BLOB_LZC
 )
 
 // SetBlobMode makes the stream encode a DataBlob for every new chunk on the GPU (before the first byte).
@@ -705,6 +706,14 @@ func (b *Batch) BlobEncodeLZL(off, length []uint64) ([][]byte, error) {
 	return b.blobEncodeCompressed(off, length, blobLZL)
 }
 
+// BlobEncodeLZC is BlobEncodeLZH with a stronger match search: the longest of the 16 latest earlier positions of the
+// chunk with the same 4 bytes, up to 2^24 - 4 bytes back, and a lazy parse.  Text-like chunks get smaller blobs for more
+// GPU time; ranges must be shorter than 2^32 bytes.  Like the rest of this shim, it has not been compiled against a Go
+// toolchain.
+func (b *Batch) BlobEncodeLZC(off, length []uint64) ([][]byte, error) {
+	return b.blobEncodeCompressed(off, length, blobLZC)
+}
+
 // which compressed DataBlob encoder blobEncodeCompressed calls
 type blobMode int
 
@@ -714,6 +723,7 @@ const (
 	blobLZE
 	blobLZH
 	blobLZL
+	blobLZC
 )
 
 func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]byte, error) {
@@ -734,6 +744,8 @@ func (b *Batch) blobEncodeCompressed(off, length []uint64, mode blobMode) ([][]b
 	dst := (*C.uint8_t)(unsafe.Pointer(&out[0]))
 	var rc C.int
 	switch mode {
+	case blobLZC:
+		rc = C.pbsgpu_blob_encode_batch_lzc(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	case blobLZL:
 		rc = C.pbsgpu_blob_encode_batch_lzl(b.e.ctx, b.buf, &o[0], &l[0], C.uint32_t(n), dst, &oo[0], &ol[0], nil)
 	case blobLZH:
@@ -845,7 +857,7 @@ func (c *Crypt) Close() { C.pbsgpu_crypt_destroy(c.c) }
 // library draws from the OS CSPRNG.
 func (st *Stream) SetCrypt(c *Crypt) error { return st.e.err(C.pbsgpu_stream_crypt(st.s, c.c, nil)) }
 
-// BlobEncodeEnc returns encrypted DataBlobs of the ranges: mode (BlobRaw .. BlobLZH, BlobLZL) picks the compressor whose frame
+// BlobEncodeEnc returns encrypted DataBlobs of the ranges: mode (BlobRaw .. BlobLZH, BlobLZL, BlobLZC) picks the compressor whose frame
 // is encrypted when smaller.  Every blob gets a fresh IV from crypto/rand; an IV must never repeat under one key.
 func (b *Batch) BlobEncodeEnc(c *Crypt, mode int, off, length []uint64) ([][]byte, error) {
 	n := len(off)
@@ -1095,7 +1107,7 @@ type ImageWriter struct {
 	e         *Engine
 	known     *KnownSet
 	crypt     *Crypt
-	mode      int // BlobRaw .. BlobLZH, BlobLZL; 0 = no blobs
+	mode      int // BlobRaw .. BlobLZH, BlobLZL, BlobLZC; 0 = no blobs
 	chunkSize uint64
 	buf       unsafe.Pointer
 	cap       uint64
@@ -1196,6 +1208,8 @@ func (w *ImageWriter) slice(n uint64) error {
 			blobs, err = b.BlobEncodeLZE(newOff, newLen)
 		case w.mode == int(BlobLZH):
 			blobs, err = b.BlobEncodeLZH(newOff, newLen)
+		case w.mode == int(BlobLZC):
+			blobs, err = b.BlobEncodeLZC(newOff, newLen)
 		default:
 			blobs, err = b.BlobEncodeLZL(newOff, newLen)
 		}

@@ -230,12 +230,12 @@ int pbsgpu_stream_suggest(pbsgpu_stream *s, uint64_t offset);
 uint64_t pbsgpu_stream_position(const pbsgpu_stream *s);
 /* DataBlobs of the stream's NEW chunks, encoded on the device from the window that holds them.  The mode is set before
  * the first byte (PBSGPU_ESTATE after that) and has the meaning of pbsgpu_blob_encode_batch (RAW), _z, _lz, _lze, _lzh
- * and _lzl (LZL = 7; the value 6 is not assigned and is rejected); NONE, the default, encodes nothing.  Blob k belongs to the k-th record without PBSGPU_CHUNK_KNOWN in poll() order, so
+ * and _lzl (LZL = 7), and _lzc (LZC = 10; the values 6, 8 and 9 are not assigned and are rejected); NONE, the default, encodes nothing.  Blob k belongs to the k-th record without PBSGPU_CHUNK_KNOWN in poll() order, so
  * with a digest set every new digest gets exactly one blob.  A window's blobs become available when its records do, all
  * of them after finish().  poll_blobs copies whole blobs back to back into out[0, out_cap) and their lengths into
  * blob_len[0, cap); out_cap must be at least pbsgpu_blob_size(cfg.max), so every call makes progress. */
 enum { PBSGPU_BLOB_NONE = 0, PBSGPU_BLOB_RAW = 1, PBSGPU_BLOB_Z = 2, PBSGPU_BLOB_LZ = 3, PBSGPU_BLOB_LZE = 4,
-       PBSGPU_BLOB_LZH = 5, PBSGPU_BLOB_LZL = 7 };
+       PBSGPU_BLOB_LZH = 5, PBSGPU_BLOB_LZL = 7, PBSGPU_BLOB_LZC = 10 };
 int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode);
 int pbsgpu_stream_poll_blobs(pbsgpu_stream *s, uint8_t *out, uint64_t out_cap, uint64_t *blob_len, uint64_t cap,
                              uint64_t *n_out);
@@ -375,6 +375,14 @@ int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, const uint64
  * blob.  Same arguments, limits and errors as _lzh.  The output is a deterministic function of the chunk bytes. */
 int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                  uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+/* pbsgpu_blob_encode_batch_lzh with a stronger match search: the match at a position is the longest among the 16
+ * latest earlier positions of the same chunk with the same 4 bytes, up to 2^24 - 4 bytes back (so sources may lie in
+ * any earlier block), and the parse is lazy (it may move on up to 2 bytes to a longer match).  The frame, the entropy
+ * stage and the block forms are _lzh's; no block refers to another's state.  Blobs of text-like data come out smaller
+ * than libzstd level 3's (DESIGN.md K16 has the measurements); the search costs more device time than _lzh's.  Same
+ * arguments and errors as _lzh; ranges < 2^32 bytes.  The output is a deterministic function of the chunk bytes. */
+int pbsgpu_blob_encode_batch_lzc(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                 uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 
 /* ---- f3, read side: decode and verify unencrypted DataBlobs (restore, mount, verify jobs) ------------------------
  * Blob i is [base + off[i], + len[i]) (HOST or DEVICE); its chunk has chunk_len[i] bytes (the difference of consecutive
@@ -417,7 +425,7 @@ int pbsgpu_blob_decode_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *
  * IVs: iv holds n x 16 bytes, one per blob, supplied by the caller, so the output is a pure function of the inputs.
  * GCM's security rests on never using one IV twice under one key: draw every IV from a CSPRNG (upstream draws them at
  * random) and never reuse one.  The library never generates or stores IVs.
- * mode: PBSGPU_BLOB_RAW (encrypt every chunk uncompressed) or PBSGPU_BLOB_Z .. PBSGPU_BLOB_LZH, PBSGPU_BLOB_LZL (the
+ * mode: PBSGPU_BLOB_RAW (encrypt every chunk uncompressed) or PBSGPU_BLOB_Z .. PBSGPU_BLOB_LZH, _LZL, _LZC (the
  * compressor whose frame is used when smaller).  Blob i goes to out + out_off[i] (HOST memory), which must hold pbsgpu_blob_size_enc(len[i])
  * bytes; out_len[i] receives its size.  base is HOST or DEVICE; ranges < 2^36 bytes.  crc_out may be NULL. */
 /* create also derives the id_key of keyed digests: PBKDF2-HMAC-SHA256(password = key, salt = "_id_key", 10 iterations,

@@ -168,7 +168,7 @@ class DedupWriter {
 // Start marker, then per file a 16-byte PAYLOAD header + content (reference internal/pxarmount/pxarfs.go:408-411),
 // chunker state carried across files, a suggested boundary at every file start, bytes read straight into the
 // library's pinned ring.  WriteEntryReader (commit.go:720) returns the entry's payload offset.
-// Optional: `blob_mode` (PBSGPU_BLOB_RAW .. _LZH, _LZL) hands the DataBlob of every new chunk to `upload_blob(digest, blob,
+// Optional: `blob_mode` (PBSGPU_BLOB_RAW .. _LZH, _LZL, _LZC) hands the DataBlob of every new chunk to `upload_blob(digest, blob,
 // len)`, encoded on the GPU from the stream's windows; `hash_files` records every file's XXH3-64 in BackedHashes()
 // (commitWalkState.backedHashes, commit.go:725); `crypt` gives keyed digests and encrypted blobs, their IVs drawn from the
 // OS CSPRNG by the stream.
@@ -288,7 +288,7 @@ class PayloadStreamWriter {
 // The image is cut at every multiple of `chunk_size` (upstream writes 4 MiB).  WriteSlice takes the next bytes of the
 // image (HOST or DEVICE memory); every slice but the last is a multiple of chunk_size.  Each chunk is digested on the
 // GPU (keyed with `crypt`) and probed against `known` (seed it with KnownSet::SeedFromFidx); with a blob mode
-// (PBSGPU_BLOB_RAW .. _LZH, _LZL), every new chunk's DataBlob goes to `upload_blob` (encrypted with `crypt`, IVs from
+// (PBSGPU_BLOB_RAW .. _LZH, _LZL, _LZC), every new chunk's DataBlob goes to `upload_blob` (encrypted with `crypt`, IVs from
 // getrandom).  Finish() renders the .fidx.
 class FixedIndexWriter {
   public:
@@ -353,7 +353,8 @@ class FixedIndexWriter {
         } else {
             auto fn = mode_ == PBSGPU_BLOB_Z ? pbsgpu_blob_encode_batch_z : mode_ == PBSGPU_BLOB_LZ ? pbsgpu_blob_encode_batch_lz
                     : mode_ == PBSGPU_BLOB_LZE ? pbsgpu_blob_encode_batch_lze : mode_ == PBSGPU_BLOB_LZH ? pbsgpu_blob_encode_batch_lzh
-                    : mode_ == PBSGPU_BLOB_LZL ? pbsgpu_blob_encode_batch_lzl : nullptr;
+                    : mode_ == PBSGPU_BLOB_LZL ? pbsgpu_blob_encode_batch_lzl : mode_ == PBSGPU_BLOB_LZC ? pbsgpu_blob_encode_batch_lzc
+                    : nullptr;
             if (!fn) throw Error(PBSGPU_EINVAL, "transfer: unknown blob mode " + std::to_string(mode_));
             e_.check(fn(e_.ctx(), data, off.data(), len.data(), n, buf.data(), out_off.data(), out_len.data(), nullptr));
         }

@@ -37,7 +37,7 @@ CHUNK_DTYPE = np.dtype([("stream", "<u4"), ("flags", "<u4"), ("end_off", "<u8"),
 assert CHUNK_DTYPE.itemsize == C.sizeof(Chunk) == 48
 CHUNK_KNOWN = 1
 # pbsgpu_stream_blob_mode: the DataBlob encoder of a stream's new chunks (None = no blobs)
-BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5, "lzl": 7}   # 6 is not assigned
+BLOB_MODES = {None: 0, "raw": 1, "z": 2, "lz": 3, "lze": 4, "lzh": 5, "lzl": 7, "lzc": 10}   # 6, 8, 9 are not assigned
 # pbsgpu_blob_decode_batch: per-blob status (PBSGPU_DEC_*)
 DEC_OK, DEC_BAD_MAGIC, DEC_BAD_CRC, DEC_ENCRYPTED, DEC_BAD_FRAME, DEC_BAD_SIZE, DEC_BAD_CHECKSUM, DEC_BAD_DIGEST = range(8)
 DEC_BAD_TAG = 8   # pbsgpu_blob_decode_batch_enc only: the AES-256-GCM tag did not verify
@@ -164,6 +164,7 @@ _SIGNATURES = {
     "pbsgpu_blob_encode_batch_lze": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
     "pbsgpu_blob_encode_batch_lzh": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
     "pbsgpu_blob_encode_batch_lzl": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
+    "pbsgpu_blob_encode_batch_lzc": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
     "pbsgpu_crypt_create": [_vp, _vp, C.POINTER(_vp)],
     "pbsgpu_crypt_destroy": ([_vp], None),
     "pbsgpu_blob_size_enc": ([C.c_uint64], C.c_uint64),

@@ -28,14 +28,15 @@ extern "C" uint64_t pbsgpu_blob_size(uint64_t payload_len) { return payload_len 
 extern "C" uint64_t pbsgpu_blob_size_enc(uint64_t payload_len) { return payload_len + 44; }
 
 // Which DataBlob encoder a call is: uncompressed only, RLE / raw frames (_z), with the match stage (_lz), with the match
-// and entropy stages (_lze), with Huffman literals over every byte value (_lzh), and _lzh with long-distance matches
-// across the whole chunk (_lzl).
-enum class BlobMode { raw, z, lz, lze, lzh, lzl };
-// the encoders by their PBSGPU_BLOB_* value (PBSGPU_BLOB_RAW ..); value 6 is not assigned
+// and entropy stages (_lze), with Huffman literals over every byte value (_lzh), _lzh with long-distance matches
+// across the whole chunk (_lzl), and _lzh with K16's hash-chain search over the whole chunk and lazy parse (_lzc).
+enum class BlobMode { raw, z, lz, lze, lzh, lzl, lzc };
+// the encoders by their PBSGPU_BLOB_* value (PBSGPU_BLOB_RAW ..); values 6, 8 and 9 are not assigned
 static bool blob_mode_of(int mode, BlobMode *m) {
     static const BlobMode modes[] = {BlobMode::raw, BlobMode::z, BlobMode::lz, BlobMode::lze, BlobMode::lzh};
     if (mode >= PBSGPU_BLOB_RAW && mode <= PBSGPU_BLOB_LZH) { *m = modes[mode - PBSGPU_BLOB_RAW]; return true; }
     if (mode == PBSGPU_BLOB_LZL) { *m = BlobMode::lzl; return true; }
+    if (mode == PBSGPU_BLOB_LZC) { *m = BlobMode::lzc; return true; }
     return false;
 }
 
@@ -113,6 +114,37 @@ static int ldm_spans_of(Blocking &b, const uint8_t *dbase, const uint64_t *off, 
     return PBSGPU_OK;
 }
 
+// K16 (lzc): the passes of whole chunks (at most CH_PASS_BYTES, or one longer chunk) that hold blocks of the match
+// stage's list (zfirst[i]: chunk i's first; vfirst, vpos: zchain.cuh's numbering, vpos uploaded here); per pass the chain
+// search, then parse(args, scratch) enqueues K16c and the encoders.  The scratch is sized once for the largest pass.
+template <class Parse>
+static int chain_passes(Blocking &b, const uint8_t *dbase, const uint64_t *d_off, const uint64_t *d_len, uint32_t n,
+                        const std::vector<uint64_t> &vfirst, const std::vector<uint64_t> &zfirst,
+                        const std::vector<uint64_t> &vpos, const uint64_t *d_zsrc, const uint32_t *d_zsize, Parse parse) {
+    pbsgpu_ctx *ctx = b.ctx;
+    std::vector<uint32_t> pass_c0;
+    for (uint32_t i = 0; i < n; i++)
+        if (pass_c0.empty() || vfirst[i + 1] - vfirst[pass_c0.back()] > CH_PASS_BYTES) pass_c0.push_back(i);
+    pass_c0.push_back(n);
+    size_t scratch_bytes = 0;
+    for (size_t p = 0; p + 1 < pass_c0.size(); p++)
+        if (zfirst[pass_c0[p + 1]] > zfirst[pass_c0[p]])
+            scratch_bytes = std::max(scratch_bytes, chain_scratch_bytes(vfirst[pass_c0[p + 1]] - vfirst[pass_c0[p]]));
+    uint64_t *d_vfirst = b.upload(vfirst.data(), n + 1), *d_vpos = b.upload(vpos.data(), vpos.size());
+    uint8_t *scratch = b.get<uint8_t>(scratch_bytes);
+    if (!d_vfirst || !d_vpos || !scratch)
+        return fail(ctx, PBSGPU_ENOMEM, "chain search scratch of %llu bytes failed", (unsigned long long)scratch_bytes);
+    for (size_t p = 0; b.ok() && p + 1 < pass_c0.size(); p++) {
+        const uint32_t c0 = pass_c0[p], c1 = pass_c0[p + 1];
+        const ChainArgs a{dbase, d_off, d_len, d_vfirst, c0, c1, vfirst[c1] - vfirst[c0], vfirst[c0], d_zsrc, d_vpos, d_zsize,
+                          zfirst[c0], zfirst[c1]};
+        if (a.z1 == a.z0) continue;
+        b.e = launch_chain_search(a, scratch, b.st);
+        parse(a, (void *)scratch);
+    }
+    return PBSGPU_OK;
+}
+
 // Compressed form: a blob's payload is a zstd frame when that is smaller than the raw bytes (upstream
 // `DataBlob::encode` keeps the compressed form only then).  The frame is built on the device (zframe.cu, zlz.cu,
 // zent.cu): a 128 KiB block of one repeated byte is an RLE_Block (K8a decides); with lz / lze / lzh every other block
@@ -139,9 +171,11 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
     auto block_size = [&](uint32_t i, uint64_t k) { return (uint32_t)std::min<uint64_t>(ZFRAME_BLOCK, len[i] - k * ZFRAME_BLOCK); };
     // K9 (+ K10): the match stage and encoding of the blocks that are not constant, in passes of LZ_PASS_BLOCKS.  With
     // lzl, K12 first finds the long spans; the blocks that hold one are parsed again with them (K9a's span parse, K9b,
-    // K10) into slots nz + y, and each such block keeps the smaller content, K9's on ties.
-    const bool ent = mode == BlobMode::lze || mode == BlobMode::lzh || mode == BlobMode::lzl, lz = mode == BlobMode::lz || ent;
-    const bool full = mode == BlobMode::lzh || mode == BlobMode::lzl;
+    // K10) into slots nz + y, and each such block keeps the smaller content, K9's on ties.  With lzc, K16 is the parse
+    // instead of K9a, per pass of whole chunks (CH_PASS_BYTES, or one longer chunk).
+    const bool lzc = mode == BlobMode::lzc;
+    const bool ent = mode == BlobMode::lze || mode == BlobMode::lzh || mode == BlobMode::lzl || lzc, lz = mode == BlobMode::lz || ent;
+    const bool full = mode == BlobMode::lzh || mode == BlobMode::lzl || lzc;
     std::vector<uint32_t> info;
     std::vector<uint64_t> slot_of;   // the slot of block z's content
     const uint8_t *slots = nullptr;
@@ -149,12 +183,18 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
         std::vector<uint64_t> zsrc;
         std::vector<uint32_t> zsize;
         std::vector<int64_t> zof(n_blocks, -1);
-        for (uint32_t i = 0; i < n; i++)
+        std::vector<uint64_t> zfirst(n + 1), vfirst(n + 1), vpos;   // lzc: K16's numbering (zchain.cuh, ChainArgs)
+        for (uint32_t i = 0; i < n; i++) {
+            zfirst[i] = zsrc.size();
+            vfirst[i + 1] = vfirst[i] + len[i];
             for (uint64_t k = 0; k < blk_first[i + 1] - blk_first[i]; k++)
                 if (!(flags[blk_first[i] + k] & 0x100u)) {
                     zof[blk_first[i] + k] = (int64_t)zsrc.size();
                     zsrc.push_back(off[i] + k * ZFRAME_BLOCK); zsize.push_back(block_size(i, k));
+                    if (lzc) vpos.push_back(vfirst[i] + k * ZFRAME_BLOCK);
                 }
+        }
+        zfirst[n] = zsrc.size();
         const uint64_t nz = zsrc.size();
         std::vector<uint32_t> span_z, span_first;
         std::vector<uint64_t> spans;
@@ -176,6 +216,13 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
             if (!d_zsrc || !d_zsize || !d_slots || !d_seqs || !d_nseq || !d_nlit || !d_info || (ent && !d_ent) ||
                 (ny && (!d_spans || !d_span_first)))
                 return fail(ctx, PBSGPU_ENOMEM, "match stage: device allocation failed");
+            // K9b and K10 over blocks [f, f + pn), parsed into the pass scratch
+            auto encode = [&](uint64_t f, uint32_t pn) {
+                if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
+                if (b.ok() && d_ent)
+                    b.e = launch_ent_encode((const LzTables *)ctx->d_lz_tab, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
+                                            d_info, d_ent, full, b.st);
+            };
             // the blocks [0, nz), then the span blocks [nz, nz + ny), each list in passes of its own
             auto passes = [&](uint64_t lo, uint64_t hi, bool span_parse) {
                 for (uint64_t f = lo; b.ok() && f < hi; f += LZ_PASS_BLOCKS) {
@@ -183,13 +230,21 @@ static int zstd_frames(Blocking &b, const uint8_t *dbase, const uint64_t *off, c
                     b.e = span_parse ? launch_lz_parse_spans(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
                                                              d_spans, d_span_first, nz, b.st)
                                      : launch_lz_parse(dbase, d_zsrc, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit, b.st);
-                    if (b.ok()) b.e = launch_lz_encode((const LzTables *)ctx->d_lz_tab, f, pn, d_slots, d_seqs, d_nseq, d_nlit, d_info, b.st);
-                    if (b.ok() && d_ent)
-                        b.e = launch_ent_encode((const LzTables *)ctx->d_lz_tab, d_zsize, f, pn, d_slots, d_seqs, d_nseq, d_nlit,
-                                                d_info, d_ent, full, b.st);
+                    encode(f, pn);
                 }
             };
-            passes(0, nz, false);
+            if (lzc) {   // K16c and the encoders per pass, LZ_PASS_BLOCKS blocks at a time
+                auto parse = [&](const ChainArgs &a, void *scratch) {
+                    for (uint64_t f = a.z0; b.ok() && f < a.z1; f += LZ_PASS_BLOCKS) {
+                        const uint32_t pn = (uint32_t)std::min<uint64_t>(LZ_PASS_BLOCKS, a.z1 - f);
+                        b.e = launch_chain_parse(a, scratch, f, pn, d_slots, d_seqs, d_nseq, d_nlit, b.st);
+                        encode(f, pn);
+                    }
+                };
+                if (int rc = chain_passes(b, dbase, d_off, d_len, n, vfirst, zfirst, vpos, d_zsrc, d_zsize, parse)) return rc;
+            } else {
+                passes(0, nz, false);
+            }
             passes(nz, nall, true);
             info.resize(nall);
             if (b.ok()) b.e = cudaMemcpyAsync(info.data(), d_info, nall * 4, cudaMemcpyDeviceToHost, b.st);
@@ -316,6 +371,8 @@ int pbsgpu_blob_encode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, con
     const unsigned max_log2 = crypt ? 36 : 40;   // plain raw blobs have no limit
     for (uint32_t i = 0; (crypt || bm != BlobMode::raw) && i < n; i++)
         if (len[i] >= (1ull << max_log2)) return fail(ctx, PBSGPU_EINVAL, "blob %u longer than 2^%u bytes", i, max_log2);
+    for (uint32_t i = 0; bm == BlobMode::lzc && i < n; i++)   // K16 numbers a pass's positions in 32 bits
+        if (len[i] >= (1ull << 32)) return fail(ctx, PBSGPU_EINVAL, "lzc blob %u longer than 2^32 - 1 bytes", i);
     Blocking b(ctx, ctx->streams[0]);
     const uint8_t *dbase, *frames = nullptr;
     if (int rc = b.stage(base, off, len, n, &dbase)) return rc;
@@ -420,6 +477,11 @@ extern "C" int pbsgpu_blob_encode_batch_lzh(pbsgpu_ctx *ctx, const void *base, c
 extern "C" int pbsgpu_blob_encode_batch_lzl(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                                             uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
     return blob_encode_plain(ctx, PBSGPU_BLOB_LZL, base, off, len, n, out, out_off, out_len, crc_out);
+}
+
+extern "C" int pbsgpu_blob_encode_batch_lzc(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                            uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out) {
+    return blob_encode_plain(ctx, PBSGPU_BLOB_LZC, base, off, len, n, out, out_off, out_len, crc_out);
 }
 
 extern "C" int pbsgpu_blob_encode_batch_enc(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, const void *base,

@@ -468,7 +468,7 @@ extern "C" int pbsgpu_stream_suggest(pbsgpu_stream *s, uint64_t offset) {
 extern "C" int pbsgpu_stream_blob_mode(pbsgpu_stream *s, int mode) {
     if (!s) return PBSGPU_EINVAL;
     Guard g(s->ctx);
-    if ((mode < PBSGPU_BLOB_NONE || mode > PBSGPU_BLOB_LZH) && mode != PBSGPU_BLOB_LZL)
+    if ((mode < PBSGPU_BLOB_NONE || mode > PBSGPU_BLOB_LZH) && mode != PBSGPU_BLOB_LZL && mode != PBSGPU_BLOB_LZC)
         return fail(s->ctx, PBSGPU_EINVAL, "unknown blob mode %d", mode);
     if (s->started || s->finished) return fail(s->ctx, PBSGPU_ESTATE, "the blob mode is set before the first byte");
     s->blob_mode = mode;

@@ -260,7 +260,7 @@ int pbsgpu_xxh3_enqueue(pbsgpu_ctx *ctx, const uint8_t *dbase, const uint64_t *o
 int pbsgpu_xxh3_collect(pbsgpu_ctx *ctx, XxhRun *r, uint64_t *hash_out, cudaStream_t st);
 void pbsgpu_xxh3_release(pbsgpu_ctx *ctx, XxhRun *r);
 int pbsgpu_xxh3_table(pbsgpu_ctx *ctx, const void **tab);   // K7's device table (uploaded on first use)
-// DataBlobs (capi_blob.cu) of n ranges with the encoder of `mode` (PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH, PBSGPU_BLOB_LZL),
+// DataBlobs (capi_blob.cu) of n ranges with the encoder of `mode` (PBSGPU_BLOB_RAW .. PBSGPU_BLOB_LZH, _LZL, _LZC),
 // encrypted with crypt and the IVs iv[16 n] or plain (crypt NULL): blob i at out + out_off[i], out_len[i] bytes (out_len
 // and crc_out may be NULL).  Device ranges are encoded in place.  The body of every pbsgpu_blob_encode_batch* call.
 int pbsgpu_blob_encode(pbsgpu_ctx *ctx, const pbsgpu_crypt *crypt, int mode, const uint8_t *iv, const void *base,

@@ -136,6 +136,7 @@ cudaError_t launch_zframe_hdr(uint8_t *stage, const uint64_t *frame_off, const u
 #include "zlz.cuh"   // f3: LZ77 match stage + Predefined_Mode sequences (K9)
 #include "zent.cuh"  // f3: entropy stage: FSE_Compressed_Mode sequences + Huffman literals (K10)
 #include "zldm.cuh"  // f3: long-distance matches of _lzl (K12)
+#include "zchain.cuh"  // f3: hash-chain match search and lazy parse of _lzc (K16)
 #include "zdec.cuh"  // f3, read side: the zstd decoder (K13)
 #include "deflate.cuh"  // f3, read side: raw Deflate streams of the zip restore (K15)
 namespace pbsgpu {

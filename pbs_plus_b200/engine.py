@@ -405,6 +405,12 @@ class Engine:
         most its _lzh blob (pbsgpu_blob_encode_batch_lzl) -> list of n `bytes` blobs, crc[n]."""
         return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lzl, base, off, length)
 
+    def blob_encode_batch_lzc(self, base, off, length):
+        """blob_encode_batch_lzh with K16's match search: the longest of 16 hash-chain candidates anywhere up to 2^24 - 4
+        bytes back in the chunk and a lazy parse, for smaller blobs of text-like data at more device time
+        (pbsgpu_blob_encode_batch_lzc; ranges < 2^32 bytes) -> list of n `bytes` blobs, crc[n]."""
+        return self._blob_encode_sized(self._L.pbsgpu_blob_encode_batch_lzc, base, off, length)
+
     @staticmethod
     def _blob_layout(l, head: int):
         """Room for n blobs back to back, each its uncompressed payload behind a `head`-byte header (12, or 44 encrypted)
@@ -480,7 +486,7 @@ class Engine:
 
     def blob_encode_batch_enc(self, crypt: "Crypt", mode: str, base, off, length, iv: bytes):
         """Encrypted DataBlobs (AES-256-GCM, pbsgpu_blob_encode_batch_enc) of n ranges: the payload is `mode`'s zstd
-        frame ("z", "lz", "lze", "lzh", "lzl") where smaller, else the raw chunk ("raw": always).  `iv` holds n x 16 bytes, one
+        frame ("z", "lz", "lze", "lzh", "lzl", "lzc") where smaller, else the raw chunk ("raw": always).  `iv` holds n x 16 bytes, one
         IV per blob; an IV must never be used twice under one key (draw them with os.urandom).
         -> list of n `bytes` blobs, crc[n]."""
         def enc(h, base, o, l, n, *outputs):
@@ -856,7 +862,8 @@ class Stream(_Handle):
 
     def blob_mode(self, mode: str | None):
         """DataBlobs for the new chunks (pbsgpu_stream_blob_mode), set before the first byte: None (no blobs), "raw",
-        "z", "lz", "lze", "lzh" or "lzl" -- the encoders of Engine.blob_encode_batch, _z, _lz, _lze, _lzh and _lzl."""
+        "z", "lz", "lze", "lzh", "lzl" or "lzc" -- the encoders of Engine.blob_encode_batch, _z, _lz, _lze, _lzh, _lzl
+        and _lzc."""
         if mode not in BLOB_MODES:
             raise ValueError(f"blob mode must be one of {list(BLOB_MODES)}, not {mode!r}")
         self._eng._ck(self._eng._L.pbsgpu_stream_blob_mode(self._h, BLOB_MODES[mode]))

@@ -75,7 +75,8 @@ class DedupWriter:
     # "z": frames of RLE and raw blocks; "lz": also compressed blocks from the LZ77 match stage (pbsgpu_blob_encode_batch_lz);
     # "lze": those blocks also through zstd's entropy stage (pbsgpu_blob_encode_batch_lze); "lzh": with Huffman literals
     # whatever their largest value, for binary data (pbsgpu_blob_encode_batch_lzh); "lzl": also long matches anywhere
-    # earlier in the chunk, for repeats beyond one 128 KiB block (pbsgpu_blob_encode_batch_lzl)
+    # earlier in the chunk, for repeats beyond one 128 KiB block (pbsgpu_blob_encode_batch_lzl); "lzc": _lzh with a
+    # hash-chain match search over the whole chunk and a lazy parse, for smaller text-like blobs (pbsgpu_blob_encode_batch_lzc)
     blob_compression: str = "z"
     # encrypt mode (CryptMode encrypt, commit.go:314): the 32-byte client key.  Digests become keyed (SHA-256(chunk ||
     # id_key)) and upload_blob receives encrypted blobs (pbsgpu_blob_encode_batch_enc, IVs from os.urandom)
@@ -187,7 +188,7 @@ class PayloadStreamWriter:
     index: list[tuple[int, bytes, bool]] = field(default_factory=list)   # (end offset in the NEW stream, digest, known)
     payload_offsets: dict[str, int] = field(default_factory=dict)        # entry path -> offset of its PAYLOAD header
     # (digest, DataBlob) for NEW chunks, encoded on the GPU from the stream's windows (pbsgpu_stream_blob_mode) with the
-    # encoder `blob_compression` names ("z", "lz", "lze", "lzh" or "lzl", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
+    # encoder `blob_compression` names ("z", "lz", "lze", "lzh", "lzl" or "lzc", as for DedupWriter).  Chunks injected by WriteEntryRef get none.
     upload_blob: Callable[[bytes, bytes], None] | None = None
     blob_compression: str = "z"
     # hash_files: relPath -> XXH3-64 of every file written through WriteEntryReader in backed_hashes
@@ -333,7 +334,7 @@ class FixedIndexWriter:
     """Backs up a disk image as a fixed index (`<name>.img.fidx`): the image is cut at every multiple of `chunk_size`
     (upstream writes 4 MiB chunks), and each chunk is digested on the GPU, probed against `known` (seed it from the
     previous snapshot's index with DigestSet.seed_fidx) and, when new, handed to `upload_blob(digest, blob)` as a
-    DataBlob made by the encoder `blob_compression` names ("z", "lz", "lze", "lzh" or "lzl", as for DedupWriter).  No
+    DataBlob made by the encoder `blob_compression` names ("z", "lz", "lze", "lzh", "lzl" or "lzc", as for DedupWriter).  No
     state crosses a chunk boundary, so the image is fed in slices of any size that are multiples of `chunk_size` -- only
     the last may end inside a chunk -- one batch call per slice, from host memory or straight from device memory."""
     engine: Engine

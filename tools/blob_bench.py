@@ -3,10 +3,11 @@ the raw C calls (no Python-side allocation or slicing inside the timed region). 
 them zero runs, a text-like image (tests/zstd_lz_ref.py text_corpus, 32 MiB repeated), a binary-like one
 (tests/zstd_huf_ref.py binary_corpus, 32 MiB repeated) and one with repeats far beyond one block (every 4 MiB chunk is
 4 copies of 1 MiB of binary_corpus with 2000 random byte edits, tests/zstd_ldm_ref.py repeated_image).  For each: GB/s
-of input and output / input of every encoder, and for context libzstd level 1 (pyarrow) on a 64 MiB host sample of the
-same image (8 MiB from each GiB), its ratio and single-thread rate on the HOST CPU.
+of input and output / input of every encoder, and for context libzstd levels 1 and 3 (pyarrow, one host thread) on a
+64 MiB host sample of the same image (8 MiB from each GiB), their ratios and single-thread rates on the HOST CPU.
+blob_encode_batch_enc_lzc is the encrypted call in _lzc mode (random IVs).
 
-    python tools/blob_bench.py [call ...]     # e.g. blob_encode_batch_lzh blob_encode_batch_lzl; default: every call"""
+    python tools/blob_bench.py [call ...]     # e.g. blob_encode_batch_lzh blob_encode_batch_lzc; default: every call"""
 import subprocess
 import sys
 import time
@@ -30,14 +31,17 @@ n = 8 << 30
 CH = 4 << 20
 off = np.arange(0, n, CH, dtype=np.uint64)
 ln = np.full(len(off), CH, dtype=np.uint64)
-boff = (np.arange(len(off), dtype=np.uint64) * np.uint64(CH + 12))
-out = e.host_alloc(int(len(off)) * (CH + 12))
+boff = (np.arange(len(off), dtype=np.uint64) * np.uint64(CH + 44))   # room for an encrypted blob's header
+out = e.host_alloc(int(len(off)) * (CH + 44))
+ivs = np.random.default_rng(0).integers(0, 256, 16 * len(off), dtype=np.uint8)
+crypt = e.crypt(bytes(range(32)))
 blen = np.zeros(len(off), dtype=np.uint64)
 crc = np.zeros(len(off), dtype=np.uint32)
 
 
 CALLS = sys.argv[1:] or ["crc32_batch", "blob_encode_batch", "blob_encode_batch_z", "blob_encode_batch_lz",
-                         "blob_encode_batch_lze", "blob_encode_batch_lzh", "blob_encode_batch_lzl"]
+                         "blob_encode_batch_lze", "blob_encode_batch_lzh", "blob_encode_batch_lzl",
+                         "blob_encode_batch_lzc", "blob_encode_batch_enc_lzc"]
 
 
 def images():
@@ -65,6 +69,11 @@ for label, d in images():
             if name == "crc32_batch":
                 rc = L_.pbsgpu_crc32_batch(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), crc.ctypes.data)
                 size = 0
+            elif name == "blob_encode_batch_enc_lzc":
+                rc = L_.pbsgpu_blob_encode_batch_enc(e._h, crypt._h, 10, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off),
+                                                     ivs.ctypes.data, out.ctypes.data, boff.ctypes.data, blen.ctypes.data,
+                                                     crc.ctypes.data)
+                size = int(blen.sum())
             elif name == "blob_encode_batch":
                 rc = L_.pbsgpu_blob_encode_batch(e._h, d.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), out.ctypes.data,
                                                  boff.ctypes.data, crc.ctypes.data)
@@ -81,13 +90,15 @@ for label, d in images():
     try:
         import pyarrow as pa
         sample = b"".join(d[k * (n // 8): k * (n // 8) + (8 << 20)].cpu().numpy().tobytes() for k in range(8))
-        t0 = time.perf_counter()
-        z = pa.Codec("zstd", compression_level=1).compress(sample, asbytes=True)
-        dt = time.perf_counter() - t0
-        print(f"libzstd level 1 (host CPU, one thread, 8 x 8 MiB sample): output / input {len(z) / len(sample):.4f}, "
-              f"{len(sample) / dt / 1e9:.2f} GB/s")
+        for level in (1, 3):
+            t0 = time.perf_counter()
+            z = pa.Codec("zstd", compression_level=level).compress(sample, asbytes=True)
+            dt = time.perf_counter() - t0
+            print(f"libzstd level {level} (host CPU, one thread, 8 x 8 MiB sample): output / input {len(z) / len(sample):.4f}, "
+                  f"{len(sample) / dt / 1e9:.2f} GB/s")
     except ImportError:
-        print("libzstd level 1: pyarrow not available")
+        print("libzstd: pyarrow not available")
     del d
+crypt.close()
 e.host_free(out)
 e.close()
