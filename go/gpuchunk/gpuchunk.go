@@ -998,8 +998,9 @@ func (p *PayloadReader) read(off, length []uint64, payload bool, out []byte, out
 }
 
 // readDeflate is read whose outputs are the ranges' raw Deflate streams, compressed on the GPU
-// (pbsgpu_reader_read_deflate); more[i] != 0: a later call continues stream i.  Returns the streams and CRC-32s.
-func (p *PayloadReader) readDeflate(off, length []uint64, payload bool, more []uint8) ([][]byte, []uint32, error) {
+// (pbsgpu_reader_read_deflate); more[i] != 0: a later call continues stream i; lzc: the hash-chain parse
+// (PBSGPU_READ_DEFLATE_LZC).  Returns the streams and CRC-32s.
+func (p *PayloadReader) readDeflate(off, length []uint64, payload bool, more []uint8, lzc bool) ([][]byte, []uint32, error) {
 	n := len(off)
 	if n == 0 {
 		return nil, nil, nil
@@ -1025,6 +1026,9 @@ func (p *PayloadReader) readDeflate(off, length []uint64, payload bool, more []u
 	var mp *C.uint8_t
 	if more != nil {
 		mp = (*C.uint8_t)(unsafe.Pointer(&more[0]))
+	}
+	if lzc {
+		flags |= C.PBSGPU_READ_DEFLATE_LZC
 	}
 	rc := C.pbsgpu_reader_read_deflate(p.r, (*C.uint64_t)(unsafe.Pointer(&off[0])), (*C.uint64_t)(unsafe.Pointer(&length[0])),
 		C.uint32_t(n), flags, mp, unsafe.Pointer(&blobs[0]), (*C.uint64_t)(unsafe.Pointer(&bo[0])),
@@ -1272,11 +1276,13 @@ func (e *Engine) NewImageReader(fidx []byte, c *Crypt, cacheBytes uint64, source
 // (pbsgpu_reader_read_deflate) and the container is written by pbsgpu_zip_*.  Every entry but a directory has flag bit
 // 3 and a data descriptor; Close writes the central directory.  Files up to PieceBytes go in batches of about PieceBytes
 // file bytes, one read per batch; a larger file goes in 128 KiB-aligned pieces of plain ranges continued with `more`,
-// after one plain read of its 16-byte PAYLOAD header, and its CRC-32 is combined from the pieces'.
+// after one plain read of its 16-byte PAYLOAD header, and its CRC-32 is combined from the pieces'.  LZC: deflate with
+// the hash-chain parse (pbsgpu_deflate_batch_lzc), for a smaller zip at a lower rate; false writes the greedy parse's.
 type ZipWriter struct {
 	pr         *PayloadReader
 	w          io.Writer
 	PieceBytes uint64
+	LZC        bool
 	pos        uint64
 	entries    []C.pbsgpu_zip_entry
 }
@@ -1359,7 +1365,7 @@ func (z *ZipWriter) AddFiles(files []ZipFile) error {
 		for i, f := range batch {
 			off[i], size[i] = f.PayloadOffset, f.Size
 		}
-		streams, crcs, err := z.pr.readDeflate(off, size, true, nil)
+		streams, crcs, err := z.pr.readDeflate(off, size, true, nil, z.LZC)
 		if err != nil {
 			return err
 		}
@@ -1423,7 +1429,7 @@ func (z *ZipWriter) large(f ZipFile, piece uint64) error {
 		if lo+n < f.Size {
 			more[0] = 1
 		}
-		s, c, err := z.pr.readDeflate([]uint64{f.PayloadOffset + 16 + lo}, []uint64{n}, false, more)
+		s, c, err := z.pr.readDeflate([]uint64{f.PayloadOffset + 16 + lo}, []uint64{n}, false, more, z.LZC)
 		if err != nil {
 			return err
 		}

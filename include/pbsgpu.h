@@ -504,6 +504,7 @@ int pbsgpu_reader_open_fidx(pbsgpu_ctx *ctx, const uint8_t *fidx, uint64_t bytes
 void pbsgpu_reader_close(pbsgpu_reader *r);
 uint64_t pbsgpu_reader_size(const pbsgpu_reader *r);
 #define PBSGPU_READ_PAYLOAD 1u
+#define PBSGPU_READ_DEFLATE_LZC 2u   /* pbsgpu_reader_read_deflate only: deflate as pbsgpu_deflate_batch_lzc */
 int pbsgpu_reader_plan(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
                        uint64_t *chunk, uint8_t *digest, uint64_t cap, uint64_t *n_out);
 int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
@@ -530,10 +531,19 @@ enum { PBSGPU_DEC_MISSING = PBSGPU_DEC_BAD_TAG + 1,   /* 9: a chunk the range ne
  * byte-aligned end, and len[i] must be a multiple of 128 KiB (EINVAL otherwise; a piece of 0 bytes is no bytes).
  * Concatenating the pieces gives exactly the one-call stream.  Scratch is bounded per pass of 4096 segments, so a call
  * of any size works.
+ * pbsgpu_deflate_batch_lzc: pbsgpu_deflate_batch's arguments, rules and format (segments, more, forms, bound), with a
+ * hash-chain search and lazy parse in each segment instead of the greedy one (tests/deflate_chain_ref.py restates it;
+ * DESIGN.md K16d): a match is the longest of the first 32 earlier positions of the segment with the same 3 bytes, at
+ * most 32768 back and 258 long (ties to the nearer); the parse may move on
+ * up to 2 positions when the next match's gain (4 length - the distance code's extra bits) is larger by more than 4;
+ * a segment takes at most 32768 matches.  Smaller streams at a lower rate; passes of 1024 segments, each with about
+ * 3.5 GiB of device scratch.
  * pbsgpu_crc32_combine: the CRC-32 of A || B from crc1 = CRC-32(A), crc2 = CRC-32(B) and len2 = |B| (host only). */
 uint64_t pbsgpu_deflate_bound(uint64_t len);
 int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
                          const uint8_t *more, uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
+int pbsgpu_deflate_batch_lzc(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                             const uint8_t *more, uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out);
 uint32_t pbsgpu_crc32_combine(uint32_t crc1, uint32_t crc2, uint64_t len2);
 /* The zip container (host only, no ctx).  An entry: its name bytes (a directory's ends in '/'), Unix st_mode, mtime in
  * seconds since the epoch, method (0 stored, 8 deflate), the CRC-32 and the compressed and uncompressed sizes of its
@@ -565,7 +575,8 @@ typedef struct pbsgpu_zip_entry {
  * crc_out as there): out is HOST memory with pbsgpu_deflate_bound(len[i]) reserved at out + out_off[i] (a device out is
  * EINVAL), out_len[i] is the stream's size, and 0 when status[i] is not OK; no byte of a failed range is written.  The
  * ranges are read into a device stage of the call's total range bytes and deflated there: file bytes never cross PCIe
- * uncompressed. */
+ * uncompressed.  flags may add PBSGPU_READ_DEFLATE_LZC: the streams are then pbsgpu_deflate_batch_lzc's (plan and read
+ * refuse that flag with EINVAL). */
 int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
                                const uint8_t *more, const void *blob_base, const uint64_t *blob_off, const uint64_t *blob_len,
                                const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out, const uint64_t *out_off,

@@ -44,6 +44,7 @@ DEC_BAD_TAG = 8   # pbsgpu_blob_decode_batch_enc only: the AES-256-GCM tag did n
 # pbsgpu_reader_read: a range's chunk was neither cached nor given; a file's 16-byte PAYLOAD header did not match
 DEC_MISSING, DEC_BAD_HEADER = 9, 10
 READ_PAYLOAD = 1   # pbsgpu_reader_plan / _read flags: ranges are (payload offset, file size)
+READ_DEFLATE_LZC = 2   # pbsgpu_reader_read_deflate only: the streams are pbsgpu_deflate_batch_lzc's
 
 
 class DevInfo(C.Structure):
@@ -178,6 +179,7 @@ _SIGNATURES = {
     "pbsgpu_reader_read": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp],
     "pbsgpu_deflate_bound": ([C.c_uint64], C.c_uint64),
     "pbsgpu_deflate_batch": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp],
+    "pbsgpu_deflate_batch_lzc": [_vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp],
     "pbsgpu_crc32_combine": ([C.c_uint32, C.c_uint32, C.c_uint64], C.c_uint32),
     "pbsgpu_reader_read_deflate": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
                                    _vp, _vp],

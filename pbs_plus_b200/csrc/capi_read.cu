@@ -358,8 +358,9 @@ extern "C" int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const u
 }
 
 // The zip restore's read: the ranges go through pbsgpu_reader_read into a device stage owned by this call, and only the
-// ranges whose status is OK are deflated from there (pbsgpu_deflate_batch) into the caller's host memory, so file bytes
-// cross PCIe compressed and no byte of a failed range reaches `out`.
+// ranges whose status is OK are deflated from there (pbsgpu_deflate_batch, or pbsgpu_deflate_batch_lzc with
+// PBSGPU_READ_DEFLATE_LZC) into the caller's host memory, so file bytes cross PCIe compressed and no byte of a failed
+// range reaches `out`.
 extern "C" int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
                                           const uint8_t *more, const void *blob_base, const uint64_t *blob_off,
                                           const uint64_t *blob_len, const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out,
@@ -370,6 +371,8 @@ extern "C" int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off,
         return PBSGPU_EINVAL;
     pbsgpu_ctx *ctx = r->ctx;
     Guard g(ctx);
+    const bool lzc = flags & PBSGPU_READ_DEFLATE_LZC;   // this call's flag alone: the read below never sees it
+    flags &= ~PBSGPU_READ_DEFLATE_LZC;
     if (n && pbsgpu_is_device_ptr(out)) return fail(ctx, PBSGPU_EINVAL, "read_deflate: out must be host memory");
     for (uint32_t i = 0; i < n; i++)
         if (more && more[i] && len[i] % DEFLATE_SEGMENT)
@@ -397,8 +400,8 @@ extern "C" int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off,
     const uint32_t k = (uint32_t)idx.size();
     if (k == 0) return PBSGPU_OK;
     klen.resize(k); kcrc.resize(k);
-    if (int rc = pbsgpu_deflate_batch(ctx, stage, ko.data(), kl.data(), k, km.data(), out, koo.data(), klen.data(),
-                                      crc_out ? kcrc.data() : nullptr))
+    if (int rc = (lzc ? pbsgpu_deflate_batch_lzc : pbsgpu_deflate_batch)(ctx, stage, ko.data(), kl.data(), k, km.data(), out,
+                                                                         koo.data(), klen.data(), crc_out ? kcrc.data() : nullptr))
         return rc;
     for (uint32_t j = 0; j < k; j++) {
         out_len[idx[j]] = klen[j];

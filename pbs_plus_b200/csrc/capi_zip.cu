@@ -1,5 +1,6 @@
 // pbs_plus_b200/csrc/capi_zip.cu -- C ABI of the zip restore (f3, read side): raw Deflate streams of byte ranges (K9a's
-// Deflate parse + K15, deflate.cu), the CRC-32 combination of pieces, and the zip container written on the host.
+// Deflate parse, or with _lzc K16's hash-chain parse, then K15, deflate.cu), the CRC-32 combination of pieces, and the
+// zip container written on the host.
 #include <time.h>
 
 #include <algorithm>
@@ -36,9 +37,11 @@ extern "C" uint32_t pbsgpu_crc32_combine(uint32_t crc1, uint32_t crc2, uint64_t 
     return multmodp(p, crc1) ^ crc2;
 }
 
-extern "C" int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
-                                    const uint8_t *more, uint8_t *out, const uint64_t *out_off, uint64_t *out_len,
-                                    uint32_t *crc_out) {
+// lzc: K16's DEFLATE instantiation parses each pass of DCH_PASS_SEGS segments (every segment one chunk of one block of
+// ChainArgs) instead of K9a; K15 and the compaction are the same.
+static int deflate_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                         const uint8_t *more, uint8_t *out, const uint64_t *out_off, uint64_t *out_len, uint32_t *crc_out,
+                         bool lzc) {
     if (!ctx || (n && (!off || !len || !out || !out_off || !out_len))) return PBSGPU_EINVAL;
     Guard g(ctx);
     for (uint32_t i = 0; i < n; i++)
@@ -79,7 +82,7 @@ extern "C" int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uin
             out_len[i] = 2;
         }
     if (nseg) {
-        const uint64_t pcap = std::min<uint64_t>(nseg, DEFLATE_PASS_SEGS);
+        const uint64_t pass = lzc ? DCH_PASS_SEGS : DEFLATE_PASS_SEGS, pcap = std::min<uint64_t>(nseg, pass);
         uint64_t *d_src = b.upload(src.data(), nseg);
         uint32_t *d_size = b.upload(size.data(), nseg);
         uint8_t *d_fin = b.upload(fin.data(), nseg);
@@ -93,14 +96,38 @@ extern "C" int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uin
         if (!d_src || !d_size || !d_fin || !d_lits || !d_seqs || !d_nseq || !d_nlit || !d_len || !d_out ||
             (!out_dev && !stage) || !d_pieces || !d_first)
             return fail(ctx, PBSGPU_ENOMEM, "deflate: device allocation failed");
+        // lzc: the segments' sizes as K16 takes them, their first positions in the call, and the scratch of one pass
+        std::vector<uint64_t> vfirst, len64;
+        uint64_t *d_vfirst = nullptr, *d_len64 = nullptr;
+        uint8_t *scratch = nullptr;
+        if (lzc) {
+            vfirst.assign(nseg + 1, 0);
+            len64.assign(size.begin(), size.end());
+            for (uint64_t s = 0; s < nseg; s++) vfirst[s + 1] = vfirst[s] + size[s];
+            uint64_t most = 0;
+            for (uint64_t f = 0; f < nseg; f += pass) most = std::max(most, vfirst[std::min(nseg, f + pass)] - vfirst[f]);
+            const size_t sb = chain_scratch_bytes(most);
+            d_vfirst = b.upload(vfirst.data(), nseg + 1);
+            d_len64 = b.upload(len64.data(), nseg);
+            scratch = b.get<uint8_t>(sb);
+            if (!d_vfirst || !d_len64 || !scratch)
+                return fail(ctx, PBSGPU_ENOMEM, "deflate: chain search scratch of %llu bytes failed", (unsigned long long)sb);
+        }
         std::vector<uint32_t> slen(pcap);
         std::vector<ReadPiece> pieces(pcap);
         std::vector<uint64_t> first(pcap + 1);
         struct Run { uint64_t stage, out, len; };
         std::vector<Run> runs;
-        for (uint64_t f = 0; f < nseg; f += DEFLATE_PASS_SEGS) {
-            const uint32_t pn = (uint32_t)std::min<uint64_t>(DEFLATE_PASS_SEGS, nseg - f);
-            if (b.ok()) b.e = launch_lz_parse_deflate(dbase, d_src + f, d_size + f, pn, d_lits, d_seqs, d_nseq, d_nlit, b.st);
+        for (uint64_t f = 0; f < nseg; f += pass) {
+            const uint32_t pn = (uint32_t)std::min<uint64_t>(pass, nseg - f);
+            if (lzc) {
+                const ChainArgs a{dbase, d_src, d_len64, d_vfirst, (uint32_t)f, (uint32_t)(f + pn), vfirst[f + pn] - vfirst[f],
+                                  vfirst[f], d_src, d_vfirst, d_size, f, f + pn};
+                if (b.ok()) b.e = launch_chain_search(a, scratch, b.st, true);
+                if (b.ok()) b.e = launch_chain_parse(a, scratch, f, pn, d_lits, d_seqs, d_nseq, d_nlit, b.st, true);
+            } else if (b.ok()) {
+                b.e = launch_lz_parse_deflate(dbase, d_src + f, d_size + f, pn, d_lits, d_seqs, d_nseq, d_nlit, b.st);
+            }
             if (b.ok()) b.e = launch_deflate_encode(dbase, d_src + f, d_size + f, d_fin + f, pn, d_lits, d_seqs, d_nseq, d_nlit,
                                                     d_out, d_len, b.st);
             if (b.ok()) b.e = cudaMemcpyAsync(slen.data(), d_len, pn * 4ull, cudaMemcpyDeviceToHost, b.st);
@@ -132,6 +159,18 @@ extern "C" int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uin
     }
     if (crc_out && b.ok()) b.e = cudaMemcpyAsync(crc_out, d_crc, n * 4ull, cudaMemcpyDeviceToHost, b.st);
     return b.finish("deflate batch");
+}
+
+extern "C" int pbsgpu_deflate_batch(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len, uint32_t n,
+                                    const uint8_t *more, uint8_t *out, const uint64_t *out_off, uint64_t *out_len,
+                                    uint32_t *crc_out) {
+    return deflate_batch(ctx, base, off, len, n, more, out, out_off, out_len, crc_out, false);
+}
+
+extern "C" int pbsgpu_deflate_batch_lzc(pbsgpu_ctx *ctx, const void *base, const uint64_t *off, const uint64_t *len,
+                                        uint32_t n, const uint8_t *more, uint8_t *out, const uint64_t *out_off,
+                                        uint64_t *out_len, uint32_t *crc_out) {
+    return deflate_batch(ctx, base, off, len, n, more, out, out_off, out_len, crc_out, true);
 }
 
 // ---- the zip container --------------------------------------------------------------------------------------------

@@ -18,6 +18,11 @@
 //                  next entries.  A CH_SAT entry the parse reaches is searched again by the warp, 32 bytes per ballot
 //                  step over the full chain walk; the parse jumps past the match, so that costs about
 //                  CH_DEPTH * (1 + CH_LAZY) / 32 steps per byte of a long match.
+//
+// K16d, the DEFLATE instantiation of the same kernels (pbsgpu_deflate_batch_lzc, tests/deflate_chain_ref.py): each
+// 128 KiB Deflate segment is one chunk of one block; the key is DCH_MINMATCH bytes, offsets reach DEFLATE_WINDOW, a
+// match and K16c's re-search stop at DEFLATE_MAX_MATCH, the gain counts the distance code's extra bits, and a segment
+// takes at most LZ_MAX_SEQ matches (the rest are literals).  K15 codes the output unchanged.
 #include "internal.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -30,7 +35,20 @@ constexpr int CH_THREADS = 256;
 constexpr uint32_t CH_BEST_SPAN = 8192;    // K16b positions per CTA
 static_assert(CH_CAP < CH_SAT, "best[] keeps a length below CH_CAP in 8 bits");
 
+template <bool DEFLATE> struct ChainRule;
+template <> struct ChainRule<false> {   // _lzc
+    static constexpr uint32_t MINMATCH = CH_MINMATCH, DEPTH = CH_DEPTH, LAZY = CH_LAZY, MAXDIST = CH_MAXDIST;
+    static constexpr int MARGIN = CH_MARGIN;
+};
+template <> struct ChainRule<true> {    // Deflate
+    static constexpr uint32_t MINMATCH = DCH_MINMATCH, DEPTH = DCH_DEPTH, LAZY = DCH_LAZY, MAXDIST = DEFLATE_WINDOW;
+    static constexpr int MARGIN = DCH_MARGIN;
+};
+static_assert(DCH_MINMATCH >= 3 && DCH_MINMATCH <= 4 && DEFLATE_MAX_MATCH > CH_CAP, "Deflate keys and lengths");
+
+template <bool DEFLATE>
 __global__ void __launch_bounds__(CH_THREADS) k_ch_keys(const ChainArgs a, uint64_t *key, uint32_t *val) {
+    using C = ChainRule<DEFLATE>;
     const uint64_t p = (uint64_t)blockIdx.x * CH_THREADS + threadIdx.x;
     if (p >= a.n) return;
     uint32_t lo = a.c0, hi = a.c1 - 1;   // the chunk: the last c with vfirst[c] - vbase <= p
@@ -40,10 +58,10 @@ __global__ void __launch_bounds__(CH_THREADS) k_ch_keys(const ChainArgs a, uint6
     }
     const uint64_t x = p - (a.vfirst[lo] - a.vbase);
     uint64_t k = (uint64_t)(a.c1 - a.c0) << 32;
-    if (x + CH_MINMATCH <= a.len[lo]) {
+    if (x + C::MINMATCH <= a.len[lo]) {
         const uint8_t *q = a.base + a.off[lo] + x;
-        k = (uint64_t)(lo - a.c0) << 32 | __ldg(q) | (uint32_t)__ldg(q + 1) << 8 | (uint32_t)__ldg(q + 2) << 16 |
-            (uint32_t)__ldg(q + 3) << 24;
+        k = (uint64_t)(lo - a.c0) << 32 | __ldg(q) | (uint32_t)__ldg(q + 1) << 8 | (uint32_t)__ldg(q + 2) << 16;
+        if (C::MINMATCH == 4) k |= (uint32_t)__ldg(q + 3) << 24;
     }
     key[p] = k;
     val[p] = (uint32_t)p;
@@ -57,21 +75,23 @@ __global__ void __launch_bounds__(CH_THREADS) k_ch_prev(const uint64_t *key, con
     prev[val[k]] = k > 0 && key[k - 1] == v && (v >> 32) != nc ? val[k - 1] : CH_NONE;
 }
 
+template <bool DEFLATE>
 __global__ void __launch_bounds__(CH_THREADS) k_ch_best(const ChainArgs a, const uint32_t *prev, uint32_t *best) {
+    using C = ChainRule<DEFLATE>;
     const uint64_t z = a.z0 + blockIdx.x;
     const uint32_t S = a.zsize[z], P = (uint32_t)(a.vpos[z] - a.vbase);
     const uint8_t *p = a.base + a.zsrc[z];
     const uint32_t t1 = min(S, (blockIdx.y + 1) * CH_BEST_SPAN);
     for (uint32_t t = blockIdx.y * CH_BEST_SPAN + threadIdx.x; t < t1; t += CH_THREADS) {
-        const uint32_t lim = S - t, i = P + t;
+        const uint32_t lim = DEFLATE ? min(S - t, DEFLATE_MAX_MATCH) : S - t, i = P + t;
         uint32_t out = 0;
-        if (lim >= CH_MINMATCH) {
+        if (lim >= C::MINMATCH) {
             const uint32_t cap = min(lim, CH_CAP);
             const uint8_t *q = p + t;
             uint32_t j = prev[i], bl = 0, bo = 0;
-            for (uint32_t k = 0; k < CH_DEPTH && j != CH_NONE && i - j <= CH_MAXDIST; k++) {
+            for (uint32_t k = 0; k < C::DEPTH && j != CH_NONE && i - j <= C::MAXDIST; k++) {
                 const uint8_t *s = q - (i - j);
-                uint32_t L = CH_MINMATCH;   // the key's bytes are equal
+                uint32_t L = C::MINMATCH;   // the key's bytes are equal
                 while (L < cap && __ldg(s + L) == __ldg(q + L)) L++;
                 if (L == cap && cap < lim) { bl = CH_SAT; break; }
                 if (L > bl) {
@@ -86,28 +106,33 @@ __global__ void __launch_bounds__(CH_THREADS) k_ch_best(const ChainArgs a, const
     }
 }
 
-// gain of a match: 4 L - floor(log2(offset + 3))
-__device__ __forceinline__ int ch_gain(uint32_t L, uint32_t o) { return 4 * (int)L - (31 - __clz(o + 3)); }
+// gain of a match: 4 L - floor(log2(offset + 3)); Deflate: 4 L - the extra bits of the distance code
+template <bool DEFLATE> __device__ __forceinline__ int ch_gain(uint32_t L, uint32_t o) {
+    if (DEFLATE) return 4 * (int)L - (o <= 2 ? 0 : 30 - __clz(o - 1));
+    return 4 * (int)L - (31 - __clz(o + 3));
+}
 
+template <bool DEFLATE>
 __global__ void __launch_bounds__(128) k_ch_parse(const ChainArgs a, const uint32_t *prev, const uint32_t *best,
                                                   uint64_t first, uint32_t nb, uint8_t *slots, uint64_t *seqs, uint32_t *nseq,
                                                   uint32_t *nlit) {
     const uint32_t w = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    using C = ChainRule<DEFLATE>;
     if (w >= nb) return;
-    const uint64_t z = first + w;
+    const uint64_t z = first + w, zo = DEFLATE ? w : z;   // zo: the block's slot and counts
     const uint32_t S = a.zsize[z], P = (uint32_t)(a.vpos[z] - a.vbase);
     const uint8_t *p = a.base + a.zsrc[z];
     const uint32_t *bst = best + P;
-    uint8_t *lit = slots + z * LZ_SLOT + 3;
+    uint8_t *lit = slots + zo * LZ_SLOT + 3;
     uint64_t *sq = seqs + (uint64_t)w * LZ_MAX_SEQ;
     // the match at block position m: best[]'s, or the full chain walk for a CH_SAT entry
     auto match = [&](uint32_t m, uint32_t &L, uint32_t &o) {
         const uint32_t e = bst[m];
         if ((e & 0xFF) != CH_SAT) { L = e & 0xFF; o = e >> 8; return; }
-        const uint32_t i = P + m, lim = S - m;
+        const uint32_t i = P + m, lim = DEFLATE ? min(S - m, DEFLATE_MAX_MATCH) : S - m;
         const uint8_t *q = p + m;
         uint32_t j = prev[i], bl = 0, bo = 0;
-        for (uint32_t k = 0; k < CH_DEPTH && j != CH_NONE && i - j <= CH_MAXDIST; k++) {
+        for (uint32_t k = 0; k < C::DEPTH && j != CH_NONE && i - j <= C::MAXDIST; k++) {
             const uint8_t *s = q - (i - j);
             uint32_t len = 0;
             for (;;) {
@@ -127,7 +152,7 @@ __global__ void __launch_bounds__(128) k_ch_parse(const ChainArgs a, const uint3
     uint32_t pos = 0, run = 0, nl = 0, ns = 0;   // the same in every lane
     while (pos < S) {
         const uint32_t q = pos + lane;
-        const uint32_t hits = __ballot_sync(~0u, q < S && bst[q] != 0);
+        const uint32_t hits = __ballot_sync(~0u, (!DEFLATE || ns < LZ_MAX_SEQ) && q < S && bst[q] != 0);
         uint32_t m = hits ? pos + __ffs(hits) - 1 : min(pos + 32, S);
         if (q < m) lit[nl + lane] = __ldg(p + q);
         nl += m - pos;
@@ -135,10 +160,10 @@ __global__ void __launch_bounds__(128) k_ch_parse(const ChainArgs a, const uint3
         if (!hits) continue;
         uint32_t L, o;
         match(m, L, o);
-        for (uint32_t k = 0; k < CH_LAZY && m + 1 < S && bst[m + 1] != 0; k++) {
+        for (uint32_t k = 0; k < C::LAZY && m + 1 < S && bst[m + 1] != 0; k++) {
             uint32_t L2, o2;
             match(m + 1, L2, o2);
-            if (ch_gain(L2, o2) <= ch_gain(L, o) + CH_MARGIN) break;
+            if (ch_gain<DEFLATE>(L2, o2) <= ch_gain<DEFLATE>(L, o) + C::MARGIN) break;
             if (lane == 0) lit[nl] = __ldg(p + m);
             nl++; m++; L = L2; o = o2;
         }
@@ -146,7 +171,7 @@ __global__ void __launch_bounds__(128) k_ch_parse(const ChainArgs a, const uint3
         ns++;
         pos = run = m + L;
     }
-    if (lane == 0) { nseq[z] = ns; nlit[z] = nl; }
+    if (lane == 0) { nseq[zo] = ns; nlit[zo] = nl; }
 }
 
 // scratch: key[2][n] (u64) | val[2][n] prev[n] (u32) | cub temp; best[] takes the key buffers once prev[] is done
@@ -166,7 +191,7 @@ size_t chain_scratch_bytes(uint64_t n) { return chain_layout(n).total; }
 
 #define CH_CK(call) do { const cudaError_t e__ = (call); if (e__ != cudaSuccess) return e__; } while (0)
 
-cudaError_t launch_chain_search(const ChainArgs &a, void *scratch, cudaStream_t st) {
+template <bool DEFLATE> static cudaError_t chain_search(const ChainArgs &a, void *scratch, cudaStream_t st) {
     if (a.z1 <= a.z0 || a.n == 0) return cudaSuccess;
     const ChainLayout L = chain_layout(a.n);
     uint8_t *b = (uint8_t *)scratch;
@@ -176,7 +201,7 @@ cudaError_t launch_chain_search(const ChainArgs &a, void *scratch, cudaStream_t 
     int end_bit = 32;
     while (end_bit < 64 && (nc >> (end_bit - 32)) != 0) end_bit++;   // the chunk field holds 0 .. nc
     const unsigned g = (unsigned)((a.n + CH_THREADS - 1) / CH_THREADS);
-    k_ch_keys<<<g, CH_THREADS, 0, st>>>(a, k0, v0);
+    k_ch_keys<DEFLATE><<<g, CH_THREADS, 0, st>>>(a, k0, v0);
     CH_CK(cudaGetLastError());
     cub::DoubleBuffer<uint64_t> dk(k0, k1);
     cub::DoubleBuffer<uint32_t> dv(v0, v1);
@@ -185,17 +210,23 @@ cudaError_t launch_chain_search(const ChainArgs &a, void *scratch, cudaStream_t 
     k_ch_prev<<<g, CH_THREADS, 0, st>>>(dk.Current(), dv.Current(), a.n, nc, prev);
     CH_CK(cudaGetLastError());
     const dim3 bg((unsigned)(a.z1 - a.z0), ZFRAME_BLOCK / CH_BEST_SPAN);
-    k_ch_best<<<bg, CH_THREADS, 0, st>>>(a, prev, (uint32_t *)(b + L.k0));
+    k_ch_best<DEFLATE><<<bg, CH_THREADS, 0, st>>>(a, prev, (uint32_t *)(b + L.k0));
     return cudaGetLastError();
+}
+static_assert(DEFLATE_SEGMENT == ZFRAME_BLOCK, "K16b's grid covers a Deflate segment as a block");
+
+cudaError_t launch_chain_search(const ChainArgs &a, void *scratch, cudaStream_t st, bool deflate) {
+    return deflate ? chain_search<true>(a, scratch, st) : chain_search<false>(a, scratch, st);
 }
 
 cudaError_t launch_chain_parse(const ChainArgs &a, const void *scratch, uint64_t first, uint32_t nb, uint8_t *slots,
-                               uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, cudaStream_t st) {
+                               uint64_t *seqs, uint32_t *nseq, uint32_t *nlit, cudaStream_t st, bool deflate) {
     if (nb == 0) return cudaSuccess;
     const ChainLayout L = chain_layout(a.n);
     const uint8_t *b = (const uint8_t *)scratch;
-    k_ch_parse<<<(nb + 3) / 4, 128, 0, st>>>(a, (const uint32_t *)(b + L.prev), (const uint32_t *)(b + L.k0), first, nb,
-                                             slots, seqs, nseq, nlit);
+    const uint32_t *prev = (const uint32_t *)(b + L.prev), *best = (const uint32_t *)(b + L.k0);
+    if (deflate) k_ch_parse<true><<<(nb + 3) / 4, 128, 0, st>>>(a, prev, best, first, nb, slots, seqs, nseq, nlit);
+    else k_ch_parse<false><<<(nb + 3) / 4, 128, 0, st>>>(a, prev, best, first, nb, slots, seqs, nseq, nlit);
     return cudaGetLastError();
 }
 

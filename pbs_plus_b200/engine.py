@@ -355,6 +355,14 @@ class Engine:
         """Raw Deflate streams (RFC 1951) of n byte ranges (host or device base) on the GPU (pbsgpu_deflate_batch).
         more: per range, a later call continues the stream (its length a multiple of DEFLATE_SEGMENT).
         out: "host" -> list of bytes, "device" -> list of torch CUDA tensor views.  -> (streams, crc32 u32[n])"""
+        return self._deflate(self._L.pbsgpu_deflate_batch, base, off, length, more, out)
+
+    def deflate_batch_lzc(self, base, off, length, more=None, out: str = "host"):
+        """deflate_batch with a hash-chain search and lazy parse in each segment (pbsgpu_deflate_batch_lzc): smaller
+        streams, at a lower rate."""
+        return self._deflate(self._L.pbsgpu_deflate_batch_lzc, base, off, length, more, out)
+
+    def _deflate(self, fn, base, off, length, more, out):
         if out not in ("host", "device"):
             raise ValueError(f"out must be 'host' or 'device', not {out!r}")
         o, l = self._offlen(off, length)
@@ -363,9 +371,8 @@ class Engine:
         buf = self._alloc(total, out)
         olen = np.zeros(n, dtype=np.uint64)
         crc = np.zeros(n, dtype=np.uint32)
-        self._ck(self._L.pbsgpu_deflate_batch(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, n,
-                                              None if m is None else m.ctypes.data, _ptr(buf), ooff.ctypes.data,
-                                              olen.ctypes.data, crc.ctypes.data))
+        self._ck(fn(self._h, _ptr(base), o.ctypes.data, l.ctypes.data, n, None if m is None else m.ctypes.data, _ptr(buf),
+                    ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data))
         return _split(buf, ooff, olen), crc
 
     def blob_encode_batch(self, base, off, length):
@@ -726,11 +733,12 @@ class Reader(_Handle):
             bl.ctypes.data, bc.ctypes.data, k, _ptr(buf), ooff.ctypes.data, status.ctypes.data, bst.ctypes.data))
         return status, _split(buf, ooff, l, status == _lib.DEC_OK), bst
 
-    def read_deflate(self, off, length, blobs, payload: bool = False, more=None):
+    def read_deflate(self, off, length, blobs, payload: bool = False, more=None, lzc: bool = False):
         """read() whose outputs are the ranges' raw Deflate streams (pbsgpu_reader_read_deflate): the ranges are
         deflated on the device.  more: per range, a later call continues its stream (length a multiple of
-        DEFLATE_SEGMENT).  `blobs` as in read().  -> (status int32[n], streams (bytes, None where the status is not
-        DEC_OK), crc32 u32[n], blob_status int32[k])"""
+        DEFLATE_SEGMENT).  lzc: the streams of Engine.deflate_batch_lzc instead of deflate_batch.  `blobs` as in
+        read().  -> (status int32[n], streams (bytes, None where the status is not DEC_OK), crc32 u32[n],
+        blob_status int32[k])"""
         o, l = Engine._offlen(off, length)
         base, bo, bl, bc = _blob_args(blobs)
         n, k = len(o), len(bo)
@@ -741,8 +749,8 @@ class Reader(_Handle):
         status = np.zeros(n, dtype=np.int32)
         bst = np.zeros(k, dtype=np.int32)
         self._eng._ck(self._eng._L.pbsgpu_reader_read_deflate(
-            self._h, o.ctypes.data, l.ctypes.data, n, _lib.READ_PAYLOAD if payload else 0,
-            None if m is None else m.ctypes.data, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
+            self._h, o.ctypes.data, l.ctypes.data, n,
+            (_lib.READ_PAYLOAD if payload else 0) | (_lib.READ_DEFLATE_LZC if lzc else 0), None if m is None else m.ctypes.data, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
             buf.ctypes.data, ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data, status.ctypes.data, bst.ctypes.data))
         return status, _split(buf, ooff, olen, status == _lib.DEC_OK), crc, bst
 

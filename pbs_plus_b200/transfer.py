@@ -441,9 +441,10 @@ class PayloadReader:
         self._check(status, off, size, payload)
         return data
 
-    def _read_deflate(self, off: list[int], size: list[int], payload: bool, more=None):
-        """_read whose outputs are raw Deflate streams -> (streams, crc32s)."""
-        status, streams, crc, _ = self._reader.read_deflate(off, size, self._fetch(off, size, payload), payload, more)
+    def _read_deflate(self, off: list[int], size: list[int], payload: bool, more=None, lzc: bool = False):
+        """_read whose outputs are raw Deflate streams (with lzc, Engine.deflate_batch_lzc's) -> (streams, crc32s)."""
+        status, streams, crc, _ = self._reader.read_deflate(off, size, self._fetch(off, size, payload), payload, more,
+                                                            lzc)
         self._check(status, off, size, payload)
         return streams, [int(c) for c in crc]
 
@@ -481,10 +482,11 @@ class ZipWriter:
     AddFiles takes (path, st_mode, mtime, payload offset, size) tuples.  Files up to `piece_bytes` go in batches of
     about `piece_bytes` file bytes, one plan / fetch / read_deflate per batch; a larger file goes in 128 KiB-aligned
     pieces of plain ranges continued with `more`, after one plain read of its 16-byte PAYLOAD header, and its CRC-32 is
-    combined from the pieces'."""
+    combined from the pieces'.  lzc: deflate with the hash-chain parse (Engine.deflate_batch_lzc), for a smaller zip
+    at a lower rate; the default writes the greedy parse's streams."""
 
-    def __init__(self, reader: PayloadReader, w: BinaryIO, piece_bytes: int = 1 << 30):
-        self._r, self._w = reader, w
+    def __init__(self, reader: PayloadReader, w: BinaryIO, piece_bytes: int = 1 << 30, lzc: bool = False):
+        self._r, self._w, self._lzc = reader, w, lzc
         self._piece = max(_lib.DEFLATE_SEGMENT, piece_bytes // _lib.DEFLATE_SEGMENT * _lib.DEFLATE_SEGMENT)
         self._pos, self._entries = 0, []
 
@@ -526,7 +528,7 @@ class ZipWriter:
     def _flush(self, batch) -> None:
         if not batch:
             return
-        streams, crcs = self._r._read_deflate([f[3] for f in batch], [f[4] for f in batch], True)
+        streams, crcs = self._r._read_deflate([f[3] for f in batch], [f[4] for f in batch], True, None, self._lzc)
         for (path, mode, mtime, _, size), s, c in zip(batch, streams, crcs):
             self._entry(path, mode, mtime, 8, [s], c, len(s), size)
 
@@ -540,7 +542,7 @@ class ZipWriter:
         lo, crc, csize = 0, 0, 0
         while lo < size:
             n = min(self._piece, size - lo)
-            (s,), (c,) = self._r._read_deflate([payload_offset + 16 + lo], [n], False, [int(lo + n < size)])
+            (s,), (c,) = self._r._read_deflate([payload_offset + 16 + lo], [n], False, [int(lo + n < size)], self._lzc)
             crc, csize, lo = _engine.crc32_combine(crc, c, n), csize + len(s), lo + n
             self._write(s)
         e.crc, e.comp_size = crc, csize

@@ -1,12 +1,13 @@
 """The zip restore's Deflate stage and the zip restore itself, all arms in one process:
 
-  1. pbsgpu_deflate_batch on 8 GiB device-resident images (64 ranges of 128 MiB, device out): the half-zero random,
-     tests/zstd_lz_ref.text_corpus and tests/zstd_huf_ref.binary_corpus generators (a 32 MiB tile repeated; segments
-     are coded independently, so the repeat gives no cross-tile matches).  GB/s of input and output / input.
-  2. host zlib (raw Deflate) levels 1 and 6 on one core, 8 samples of 8 MiB of each image, for context only.
+  1. pbsgpu_deflate_batch and pbsgpu_deflate_batch_lzc on 8 GiB device-resident images (64 ranges of 128 MiB, device
+     out): the half-zero random, tests/zstd_lz_ref.text_corpus and tests/zstd_huf_ref.binary_corpus generators (a
+     32 MiB tile repeated; segments are coded independently, so the repeat gives no cross-tile matches).  GB/s of
+     input and output / input.
+  2. host zlib (raw Deflate) levels 1, 4 and 6 on one core, 8 samples of 8 MiB of each image, for context only.
   3. a zip restore of an 8 GiB _lzh payload archive (text-like, then half-zero, files of 4 KiB to 8 MiB, as
-     tools/read_bench.py builds it) through transfer.ZipWriter into a byte-counting sink, against
-     PayloadReader.ReadFileContents of the same files in the same run.  GB/s of file bytes.
+     tools/read_bench.py builds it) through transfer.ZipWriter, default and lzc=True, into a byte-counting sink,
+     against PayloadReader.ReadFileContents of the same files in the same run.  GB/s of file bytes.
 
 Prints the card and its power limit, then one JSON line.
 
@@ -59,20 +60,22 @@ for kind in ("half_zero_random", "text", "binary"):
     out = torch.empty(int(bound.sum()), dtype=torch.uint8, device="cuda")
     olen = np.zeros(len(off), np.uint64)
     crc = np.zeros(len(off), np.uint32)
-    best = None
-    for _ in range(3):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        e._ck(e._L.pbsgpu_deflate_batch(e._h, a.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), None,
-                                        out.data_ptr(), ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data))
-        dt = time.perf_counter() - t0
-        best = dt if best is None else min(best, dt)
-    s0 = out[:int(olen[0])].cpu().numpy().tobytes()
-    assert zlib.decompress(s0, -15) == a[:RANGE].cpu().numpy().tobytes(), kind
-    ratio = float(olen.sum()) / n
+    gpu = {}
+    for arm in ("deflate_batch", "deflate_batch_lzc"):
+        best = None
+        for _ in range(3):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            e._ck(getattr(e._L, "pbsgpu_" + arm)(e._h, a.data_ptr(), off.ctypes.data, ln.ctypes.data, len(off), None,
+                                                 out.data_ptr(), ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data))
+            dt = time.perf_counter() - t0
+            best = dt if best is None else min(best, dt)
+        s0 = out[:int(olen[0])].cpu().numpy().tobytes()
+        assert zlib.decompress(s0, -15) == a[:RANGE].cpu().numpy().tobytes(), (kind, arm)
+        gpu[arm] = (n / best / 1e9, float(olen.sum()) / n)
     h = a[:64 << 20].cpu().numpy()
     host = {}
-    for lvl in (1, 6):
+    for lvl in (1, 4, 6):
         t0 = time.perf_counter()
         outb = 0
         for k in range(8):
@@ -80,10 +83,12 @@ for kind in ("half_zero_random", "text", "binary"):
             outb += len(c.compress(h[k << 23:(k + 1) << 23].tobytes()) + c.flush())
         dt = time.perf_counter() - t0
         host[f"zlib{lvl}"] = {"GBps": (64 << 20) / dt / 1e9, "ratio": outb / (64 << 20)}
-    result[kind] = {"deflate_batch_GBps": n / best / 1e9, "ratio": ratio, "host_one_core": host}
-    print(f"{kind:16s} deflate_batch {n / best / 1e9:7.2f} GB/s, out/in {ratio:.4f}; host zlib-1 "
-          f"{host['zlib1']['GBps']:.3f} GB/s ({host['zlib1']['ratio']:.4f}), zlib-6 {host['zlib6']['GBps']:.3f} GB/s "
-          f"({host['zlib6']['ratio']:.4f})")
+    result[kind] = {"deflate_batch_GBps": gpu["deflate_batch"][0], "ratio": gpu["deflate_batch"][1],
+                    "deflate_batch_lzc_GBps": gpu["deflate_batch_lzc"][0], "ratio_lzc": gpu["deflate_batch_lzc"][1],
+                    "host_one_core": host}
+    print(f"{kind:16s} " + ", ".join(f"{arm} {g:7.2f} GB/s, out/in {r:.4f}" for arm, (g, r) in gpu.items()) + "; host "
+          + ", ".join(f"zlib-{lvl} {host[f'zlib{lvl}']['GBps']:.3f} GB/s ({host[f'zlib{lvl}']['ratio']:.4f})"
+                      for lvl in (1, 4, 6)))
     del a, out
     torch.cuda.empty_cache()
 
@@ -149,11 +154,11 @@ class Count(io.RawIOBase):
         return len(b)
 
 
-def zip_restore():
+def zip_restore(lzc=False):
     sink = Count()
     t0 = time.perf_counter()
     with transfer.PayloadReader(e, didx, src, cache_bytes=CACHE) as r:
-        z = transfer.ZipWriter(r, sink)
+        z = transfer.ZipWriter(r, sink, lzc=lzc)
         z.AddFiles(files)
         z.Close()
     return time.perf_counter() - t0, sink.n
@@ -174,9 +179,11 @@ def read_files():
 
 
 tz, zbytes = min(zip_restore() for _ in range(2))
+tc, cbytes = min(zip_restore(True) for _ in range(2))
 tr = min(read_files() for _ in range(2))
 result["zip_restore"] = {"files": len(files), "file_bytes": fbytes, "zip_bytes": zbytes, "zip_GBps": fbytes / tz / 1e9,
-                         "read_files_GBps": fbytes / tr / 1e9}
+                         "zip_bytes_lzc": cbytes, "zip_lzc_GBps": fbytes / tc / 1e9, "read_files_GBps": fbytes / tr / 1e9}
 print(f"zip restore: {len(files)} files, {fbytes / 2**30:.2f} GiB -> zip {zbytes / fbytes:.4f} of the file bytes: "
-      f"ZipWriter {fbytes / tz / 1e9:.2f} GB/s, ReadFileContents {fbytes / tr / 1e9:.2f} GB/s")
+      f"ZipWriter {fbytes / tz / 1e9:.2f} GB/s; lzc=True {cbytes / fbytes:.4f} at {fbytes / tc / 1e9:.2f} GB/s; "
+      f"ReadFileContents {fbytes / tr / 1e9:.2f} GB/s")
 print(json.dumps(result))
