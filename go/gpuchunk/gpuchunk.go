@@ -31,6 +31,7 @@ import (
 	"fmt"
 	"hash/crc32"
 	"io"
+	"os"
 	"runtime"
 	"strings"
 	"unsafe"
@@ -943,7 +944,7 @@ func (p *PayloadReader) fetch(off, length []uint64, flags C.uint32_t) (blobs []b
 		return
 	}
 	need = need[:k]
-	if k > 0 {
+	if k > 0 && flags&C.PBSGPU_READ_SPARSE == 0 { // a sparse restore must not fetch the zero chunks after its range
 		for c := need[k-1] + 1; c < uint64(len(p.digests)) && c <= need[k-1]+uint64(p.Prefetch); c++ {
 			need = append(need, c)
 		}
@@ -1269,6 +1270,65 @@ func (e *Engine) NewImageReader(fidx []byte, c *Crypt, cacheBytes uint64, source
 		copy(dg[i][:], fidx[4096+32*i:4096+32*i+32])
 	}
 	return &PayloadReader{e: e, r: r, source: source, digests: dg, size: uint64(C.pbsgpu_reader_size(r))}, nil
+}
+
+// RestoreImage writes the whole image of an image reader (NewImageReader) to f, sparsely
+// (pbsgpu_reader_read_sparse): per slice of sliceBytes (0 = 1 GiB), one plan that leaves out the zero chunks, one fetch
+// of the named blobs, one read that returns only the data extents, and a WriteAt of each; then f.Truncate to the image's
+// size.  Zero chunks are never fetched or decoded and no all-zero 4 KiB block is written, so f must read as zeros where
+// nothing is written: a new file (which stays thin) or a device the caller zeroed, as upstream's skip-zero restore.
+func (p *PayloadReader) RestoreImage(f *os.File, sliceBytes uint64) error {
+	if sliceBytes == 0 {
+		sliceBytes = 1 << 30
+	}
+	if sliceBytes > p.size {
+		sliceBytes = p.size
+	}
+	out := make([]byte, sliceBytes+1) // the packed data of one slice, reused by every slice (+1: never empty)
+	for off := uint64(0); off < p.size; off += sliceBytes {
+		n := p.size - off
+		if n > sliceBytes {
+			n = sliceBytes
+		}
+		o, l := []uint64{off}, []uint64{n}
+		blobs, bo, bl, need, err := p.fetch(o, l, C.PBSGPU_READ_SPARSE)
+		if err != nil {
+			return err
+		}
+		parts := (off+n-1)/4096 - off/4096 + 1
+		extCap := (parts + 1) / 2
+		ext := make([]uint64, 2*extCap)
+		extFirst := make([]uint64, 2)
+		outOff := []uint64{0}
+		status := make([]int32, 1)
+		blobStatus := make([]int32, len(need))
+		rc := C.pbsgpu_reader_read_sparse(p.r, (*C.uint64_t)(unsafe.Pointer(&o[0])), (*C.uint64_t)(unsafe.Pointer(&l[0])), 1, 0,
+			unsafe.Pointer(&blobs[0]), (*C.uint64_t)(unsafe.Pointer(&bo[0])), (*C.uint64_t)(unsafe.Pointer(&bl[0])),
+			(*C.uint64_t)(unsafe.Pointer(&need[0])), C.uint32_t(len(need)-1), (*C.uint8_t)(unsafe.Pointer(&out[0])),
+			(*C.uint64_t)(unsafe.Pointer(&outOff[0])), (*C.uint64_t)(unsafe.Pointer(&ext[0])), C.uint64_t(extCap),
+			(*C.uint64_t)(unsafe.Pointer(&extFirst[0])), (*C.int32_t)(unsafe.Pointer(&status[0])),
+			(*C.int32_t)(unsafe.Pointer(&blobStatus[0])))
+		if err := p.e.err(rc); err != nil {
+			return err
+		}
+		if status[0] != int32(C.PBSGPU_DEC_OK) {
+			for j, s := range blobStatus[:len(need)-1] {
+				if s != int32(C.PBSGPU_DEC_OK) {
+					return fmt.Errorf("pbsgpu: image chunk %d (%x): status %d", need[j], p.digests[need[j]], s)
+				}
+			}
+			return fmt.Errorf("pbsgpu: image slice at %d: status %d", off, status[0])
+		}
+		var at uint64
+		for e := extFirst[0]; e < extFirst[1]; e++ {
+			eo, el := ext[2*e], ext[2*e+1]
+			if _, err := f.WriteAt(out[at:at+el], int64(eo)); err != nil {
+				return err
+			}
+			at += el
+		}
+	}
+	return f.Truncate(int64(p.size))
 }
 
 // ZipWriter writes one <name>.zip of a restore (the replacement for zip.NewWriter + io.Copy(rangeReader) in

@@ -505,6 +505,7 @@ void pbsgpu_reader_close(pbsgpu_reader *r);
 uint64_t pbsgpu_reader_size(const pbsgpu_reader *r);
 #define PBSGPU_READ_PAYLOAD 1u
 #define PBSGPU_READ_DEFLATE_LZC 2u   /* pbsgpu_reader_read_deflate only: deflate as pbsgpu_deflate_batch_lzc */
+#define PBSGPU_READ_SPARSE 4u        /* pbsgpu_reader_plan of a .fidx reader only: leave out zero chunks */
 int pbsgpu_reader_plan(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
                        uint64_t *chunk, uint8_t *digest, uint64_t cap, uint64_t *n_out);
 int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
@@ -513,6 +514,42 @@ int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const uint64_t *le
                        uint8_t *out, const uint64_t *out_off, int32_t *status, int32_t *blob_status);
 enum { PBSGPU_DEC_MISSING = PBSGPU_DEC_BAD_TAG + 1,   /* 9: a chunk the range needs was neither cached nor given */
        PBSGPU_DEC_BAD_HEADER };                        /* 10: READ_PAYLOAD and the 16-byte header does not match */
+
+/* ---- f3, read side: sparse image restore ----------------------------------------------------------------------------
+ * A thin-provisioned disk image is mostly zeros.  The sparse restore serves its zero chunks without their blobs and
+ * hands back only the data bytes of each range with where they go, so a restore into a zero-initialised target (a new
+ * file, or a device the caller zeroed, as upstream's skip-zero restore) writes only the data and keeps the image thin.
+ * Zero chunk: chunk i of a .fidx reader is a zero chunk when its index digest equals the digest of clen[i] zero bytes:
+ * plain SHA-256, or with the reader's crypt the keyed SHA-256(zeros || id_key).  Those digests (chunk_size and the short
+ * last chunk) are computed on the GPU on the reader's first sparse call, not at open.  A zero chunk whose start and end
+ * lie on 4 KiB block boundaries (or end at the image's end) -- every zero chunk when chunk_size is a multiple of 4096, as
+ * upstream's 4 MiB -- is served by its digest: no blob, no decode, no cache slot.  Any other zero chunk shares a block
+ * with its neighbours and is read like a data chunk (planned, given, decoded and scanned).  This trusts the index digest, as dedup does (the index checksum was
+ * verified at open); a damaged zero-chunk blob in the store is not noticed here -- checking blobs is
+ * pbsgpu_blob_decode_batch's job.
+ * Holes: image offsets are cut into 4096-byte blocks aligned to the image (block b is [4096 b, 4096 (b + 1))), not to
+ * the range.  Within range i, a block's part inside the range is a hole when all of its bytes are zero.  The data
+ * extents of the range are the maximal runs of non-hole block parts, as (image offset, length) pairs, ascending.  They
+ * depend only on the image bytes and the range: the zero-chunk rule only saves work.
+ * pbsgpu_reader_plan with PBSGPU_READ_SPARSE (a .fidx reader only; EINVAL otherwise) leaves out zero chunks; without
+ * the flag it is unchanged and names them.  "Zero chunks" below are the ones served by digest.  pbsgpu_reader_read and _read_deflate refuse the flag with EINVAL.
+ * pbsgpu_reader_read_sparse: pbsgpu_reader_read's arguments, blob handling, groups, statuses and argument errors, with
+ * these differences:
+ *  - a .fidx reader only, and flags 0: a .didx reader, or PBSGPU_READ_PAYLOAD, is EINVAL;
+ *  - out is HOST memory (a device out is EINVAL) with len[i] bytes reserved at out + out_off[i]; it receives range i's
+ *    data bytes packed, in extent order.  No hole byte is copied from the device;
+ *  - ext receives (offset, length) u64 pairs, range i's at ext[2 ext_first[i] ..  2 ext_first[i + 1]) (ext_first has
+ *    n + 1 entries).  ext_cap (pairs) must be at least sum ceil(B_i / 2), with B_i the number of 4 KiB blocks range i
+ *    touches -- the most extents a range can have -- or the call is EINVAL before any work;
+ *  - a range whose status is not OK has no extents, and none of its out bytes are written;
+ *  - a blob given for a zero chunk is checked and cached like any other, and its blob_status reported; the range's
+ *    output does not depend on it.  A range that touches only zero chunks needs no blob and reads no byte of the cache.
+ * The data chunks are read into a device stage of their bytes in the call, K17 maps their all-zero block parts there
+ * and K14 copies the data extents out. */
+int pbsgpu_reader_read_sparse(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
+                              const void *blob_base, const uint64_t *blob_off, const uint64_t *blob_len,
+                              const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out, const uint64_t *out_off,
+                              uint64_t *ext, uint64_t ext_cap, uint64_t *ext_first, int32_t *status, int32_t *blob_status);
 
 /* ---- f3, read side: zip restore ------------------------------------------------------------------------------------
  * Restore as zip (reference internal/pxar/zip.go, RestoreModeZip): files are compressed on the GPU into raw Deflate

@@ -45,6 +45,8 @@ DEC_BAD_TAG = 8   # pbsgpu_blob_decode_batch_enc only: the AES-256-GCM tag did n
 DEC_MISSING, DEC_BAD_HEADER = 9, 10
 READ_PAYLOAD = 1   # pbsgpu_reader_plan / _read flags: ranges are (payload offset, file size)
 READ_DEFLATE_LZC = 2   # pbsgpu_reader_read_deflate only: the streams are pbsgpu_deflate_batch_lzc's
+READ_SPARSE = 4   # pbsgpu_reader_plan of a .fidx reader only: zero chunks are left out
+SPARSE_BLOCK = 4096   # pbsgpu_reader_read_sparse: holes are image-aligned blocks of this size, or their parts in a range
 
 
 class DevInfo(C.Structure):
@@ -183,6 +185,8 @@ _SIGNATURES = {
     "pbsgpu_crc32_combine": ([C.c_uint32, C.c_uint32, C.c_uint64], C.c_uint32),
     "pbsgpu_reader_read_deflate": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
                                    _vp, _vp],
+    "pbsgpu_reader_read_sparse": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp,
+                                  C.c_uint64, _vp, _vp, _vp],
     "pbsgpu_zip_local_header": ([C.POINTER(ZipEntry), _vp, C.c_uint64], C.c_uint64),
     "pbsgpu_zip_data_descriptor": ([C.POINTER(ZipEntry), _vp, C.c_uint64], C.c_uint64),
     "pbsgpu_zip_directory": ([_vp, C.c_uint64, C.c_uint64, _vp, C.c_uint64], C.c_uint64),

@@ -18,7 +18,8 @@ OBJ = HERE / "_obj"
 LIB = HERE / "libpbsgpu.so"
 SOURCES = ["scan.cu", "resolve.cu", "sha256.cu", "digestset.cu", "crc32.cu", "xxh3.cu", "corpus.cu", "capi.cu", "capi_set.cu",
            "capi_stream.cu", "capi_aux.cu", "capi_blob.cu", "capi_crypt.cu", "zframe.cu", "zlz.cu", "zent.cu", "aesgcm.cu",
-           "zldm.cu", "zchain.cu", "zdec.cu", "reader.cu", "capi_read.cu", "deflate.cu", "capi_zip.cu"]
+           "zldm.cu", "zchain.cu", "zdec.cu", "reader.cu", "capi_read.cu", "deflate.cu", "capi_zip.cu",
+           "zeromap.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [

@@ -32,6 +32,10 @@ struct pbsgpu_reader {
     std::deque<Slot> ring;
     std::unordered_map<uint64_t, Held> held;
     bool image = false;   // over a fixed index: no pxar headers, PBSGPU_READ_PAYLOAD is refused
+    // sparse calls of an image: the digests of clen zero bytes for the (at most two) chunk lengths, computed on first use
+    bool zero_known = false;
+    uint64_t zero_len[2] = {0, 0};
+    uint8_t zero_dig[2][32];
 };
 
 static uint64_t slot_bytes(uint64_t len) { return std::max<uint64_t>(256, (len + 255) & ~255ull); }
@@ -141,6 +145,31 @@ template <typename F> static void for_pieces(const pbsgpu_reader *r, uint64_t lo
     }
 }
 
+// The digests of clen zero bytes for the image's two chunk lengths (chunk_size and the last chunk's), plain or keyed with
+// the reader's crypt as the index's digests are: K3 through the SHA-256 batch calls, once per reader.
+static int zero_digests(pbsgpu_reader *r) {
+    if (r->zero_known || r->ends.empty()) return PBSGPU_OK;
+    r->zero_len[0] = r->clen.front();   // the longest: every chunk but the last is chunk_size
+    r->zero_len[1] = r->clen.back();
+    const std::vector<uint8_t> zeros(r->zero_len[0]);
+    const uint64_t at[2] = {0, 0};
+    if (int rc = r->crypt ? pbsgpu_sha256_keyed_batch(r->ctx, r->crypt, zeros.data(), at, r->zero_len, 2, r->zero_dig[0])
+                          : pbsgpu_sha256_batch(r->ctx, zeros.data(), at, r->zero_len, 2, r->zero_dig[0]))
+        return rc;
+    r->zero_known = true;
+    return PBSGPU_OK;
+}
+// chunk c is served by its digest in a sparse call (after zero_digests): a zero chunk -- its index digest is the digest
+// of clen[c] zero bytes -- whose start and end lie on 4 KiB block boundaries (the end may be the image's end), so no
+// block part holds both its zeros and another chunk's bytes.  A zero chunk that cuts a block (a chunk size that is not
+// a multiple of 4096) is read like a data chunk: skipping it would split that block's data between two runs.
+static bool zero_chunk(const pbsgpu_reader *r, uint64_t c) {
+    const uint64_t start = r->ends[c] - r->clen[c];
+    if (start % ZERO_BLOCK || (r->ends[c] % ZERO_BLOCK && r->ends[c] != r->ends.back())) return false;
+    const int k = r->clen[c] == r->zero_len[0] ? 0 : r->clen[c] == r->zero_len[1] ? 1 : -1;
+    return k >= 0 && memcmp(r->digests.data() + 32 * c, r->zero_dig[k], 32) == 0;
+}
+
 // The arguments every call checks: flags, and every range (with its PAYLOAD header) inside the archive.
 static int check_ranges(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags) {
     if (flags & ~PBSGPU_READ_PAYLOAD) return fail(r->ctx, PBSGPU_EINVAL, "unknown read flags 0x%x", flags);
@@ -156,12 +185,17 @@ extern "C" int pbsgpu_reader_plan(pbsgpu_reader *r, const uint64_t *off, const u
                                   uint64_t *chunk, uint8_t *digest, uint64_t cap, uint64_t *n_out) {
     if (!r || !n_out || (n && (!off || !len)) || (cap && !chunk)) return PBSGPU_EINVAL;
     Guard g(r->ctx);
+    const bool sparse = flags & PBSGPU_READ_SPARSE;   // plan's flag alone: check_ranges refuses it for the reads
+    flags &= ~PBSGPU_READ_SPARSE;
+    if (sparse && !r->image) return fail(r->ctx, PBSGPU_EINVAL, "PBSGPU_READ_SPARSE needs a .fidx reader");
     if (int rc = check_ranges(r, off, len, n, flags)) return rc;
+    if (sparse)
+        if (int rc = zero_digests(r)) return rc;
     const uint64_t hs = flags & PBSGPU_READ_PAYLOAD ? 16 : 0;
     std::vector<uint64_t> need;
     for (uint32_t i = 0; i < n; i++)
         for_pieces(r, off[i], off[i] + hs + len[i], [&](uint64_t c, uint64_t, uint64_t, uint64_t) {
-            if (!r->held.count(c)) need.push_back(c);
+            if (!r->held.count(c) && !(sparse && zero_chunk(r, c))) need.push_back(c);
         });
     std::sort(need.begin(), need.end());
     need.erase(std::unique(need.begin(), need.end()), need.end());
@@ -208,7 +242,7 @@ struct Gather {
         pieces.clear(); runs.clear(); stage_used = 0;
         return b.finish("reader gather");
     }
-    int add(const RawPiece &q, uint64_t slot) {
+    int add(const RawPiece &q, const uint8_t *src) {   // src: the chunk's cache slot (or the stage q.coff is into)
         uint64_t done = 0;
         while (done < q.len) {
             if (pieces.size() == READER_PIECE_BATCH || (!q.hdr && !out_dev && stage_used == stage_cap))
@@ -225,7 +259,7 @@ struct Gather {
                     runs.push_back({stage_used, q.dst + done, take});
                 stage_used += take;
             }
-            pieces.push_back({(uint64_t)(uintptr_t)r->cache + slot + q.coff + done, dst, take});
+            pieces.push_back({(uint64_t)(uintptr_t)src + q.coff + done, dst, take});
             done += take;
         }
         return PBSGPU_OK;
@@ -285,7 +319,7 @@ extern "C" int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const u
     // 2. the pieces of chunks that were cached, before any decode can overwrite them
     for (const RawPiece &q : raw)
         if (q.cached)
-            if (int rc = ga.add(q, r->held[q.chunk].off)) return rc;
+            if (int rc = ga.add(q, r->cache + r->held[q.chunk].off)) return rc;
     if (int rc = ga.flush()) return rc;
     // 3. the blobs, in groups whose slots do not overwrite each other; each group's pieces are copied right after it
     std::vector<int32_t> bst(n_blobs, PBSGPU_DEC_OK);
@@ -318,7 +352,7 @@ extern "C" int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const u
         }
         std::sort(mine.begin(), mine.end());   // range order: runs of a host `out` coalesce
         for (uint64_t k : mine)
-            if (int rc = ga.add(raw[k], slot[given[raw[k].chunk]])) return rc;
+            if (int rc = ga.add(raw[k], r->cache + slot[given[raw[k].chunk]])) return rc;
         return ga.flush();
     };
     uint32_t j0 = 0;
@@ -408,4 +442,136 @@ extern "C" int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off,
         if (crc_out) crc_out[idx[j]] = kcrc[j];
     }
     return PBSGPU_OK;
+}
+
+// The sparse image restore's read: the ranges' data chunks (every chunk but the zero chunks) go through
+// pbsgpu_reader_read into a device stage owned by this call, K17 maps their 4 KiB block parts that are all zero, and K14
+// copies only the data extents of the ranges whose status is OK to the caller's host memory, packed.  Zero chunks
+// (zero_chunk) are neither fetched, decoded, cached nor scanned: their block parts are holes by construction.
+extern "C" int pbsgpu_reader_read_sparse(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags,
+                                         const void *blob_base, const uint64_t *blob_off, const uint64_t *blob_len,
+                                         const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out, const uint64_t *out_off,
+                                         uint64_t *ext, uint64_t ext_cap, uint64_t *ext_first, int32_t *status,
+                                         int32_t *blob_status) {
+    if (!r || (n && (!off || !len || !out || !out_off || !ext_first || !status)) || (ext_cap && !ext) ||
+        (n_blobs && (!blob_base || !blob_off || !blob_len || !blob_chunk)))
+        return PBSGPU_EINVAL;
+    pbsgpu_ctx *ctx = r->ctx;
+    Guard g(ctx);
+    if (!r->image) return fail(ctx, PBSGPU_EINVAL, "read_sparse: a .didx reader has no sparse read");
+    if (int rc = check_ranges(r, off, len, n, flags)) return rc;
+    if (n && pbsgpu_is_device_ptr(out)) return fail(ctx, PBSGPU_EINVAL, "read_sparse: out must be host memory");
+    // bit0[i]: the bit of range i's first block part; a range of B block parts has at most ceil(B / 2) extents
+    std::vector<uint64_t> bit0(n + 1, 0);
+    uint64_t bound = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t parts = len[i] ? (off[i] + len[i] - 1) / ZERO_BLOCK - off[i] / ZERO_BLOCK + 1 : 0;
+        bit0[i + 1] = bit0[i] + parts;
+        bound += (parts + 1) / 2;
+    }
+    if (ext_cap < bound)
+        return fail(ctx, PBSGPU_EINVAL, "read_sparse: ext_cap %llu < %llu, the most extents the ranges can have",
+                    (unsigned long long)ext_cap, (unsigned long long)bound);
+    if (int rc = zero_digests(r)) return rc;
+    // the data runs: maximal runs of data chunks within a range, staged at offsets congruent to their image offsets
+    // mod 16 so K17's vector loads are aligned on whole blocks
+    struct Run { uint64_t off, len, soff; uint32_t range; };
+    std::vector<Run> runs;
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n; i++)
+        for_pieces(r, off[i], off[i] + len[i], [&](uint64_t c, uint64_t, uint64_t l, uint64_t at) {
+            if (zero_chunk(r, c)) return;
+            const uint64_t a = off[i] + at;
+            if (!runs.empty() && runs.back().range == i && runs.back().off + runs.back().len == a) {
+                runs.back().len += l;
+            } else {
+                total += (a - total) & 15;
+                runs.push_back({a, l, total, i});
+            }
+            total += l;
+        });
+    if (runs.size() > UINT32_MAX) return fail(ctx, PBSGPU_EINVAL, "read_sparse: more than 2^32 - 1 data runs");
+    const uint32_t nr = (uint32_t)runs.size();
+    Blocking b(ctx, ctx->streams[0]);
+    uint8_t *dstage = nr ? b.get<uint8_t>(total + 16) : nullptr;
+    if (nr && !dstage) return fail(ctx, PBSGPU_ENOMEM, "read_sparse: device stage of %llu bytes failed", (unsigned long long)total);
+    std::vector<uint64_t> ro(nr), rl(nr), rs(nr);
+    std::vector<int32_t> rst(nr);
+    for (uint32_t k = 0; k < nr; k++) { ro[k] = runs[k].off; rl[k] = runs[k].len; rs[k] = runs[k].soff; }
+    if (int rc = pbsgpu_reader_read(r, ro.data(), rl.data(), nr, 0, blob_base, blob_off, blob_len, blob_chunk, n_blobs,
+                                    dstage, rs.data(), rst.data(), blob_status))
+        return rc;
+    // a range's status: its first failing data run's (runs are in range order, then chunk order)
+    for (uint32_t i = 0; i < n; i++) status[i] = PBSGPU_DEC_OK;
+    for (uint32_t k = 0; k < nr; k++)
+        if (status[runs[k].range] == PBSGPU_DEC_OK) status[runs[k].range] = rst[k];
+    // K17 over the runs of the ranges that are OK
+    std::vector<ZeroRun> zr;
+    std::vector<uint64_t> part_first(1, 0);
+    for (const Run &u : runs) {
+        if (status[u.range] != PBSGPU_DEC_OK) continue;
+        const uint64_t b0 = u.off / ZERO_BLOCK, b1 = (u.off + u.len - 1) / ZERO_BLOCK;
+        zr.push_back({(uint64_t)(uintptr_t)dstage + u.soff, u.off, u.len, bit0[u.range] + b0 - off[u.range] / ZERO_BLOCK});
+        part_first.push_back(part_first.back() + b1 - b0 + 1);
+    }
+    std::vector<uint32_t> bits;
+    if (!zr.empty()) {
+        const uint64_t words = (bit0[n] + 31) / 32;
+        bits.resize(words);
+        uint32_t *d_bits = b.get<uint32_t>(words);
+        const ZeroRun *d_runs = b.upload(zr.data(), zr.size());
+        const uint64_t *d_first = b.upload(part_first.data(), part_first.size());
+        if (!d_bits || !d_runs || !d_first) return fail(ctx, PBSGPU_ENOMEM, "read_sparse: zero map buffers failed");
+        if (b.ok()) b.e = cudaMemsetAsync(d_bits, 0xff, words * 4, b.st);
+        if (b.ok()) b.e = launch_zero_map(d_runs, d_first, (uint32_t)zr.size(), part_first.back(), d_bits, ctx->sm_count, b.st);
+        if (b.ok()) b.e = cudaMemcpyAsync(bits.data(), d_bits, words * 4, cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("read_sparse zero map")) return rc;
+    }
+    // the extents: maximal runs of non-hole block parts.  Two runs of a range are apart by at least one zero chunk whose
+    // bounds are block boundaries (zero_chunk), so no block part spans two runs, an extent lies in one run, its dstage
+    // bytes are contiguous, and a range has at most ceil(B / 2) extents.
+    std::vector<uint64_t> esrc;   // per extent: its offset in dstage
+    uint64_t ne = 0, host_bytes = 0;
+    if (n) ext_first[0] = 0;
+    for (uint32_t i = 0, k = 0; i < n; i++) {
+        const uint64_t e0 = ne;
+        for (; k < nr && runs[k].range == i; k++) {
+            const Run &u = runs[k];
+            if (status[i] != PBSGPU_DEC_OK) continue;
+            const uint64_t b0 = u.off / ZERO_BLOCK, b1 = (u.off + u.len - 1) / ZERO_BLOCK;
+            for (uint64_t blk = b0; blk <= b1; blk++) {
+                const uint64_t bit = bit0[i] + blk - off[i] / ZERO_BLOCK;
+                if (bits[bit >> 5] >> (bit & 31) & 1) continue;   // a hole
+                const uint64_t lo = std::max(u.off, blk * ZERO_BLOCK), hi = std::min(u.off + u.len, (blk + 1) * ZERO_BLOCK);
+                if (ne > e0 && ext[2 * ne - 2] + ext[2 * ne - 1] == lo) {
+                    ext[2 * ne - 1] += hi - lo;
+                } else {
+                    ext[2 * ne] = lo; ext[2 * ne + 1] = hi - lo;
+                    esrc.push_back(u.soff + (lo - u.off));
+                    ne++;
+                }
+                host_bytes += hi - lo;
+            }
+        }
+        ext_first[i + 1] = ne;
+    }
+    if (ne == 0) return PBSGPU_OK;
+    // K14: the data extents, packed per range, through the host-out staging buffer
+    Gather ga{b, r, out, nullptr};
+    ga.out_dev = false;
+    const uint32_t pcap = (uint32_t)std::min<uint64_t>(ne + 1, READER_PIECE_BATCH) * 2;   // a split piece adds one
+    ga.d_pieces = b.get<ReadPiece>(pcap);
+    ga.d_first = b.get<uint64_t>(pcap + 1);
+    ga.pieces.reserve(pcap);
+    ga.stage_cap = std::min(host_bytes, READER_STAGE_MAX);
+    ga.stage = b.get<uint8_t>(ga.stage_cap);
+    if (!ga.d_pieces || !ga.d_first || !ga.stage) return fail(ctx, PBSGPU_ENOMEM, "read_sparse gather buffers failed");
+    for (uint32_t i = 0; i < n; i++) {
+        uint64_t packed = 0;
+        for (uint64_t e = ext_first[i]; e < ext_first[i + 1]; e++) {
+            if (int rc = ga.add({0, esrc[e], ext[2 * e + 1], out_off[i] + packed, i, false, false}, dstage)) return rc;
+            packed += ext[2 * e + 1];
+        }
+    }
+    return ga.flush();
 }

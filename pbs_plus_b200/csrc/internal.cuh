@@ -209,6 +209,15 @@ struct ReadPiece { uint64_t src, dst, len; };   // device addresses: len bytes f
 cudaError_t launch_read_gather(const ReadPiece *pieces, const uint64_t *tile_first, uint32_t n, uint64_t total_tiles,
                                int sm_count, cudaStream_t st);
 
+// ---- zero-block map of the sparse image restore (K17, zeromap.cu) ----------------------------------------------------
+constexpr uint64_t ZERO_BLOCK = 4096;   // holes are whole image-aligned blocks of this size, or their parts in a range
+// a staged run: image bytes [off, off + len) at device address src; bit: the bit of its first block part
+struct ZeroRun { uint64_t src, off, len, bit; };
+// part_first[n+1]: prefix of the runs' block-part counts.  bits (device, preset to all ones): the bit of every block
+// part with a non-zero byte is cleared.
+cudaError_t launch_zero_map(const ZeroRun *runs, const uint64_t *part_first, uint32_t n, uint64_t total_parts,
+                            uint32_t *bits, int sm_count, cudaStream_t st);
+
 // ---- corpus (K5) ------------------------------------------------------------------
 cudaError_t launch_corpus_fill(const pbsgpu_corpus &c, uint64_t first_file, uint32_t n_files, uint8_t *dst,
                                uint64_t stride, cudaStream_t st);

@@ -697,11 +697,12 @@ class Reader(_Handle):
         """The archive's length (the index's last end offset)."""
         return int(self._eng._L.pbsgpu_reader_size(self._h))
 
-    def plan(self, off, length, payload: bool = False):
+    def plan(self, off, length, payload: bool = False, sparse: bool = False):
         """The chunks the ranges touch that the cache does not hold -> (chunk indices u64[k] ascending, digests
-        u8[k, 32]).  payload: the ranges are (payload offset, file size) of files, their 16-byte headers included."""
+        u8[k, 32]).  payload: the ranges are (payload offset, file size) of files, their 16-byte headers included.
+        sparse (a .fidx reader only): leave out the zero chunks, which read_sparse serves without a blob."""
         o, l = Engine._offlen(off, length)
-        flags = _lib.READ_PAYLOAD if payload else 0
+        flags = (_lib.READ_PAYLOAD if payload else 0) | (_lib.READ_SPARSE if sparse else 0)
         n = C.c_uint64()
         rc = self._eng._L.pbsgpu_reader_plan(self._h, o.ctypes.data, l.ctypes.data, len(o), flags, None, None, 0, C.byref(n))
         if rc != _lib.ERANGE:
@@ -753,6 +754,37 @@ class Reader(_Handle):
             (_lib.READ_PAYLOAD if payload else 0) | (_lib.READ_DEFLATE_LZC if lzc else 0), None if m is None else m.ctypes.data, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
             buf.ctypes.data, ooff.ctypes.data, olen.ctypes.data, crc.ctypes.data, status.ctypes.data, bst.ctypes.data))
         return status, _split(buf, ooff, olen, status == _lib.DEC_OK), crc, bst
+
+
+    def read_sparse(self, off, length, blobs):
+        """Read ranges of a disk image sparsely (pbsgpu_reader_read_sparse): zero chunks need no blob, and per range
+        only the data extents -- the maximal runs of 4 KiB image-aligned block parts that are not all zero -- come
+        back.  `blobs` as in read().  -> (status int32[n], per range (extents [(image offset, length)], packed data
+        bytes) or None where the status is not DEC_OK, blob_status int32[k])"""
+        o, l = Engine._offlen(off, length)
+        base, bo, bl, bc = _blob_args(blobs)
+        n, k = len(o), len(bo)
+        ooff, total = _offsets(l)
+        buf = self._eng._alloc(total, "host")
+        bs = _lib.SPARSE_BLOCK
+        parts = [(int(a) + int(b) - 1) // bs - int(a) // bs + 1 if b else 0 for a, b in zip(o, l)]
+        cap = sum((p + 1) // 2 for p in parts)
+        ext = np.zeros((max(1, cap), 2), dtype=np.uint64)
+        first = np.zeros(n + 1, dtype=np.uint64)
+        status = np.zeros(n, dtype=np.int32)
+        bst = np.zeros(k, dtype=np.int32)
+        self._eng._ck(self._eng._L.pbsgpu_reader_read_sparse(
+            self._h, o.ctypes.data, l.ctypes.data, n, 0, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
+            buf.ctypes.data, ooff.ctypes.data, ext.ctypes.data, cap, first.ctypes.data, status.ctypes.data,
+            bst.ctypes.data))
+        data = []
+        for i in range(n):
+            if status[i] != _lib.DEC_OK:
+                data.append(None)
+                continue
+            e = [(int(a), int(b)) for a, b in ext[int(first[i]): int(first[i + 1])]]
+            data.append((e, buf[int(ooff[i]): int(ooff[i]) + sum(b for _, b in e)].tobytes()))
+        return status, data, bst
 
 
 class DigestSet(_Handle):

@@ -24,7 +24,8 @@ Two writers:
   * DedupWriter -- per-file batching (every file its own stream).  Faster for many small files, but its index does NOT
     describe a ppxar payload stream: use it for dedup statistics / digest computation, not to write .ppxar.didx.
 
-And for disk images (`.img.fidx` archives): FixedIndexWriter -- fixed-size chunks through the batch call, fed in slices.
+And for disk images (`.img.fidx` archives): FixedIndexWriter -- fixed-size chunks through the batch call, fed in slices;
+restore_image -- the sparse restore: zero chunks are served by digest and only the data extents are written.
 
 Restore as zip (reference internal/pxar/zip.go): ZipWriter -- files of a PayloadReader deflated on the GPU
 (pbsgpu_reader_read_deflate) inside a zip container written by pbsgpu_zip_*.
@@ -472,6 +473,44 @@ class PayloadReader:
 
     def __exit__(self, *a):
         self.Close()
+
+
+def restore_image(engine: Engine, fidx: bytes, chunk_source: Callable[[bytes], bytes], fd: int,
+                  crypt_key: bytes | None = None, slice_bytes: int = 1 << 30, cache_bytes: int = 0) -> None:
+    """Restores the disk image a `.img.fidx` describes into the file descriptor `fd`, sparsely: per slice of
+    `slice_bytes`, one plan that leaves out the zero chunks, one fetch of the named blobs by digest through
+    `chunk_source`, one pbsgpu_reader_read_sparse, and an os.pwrite of each data extent; then os.ftruncate to the image's
+    size.  Zero chunks are never fetched or decoded, and no all-zero 4 KiB block is written, so the target must read as
+    zeros where nothing is written: a new file (which stays thin), or a device the caller zeroed, as upstream's
+    skip-zero restore.  `crypt_key` and `cache_bytes` as for PayloadReader.  Raises IOError naming the first chunk whose
+    blob fails a check."""
+    crypt = engine.crypt(crypt_key) if crypt_key is not None else None
+    try:
+        reader = engine.reader_fidx(fidx, crypt, cache_bytes)
+        try:
+            size, step = reader.size, max(1, int(slice_bytes))
+            for off in range(0, size, step):
+                n = min(step, size - off)
+                chunks, digests = reader.plan([off], [n], sparse=True)
+                blobs = {int(c): chunk_source(bytes(d)) for c, d in zip(chunks, digests)}
+                status, data, bst = reader.read_sparse([off], [n], blobs)
+                if status[0] != _lib.DEC_OK:
+                    bad = [f"chunk {int(c)} ({bytes(d).hex()})" for c, d, s in zip(chunks, digests, bst) if s != _lib.DEC_OK]
+                    where = bad[0] if bad else f"the slice at {off}"
+                    raise IOError(f"transfer: image {where}: {_DEC_NAMES.get(int(status[0]), int(status[0]))}")
+                extents, packed = data[0]
+                view, at = memoryview(packed), 0
+                for eo, el in extents:
+                    done = 0
+                    while done < el:
+                        done += os.pwrite(fd, view[at + done: at + el], eo + done)
+                    at += el
+            os.ftruncate(fd, size)
+        finally:
+            reader.close()
+    finally:
+        if crypt is not None:
+            crypt.close()
 
 
 class ZipWriter:
