@@ -290,7 +290,6 @@ extern "C" int pbsgpu_open(int device, pbsgpu_ctx **out) {
         ctx->tune.head_per_sm = std::max(1, env_int("PBSGPU_HYBRID_HEAD_PER_SM", ctx->tune.head_per_sm));
         ctx->tune.mid_x10 = std::max(0, env_int("PBSGPU_BULK_MID_X10", ctx->tune.mid_x10));
         ctx->n_slots = std::max(1, std::min(N_STREAMS, env_int("PBSGPU_SLOTS", ctx->n_slots)));
-        ctx->crc_variant = env_int("PBSGPU_CRC_VARIANT", 0);
         if (getenv("PBSGPU_STREAM_WINDOW")) ctx->stream_window = strtoull(getenv("PBSGPU_STREAM_WINDOW"), nullptr, 0);
         ctx->stream_nbuf = std::max(2, std::min(32, env_int("PBSGPU_STREAM_NBUF", ctx->stream_nbuf)));
         if (getenv("PBSGPU_ARENA_MB")) ctx->arena_want = strtoull(getenv("PBSGPU_ARENA_MB"), nullptr, 0) << 20;

@@ -204,27 +204,23 @@ extern "C" int pbsgpu_sha256_keyed_batch(pbsgpu_ctx *ctx, const pbsgpu_crypt *cr
 int pbsgpu_crc32_enqueue(Blocking &b, const uint8_t *dbase, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t *d_out) {
     pbsgpu_ctx *ctx = b.ctx;
     if (int rc = pbsgpu_upload_table_once(ctx, &ctx->d_crc_tables, crc_tables_bytes(), crc_fill_tables_host)) return rc;
-    const int crc_variant = ctx->crc_variant;   // 0 = TMA-tiled kernel (default), 1 = simple lane-strided kernel (PBSGPU_CRC_VARIANT at open)
-    // work units: 128 KiB warp blocks (simple) or <= 576 KiB regions of the 16 B aligned body (tiled)
-    const uint64_t UNIT = crc_variant ? crc_wb_bytes() : crc_region_bytes();
-    std::vector<uint64_t> wb_first(n + 1);
+    // work units: <= 576 KiB regions of the 16 B aligned body, at least one per non-empty range
+    const uint64_t UNIT = crc_region_bytes();
+    std::vector<uint64_t> region_first(n + 1);
     uint64_t total = 0;
     for (uint32_t i = 0; i < n; i++) {
-        wb_first[i] = total;
-        if (crc_variant) total += (len[i] + UNIT - 1) / UNIT;
-        else if (len[i]) {
+        region_first[i] = total;
+        if (len[i]) {
             uint64_t head = (16 - ((uintptr_t)(dbase + off[i]) & 15)) & 15;
             uint64_t body = len[i] > head ? len[i] - head : 0;
             total += std::max<uint64_t>(1, (body + UNIT - 1) / UNIT);
         }
     }
-    wb_first[n] = total;
-    uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n), *d_first = b.upload(wb_first.data(), n + 1);
+    region_first[n] = total;
+    uint64_t *d_off = b.upload(off, n), *d_len = b.upload(len, n), *d_first = b.upload(region_first.data(), n + 1);
     uint32_t *d_part = b.get<uint32_t>(total + 1);
     if (!d_off || !d_len || !d_first || !d_part) return fail(ctx, PBSGPU_ENOMEM, "device allocation failed");
-    if (b.ok())
-        b.e = crc_variant ? launch_crc32(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st)
-                          : launch_crc32_tiled(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st);
+    if (b.ok()) b.e = launch_crc32_tiled(dbase, d_off, d_len, d_first, n, total, ctx->d_crc_tables, d_part, d_out, ctx->sm_count, b.st);
     return PBSGPU_OK;
 }
 

@@ -6,9 +6,9 @@
 // payload bytes are already on the host; what the GPU adds is the checksum, another full pass over
 // the new data.  zstd compression of blobs is out of scope (no compressor here).
 //
-// CRC is linear over GF(2), so a range is cut into 4 KiB segments hashed independently (one lane
-// each, slicing-by-4 with lane-replicated tables in shared memory) and the partial CRCs are merged
-// with zlib's crc32_combine algebra: crc(A||B) = crc(A) * x^(8|B|) mod P  xor  crc(B).
+// CRC is linear over GF(2), so a range is cut into regions hashed independently (k_crc32_tiled)
+// and the partial CRCs are merged with zlib's crc32_combine algebra:
+// crc(A||B) = crc(A) * x^(8|B|) mod P  xor  crc(B).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -18,8 +18,6 @@
 namespace pbsgpu {
 
 constexpr uint32_t CRC_POLY = 0xedb88320u;   // reflected IEEE polynomial
-constexpr int CRC_SEG = 4096;                // bytes per lane
-constexpr int CRC_WB = 32 * CRC_SEG;         // bytes per warp block (128 KiB)
 
 // a(x) * b(x) mod P in the reflected representation (zlib multmodp)
 __host__ __device__ inline uint32_t crc_multmodp(uint32_t a, uint32_t b) {
@@ -48,7 +46,6 @@ __host__ __device__ inline uint32_t crc_x2nmodp(const uint32_t *x2n, uint64_t n,
 struct CrcTables {
     uint32_t t[4][256];   // slicing-by-4
     uint32_t x2n[32];     // x^(2^i) mod P
-    uint32_t f_seg;       // x^(8 * CRC_SEG) mod P
 };
 
 void crc_make_tables(CrcTables *h) {
@@ -62,77 +59,14 @@ void crc_make_tables(CrcTables *h) {
     uint32_t p = 1u << 30;   // x^1
     h->x2n[0] = p;
     for (int i = 1; i < 32; i++) h->x2n[i] = p = crc_multmodp(p, p);
-    h->f_seg = crc_x2nmodp(h->x2n, CRC_SEG, 3);
-}
-
-// Persistent kernel: every warp loops over 128 KiB blocks; partial[wb] = crc of that block.
-// The four slicing tables are replicated per lane in shared memory (T[k][byte][lane], 4 x 32 KiB):
-// the bank of a lookup is the lane for every data byte, so the 4 lookups per word never conflict.
-constexpr int CRC_THREADS = 512;
-constexpr int CRC_SMEM = 4 * 256 * 32 * 4 + 32 * 4;
-
-__global__ void __launch_bounds__(CRC_THREADS, 1) k_crc32_blocks(const uint8_t *base, const uint64_t *off,
-                                                                 const uint64_t *len, const uint64_t *wb_first,
-                                                                 uint32_t n, uint64_t total_wb, const CrcTables *tab,
-                                                                 uint32_t *part_crc) {
-    extern __shared__ __align__(16) uint32_t smem_crc[];
-    uint32_t *TR = smem_crc;                       // [4][256][32]
-    uint32_t *X2N = smem_crc + 4 * 256 * 32;
-    for (int i = threadIdx.x; i < 4 * 256 * 32; i += blockDim.x) TR[i] = tab->t[i >> 13][(i >> 5) & 255];
-    if (threadIdx.x < 32) X2N[threadIdx.x] = tab->x2n[threadIdx.x];
-    __syncthreads();
-    const uint32_t f_seg = tab->f_seg;
-    const uint32_t lane = threadIdx.x & 31, lane4 = lane << 2;
-    const uint8_t *TB = (const uint8_t *)TR;       // byte-addressed: k * 32768 + (byte << 7) + lane * 4
-    auto lut = [&](uint32_t k, uint32_t byte_shl7) -> uint32_t {
-        return *(const uint32_t *)(TB + k * 32768u + ((byte_shl7 & 0x7f80u) | lane4));
-    };
-    const uint64_t warps_total = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-    for (uint64_t gw = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; gw < total_wb; gw += warps_total) {
-        const uint32_t r = owner_of(wb_first, n, gw);
-        const uint64_t wb = gw - wb_first[r], rlen = len[r];
-        const uint64_t done = wb * CRC_WB + (uint64_t)lane * CRC_SEG;
-        const uint8_t *p = base + off[r] + done;
-        const uint32_t seg = done >= rlen ? 0u : (rlen - done < (uint64_t)CRC_SEG ? (uint32_t)(rlen - done) : (uint32_t)CRC_SEG);
-        uint32_t c = 0xffffffffu, i = 0;
-#define CRC_BYTE(b) do { c = lut(0, (c ^ (b)) << 7) ^ (c >> 8); } while (0)
-#define CRC_WORD(w) do { c ^= (w); c = lut(3, c << 7) ^ lut(2, c >> 1) ^ lut(1, c >> 9) ^ lut(0, c >> 17); } while (0)
-        const uint32_t mis = (uint32_t)((uintptr_t)p & 15);
-        if (mis) for (; i < seg && i < 16 - mis; i++) CRC_BYTE(p[i]);                     // to 16 B alignment
-        // 16-byte loads: every lane touches its own cache line, so the L1 cost is per instruction, not per byte
-        for (; i + 64 <= seg; i += 64) {
-            uint4 v0 = __ldg((const uint4 *)(p + i)), v1 = __ldg((const uint4 *)(p + i + 16));
-            uint4 v2 = __ldg((const uint4 *)(p + i + 32)), v3 = __ldg((const uint4 *)(p + i + 48));
-            CRC_WORD(v0.x); CRC_WORD(v0.y); CRC_WORD(v0.z); CRC_WORD(v0.w);
-            CRC_WORD(v1.x); CRC_WORD(v1.y); CRC_WORD(v1.z); CRC_WORD(v1.w);
-            CRC_WORD(v2.x); CRC_WORD(v2.y); CRC_WORD(v2.z); CRC_WORD(v2.w);
-            CRC_WORD(v3.x); CRC_WORD(v3.y); CRC_WORD(v3.z); CRC_WORD(v3.w);
-        }
-        for (; i + 4 <= seg; i += 4) CRC_WORD(__ldg((const uint32_t *)(p + i)));
-        for (; i < seg; i++) CRC_BYTE(p[i]);
-#undef CRC_WORD
-#undef CRC_BYTE
-        c = seg ? ~c : 0u;            // standard CRC of this lane's segment (crc of empty = 0)
-        // merge the 32 segments left to right (tiny: 32 GF(2) multiplications per 128 KiB)
-        uint32_t acc = 0;
-        for (int l = 0; l < 32; l++) {
-            uint32_t cl = __shfl_sync(0xffffffffu, c, l), sl = __shfl_sync(0xffffffffu, seg, l);
-            if (lane == 0 && sl) {
-                uint32_t f = sl == (uint32_t)CRC_SEG ? f_seg : crc_x2nmodp(X2N, sl, 3);
-                acc = crc_multmodp(f, acc) ^ cl;
-            }
-        }
-        if (lane == 0) part_crc[gw] = acc;
-    }
 }
 
 // ============================================================================
-// Tuned kernel: TMA-staged tiles.  The lane-strided global reads of k_crc32_blocks (63 k concurrent
-// 64-byte streams) are what bounds it; here a warp owns REGIONS of 128 contiguous tiles of 32 x 144 B
-// that arrive by TMA bulk copies (double buffered, as in the scan kernel), each lane walks its 144 B span
-// of every tile (LDS.128, conflict free: lane stride = 9 quads) and carries its CRC state across tiles:
-// the 4464 bytes of the other lanes between two of its spans are skipped with ONE table step (the
-// "advance by n zero bytes" map is linear: 4 lookups).  At the end of a region every lane advances its
+// k_crc32_tiled: a warp owns REGIONS of 128 contiguous tiles of 32 x 144 B that arrive by TMA bulk copies
+// (double buffered, as in the scan kernel), each lane walks its 144 B span of every tile (LDS.128, conflict
+// free: lane stride = 9 quads) and carries its CRC state across tiles: the 4464 bytes of the other lanes
+// between two of its spans are skipped with ONE table step (the "advance by n zero bytes" map is linear:
+// 4 lookups).  At the end of a region every lane advances its
 // state to the region end (one GF(2) multiplication) and the 32 states are XORed -- CRC is linear, the
 // all-ones initial state rides on lane 0.  A range's unaligned head (< 16 B, TMA needs 16 B alignment) is
 // hashed byte-wise by lane 0 in front of its first span.
@@ -249,22 +183,6 @@ __global__ void __launch_bounds__(CT_WARPS * 32, 1) k_crc32_tiled(const uint8_t 
 #undef CT_BYTE
 }
 
-// one thread per range: merge its warp blocks
-__global__ void k_crc32_merge(const uint64_t *len, const uint64_t *wb_first, uint32_t n, const CrcTables *tab,
-                              const uint32_t *part_crc, uint32_t *out) {
-    uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    const uint64_t w0 = wb_first[r], w1 = wb_first[r + 1], rlen = len[r];
-    const uint32_t f_wb = crc_x2nmodp(tab->x2n, CRC_WB, 3);
-    uint32_t acc = 0;
-    for (uint64_t w = w0; w < w1; w++) {
-        uint64_t bytes = (w + 1 < w1) ? (uint64_t)CRC_WB : rlen - (w - w0) * CRC_WB;
-        uint32_t f = bytes == (uint64_t)CRC_WB ? f_wb : crc_x2nmodp(tab->x2n, bytes, 3);
-        acc = crc_multmodp(f, acc) ^ part_crc[w];
-    }
-    out[r] = acc;   // crc32 of an empty range = 0
-}
-
 // one thread per range: merge its regions (variable first-region length because of the unaligned head)
 __global__ void k_crc32_merge_regions(const uint8_t *base, const uint64_t *off, const uint64_t *len,
                                       const uint64_t *region_first, uint32_t n, const CrcTiledTables *tab,
@@ -304,30 +222,13 @@ cudaError_t launch_crc32_tiled(const uint8_t *base, const uint64_t *off, const u
 }
 uint64_t crc_region_bytes() { return (uint64_t)CT_REGION_TILES * CT_TILE; }
 
-cudaError_t launch_crc32(const uint8_t *base, const uint64_t *off, const uint64_t *len, const uint64_t *wb_first,
-                         uint32_t n, uint64_t total_wb, const void *tables, uint32_t *part_crc, uint32_t *out,
-                         int sm_count, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    if (total_wb) {
-        cudaError_t e = cudaFuncSetAttribute(k_crc32_blocks, cudaFuncAttributeMaxDynamicSharedMemorySize, CRC_SMEM);
-        if (e != cudaSuccess) return e;
-        uint64_t want = (total_wb + CRC_THREADS / 32 - 1) / (CRC_THREADS / 32);
-        unsigned grid = (unsigned)(want < (uint64_t)sm_count ? want : (uint64_t)sm_count);
-        k_crc32_blocks<<<grid, CRC_THREADS, CRC_SMEM, st>>>(base, off, len, wb_first, n, total_wb,
-                                                           (const CrcTables *)tables, part_crc);
-    }
-    k_crc32_merge<<<(n + 127) / 128, 128, 0, st>>>(len, wb_first, n, (const CrcTables *)tables, part_crc, out);
-    return cudaGetLastError();
-}
-
 size_t crc_tables_bytes() { return sizeof(CrcTiledTables); }
 void crc_fill_tables_host(void *dst) {
     CrcTiledTables *t = (CrcTiledTables *)dst;
-    crc_make_tables(&t->base);                                 // (base is the first member: the simple kernel reads it)
+    crc_make_tables(&t->base);
     const uint32_t f = crc_x2nmodp(t->base.x2n, CT_TILE - CT_SPAN, 3);   // x^(8 * 4464)
     for (int k = 0; k < 4; k++)
         for (uint32_t b = 0; b < 256; b++) t->zt[k][b] = crc_multmodp(f, b << (8 * k));
 }
-uint64_t crc_wb_bytes() { return CRC_WB; }
 
 }  // namespace pbsgpu

@@ -72,7 +72,6 @@ struct pbsgpu_ctx {
     bool scan_lanes = false;                  // PBSGPU_SCAN_LANES
     uint64_t xxh3_cap_blocks = 8ull << 20;    // PBSGPU_XXH3_CAP_BLOCKS
     pbsgpu::ShaTune tune;                     // PBSGPU_SHA_MODE / _HYBRID / HYBRID_THR_X10 / HYBRID_SERIAL / SPLIT_SPREAD_KB
-    int crc_variant = 0;                      // PBSGPU_CRC_VARIANT
     uint64_t stream_window = 2ull << 30;      // PBSGPU_STREAM_WINDOW
     int stream_nbuf = 12;                     // PBSGPU_STREAM_NBUF: windows in flight per stream
     // long-chunk arena (PBSGPU_BATCH_EARLY_INPUT jobs): one device ring, allocated on first use.  A job reserves

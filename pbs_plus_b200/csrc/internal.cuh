@@ -162,9 +162,6 @@ cudaError_t launch_set_compact_gather(const uint8_t *padded, const uint64_t *cou
                                       uint8_t *dense, cudaStream_t st);
 
 // ---- CRC-32 (K6, DataBlob checksums) -----------------------------------------------------
-cudaError_t launch_crc32(const uint8_t *base, const uint64_t *off, const uint64_t *len, const uint64_t *wb_first,
-                         uint32_t n, uint64_t total_wb, const void *tables, uint32_t *part_crc, uint32_t *out,
-                         int sm_count, cudaStream_t st);
 cudaError_t launch_crc32_tiled(const uint8_t *base, const uint64_t *off, const uint64_t *len,
                                const uint64_t *region_first, uint32_t n, uint64_t total_regions, const void *tables,
                                uint32_t *part_crc, uint32_t *out, int sm_count, cudaStream_t st);
@@ -183,7 +180,6 @@ cudaError_t launch_xxh3_pieces(const uint8_t *base, const uint64_t *off, const u
                                uint64_t *S, uint64_t *state_in, uint64_t *state_out, uint64_t *out, cudaStream_t st);
 uint64_t xxh3_empty_host();
 void crc_fill_tables_host(void *dst);
-uint64_t crc_wb_bytes();
 
 // ---- AES-256-GCM (K11, encrypted DataBlobs) ---------------------------------------------------
 constexpr uint32_t GCM_SEG_BLOCKS = 1024;   // 16-byte blocks per warp segment (32 per lane)

@@ -638,7 +638,7 @@ def test_knobs_are_read_per_context_and_results_do_not_depend_on_them(torch):
     ref = oracle.chunk_digest_streams(oracle.config(1 << 16), arrs).tobytes()
     d = to_dev(torch, buf)
     for env in ({"PBSGPU_SHA_HYBRID": "2", "PBSGPU_PARTITION_SMS": "0"}, {"PBSGPU_SHA_MODE": "0"}, {"PBSGPU_SHA_MODE": "13"},
-                {"PBSGPU_SHA_HYBRID": "0"}, {"PBSGPU_HYBRID_THR_X10": "5"}, {"PBSGPU_CRC_VARIANT": "1"},
+                {"PBSGPU_SHA_HYBRID": "0"}, {"PBSGPU_HYBRID_THR_X10": "5"},
                 {"PBSGPU_BULK_MID_X10": "12", "PBSGPU_HYBRID_THR_X10": "20"}, {"PBSGPU_SCAN_LANES": "1"}):
         os.environ.update(env)
         try:
@@ -648,8 +648,6 @@ def test_knobs_are_read_per_context_and_results_do_not_depend_on_them(torch):
                 del os.environ[k]
         try:
             assert e.chunk_digest_batch(pg.make_config(1 << 16), d, off, ln).tobytes() == ref, env
-            if "PBSGPU_CRC_VARIANT" in env:
-                assert int(e.crc32_batch(d, off[:1], ln[:1])[0]) == zlib.crc32(arrs[0].tobytes())
         finally:
             e.close()
 
