@@ -157,12 +157,11 @@ static bool adopt_partition(pbsgpu_ctx *ctx, const GreenApi &G, CUdevice dev, st
     ok = ok && G.gcreate(&gl, dA, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS;
     ok = ok && G.gcreate(&gb, dB, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS;
     ok = ok && (!three || G.gcreate(&gs, dC, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS);
-    cudaStream_t a[N_STREAMS] = {}, b[N_STREAMS] = {}, c[N_SCAN_STREAMS] = {}, m[N_STREAMS] = {};
+    cudaStream_t a[N_STREAMS] = {}, b[N_STREAMS] = {}, c[N_SCAN_STREAMS] = {};
     for (int i = 0; i < ctx->n_slots && ok; i++) {
-        CUstream sa = nullptr, sb = nullptr, sm = nullptr;
+        CUstream sa = nullptr, sb = nullptr;
         ok = G.gstream(&sb, gb, CU_STREAM_NON_BLOCKING, 0) == CUDA_SUCCESS;
         if (ok) b[i] = (cudaStream_t)sb;
-        if (ok && ctx->tune.mid_x10 > 0) { ok = G.gstream(&sm, gb, CU_STREAM_NON_BLOCKING, -1) == CUDA_SUCCESS; if (ok) m[i] = (cudaStream_t)sm; }
         ok = ok && G.gstream(&sa, gl, CU_STREAM_NON_BLOCKING, 0) == CUDA_SUCCESS;
         if (ok) a[i] = (cudaStream_t)sa;
     }
@@ -172,13 +171,13 @@ static bool adopt_partition(pbsgpu_ctx *ctx, const GreenApi &G, CUdevice dev, st
         if (ok) c[i] = (cudaStream_t)sc;
     }
     if (!ok) {
-        for (int i = 0; i < N_STREAMS; i++) { if (a[i]) cudaStreamDestroy(a[i]); if (b[i]) cudaStreamDestroy(b[i]); if (m[i]) cudaStreamDestroy(m[i]); }
+        for (int i = 0; i < N_STREAMS; i++) { if (a[i]) cudaStreamDestroy(a[i]); if (b[i]) cudaStreamDestroy(b[i]); }
         for (int i = 0; i < N_SCAN_STREAMS; i++) if (c[i]) cudaStreamDestroy(c[i]);
         if (G.gdestroy) { if (gl) G.gdestroy(gl); if (gb) G.gdestroy(gb); if (gs) G.gdestroy(gs); }
         (void)cudaGetLastError();
         return false;
     }
-    for (int i = 0; i < N_STREAMS; i++) { ctx->streams[i] = b[i]; ctx->streams2[i] = a[i]; ctx->streams3[i] = m[i]; }
+    for (int i = 0; i < N_STREAMS; i++) { ctx->streams[i] = b[i]; ctx->streams2[i] = a[i]; }
     for (int i = 0; i < N_SCAN_STREAMS; i++) ctx->scan_streams[i] = c[i];
     ctx->g_long = gl; ctx->g_bulk = gb; ctx->g_scan = gs;
     ctx->part_sms = (int)count(res_long);
@@ -232,7 +231,6 @@ static void ctx_destroy(pbsgpu_ctx *ctx) {
     for (int i = 0; i < N_STREAMS; i++) {
         if (ctx->streams[i]) cudaStreamDestroy(ctx->streams[i]);
         if (ctx->streams2[i]) cudaStreamDestroy(ctx->streams2[i]);
-        if (ctx->streams3[i]) cudaStreamDestroy(ctx->streams3[i]);
     }
     for (int i = 0; i < N_SCAN_STREAMS; i++) if (ctx->scan_streams[i]) cudaStreamDestroy(ctx->scan_streams[i]);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
@@ -282,21 +280,15 @@ extern "C" int pbsgpu_open(int device, pbsgpu_ctx **out) {
         ctx->variant = env_int("PBSGPU_VARIANT", 0);
         ctx->scan_lanes = env_int("PBSGPU_SCAN_LANES", 0) != 0;
         if (env_int("PBSGPU_XXH3_CAP_BLOCKS", 0) > 0) ctx->xxh3_cap_blocks = (uint64_t)atoll(getenv("PBSGPU_XXH3_CAP_BLOCKS"));
-        ctx->tune.mode = env_int("PBSGPU_SHA_MODE", ctx->tune.mode);
         ctx->tune.hybrid = env_int("PBSGPU_SHA_HYBRID", ctx->tune.hybrid);
         ctx->tune.thr_x10 = env_int("PBSGPU_HYBRID_THR_X10", ctx->tune.thr_x10);
-        ctx->tune.serial = env_int("PBSGPU_HYBRID_SERIAL", ctx->tune.serial);
         ctx->tune.spread_kb = env_int("PBSGPU_SPLIT_SPREAD_KB", ctx->tune.spread_kb);
         ctx->tune.head_per_sm = std::max(1, env_int("PBSGPU_HYBRID_HEAD_PER_SM", ctx->tune.head_per_sm));
-        ctx->tune.mid_x10 = std::max(0, env_int("PBSGPU_BULK_MID_X10", ctx->tune.mid_x10));
         ctx->n_slots = std::max(1, std::min(N_STREAMS, env_int("PBSGPU_SLOTS", ctx->n_slots)));
         if (getenv("PBSGPU_STREAM_WINDOW")) ctx->stream_window = strtoull(getenv("PBSGPU_STREAM_WINDOW"), nullptr, 0);
         ctx->stream_nbuf = std::max(2, std::min(32, env_int("PBSGPU_STREAM_NBUF", ctx->stream_nbuf)));
         if (getenv("PBSGPU_ARENA_MB")) ctx->arena_want = strtoull(getenv("PBSGPU_ARENA_MB"), nullptr, 0) << 20;
         ctx->arena_frac_x16 = std::max(1, std::min(16, env_int("PBSGPU_ARENA_FRAC_X16", ctx->arena_frac_x16)));
-        int prio_lo = 0, prio_hi = 0;
-        cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-        const int side_prio = env_int("PBSGPU_HYBRID_PRIO", 0) ? prio_hi : prio_lo;   // 1: long-chunk kernels on a high-priority stream
         // default: 24 SMs reserved for the long-chunk latency kernels (green contexts); 0 disables
         const int want_part = env_int("PBSGPU_PARTITION_SMS", 24);
         // + PBSGPU_SCAN_SMS SMs that run only the front halves (K1 scan / sort / K2); default 0 = scans share the bulk partition
@@ -305,8 +297,7 @@ extern "C" int pbsgpu_open(int device, pbsgpu_ctx **out) {
         bool ok = true;
         for (int i = 0; i < ctx->n_slots && !partitioned && ok; i++)
             ok = cudaStreamCreateWithFlags(&ctx->streams[i], cudaStreamNonBlocking) == cudaSuccess &&
-                 cudaStreamCreateWithPriority(&ctx->streams2[i], cudaStreamNonBlocking, side_prio) == cudaSuccess &&
-                 (ctx->tune.mid_x10 <= 0 || cudaStreamCreateWithPriority(&ctx->streams3[i], cudaStreamNonBlocking, prio_hi) == cudaSuccess);
+                 cudaStreamCreateWithFlags(&ctx->streams2[i], cudaStreamNonBlocking) == cudaSuccess;
         if (!ok || cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
             cudaStreamCreateWithFlags(&ctx->tail_stream, cudaStreamNonBlocking) != cudaSuccess) { rc = PBSGPU_ECUDA; break; }
         ctx->streams_made = true;
@@ -385,7 +376,6 @@ cudaError_t pbsgpu_job_sync(pbsgpu_job *j) {   // everything the job enqueued, o
     if (j->ss && j->ss != j->st && (r = cudaStreamSynchronize(j->ss)) != cudaSuccess) e = r;
     if (j->st && (r = cudaStreamSynchronize(j->st)) != cudaSuccess) e = r;
     if (j->st2 && (r = cudaStreamSynchronize(j->st2)) != cudaSuccess) e = r;
-    if (j->st3 && (r = cudaStreamSynchronize(j->st3)) != cudaSuccess) e = r;
     if (j->state == JOB_ENQUEUED && (r = cudaEventSynchronize(j->ev[EV_END])) != cudaSuccess) e = r;   // the tail may run on the tail stream
     if (e != cudaSuccess) (void)cudaGetLastError();
     return e;
@@ -561,7 +551,6 @@ static int job_place(pbsgpu_job *j, pbsgpu_job **out) {
     pbsgpu_ctx *ctx = j->ctx;
     j->st = ctx->streams[ctx->next_stream];
     j->st2 = ctx->streams2[ctx->next_stream];
-    j->st3 = ctx->streams3[ctx->next_stream];
     ctx->next_stream = (ctx->next_stream + 1) % ctx->n_slots;
     if (ctx->scan_sms > 0) { j->ss = ctx->scan_streams[ctx->next_scan]; ctx->next_scan = (ctx->next_scan + 1) % N_SCAN_STREAMS; }
     else j->ss = j->st;
@@ -624,7 +613,7 @@ static bool arena_reserve(pbsgpu_job *j, cudaStream_t side) {
 // a partition their CTAs pin shared memory for ~0.3 s and starve the whole-SM scan CTAs of later batches
 // and the pipelined step gets slower.  PBSGPU_SHA_HYBRID=2 forces it on regardless, 0 turns it off.
 static bool hybrid_for(const pbsgpu_ctx *ctx) {
-    if (ctx->tune.mode >= 10 || ctx->tune.hybrid == 0) return false;
+    if (ctx->tune.hybrid == 0) return false;
     return ctx->part_sms > 0 || ctx->tune.hybrid == 2;
 }
 
@@ -705,57 +694,42 @@ int pbsgpu_job_enqueue_back(pbsgpu_job *j) {
         ShaArgs ha;
         ha.base = j->base; ha.off = j->d_off; ha.chunks = j->d_chunks; ha.order = j->d_vals2;
         ha.n_chunks = &j->d_counters[CTR_CHUNKS]; ha.chunk_cap = j->chunk_cap; ha.digests = j->d_digests;
-        ha.n_head = nullptr; ha.n_mid = nullptr; ha.part = 0;
+        ha.n_head = nullptr; ha.part = 0;
         if (j->variant == 1) CK(launch_sha_simple(ha, st, j->sha_suffix));
-        else if (!hybrid_for(ctx)) CK(launch_sha_tuned(ha, ctx->tune, st, j->sha_suffix));
+        else if (!hybrid_for(ctx)) CK(launch_sha_tuned(ha, st, j->sha_suffix));
         else {
             // hybrid: chunks longer than 2.5 x avg (their serial chains bound the batch's makespan) run on
             // the latency-optimised split kernel on a forked stream, concurrently with the rest
-            const bool serial = ctx->tune.serial != 0;
-            cudaStream_t side = serial ? st : j->st2;
             uint64_t thr64 = (uint64_t)j->cfg.avg * (uint64_t)ctx->tune.thr_x10 / 10;
             uint32_t thr = thr64 > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)thr64;
             // at most one latency CTA (32 chunks) per SM of the partition and job; the longest chunks first
             const unsigned long long max_head = (unsigned long long)ctx->tune.head_per_sm * (unsigned long long)(ctx->part_sms > 0 ? ctx->part_sms : 24);
-            const bool use_mid = ctx->tune.mid_x10 > 0 && j->st3 != nullptr;
-            uint64_t thr_mid64 = (uint64_t)j->cfg.avg * (uint64_t)ctx->tune.mid_x10 / 10;
-            uint32_t thr_mid = thr_mid64 > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)thr_mid64;
-            CK(launch_split_point(j->d_keys2, &j->d_counters[CTR_CHUNKS], j->chunk_cap, thr, max_head, &j->d_counters[CTR_HEAD], thr_mid,
-                                  use_mid ? &j->d_counters[CTR_MID] : nullptr, st));
+            CK(launch_split_point(j->d_keys2, &j->d_counters[CTR_CHUNKS], j->chunk_cap, thr, max_head, &j->d_counters[CTR_HEAD], st));
             ha.n_head = &j->d_counters[CTR_HEAD];
             // early input release: the head chunks are copied to the arena and hashed from there
             // (the copy runs HERE, on the job's own stream and the big partition -- a few ms -- not on the side stream,
             // where it would queue behind the 0.3 s latency kernel of the slot's previous job)
             // (a fixed-cut job has no head chunks: its bulk pass is the whole job, so it takes no arena)
-            early = j->early && !j->fixed_log2 && !serial && !use_mid && arena_reserve(j, st);
+            early = j->early && !j->fixed_log2 && arena_reserve(j, st);
             if (early) {
                 CK(launch_arena_plan(ha, &j->d_counters[CTR_HEAD], j->arena_len, j->d_arena_off, st));
                 CK(launch_arena_gather(ha, ctx->arena + j->arena_lo, j->d_arena_off, ctx->sm_count, st));
                 ha.arena = ctx->arena + j->arena_lo; ha.arena_off = j->d_arena_off;
             }
             CK(cudaEventRecord(j->ev[EV_FORK], st));
-            if (!serial) CK(cudaStreamWaitEvent(side, j->ev[EV_FORK], 0));
-            ha.n_mid = use_mid ? &j->d_counters[CTR_MID] : nullptr;
-            ha.part = 1; CK(launch_sha_split(ha, ctx->tune, side, j->sha_suffix));
+            CK(cudaStreamWaitEvent(j->st2, j->ev[EV_FORK], 0));
+            ha.part = 1; CK(launch_sha_split(ha, ctx->tune.spread_kb, j->st2, j->sha_suffix));
             ha.arena = nullptr; ha.arena_off = nullptr;
-            CK(cudaEventRecord(j->ev[EV_JOIN], side));
-            if (early) CK(cudaEventRecord(ctx->arena_recs.back().ev, side));   // the region may be reused after this
-            if (use_mid) {   // the longer bulk chunks of every job in flight start first (high-priority stream), the short ones fill in
-                CK(cudaStreamWaitEvent(j->st3, j->ev[EV_FORK], 0));
-                ha.part = 3; CK(launch_sha_tuned(ha, ctx->tune, j->st3, j->sha_suffix));
-                CK(cudaEventRecord(j->ev[EV_MID], j->st3));
-                ha.part = 4; CK(launch_sha_tuned(ha, ctx->tune, st, j->sha_suffix));
-                CK(cudaStreamWaitEvent(st, j->ev[EV_MID], 0));
-            } else {
-                ha.part = 2; CK(launch_sha_tuned(ha, ctx->tune, st, j->sha_suffix));
-            }
+            CK(cudaEventRecord(j->ev[EV_JOIN], j->st2));
+            if (early) CK(cudaEventRecord(ctx->arena_recs.back().ev, j->st2));   // the region may be reused after this
+            ha.part = 2; CK(launch_sha_tuned(ha, st, j->sha_suffix));
             CK(cudaEventRecord(j->ev[EV_BULK], st));
             if (early) {
                 // the caller's buffer is free once the bulk pass and the gather are done -- provided the candidate buffer
                 // did not overflow (then the job is rerun from the input; pbsgpu_batch_wait_input checks the count)
                 CK(cudaMemcpyAsync(j->h_early, &j->d_counters[CTR_CANDIDATES], sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
                 CK(cudaEventRecord(j->ev[EV_INPUT], st));
-            } else if (!serial) CK(cudaStreamWaitEvent(st, j->ev[EV_JOIN], 0));
+            } else CK(cudaStreamWaitEvent(st, j->ev[EV_JOIN], 0));
         }
     }
     j->early_active = early;

@@ -159,8 +159,8 @@ extern "C" int pbsgpu_fidx_parse(pbsgpu_ctx *ctx, const uint8_t *fidx, uint64_t 
 // ---------------------------------------------------------------------------
 void pbsgpu_sha256_enqueue(Blocking &b, const uint8_t *base, const ChunkRef *d_refs, const unsigned long long *d_n, uint32_t n,
                            const uint8_t *suffix, uint8_t *d_dig) {
-    const ShaArgs ha{base, nullptr, d_refs, nullptr, d_n, n, d_dig, nullptr, nullptr, 0};
-    if (b.ok()) b.e = b.ctx->variant == 1 ? launch_sha_simple(ha, b.st, suffix) : launch_sha_tuned(ha, b.ctx->tune, b.st, suffix);
+    const ShaArgs ha{base, nullptr, d_refs, nullptr, d_n, n, d_dig, nullptr, 0};
+    if (b.ok()) b.e = b.ctx->variant == 1 ? launch_sha_simple(ha, b.st, suffix) : launch_sha_tuned(ha, b.st, suffix);
 }
 
 // suffix: encrypt mode's device id_key (keyed digests), or NULL

@@ -40,7 +40,6 @@ struct pbsgpu_ctx {
     std::recursive_mutex mu;
     cudaStream_t streams[N_STREAMS] = {};
     cudaStream_t streams2[N_STREAMS] = {};   // forked side stream per job stream (latency kernel of the hybrid SHA launch)
-    cudaStream_t streams3[N_STREAMS] = {};   // PBSGPU_BULK_MID_X10 > 0: high-priority bulk stream per slot (mid class)
     cudaStream_t scan_streams[N_SCAN_STREAMS] = {};   // front halves (K1 scan, sort, K2 resolve) in submission order on the scan partition
     int next_scan = 0;
     cudaStream_t copy_stream = nullptr;
@@ -71,7 +70,7 @@ struct pbsgpu_ctx {
     uint64_t stage_bytes = 0;                 // PBSGPU_STAGE_BYTES: host-input staging group size (0 = auto)
     bool scan_lanes = false;                  // PBSGPU_SCAN_LANES
     uint64_t xxh3_cap_blocks = 8ull << 20;    // PBSGPU_XXH3_CAP_BLOCKS
-    pbsgpu::ShaTune tune;                     // PBSGPU_SHA_MODE / _HYBRID / HYBRID_THR_X10 / HYBRID_SERIAL / SPLIT_SPREAD_KB
+    pbsgpu::ShaTune tune;                     // PBSGPU_SHA_HYBRID / HYBRID_THR_X10 / SPLIT_SPREAD_KB / HYBRID_HEAD_PER_SM
     uint64_t stream_window = 2ull << 30;      // PBSGPU_STREAM_WINDOW
     int stream_nbuf = 12;                     // PBSGPU_STREAM_NBUF: windows in flight per stream
     // long-chunk arena (PBSGPU_BATCH_EARLY_INPUT jobs): one device ring, allocated on first use.  A job reserves
@@ -179,16 +178,16 @@ int pbsgpu_set_process_dev(pbsgpu_set *s, const uint8_t *d_dig, uint64_t n, int 
 // ---------------------------------------------------------------------------
 // Job: one batch of device-resident streams through K1..K4 on one CUDA stream (capi.cu)
 // ---------------------------------------------------------------------------
-enum { EV_START, EV_SCAN, EV_SORT, EV_RESOLVE, EV_SHA, EV_END, EV_FORK, EV_JOIN, EV_BULK, EV_BACK, EV_SET, EV_MID, EV_INPUT, EV_COUNT };
+enum { EV_START, EV_SCAN, EV_SORT, EV_RESOLVE, EV_SHA, EV_END, EV_FORK, EV_JOIN, EV_BULK, EV_BACK, EV_SET, EV_INPUT, EV_COUNT };
 // Slots of j->d_counters, zeroed by every front half.  The first CTR_HOST slots are copied back to j->h_counters.
-enum { CTR_CANDIDATES, CTR_CHUNKS, CTR_HEAD, CTR_NEW, CTR_MID, CTR_HOST = CTR_MID, CTR_DEVICE = 8 };
+enum { CTR_CANDIDATES, CTR_CHUNKS, CTR_HEAD, CTR_NEW, CTR_HOST, CTR_DEVICE = 8 };
 // CREATED: nothing in flight.  FRONT: the front half was (perhaps partly) enqueued.  ENQUEUED: both halves are enqueued,
 // EV_END recorded, and a fused probe still has to be settled with the set.  FINISHED: results are on the host.
 enum JobState { JOB_CREATED, JOB_FRONT, JOB_ENQUEUED, JOB_FINISHED };
 
 struct pbsgpu_job {
     pbsgpu_ctx *ctx = nullptr;
-    cudaStream_t st = nullptr, st2 = nullptr, ss = nullptr, st3 = nullptr;   // back half / long-chunk kernel / front half / mid class
+    cudaStream_t st = nullptr, st2 = nullptr, ss = nullptr;   // back half / long-chunk kernel / front half
     pbsgpu_cfg cfg;
     const uint8_t *base = nullptr;
     std::vector<uint64_t> off, len, tile_first, forced_keys;   // forced_keys: (stream << 40 | offset-1) suggested boundaries

@@ -87,9 +87,7 @@ struct ShaArgs {
     // hybrid launch: the first *n_head entries of `order` (the longest chunks) go to the
     // latency-optimised split kernel (part 1), the rest to the throughput kernel (part 2).
     const unsigned long long *n_head;    // device; NULL with part 0
-    const unsigned long long *n_mid;     // device; end of the "mid" class (>= *n_head); NULL unless part is 3 or 4
-    int part;                            // 0 = everything, 1 = head only, 2 = everything but the head,
-                                         // 3 = mid class [head, mid), 4 = short class [mid, n)
+    int part;                            // 0 = everything, 1 = head only, 2 = everything but the head
     // long-chunk arena (part 1 only; NULL = read the chunks where they lie): head chunk t was copied to
     // arena + arena_off[t] + (its source address mod 16) by k_arena_gather
     const uint8_t *arena = nullptr;
@@ -97,23 +95,18 @@ struct ShaArgs {
 };
 // per-context tuning knobs of K3 (read from the environment once per pbsgpu_open)
 struct ShaTune {
-    int mode = 2;        // PBSGPU_SHA_MODE: instruction mix of the throughput kernel (0,1,2,3,7) or split-only (10..13)
     int hybrid = 1;      // PBSGPU_SHA_HYBRID: 0 throughput kernel only, 1 hybrid when partitioned, 2 hybrid always
     int thr_x10 = 25;    // PBSGPU_HYBRID_THR_X10: chunks longer than thr_x10/10 x avg take the latency kernel
-    int serial = 0;      // PBSGPU_HYBRID_SERIAL: latency kernel on the job's own stream (diagnostic)
     int spread_kb = 30;  // PBSGPU_SPLIT_SPREAD_KB: dummy dynamic shared memory per latency CTA (caps CTAs per SM)
     int head_per_sm = 32; // PBSGPU_HYBRID_HEAD_PER_SM: chunks per SM of the long partition (and job) that may take the latency kernel
-    int mid_x10 = 0;      // PBSGPU_BULK_MID_X10: > 0: bulk chunks longer than mid_x10/10 x avg are launched on a HIGH-PRIORITY bulk
-                          // stream of their own, so the longer chains of every job in flight start before the short ones
 };
 // suffix (device, 32 bytes; encrypt mode's id_key): the digests are SHA-256(chunk || suffix), from the keyed kernels;
 // NULL = plain digests
 cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st, const uint8_t *suffix = nullptr);
-cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix = nullptr);   // throughput kernel
-cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix = nullptr);   // latency kernel
+cudaError_t launch_sha_tuned(const ShaArgs &a, cudaStream_t st, const uint8_t *suffix = nullptr);   // throughput kernel
+cudaError_t launch_sha_split(const ShaArgs &a, int spread_kb, cudaStream_t st, const uint8_t *suffix = nullptr);   // latency kernel
 cudaError_t launch_split_point(const uint32_t *len_sorted_desc, const unsigned long long *n_chunks, uint64_t cap,
-                               uint32_t threshold, unsigned long long max_head, unsigned long long *n_head,
-                               uint32_t threshold_mid, unsigned long long *n_mid, cudaStream_t st);
+                               uint32_t threshold, unsigned long long max_head, unsigned long long *n_head, cudaStream_t st);
 // long-chunk arena: plan the placement of the head chunks inside a reservation of `arena_cap` bytes (trims *n_head, whole
 // groups of 32, to what fits), then copy them there
 cudaError_t launch_arena_plan(const ShaArgs &a, unsigned long long *n_head, uint64_t arena_cap, uint64_t *arena_off,

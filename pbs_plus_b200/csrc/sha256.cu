@@ -205,13 +205,6 @@ __device__ __forceinline__ bool sha_slot(const ShaArgs &a, uint64_t t, uint64_t 
     const unsigned long long n = live_count(*a.n_chunks, a.chunk_cap);
     const unsigned long long head = live_count(a.part ? *a.n_head : 0ull, n);
     if (a.part == 1) { pos = t; return t < head; }
-    if (a.part >= 3) {
-        unsigned long long mid = live_count(*a.n_mid, n);
-        if (mid < head) mid = head;
-        if (a.part == 3) { pos = t + head; return pos < mid; }
-        pos = t + mid;
-        return pos < n;
-    }
     pos = t + head;
     return pos < n;
 }
@@ -249,79 +242,63 @@ cudaError_t launch_sha_simple(const ShaArgs &a, cudaStream_t st, const uint8_t *
 // ---------------------------------------------------------------------------
 // Pipe balancing: the SM's integer work splits over the ALU pipe (LOP3/SHF/PRMT/IADD3) and the FMA pipe (IMAD), 64
 // lanes/clk/SM each.  ptxas puts almost all of SHA-256 on the ALU pipe.  Multiplying by constants the compiler cannot
-// see (kernel arguments 1, 2^29, 2^22, 2^7) forces the additions (a*1+b), the two logical shifts of the message
-// schedule (mul.hi by 2^(32-n)) and one rotation per round (mul.lo + mad.hi) onto IMAD / IMAD.HI, taking the ALU pipe
-// from ~1280 to ~880 instructions per block with ~870 on the FMA pipe.  MODE bit0: adds, bit1: shifts, bit2: rotr25.
+// see (kernel arguments 1, 2^29, 2^22) forces the two logical shifts of the message schedule (mul.hi by 2^(32-n)) and,
+// where asked for, the additions (a*1+b) onto IMAD / IMAD.HI.  The throughput kernel moves the shifts only; the split
+// kernel's producer moves the shifts and every addition.  tools/sha_lab.cu times other mixes.
 // ---------------------------------------------------------------------------
-struct Opq { uint32_t one, p29, p22, p7; };
+struct Opq { uint32_t one, p29, p22; };
 
-template <int MODE> struct Ops {
-    static __device__ __forceinline__ uint32_t add(uint32_t a, uint32_t b, const Opq &o) {
-        if (MODE & 1) { uint32_t d; asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(o.one), "r"(b)); return d; }
-        return a + b;
-    }
-    static __device__ __forceinline__ uint32_t shr3(uint32_t x, const Opq &o) {
-        if (MODE & 2) { uint32_t d; asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(o.p29)); return d; }
-        return x >> 3;
-    }
-    static __device__ __forceinline__ uint32_t shr10(uint32_t x, const Opq &o) {
-        if (MODE & 2) { uint32_t d; asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(o.p22)); return d; }
-        return x >> 10;
-    }
-    static __device__ __forceinline__ uint32_t rotr25(uint32_t x, const Opq &o) {
-        if (MODE & 4) {
-            uint32_t lo, d;
-            asm("mul.lo.u32 %0, %1, %2;" : "=r"(lo) : "r"(x), "r"(o.p7));
-            asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(x), "r"(o.p7), "r"(lo));
-            return d;
-        }
-        return __funnelshift_r(x, x, 25);
-    }
-};
+__device__ __forceinline__ uint32_t fma_add(uint32_t a, uint32_t b, const Opq &o) {
+    uint32_t d; asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(o.one), "r"(b)); return d;
+}
+__device__ __forceinline__ uint32_t fma_shr3(uint32_t x, const Opq &o) {
+    uint32_t d; asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(o.p29)); return d;
+}
+__device__ __forceinline__ uint32_t fma_shr10(uint32_t x, const Opq &o) {
+    uint32_t d; asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(o.p22)); return d;
+}
 
-// Message schedule step of round i on the 16-word ring w (FIPS 180-4 6.2.2 step 1): expands W[i] in place when
-// i >= 16 and returns W[i] + K[i].
-template <class P>
+// Message schedule step of round i on the 16-word ring w (FIPS 180-4 6.2.2 step 1), shifts and additions on the FMA
+// pipe: expands W[i] in place when i >= 16 and returns W[i] + K[i].
 __device__ __forceinline__ uint32_t sched(uint32_t (&w)[16], int i, const Opq &o) {
     constexpr uint32_t K[64] = {K256_LIST};
     if (i >= 16) {
         uint32_t w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
-        uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ P::shr3(w15, o);
-        uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ P::shr10(w2, o);
-        w[i & 15] = P::add(P::add(w[i & 15], s0, o), P::add(w[(i + 9) & 15], s1, o), o);
+        uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ fma_shr3(w15, o);
+        uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ fma_shr10(w2, o);
+        w[i & 15] = fma_add(fma_add(w[i & 15], s0, o), fma_add(w[(i + 9) & 15], s1, o), o);
     }
-    return P::add(w[i & 15], K[i], o);
+    return fma_add(w[i & 15], K[i], o);
 }
 
-template <int MODE>
+// sha_compress with the schedule's shifts on the FMA pipe
 __device__ __forceinline__ void sha_compress_t(Sha256State &s, uint32_t (&w)[16], const Opq &o) {
     constexpr uint32_t K[64] = {K256_LIST};
-    typedef Ops<MODE> P;
     uint32_t a = s.h[0], b = s.h[1], c = s.h[2], d = s.h[3], e = s.h[4], f = s.h[5], g = s.h[6], h = s.h[7];
 #pragma unroll
     for (int i = 0; i < 64; i++) {
         // the schedule stays inline: sched() puts W+K ahead of S1/ch, and ptxas then picks another pipe mix for this loop
         if (i >= 16) {
             uint32_t w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
-            uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ P::shr3(w15, o);
-            uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ P::shr10(w2, o);
-            w[i & 15] = P::add(P::add(w[i & 15], s0, o), P::add(w[(i + 9) & 15], s1, o), o);
+            uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ fma_shr3(w15, o);
+            uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ fma_shr10(w2, o);
+            w[i & 15] = (w[i & 15] + s0) + (w[(i + 9) & 15] + s1);
         }
-        uint32_t S1 = rotr(e, 6) ^ rotr(e, 11) ^ P::rotr25(e, o);
+        uint32_t S1 = rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25);
         uint32_t ch = (e & f) ^ (~e & g);
-        uint32_t kw = P::add(w[i & 15], K[i], o);
-        uint32_t t1 = P::add(P::add(h, kw, o), P::add(S1, ch, o), o);
+        uint32_t kw = w[i & 15] + K[i];
+        uint32_t t1 = (h + kw) + (S1 + ch);
         uint32_t S0 = rotr(a, 2) ^ rotr(a, 13) ^ rotr(a, 22);
         uint32_t mj = (a & b) ^ (a & c) ^ (b & c);
-        uint32_t t2 = P::add(S0, mj, o);
-        h = g; g = f; f = e; e = P::add(d, t1, o); d = c; c = b; b = a; a = P::add(t1, t2, o);
+        uint32_t t2 = S0 + mj;
+        h = g; g = f; f = e; e = d + t1; d = c; c = b; b = a; a = t1 + t2;
     }
     s.h[0] += a; s.h[1] += b; s.h[2] += c; s.h[3] += d; s.h[4] += e; s.h[5] += f; s.h[6] += g; s.h[7] += h;
 }
 
 // Tuned kernel.  Same one-lane-per-chunk mapping, but BlockStream's loads and the pipe-balanced compression above.
-// KEYED: encrypt mode's digest SHA-256(chunk || suffix); the plain instantiations ignore `suffix`
-template <int MODE, bool KEYED>
+// KEYED: encrypt mode's digest SHA-256(chunk || suffix); the plain instantiation ignores `suffix`
+template <bool KEYED>
 __global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o, const uint8_t *suffix) {
     uint64_t t;
     if (!sha_slot(a, (uint64_t)blockIdx.x * 32 + threadIdx.x, t)) return;
@@ -334,7 +311,7 @@ __global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o, const uint8_
     for (uint32_t b = 0; b < nblk; b++) {
         uint32_t w[16];
         in.next(b, w);
-        sha_compress_t<MODE>(s, w, o);
+        sha_compress_t(s, w, o);
     }
     sha_done<KEYED>(a, suffix, s, p + (uint64_t)nblk * 64, c, id);
 }
@@ -356,45 +333,28 @@ __global__ void __launch_bounds__(32) k_sha_tuned(ShaArgs a, Opq o, const uint8_
 // ---------------------------------------------------------------------------
 constexpr int SPLIT_STAGES = 3;
 
-// consumer: 64 rounds with W+K supplied.  CMODE 0: IADD3 forms (fewest instructions),
-// CMODE 1: all additions on the FMA pipe (a*1+b with an opaque 1),
-// CMODE 2: the two additions on the chain (e', a') stay IADD3, everything that only depends on values known at the
-//          start of the round (h+kw, d+h+kw, h+kw+maj) and the Sigma0 add go to the FMA pipe: 12 ALU + 4 FMA per round.
-template <int CMODE>
-__device__ __forceinline__ void sha_rounds(Sha256State &s, const uint4 (&kwv)[16], const Opq &o) {
-    typedef Ops<CMODE ? 1 : 0> P;
+// consumer: 64 rounds with W+K supplied, in IADD3 forms (fewest instructions)
+__device__ __forceinline__ void sha_rounds(Sha256State &s, const uint4 (&kwv)[16]) {
     uint32_t a = s.h[0], b = s.h[1], c = s.h[2], d = s.h[3], e = s.h[4], f = s.h[5], g = s.h[6], h = s.h[7];
 #pragma unroll
     for (int i = 0; i < 64; i++) {
         const uint4 v = kwv[i >> 2];
         const uint32_t kw = (i & 3) == 0 ? v.x : (i & 3) == 1 ? v.y : (i & 3) == 2 ? v.z : v.w;
-        uint32_t hk = P::add(h, kw, o);            // off the critical path (h is 3 rounds old)
-        uint32_t dhk = P::add(d, hk, o);
+        uint32_t hk = h + kw;                     // off the critical path (h is 3 rounds old)
+        uint32_t dhk = d + hk;
         uint32_t S1 = rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25);
         uint32_t ch = (e & f) ^ (~e & g);
         uint32_t S0 = rotr(a, 2) ^ rotr(a, 13) ^ rotr(a, 22);
         uint32_t mj = (a & b) ^ (a & c) ^ (b & c);
-        uint32_t en, an;
-        if (CMODE == 2) {
-            uint32_t m = P::add(P::add(hk, mj, o), S0, o);
-            en = S1 + ch + dhk;                   // IADD3 (on the e chain)
-            an = S1 + ch + m;                     // IADD3 (on the a chain)
-        } else if (CMODE) {
-            uint32_t s1ch = P::add(S1, ch, o);
-            en = P::add(s1ch, dhk, o);
-            uint32_t x = P::add(P::add(S0, mj, o), hk, o);
-            an = P::add(s1ch, x, o);
-        } else {
-            en = S1 + ch + dhk;                   // IADD3
-            uint32_t x = S0 + mj + hk;            // IADD3
-            an = x + S1 + ch;                     // IADD3
-        }
+        uint32_t en = S1 + ch + dhk;              // IADD3
+        uint32_t x = S0 + mj + hk;                // IADD3
+        uint32_t an = x + S1 + ch;                // IADD3
         h = g; g = f; f = e; e = en; d = c; c = b; b = a; a = an;
     }
     s.h[0] += a; s.h[1] += b; s.h[2] += c; s.h[3] += d; s.h[4] += e; s.h[5] += f; s.h[6] += g; s.h[7] += h;
 }
 
-template <int PMODE, int CMODE, bool KEYED>
+template <bool KEYED>
 __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o, const uint8_t *suffix) {
     __shared__ __align__(16) uint4 ring[SPLIT_STAGES][16][32];   // [stage][4 rounds][lane] = W+K
     __shared__ __align__(8) uint64_t bars[2 * SPLIT_STAGES];
@@ -431,7 +391,7 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o, const uint8_
                 in.next(b, w);
 #pragma unroll
                 for (int i = 0; i < 64; i++) {
-                    kw[i & 3] = sched<Ops<PMODE>>(w, i, o);
+                    kw[i & 3] = sched(w, i, o);
                     if ((i & 3) == 3) ring[stage][i >> 2][lane] = make_uint4(kw[0], kw[1], kw[2], kw[3]);
                 }
             }
@@ -449,7 +409,7 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o, const uint8_
                 uint4 kwv[16];
 #pragma unroll
                 for (int k = 0; k < 16; k++) kwv[k] = ring[stage][k][lane];
-                sha_rounds<CMODE>(s, kwv, o);
+                sha_rounds(s, kwv);
             }
             mbar_arrive(empty[stage]);
             if (++stage == SPLIT_STAGES) { stage = 0; phase ^= 1; }
@@ -458,28 +418,13 @@ __global__ void __launch_bounds__(64) k_sha_split(ShaArgs a, Opq o, const uint8_
     }
 }
 
-// throughput kernel (mode 0: the compiler's own pipe choice; 2: + schedule shifts on the FMA pipe;
-// 1/3/7: more aggressive offloads -- see DESIGN.md and tools/sha_lab.cu).  `mode` comes from the context
-// (PBSGPU_SHA_MODE read once per pbsgpu_open), never from process-wide state.
-cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix) {
+// throughput kernel
+cudaError_t launch_sha_tuned(const ShaArgs &a, cudaStream_t st, const uint8_t *suffix) {
     if (a.chunk_cap == 0) return cudaSuccess;
-    if (tune.mode >= 10 && a.part == 0) return launch_sha_split(a, tune, st, suffix);
-    Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
+    Opq o{1u, 1u << 29, 1u << 22};
     unsigned blocks = (unsigned)((a.chunk_cap + 31) / 32);
-    if (suffix) switch (tune.mode) {
-        case 0: k_sha_tuned<0, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
-        case 1: k_sha_tuned<1, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
-        case 3: k_sha_tuned<3, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
-        case 7: k_sha_tuned<7, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
-        default: k_sha_tuned<2, true><<<blocks, 32, 0, st>>>(a, o, suffix); break;
-    }
-    else switch (tune.mode) {
-        case 0: k_sha_tuned<0, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
-        case 1: k_sha_tuned<1, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
-        case 3: k_sha_tuned<3, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
-        case 7: k_sha_tuned<7, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
-        default: k_sha_tuned<2, false><<<blocks, 32, 0, st>>>(a, o, nullptr); break;
-    }
+    if (suffix) k_sha_tuned<true><<<blocks, 32, 0, st>>>(a, o, suffix);
+    else k_sha_tuned<false><<<blocks, 32, 0, st>>>(a, o, nullptr);
     return cudaGetLastError();
 }
 
@@ -489,31 +434,20 @@ cudaError_t launch_sha_tuned(const ShaArgs &a, const ShaTune &tune, cudaStream_t
 // (part 1) each CTA therefore also asks for `spread_kb` KiB of dummy dynamic shared memory, which caps the
 // CTAs per SM (30 -> 4, 85 -> 2, 112 -> 1) and forces the spread; the throughput kernel uses no shared
 // memory and still co-resides.
-template <int PM, int CM>
-static cudaError_t launch_split_t(const ShaArgs &a, const Opq &o, unsigned blocks, int spread_kb, cudaStream_t st,
-                                  const uint8_t *suffix) {
+cudaError_t launch_sha_split(const ShaArgs &a, int spread_kb, cudaStream_t st, const uint8_t *suffix) {
+    if (a.chunk_cap == 0) return cudaSuccess;
+    Opq o{1u, 1u << 29, 1u << 22};
+    unsigned blocks = (unsigned)((a.chunk_cap + 31) / 32);
     size_t dyn = 0;
     if (a.part == 1 && spread_kb > 0) {
         dyn = (size_t)spread_kb * 1024;
-        cudaError_t e = cudaFuncSetAttribute(suffix ? k_sha_split<PM, CM, true> : k_sha_split<PM, CM, false>,
+        cudaError_t e = cudaFuncSetAttribute(suffix ? k_sha_split<true> : k_sha_split<false>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
         if (e != cudaSuccess) return e;
     }
-    if (suffix) k_sha_split<PM, CM, true><<<blocks, 64, dyn, st>>>(a, o, suffix);
-    else k_sha_split<PM, CM, false><<<blocks, 64, dyn, st>>>(a, o, nullptr);
+    if (suffix) k_sha_split<true><<<blocks, 64, dyn, st>>>(a, o, suffix);
+    else k_sha_split<false><<<blocks, 64, dyn, st>>>(a, o, nullptr);
     return cudaGetLastError();
-}
-cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t st, const uint8_t *suffix) {
-    if (a.chunk_cap == 0) return cudaSuccess;
-    Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
-    unsigned blocks = (unsigned)((a.chunk_cap + 31) / 32);
-    switch (tune.mode) {
-        case 10: return launch_split_t<0, 0>(a, o, blocks, tune.spread_kb, st, suffix);
-        case 12: return launch_split_t<0, 1>(a, o, blocks, tune.spread_kb, st, suffix);
-        case 13: return launch_split_t<3, 1>(a, o, blocks, tune.spread_kb, st, suffix);
-        case 14: return launch_split_t<3, 2>(a, o, blocks, tune.spread_kb, st, suffix);
-        default: return launch_split_t<3, 0>(a, o, blocks, tune.spread_kb, st, suffix);   // producer balanced, consumer IADD3
-    }
 }
 
 // number of leading entries (lengths sorted descending) longer than `threshold`, rounded up to 32 and
@@ -521,31 +455,21 @@ cudaError_t launch_sha_split(const ShaArgs &a, const ShaTune &tune, cudaStream_t
 // otherwise structured data cuts every chunk at max) only the longest ones go there and the rest stays
 // with the throughput kernel on the big partition
 __global__ void k_split_point(const uint32_t *len_sorted_desc, const unsigned long long *n_chunks, uint64_t cap,
-                              uint32_t threshold, unsigned long long max_head, unsigned long long *n_head,
-                              uint32_t threshold_mid, unsigned long long *n_mid) {
+                              uint32_t threshold, unsigned long long max_head, unsigned long long *n_head) {
     const unsigned long long n = live_count(*n_chunks, cap);
-    auto first_le = [&](uint32_t thr) {     // first index with len <= thr (lengths sorted descending)
-        unsigned long long lo = 0, hi = n;
-        while (lo < hi) {
-            unsigned long long mid = (lo + hi) >> 1;
-            if (len_sorted_desc[mid] > thr) lo = mid + 1; else hi = mid;
-        }
-        return lo;
-    };
-    unsigned long long h = (first_le(threshold) + 31) & ~31ull;
+    unsigned long long lo = 0, hi = n;      // first index with len <= threshold (lengths sorted descending)
+    while (lo < hi) {
+        unsigned long long mid = (lo + hi) >> 1;
+        if (len_sorted_desc[mid] > threshold) lo = mid + 1; else hi = mid;
+    }
+    unsigned long long h = (lo + 31) & ~31ull;
     if (h > max_head) h = max_head & ~31ull;
     if (h > n) h = n;
     *n_head = h;
-    if (n_mid) {
-        unsigned long long m = (first_le(threshold_mid) + 31) & ~31ull;
-        if (m > n) m = n;
-        *n_mid = m < h ? h : m;
-    }
 }
 cudaError_t launch_split_point(const uint32_t *len_sorted_desc, const unsigned long long *n_chunks, uint64_t cap,
-                               uint32_t threshold, unsigned long long max_head, unsigned long long *n_head,
-                               uint32_t threshold_mid, unsigned long long *n_mid, cudaStream_t st) {
-    k_split_point<<<1, 1, 0, st>>>(len_sorted_desc, n_chunks, cap, threshold, max_head, n_head, threshold_mid, n_mid);
+                               uint32_t threshold, unsigned long long max_head, unsigned long long *n_head, cudaStream_t st) {
+    k_split_point<<<1, 1, 0, st>>>(len_sorted_desc, n_chunks, cap, threshold, max_head, n_head);
     return cudaGetLastError();
 }
 

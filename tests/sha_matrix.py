@@ -1,10 +1,12 @@
-"""The matrix that pins K3 (csrc/sha256.cu): every kernel instantiation, every launch path, the inputs that put each
-one at its edges, and the hashlib reference.  Importing it needs no GPU; test_gpu_sha_matrix.py runs the matrix and
-test_sha_matrix_cpu.py fails when sha256.cu or capi.cu gains a mode or a knob that is not listed here.
+"""The matrix that pins K3 (csrc/sha256.cu): every kernel, every launch path, the inputs that put each one at its
+edges, and the hashlib reference.  Importing it needs no GPU; test_gpu_sha_matrix.py runs the matrix and
+test_sha_matrix_cpu.py fails when sha256.cu or capi.cu gains a kernel instantiation or a knob that is not listed here.
 
-- MODES: every PBSGPU_SHA_MODE with a kernel of its own (throughput mixes 0/1/2/3/7, split-only 10..14; 2 and 11 are
-  the defaults of their switches).  KERNELS adds the simple cross-check kernel (PBSGPU_VARIANT=1) as its own entry.
-- PATHS: the K3 launch paths of the batch job, as the environment a context is opened with.
+- KERNELS: the kernels of the blocking byte-range calls: the throughput kernel (k_sha_tuned, the default) and the
+  simple cross-check kernel (PBSGPU_VARIANT=1).
+- PATHS: the K3 launch paths of the batch job, as the environment a context is opened with.  The latency kernel
+  (k_sha_split) runs on the hybrid ones; "split_every_chunk" (without the SM partition) and
+  "split_every_chunk_partitioned" (on the long-chunk partition) give it every chunk of a job.
 - The reference is hashlib: SHA-256(chunk), and SHA-256(chunk || id_key) for encrypt mode's keyed digests, with
   id_key from crypt_ref (PBKDF2 in hashlib).  Nothing from the library computes an expected value.
 """
@@ -16,8 +18,7 @@ import numpy as np
 
 import crypt_ref
 
-MODES = [0, 1, 2, 3, 7, 10, 11, 12, 13, 14]
-KERNELS = {**{f"mode{m}": {"PBSGPU_SHA_MODE": str(m)} for m in MODES}, "simple": {"PBSGPU_VARIANT": "1"}}
+KERNELS = {"tuned": {}, "simple": {"PBSGPU_VARIANT": "1"}}
 
 AVG = 1 << 16                     # the streams' chunker: min 16 KiB, max 256 KiB = 4 x AVG
 MAX_OVER_AVG_X10 = 40
@@ -28,13 +29,15 @@ PATHS = {
     "throughput": {"PBSGPU_SHA_HYBRID": "0"},
     "hybrid_nopart": {"PBSGPU_SHA_HYBRID": "2", "PBSGPU_PARTITION_SMS": "0"},
     "partitioned": {},
-    "serial": {"PBSGPU_HYBRID_SERIAL": "1"},
     "spread0": {"PBSGPU_SPLIT_SPREAD_KB": "0"},
     "spread85": {"PBSGPU_SPLIT_SPREAD_KB": "85"},
     # 1 x 24 chunks rounded down to whole CTAs of 32: the split kernel launches with an empty head
     "head_per_sm1": {"PBSGPU_SHA_HYBRID": "2", "PBSGPU_PARTITION_SMS": "0", "PBSGPU_HYBRID_HEAD_PER_SM": "1"},
-    # parts 3 (chunks over 1.2 x avg, high-priority stream) and 4 beside the head of chunks over 2 x avg
-    "mid": {"PBSGPU_BULK_MID_X10": "12", "PBSGPU_HYBRID_THR_X10": "20"},
+    # threshold 0 and a head limit of 64 x 24 chunks (24: the default partition's SMs, and the count assumed without
+    # one): every chunk of a job with up to 1536 of them takes the latency kernel
+    "split_every_chunk": {"PBSGPU_SHA_HYBRID": "2", "PBSGPU_PARTITION_SMS": "0", "PBSGPU_HYBRID_THR_X10": "0",
+                          "PBSGPU_HYBRID_HEAD_PER_SM": "64"},
+    "split_every_chunk_partitioned": {"PBSGPU_HYBRID_THR_X10": "0", "PBSGPU_HYBRID_HEAD_PER_SM": "64"},
     "variant1": {"PBSGPU_VARIANT": "1"},
     **{name: {"PBSGPU_HYBRID_THR_X10": str(thr)} for name, thr in SPLIT_AT.items()},
 }
@@ -61,14 +64,19 @@ def layout(lens, residues, shift: int = 0):
 
 
 def edge_lens() -> tuple[list[int], list[int]]:
-    """(lengths, start residues mod 16): 0..300 twice, each length mod 64 at several start residues, then 64k + r for
-    every r in 0..63 and k in {4, 17, 1000}.  The keyed suffix moves the one-or-two final block boundary from
-    len % 64 = 56 to 24, and for residues 33..63 the suffix itself crosses a block edge."""
+    """(lengths, start residues mod 16): 0..300 twice, each length mod 64 at several start residues, 64k + d around
+    the padding edges for k in {5, 16, 63, 64}, then 64k + r for every r in 0..63 and k in {4, 17, 1000}.  The keyed
+    suffix moves the one-or-two final block boundary from len % 64 = 56 to 24, and for residues 33..63 the suffix
+    itself crosses a block edge."""
     lens, res = [], []
     for half in (0, 8):
         for n in range(301):
             lens.append(n)
             res.append((n + 7 * (n // 64) + half) % 16)
+    for k in (5, 16, 63, 64):
+        for d in (-9, -8, -1, 0, 1, 55, 56):
+            lens.append(64 * k + d)
+            res.append((k + 3 * d) % 16)
     for ki, k in enumerate((4, 17, 1000)):
         for r in range(64):
             lens.append(64 * k + r)
@@ -80,9 +88,18 @@ def edges():
     return layout(*edge_lens())
 
 
+# The edge set as streams of one chunk each: at this average the minimum chunk (avg / 4) is longer than any edge
+# range, so every stream ends in its EOF chunk, which may have any length.
+EDGE_AVG = 1 << 18
+# Messages of 512 MiB - 1, 512 MiB and 512 MiB + 1 as all-zero streams: a zero background has no boundary candidate
+# (scan_ref), so each is one chunk, and at this average (maximum 2 GiB) the job takes them whole.
+LONG_AVG = 1 << 29
+LONG_ZERO = [(1 << 29) - 1, 1 << 29, (1 << 29) + 1]
+
+
 def long_lens() -> list[int]:
     """A few multi-MiB ranges for the split kernels' many-block chains, at both keyed finish forms."""
-    return [(3 << 20) + 5, (4 << 20) + 23, (4 << 20) + 24, (5 << 20) + 63, 6 << 20]
+    return [(3 << 20) + 5, (4 << 20) + 23, (4 << 20) + 24, (5 << 20) + 63, 6 << 20, 8 << 20]
 
 
 def edges_and_long():
@@ -96,8 +113,7 @@ def edges_and_long():
 def stream_parts() -> list[np.ndarray]:
     """Random streams with zero runs (the chunker cuts them at the maximum, 4 x AVG), a short stream and an empty
     one: about ten maximum-length chunks among a few hundred, so that the SPLIT_AT thresholds put the split point at
-    0, at a multiple of 32 short of n and at n (n itself not a multiple of 32), and the "mid" path has a non-empty mid
-    class behind its head (test_sha_matrix_cpu checks each)."""
+    0, at a multiple of 32 short of n and at n (n itself not a multiple of 32) (test_sha_matrix_cpu checks each)."""
     rng = np.random.default_rng(31)
     parts = []
     for i in range(6):

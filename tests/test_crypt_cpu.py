@@ -168,16 +168,9 @@ def test_batch_opts_keeps_the_old_layout_in_front_of_crypt():
     assert _lib.BatchOpts.crypt.offset == 48 and C.sizeof(_lib.BatchOpts) == 56
 
 
-# The plain K3 kernels keep their code in encrypt mode's build: the keyed digests are separate instantiations.
-# tests/golden/k3_sass_sha256.json holds the SHA-256 of every K3 kernel's SASS (addresses stripped) as the parent commit
-# compiled it with the nvcc named there; the plain instantiations now carry a `false` KEYED argument and an unused
-# suffix parameter in their mangled names.
-def _plain_name(parent: str) -> str:
-    name = re.sub(r"^(_ZN6pbsgpu11k_sha_tunedILi\d)(EEEvNS_7ShaArgsENS_3OpqE)$", r"\1ELb0\2PKh", parent)
-    return re.sub(r"^(_ZN6pbsgpu11k_sha_splitILi\dELi\d)(EEEvNS_7ShaArgsENS_3OpqE)$", r"\1ELb0\2PKh", name)
-
-
-def test_plain_sha256_kernels_compile_to_the_parents_sass(tmp_path):
+# tests/golden/k3_sass_sha256.json holds the SHA-256 of every K3 kernel's SASS (addresses stripped), plain and keyed, as
+# the nvcc named there compiles csrc/sha256.cu: a change to the kernels' code shows up here.
+def test_sha256_kernels_compile_to_the_golden_sass(tmp_path):
     import json
     import shutil
     import subprocess
@@ -190,8 +183,8 @@ def test_plain_sha256_kernels_compile_to_the_parents_sass(tmp_path):
         pytest.skip(f"the golden SASS is from nvcc {golden['nvcc']}")
     obj = tmp_path / "sha256.o"
     subprocess.check_call([build.NVCC, *build.FLAGS, "-c", str(ROOT / "pbs_plus_b200" / "csrc" / "sha256.cu"), "-o", str(obj)])
-    for parent, want in golden["kernels"].items():
-        txt = subprocess.run(["cuobjdump", "-sass", "-fun", _plain_name(parent), str(obj)], capture_output=True, text=True).stdout
+    for name, want in golden["kernels"].items():
+        txt = subprocess.run(["cuobjdump", "-sass", "-fun", name, str(obj)], capture_output=True, text=True).stdout
         lines = [re.sub(r"/\*[0-9a-f]{4,5}\*/", "", ln).strip() for ln in txt.splitlines()
                  if re.search(r"/\*[0-9a-f]{4,5}\*/|/\* 0x", ln)]
-        assert lines and hashlib.sha256("\n".join(lines).encode()).hexdigest() == want, parent
+        assert lines and hashlib.sha256("\n".join(lines).encode()).hexdigest() == want, name

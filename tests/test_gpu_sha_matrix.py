@@ -1,9 +1,10 @@
 """The K3 matrix (tests/sha_matrix.py) on the GPU: every SHA-256 kernel instantiation, plain and keyed, against hashlib.
 
-- the blocking byte-range calls in every mode and the simple variant, over the padding edges and multi-MiB ranges,
-  from a host base and a ragged device base;
+- the blocking byte-range calls with the throughput kernel and the simple variant, over the padding edges and
+  multi-MiB ranges, from a host base and a ragged device base;
 - the batch job on every launch path: the cuts equal the oracle's and the digests are hashlib's of those cuts, for the
   chunker (blocking call and early-input-release job) and for fixed-size cuts;
+- the latency kernel over the padding edges and past 2^32 bits, each range a stream of one chunk in its head;
 - the blocking decode of encrypted DataBlobs, whose keyed digest check is the other caller of the blocking launch;
 - messages of 512 MiB and more, whose bit length needs the high length word, and the refusal of a 4 GiB range."""
 import os
@@ -129,6 +130,49 @@ def test_job_paths_give_hashlib_digests_at_the_oracle_cuts(torch, streams, path)
         e.close()
 
 
+# ---- the latency kernel at the padding edges and past 2^32 bits: one chunk per stream, every chunk in the head -----
+def one_chunk_each(rec, lens, streams, keyed, what):
+    """rec has one chunk per non-empty stream, the whole stream, with hashlib's digest of it"""
+    nz = [s for s, n in enumerate(lens) if n]
+    assert rec["stream"].tolist() == nz and rec["end_off"].tolist() == [lens[s] for s in nz], what
+    bad = [s for s, d in zip(nz, rec["digest"]) if d.tobytes() != M.digest(streams(s), keyed)]
+    assert not bad, (what, bad[:8], len(bad))
+
+
+@pytest.mark.parametrize("path", ["split_every_chunk", "split_every_chunk_partitioned"])
+def test_split_kernel_digests_at_the_padding_edges(torch, path):
+    buf, off, ln = M.edges()
+    lens = [int(n) for n in ln]
+    e = engine(M.PATHS[path])
+    try:
+        c = e.crypt(M.KEY)
+        cfg = pg.make_config(M.EDGE_AVG)
+        for keyed in (False, True):
+            rec = e.chunk_digest_batch(cfg, buf, off, ln, crypt=c if keyed else None)
+            one_chunk_each(rec, lens, lambda s: buf[int(off[s]): int(off[s]) + lens[s]], keyed, (path, "edges", keyed))
+        c.close()
+    finally:
+        e.close()
+
+
+@pytest.mark.parametrize("path", ["split_every_chunk", "split_every_chunk_partitioned"])
+def test_split_kernel_digests_past_2_pow_32_bits(torch, path):
+    lens = M.LONG_ZERO
+    off = np.cumsum([0] + lens[:-1]).astype(np.uint64) + np.arange(len(lens), dtype=np.uint64) * 7 + 3
+    dev = torch.zeros(int(off[-1]) + lens[-1] + 64, dtype=torch.uint8, device="cuda")
+    e = engine(M.PATHS[path])
+    try:
+        c = e.crypt(M.KEY)
+        cfg = pg.make_config(M.LONG_AVG)
+        for keyed in (False, True):
+            rec = e.chunk_digest_batch(cfg, dev, off, np.array(lens, np.uint64), crypt=c if keyed else None)
+            one_chunk_each(rec, lens, lambda s: np.zeros(lens[s], np.uint8), keyed, (path, "zeros", keyed))
+        c.close()
+    finally:
+        e.close()
+        del dev
+
+
 # ---- the decode of encrypted DataBlobs: the other caller of the blocking launch ---------------------------------
 @pytest.fixture(scope="module")
 def enc_blobs():
@@ -144,7 +188,7 @@ def enc_blobs():
     return blobs, ln, b"".join(expected(buf, off, ln, True))
 
 
-@pytest.mark.parametrize("kernel", ["mode2", "mode7", "mode13", "simple"])
+@pytest.mark.parametrize("kernel", list(M.KERNELS))
 def test_encrypted_blob_decode_checks_keyed_digests(enc_blobs, kernel):
     blobs, ln, keyed = enc_blobs
     e = engine(M.KERNELS[kernel])
@@ -182,7 +226,7 @@ def long_ranges(torch):
     del dev
 
 
-@pytest.mark.parametrize("kernel", ["mode2", "simple", "mode13"])
+@pytest.mark.parametrize("kernel", list(M.KERNELS))
 def test_messages_past_2_pow_32_bits(long_ranges, kernel):
     dev, off, ln, plain, keyed = long_ranges
     e = engine(M.KERNELS[kernel])

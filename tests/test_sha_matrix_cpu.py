@@ -1,6 +1,6 @@
-"""The K3 matrix covers what ships: every mode arm of csrc/sha256.cu's launch switches is in sha_matrix.MODES, every
-K3 knob capi.cu reads at open is set by sha_matrix.PATHS or KERNELS, and the matrix's inputs reach the edges they are
-meant to.  A new instantiation or knob that nobody adds to the matrix fails here, on any machine."""
+"""The K3 matrix covers what ships: csrc/sha256.cu has one throughput and one latency kernel, each plain and keyed,
+every K3 knob capi.cu reads at open is set by sha_matrix.PATHS or KERNELS, and the matrix's inputs reach the edges they
+are meant to.  A new instantiation or knob that nobody adds to the matrix fails here, on any machine."""
 import re
 from pathlib import Path
 
@@ -9,59 +9,33 @@ import numpy as np
 import sha_matrix as M
 
 CSRC = Path(__file__).resolve().parent.parent / "pbs_plus_b200" / "csrc"
+# every variable capi.cu reads: a knob added or brought back fails here until it is listed (and, for K3, in the matrix)
+CAPI_ENV = {"PBSGPU_ARENA_FRAC_X16", "PBSGPU_ARENA_MB", "PBSGPU_DEBUG", "PBSGPU_HYBRID_HEAD_PER_SM", "PBSGPU_HYBRID_THR_X10",
+            "PBSGPU_KEEP_ENV", "PBSGPU_PARTITION_SMS", "PBSGPU_SCAN_LANES", "PBSGPU_SCAN_SMS", "PBSGPU_SHA_HYBRID",
+            "PBSGPU_SLOTS", "PBSGPU_SPLIT_SPREAD_KB", "PBSGPU_STAGE_BYTES", "PBSGPU_STREAM_NBUF", "PBSGPU_STREAM_WINDOW",
+            "PBSGPU_VARIANT", "PBSGPU_XXH3_CAP_BLOCKS"}
 
 
-def function_body(src: str, signature: str) -> str:
-    """The text of the function whose definition starts with `signature`, up to its closing brace at column 0."""
-    i = src.index(signature)
-    return src[i: src.index("\n}\n", i)]
-
-
-def switches(body: str) -> list[str]:
-    """The switch statements of a function body, each up to the next switch (or the end of the body)."""
-    parts = re.split(r"\bswitch\s*\(tune\.mode\)", body)
-    assert len(parts) >= 2, "no switch on tune.mode"
-    return parts[1:]
-
-
-def cases(sw: str) -> set[int]:
-    return {int(m) for m in re.findall(r"\bcase\s+(\d+)\s*:", sw)}
-
-
-def test_every_mode_arm_is_in_the_matrix():
+def test_one_kernel_instantiation_per_keyed_value():
     src = (CSRC / "sha256.cu").read_text()
-    tuned = switches(function_body(src, "cudaError_t launch_sha_tuned("))
-    split = switches(function_body(src, "cudaError_t launch_sha_split("))
-    assert len(tuned) == 2 and len(split) == 1
-    keyed, plain = tuned
-    # the keyed and the plain switch have the same arms, and arm N launches the mode-N kernel of its kind
-    assert cases(keyed) == cases(plain)
-    for sw, kind in ((keyed, "true"), (plain, "false")):
-        for n, m, k in re.findall(r"\bcase\s+(\d+)\s*:\s*k_sha_tuned<(\d+),\s*(\w+)>", sw):
-            assert (n, k) == (m, kind), (n, m, k)
-        assert len(re.findall(r"\bcase\s+\d+\s*:\s*k_sha_tuned<", sw)) == len(cases(sw))
-    # the throughput default arm runs mode 2's kernel; the split default runs every mode >= 10 without an arm: 11
-    tuned_default = {int(m) for m in re.findall(r"default\s*:\s*k_sha_tuned<(\d+),", keyed + plain)}
-    assert tuned_default == {2} and 2 not in cases(keyed)
-    assert "default:" in split[0] and 11 not in cases(split[0]) and min(cases(split[0])) >= 10
-    shipped = cases(keyed) | tuned_default | cases(split[0]) | {11}
-    assert shipped == set(M.MODES), sorted(shipped ^ set(M.MODES))
-    assert len(M.MODES) == len(set(M.MODES))
-    # the simple cross-check kernel has its plain and keyed forms, selected by PBSGPU_VARIANT=1
-    assert "k_sha_simple_keyed" in src and M.KERNELS["simple"] == {"PBSGPU_VARIANT": "1"}
-    assert {k: v for k, v in M.KERNELS.items() if k != "simple"} == {f"mode{m}": {"PBSGPU_SHA_MODE": str(m)} for m in M.MODES}
+    # the kernels take KEYED as their only template parameter, and every use names one of its two values
+    for k in ("k_sha_tuned", "k_sha_split"):
+        assert len(re.findall(rf"\b{k}\(", src)) == 1, k
+        assert re.search(rf"template <bool KEYED>\n__global__ void __launch_bounds__\(\d+\) {k}\(", src), k
+        uses = re.findall(rf"\b{k}<([^>]*)>", src)
+        assert uses and set(uses) == {"true", "false"}, (k, uses)
+    assert "k_sha_simple_keyed" in src and M.KERNELS == {"tuned": {}, "simple": {"PBSGPU_VARIANT": "1"}}
 
 
-def test_every_k3_knob_is_in_the_matrix():
+def test_capi_reads_only_listed_knobs_and_the_matrix_sets_every_k3_knob():
     src = (CSRC / "capi.cu").read_text()
     knobs = set(re.findall(r"ctx->tune\.\w+\s*=[^;]*env_int\(\"(PBSGPU_\w+)\"", src))
-    assert {"PBSGPU_SHA_MODE", "PBSGPU_SHA_HYBRID", "PBSGPU_HYBRID_SERIAL"} <= knobs, knobs
+    assert {"PBSGPU_SHA_HYBRID", "PBSGPU_HYBRID_THR_X10", "PBSGPU_SPLIT_SPREAD_KB", "PBSGPU_HYBRID_HEAD_PER_SM"} <= knobs, knobs
     assert re.search(r"env_int\(\"PBSGPU_VARIANT\"", src)
     knobs.add("PBSGPU_VARIANT")
     set_by_paths = {k for env in M.PATHS.values() for k in env}
-    set_by_kernels = {k for env in M.KERNELS.values() for k in env}
-    assert knobs - {"PBSGPU_SHA_MODE"} <= set_by_paths, sorted(knobs - set_by_paths)
-    assert knobs <= set_by_paths | set_by_kernels
+    assert knobs <= set_by_paths, sorted(knobs - set_by_paths)
+    assert set(re.findall(r"\"(PBSGPU_\w+)\"", src)) == CAPI_ENV
 
 
 def test_edge_inputs_reach_every_padding_form_and_alignment():
@@ -79,6 +53,24 @@ def test_edge_inputs_reach_every_padding_form_and_alignment():
     assert {n % 64 for n in M.long_lens()} >= {23, 24, 63}   # keyed: one final block, two, suffix across the edge
 
 
+def test_edge_and_zero_streams_are_one_chunk_each_and_all_in_the_latency_kernels_head():
+    import oracle
+    import scan_ref
+    buf, off, ln = M.edges()
+    lens = ln.tolist()
+    assert max(lens) < M.EDGE_AVG // 4   # below the minimum chunk: no cut
+    cuts = oracle.chunk_digest_streams(oracle.config(M.EDGE_AVG), [buf[int(o): int(o) + n] for o, n in zip(off, lens)])
+    assert cuts["end_off"].tolist() == [n for n in lens if n]
+    env = M.PATHS["split_every_chunk"]
+    assert M.PATHS["split_every_chunk_partitioned"].items() <= env.items()
+    max_head = int(env["PBSGPU_HYBRID_HEAD_PER_SM"]) * 24
+    assert M.split_point(M.chunk_lens(cuts), int(env["PBSGPU_HYBRID_THR_X10"]), max_head) == len(cuts)
+    assert M.split_point(np.array(M.LONG_ZERO), 0, max_head) == 3
+    # plain bit lengths below, at and above 2^32; keyed above; all within the maximum chunk
+    assert [8 * n >= 1 << 32 for n in M.LONG_ZERO] == [False, True, True] and max(M.LONG_ZERO) <= 4 * M.LONG_AVG
+    assert len(scan_ref.candidates(oracle.default_table(), oracle.config(M.LONG_AVG).mask, np.zeros(1 << 20, np.uint8))) == 0
+
+
 def test_stream_inputs_put_the_split_point_at_its_edges():
     import oracle
     (buf, off, ln), parts = M.pack_streams(M.stream_parts())
@@ -93,10 +85,5 @@ def test_stream_inputs_put_the_split_point_at_its_edges():
     assert at["split_32k"] % 32 == 0 and 0 < at["split_32k"] < n
     # the default threshold has a head; the head limit of 1 x 24 chunks empties it
     assert M.split_point(lens, 25) > 0 and M.split_point(lens, 25, max_head=24) == 0
-    # the mid path: a head of chunks over 2 x avg and a non-empty mid class behind it
-    env = M.PATHS["mid"]
-    head = M.split_point(lens, int(env["PBSGPU_HYBRID_THR_X10"]))
-    mid = M.split_point(lens, int(env["PBSGPU_BULK_MID_X10"]))
-    assert 0 < head < mid < n
     assert M.fixed_cuts(parts, 1 << 18)[-1] == (len(parts) - 1, len(parts[-1]))
     assert np.all(np.array([e for _, e in M.fixed_cuts(parts, 1 << 18)]) > 0)

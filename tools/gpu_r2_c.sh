@@ -25,7 +25,6 @@ run p40_t15_h96 PBSGPU_PARTITION_SMS=40 PBSGPU_HYBRID_THR_X10=15 PBSGPU_HYBRID_H
 run p32_t15_h128 PBSGPU_PARTITION_SMS=32 PBSGPU_HYBRID_THR_X10=15 PBSGPU_HYBRID_HEAD_PER_SM=128 | tee -a gpurun_out/r2c_sweep.txt
 run p24_t20_h64 PBSGPU_HYBRID_THR_X10=20 PBSGPU_HYBRID_HEAD_PER_SM=64 | tee -a gpurun_out/r2c_sweep.txt
 run p16 PBSGPU_PARTITION_SMS=16 | tee -a gpurun_out/r2c_sweep.txt
-run mode0 PBSGPU_SHA_MODE=0 | tee -a gpurun_out/r2c_sweep.txt
 run lanes PBSGPU_SCAN_LANES=1 | tee -a gpurun_out/r2c_sweep.txt
 run k32 X=1 | tee -a gpurun_out/r2c_sweep.txt
 timeout 600 python bench.py --steps 20 --warmup 3 --no-e2e --no-cpu --no-verify > gpurun_out/r2c_bench_distinct.txt 2>&1; tail -c 1200 gpurun_out/r2c_bench_distinct.txt

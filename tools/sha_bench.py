@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """K3 alone at saturation: SHA-256 of N equal ranges (no length imbalance, no tail).
-usage: PBSGPU_SHA_MODE=m python tools/sha_bench.py [range_kib] [total_gib]"""
-import os, sys, time
+usage: python tools/sha_bench.py [range_kib] [total_gib]"""
+import sys, time
 from pathlib import Path
 import numpy as np
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -24,4 +24,4 @@ for _ in range(3):
     best = min(best, dt)
 import hashlib
 chk = hashlib.sha256(buf[int(off[5]): int(off[5]) + int(ln[5])].cpu().numpy().tobytes()).digest() == bytes(d[5])
-print(f"mode {os.environ.get('PBSGPU_SHA_MODE','default')} ranges {n} x {rk} KiB: {ln.sum()/best/1e9:.1f} GB/s  ({best*1e3:.1f} ms) ok={chk}")
+print(f"ranges {n} x {rk} KiB: {ln.sum()/best/1e9:.1f} GB/s  ({best*1e3:.1f} ms) ok={chk}")

@@ -16,7 +16,7 @@
 #include <string.h>
 #include <vector>
 
-#include "../pbs_plus_b200/csrc/sha256.cu"   // product kernels (k_sha_tuned<M>, k_sha_split<P,C>) for side-by-side timing, and their loader
+#include "../pbs_plus_b200/csrc/sha256.cu"   // product kernels (k_sha_tuned, k_sha_split) for side-by-side timing, and their loader
 using pbsgpu::ChunkRef;
 using pbsgpu::ShaArgs;
 
@@ -166,15 +166,15 @@ template <int V, int THREADS, int MINB> static void lab(const Work &w) {
 }
 static ShaArgs sha_args(const Work &w) {
     ShaArgs a; a.base = w.buf; a.off = nullptr; a.chunks = w.refs; a.order = nullptr; a.n_chunks = w.n_dev; a.chunk_cap = w.n;
-    a.digests = w.dig; a.n_head = nullptr; a.n_mid = nullptr; a.part = 0; return a;
+    a.digests = w.dig; a.n_head = nullptr; a.part = 0; return a;
 }
-template <int M> static void prod_tuned(const Work &w) {
-    pbsgpu::Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
-    pbsgpu::k_sha_tuned<M, false><<<(w.n + 31) / 32, 32>>>(sha_args(w), o, nullptr);
+static void prod_tuned(const Work &w) {
+    pbsgpu::Opq o{1u, 1u << 29, 1u << 22};
+    pbsgpu::k_sha_tuned<false><<<(w.n + 31) / 32, 32>>>(sha_args(w), o, nullptr);
 }
-template <int P, int C> static void prod_split(const Work &w) {
-    pbsgpu::Opq o{1u, 1u << 29, 1u << 22, 1u << 7};
-    pbsgpu::k_sha_split<P, C, false><<<(w.n + 31) / 32, 64>>>(sha_args(w), o, nullptr);
+static void prod_split(const Work &w) {
+    pbsgpu::Opq o{1u, 1u << 29, 1u << 22};
+    pbsgpu::k_sha_split<false><<<(w.n + 31) / 32, 64>>>(sha_args(w), o, nullptr);
 }
 
 static const Variant VS[] = {
@@ -183,7 +183,7 @@ static const Variant VS[] = {
     {"v7   v3 + off-critical round adds    32 thr, <=72 regs", lab<7, 32, 28>},
     {"v11  ALL adds on FMA                 32 thr, <=72 regs", lab<11, 32, 28>},
     {"v27  v11 + sched shifts IMAD.HI      32 thr, <=72 regs", lab<27, 32, 28>},
-    {"v16  sched shifts IMAD.HI (= mode 2) 32 thr, <=72 regs", lab<16, 32, 28>},
+    {"v16  sched shifts IMAD.HI (= tuned)  32 thr, <=72 regs", lab<16, 32, 28>},
     {"v0                                   32 thr, <=64 regs", lab<0, 32, 32>},
     {"v11                                  32 thr, <=64 regs", lab<11, 32, 32>},
     {"v27                                  32 thr, <=64 regs", lab<27, 32, 32>},
@@ -199,11 +199,8 @@ static const Variant VS[] = {
     {"v27                                 128 thr, <=56 regs", lab<27, 128, 9>},
     {"v11                                 128 thr, <=48 regs", lab<11, 128, 10>},
     {"v0                                  128 thr, <=48 regs", lab<0, 128, 10>},
-    {"product k_sha_tuned<2>", prod_tuned<2>},
-    {"product k_sha_tuned<3>", prod_tuned<3>},
-    {"product k_sha_split<3,0>", prod_split<3, 0>},
-    {"product k_sha_split<3,1>", prod_split<3, 1>},
-    {"product k_sha_split<3,2>", prod_split<3, 2>},
+    {"product k_sha_tuned", prod_tuned},
+    {"product k_sha_split", prod_split},
 };
 static const int NV = (int)(sizeof VS / sizeof VS[0]);
 
@@ -278,19 +275,17 @@ int main(int argc, char **argv) {
         // load curve: C concurrent chains of equal length; time per 64 B block of a chain = the chain latency that bounds
         // a batch's makespan, GB/s = throughput at that load.  C = 132 SMs x 4 sub-partitions x 32 lanes x {1/4 .. 8} warps.
         const uint64_t chain = (argc > 2 ? atoll(argv[2]) : 1024) << 10;   // bytes per chain
-        int picks[7] = {0, 3, 4, -1, -1, -1, -1};                               // v0, v11, v27, then tuned<2>, split<3,0>, split<3,1> by name
+        int picks[5] = {0, 3, 4, -1, -1};                                       // v0, v11, v27, then the product kernels by name
         for (int v = 0; v < NV; v++) {
-            if (!strcmp(VS[v].name, "product k_sha_tuned<2>")) picks[3] = v;
-            if (!strcmp(VS[v].name, "product k_sha_split<3,0>")) picks[4] = v;
-            if (!strcmp(VS[v].name, "product k_sha_split<3,1>")) picks[5] = v;
-            if (!strcmp(VS[v].name, "product k_sha_split<3,2>")) picks[6] = v;
+            if (!strcmp(VS[v].name, "product k_sha_tuned")) picks[3] = v;
+            if (!strcmp(VS[v].name, "product k_sha_split")) picks[4] = v;
         }
         const uint32_t base_c = (uint32_t)sms * 4 * 32;
         const double mult[] = {0.25, 0.5, 1, 2, 4, 8};
         const uint32_t max_n = (uint32_t)(base_c * 8);
         B.init((uint64_t)max_n * chain > (64ull << 30) ? (64ull << 30) : (uint64_t)max_n * chain, max_n);
         printf("chains of %llu KiB; C chains = m x %u (one warp per sub-partition at m = 1)\n", (unsigned long long)(chain >> 10), base_c);
-        for (int pi = (argc > 3 ? atoi(argv[3]) : 0); pi < 7; pi++) {
+        for (int pi = (argc > 3 ? atoi(argv[3]) : 0); pi < 5; pi++) {
             for (int mi = 0; mi < 6; mi++) {
                 const uint32_t n = (uint32_t)(base_c * mult[mi]);
                 uint64_t len = chain; while ((uint64_t)n * len > B.total) len >>= 1;   // keep within the buffer
