@@ -34,6 +34,7 @@ import (
 	"os"
 	"runtime"
 	"strings"
+	"time"
 	"unsafe"
 )
 
@@ -1329,6 +1330,212 @@ func (p *PayloadReader) RestoreImage(f *os.File, sliceBytes uint64) error {
 		}
 	}
 	return f.Truncate(int64(p.size))
+}
+
+// RestoreFile is one regular file of RestoreFiles: where it goes, st_mode, mtime in seconds, the payload offset of its
+// PAYLOAD header and its size.
+type RestoreFile struct {
+	Path          string
+	Mode          uint32
+	Mtime         int64
+	PayloadOffset uint64
+	Size          uint64
+}
+
+// readFileSparse reads ranges of files sparsely (pbsgpu_reader_plan_file_sparse, _read_file_sparse): range i is the
+// content bytes [pos[i], pos[i] + n[i]) of file fs[i].  It returns per range its (content offset, length) extents and
+// its packed data bytes, which are slices of out (grown only when it is too small; RestoreFiles sizes it once).
+func (p *PayloadReader) readFileSparse(fs []*RestoreFile, pos, n []uint64, out []byte) ([][][2]uint64, [][]byte, error) {
+	k := len(fs)
+	fo, sz := make([]uint64, k), make([]uint64, k)
+	outOff := make([]uint64, k)
+	var total, extCap uint64
+	for i, f := range fs {
+		fo[i], sz[i], outOff[i] = f.PayloadOffset, f.Size, total
+		total += n[i]
+		if n[i] > 0 {
+			extCap += ((pos[i]+n[i]-1)/4096 - pos[i]/4096 + 2) / 2
+		}
+	}
+	need := make([]uint64, len(p.digests)+1)
+	var nk C.uint64_t
+	if err := p.e.err(C.pbsgpu_reader_plan_file_sparse(p.r, (*C.uint64_t)(unsafe.Pointer(&fo[0])),
+		(*C.uint64_t)(unsafe.Pointer(&sz[0])), (*C.uint64_t)(unsafe.Pointer(&pos[0])), (*C.uint64_t)(unsafe.Pointer(&n[0])),
+		C.uint32_t(k), (*C.uint64_t)(unsafe.Pointer(&need[0])), nil, C.uint64_t(len(need)), &nk)); err != nil {
+		return nil, nil, err
+	}
+	need = need[:nk]
+	var blobs []byte
+	bo, bl := make([]uint64, nk+1), make([]uint64, nk+1)
+	for j, c := range need {
+		b, err := p.source(p.digests[c])
+		if err != nil {
+			return nil, nil, err
+		}
+		bo[j], bl[j] = uint64(len(blobs)), uint64(len(b))
+		blobs = append(blobs, b...)
+	}
+	blobs, need = append(blobs, 0), append(need, 0)
+	if uint64(len(out)) < total+1 {
+		out = make([]byte, total+1)
+	}
+	ext := make([]uint64, 2*extCap+2)
+	extFirst := make([]uint64, k+1)
+	status := make([]int32, k)
+	rc := C.pbsgpu_reader_read_file_sparse(p.r, (*C.uint64_t)(unsafe.Pointer(&fo[0])), (*C.uint64_t)(unsafe.Pointer(&sz[0])),
+		(*C.uint64_t)(unsafe.Pointer(&pos[0])), (*C.uint64_t)(unsafe.Pointer(&n[0])), C.uint32_t(k), unsafe.Pointer(&blobs[0]),
+		(*C.uint64_t)(unsafe.Pointer(&bo[0])), (*C.uint64_t)(unsafe.Pointer(&bl[0])), (*C.uint64_t)(unsafe.Pointer(&need[0])),
+		C.uint32_t(len(need)-1), (*C.uint8_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&outOff[0])),
+		(*C.uint64_t)(unsafe.Pointer(&ext[0])), C.uint64_t(extCap), (*C.uint64_t)(unsafe.Pointer(&extFirst[0])),
+		(*C.int32_t)(unsafe.Pointer(&status[0])), nil)
+	if err := p.e.err(rc); err != nil {
+		return nil, nil, err
+	}
+	exts, packed := make([][][2]uint64, k), make([][]byte, k)
+	for i, f := range fs {
+		if status[i] != int32(C.PBSGPU_DEC_OK) {
+			return nil, nil, fmt.Errorf("pbsgpu: restore of %s (payload offset %d, %d bytes): status %d", f.Path,
+				f.PayloadOffset, f.Size, status[i])
+		}
+		at := outOff[i]
+		for e := extFirst[i]; e < extFirst[i+1]; e++ {
+			exts[i] = append(exts[i], [2]uint64{ext[2*e], ext[2*e+1]})
+		}
+		var m uint64
+		for _, x := range exts[i] {
+			m += x[1]
+		}
+		packed[i] = out[at : at+m]
+	}
+	return exts, packed, nil
+}
+
+// writeExtents writes the packed bytes of a file's extents at their content offsets.
+func writeExtents(f *os.File, exts [][2]uint64, packed []byte) error {
+	var at uint64
+	for _, x := range exts {
+		if _, err := f.WriteAt(packed[at:at+x[1]], int64(x[0])); err != nil {
+			return err
+		}
+		at += x[1]
+	}
+	return nil
+}
+
+// RestoreFiles writes files of a payload reader into place sparsely (the replacement for restoreFile's io.Copy,
+// internal/pxar/restore.go): zero chunks are never fetched or decoded, and each file gets one WriteAt per data extent
+// (4 KiB blocks aligned to its content start that are not all zero) and a Truncate to its size, so its zero blocks stay
+// holes.  Files up to sliceBytes (0 = 1 GiB) go in batches of about sliceBytes file bytes, one read per batch; a larger
+// file is read in pieces of sliceBytes rounded down to a multiple of 4096.  A file whose size matches, and its mtime
+// too unless noAttr, is not rewritten unless it is a directory or a symlink (shouldUpdateFile, as the Python mirror).
+// One output buffer of sliceBytes serves every read.  Unless noAttr, each file gets its mode's permission bits and
+// mtime.  Directories and symlinks are the caller's (they need no archive bytes).
+func (p *PayloadReader) RestoreFiles(files []RestoreFile, noAttr bool, sliceBytes uint64) error {
+	if sliceBytes == 0 {
+		sliceBytes = 1 << 30
+	}
+	piece := sliceBytes / 4096 * 4096
+	if piece == 0 {
+		piece = 4096
+	}
+	create := func(f *RestoreFile) (*os.File, error) {
+		return os.OpenFile(f.Path, os.O_CREATE|os.O_TRUNC|os.O_WRONLY, 0666)
+	}
+	finish := func(w *os.File, f *RestoreFile) error {
+		err := w.Truncate(int64(f.Size))
+		if cerr := w.Close(); err == nil {
+			err = cerr
+		}
+		if err != nil || noAttr {
+			return err
+		}
+		if err := os.Chmod(f.Path, os.FileMode(f.Mode&0777)); err != nil {
+			return err
+		}
+		t := time.Unix(f.Mtime, 0)
+		return os.Chtimes(f.Path, t, t)
+	}
+	out := make([]byte, piece+1) // the packed data of one batch or piece, reused by every read
+	var batch []*RestoreFile
+	var acc uint64
+	flush := func() error {
+		if len(batch) == 0 {
+			return nil
+		}
+		pos, n := make([]uint64, len(batch)), make([]uint64, len(batch))
+		for i, f := range batch {
+			n[i] = f.Size
+		}
+		exts, packed, err := p.readFileSparse(batch, pos, n, out)
+		if err != nil {
+			return err
+		}
+		for i, f := range batch {
+			w, err := create(f)
+			if err != nil {
+				return err
+			}
+			if err := writeExtents(w, exts[i], packed[i]); err != nil {
+				w.Close()
+				return err
+			}
+			if err := finish(w, f); err != nil {
+				return err
+			}
+		}
+		batch, acc = batch[:0], 0
+		return nil
+	}
+	for i := range files {
+		f := &files[i]
+		// shouldUpdateFile: keep what is there unless it is a directory or a symlink, or its size (or, unless noAttr,
+		// its mtime) differs
+		if st, err := os.Lstat(f.Path); err == nil && !st.IsDir() && st.Mode()&os.ModeSymlink == 0 &&
+			uint64(st.Size()) == f.Size && (noAttr || st.ModTime().Unix() == f.Mtime) {
+			if !noAttr {
+				if err := os.Chmod(f.Path, os.FileMode(f.Mode&0777)); err != nil {
+					return err
+				}
+				t := time.Unix(f.Mtime, 0)
+				if err := os.Chtimes(f.Path, t, t); err != nil {
+					return err
+				}
+			}
+			continue
+		}
+		if f.Size > piece {
+			if err := flush(); err != nil {
+				return err
+			}
+			w, err := create(f)
+			if err != nil {
+				return err
+			}
+			for lo := uint64(0); lo < f.Size; lo += piece {
+				m := min(piece, f.Size-lo)
+				exts, packed, err := p.readFileSparse([]*RestoreFile{f}, []uint64{lo}, []uint64{m}, out)
+				if err == nil {
+					err = writeExtents(w, exts[0], packed[0])
+				}
+				if err != nil {
+					w.Close()
+					return err
+				}
+			}
+			if err := finish(w, f); err != nil {
+				return err
+			}
+			continue
+		}
+		if len(batch) > 0 && acc+f.Size > piece {
+			if err := flush(); err != nil {
+				return err
+			}
+		}
+		batch = append(batch, f)
+		acc += f.Size
+	}
+	return flush()
 }
 
 // ZipWriter writes one <name>.zip of a restore (the replacement for zip.NewWriter + io.Copy(rangeReader) in

@@ -551,6 +551,41 @@ int pbsgpu_reader_read_sparse(pbsgpu_reader *r, const uint64_t *off, const uint6
                               const uint64_t *blob_chunk, uint32_t n_blobs, uint8_t *out, const uint64_t *out_off,
                               uint64_t *ext, uint64_t ext_cap, uint64_t *ext_first, int32_t *status, int32_t *blob_status);
 
+/* ---- f3, read side: sparse file restore ----------------------------------------------------------------------------
+ * The restore of a snapshot's files into a directory (reference restoreNormal / restoreFile, internal/pxar/restore.go)
+ * reads file contents from a .didx payload archive sparsely, so files with long zero runs are written thin, as
+ * upstream's pxar extractor leaves them.  Both calls take one range form on a .didx reader (a .fidx reader is EINVAL):
+ * range i is file_off[i], the payload offset of a file's 16-byte PAYLOAD header; file_size[i], its content size; and
+ * the content bytes [pos[i], pos[i] + len[i]) with pos + len <= file_size (a file ending past the archive, or a range
+ * outside its file, is EINVAL).  A whole file is pos 0, len = size; a large file can be read in pieces.  Only a range
+ * at pos 0 reads and checks its file's header (as pbsgpu_reader_read with PBSGPU_READ_PAYLOAD: BAD_HEADER).
+ * Zero chunk: a chunk whose length is the index's longest and whose index digest equals the digest of that many zero
+ * bytes, plain or keyed with the reader's crypt (computed on the GPU on the first file-sparse call, not at open) --
+ * when two or more chunks of that length share a digest.  Otherwise no chunk is a zero chunk: that digest is one serial
+ * SHA-256 chain over the longest length, dearer than fetching and decoding the one chunk it could spare.  A
+ * window of zero bytes hashes to 0 under any table, so a zero run is cut only at the chunker's maximum: that one length
+ * carries almost all zero chunks.  Zero chunks are never planned, fetched, decoded or cached; they need not lie on
+ * block boundaries.  This trusts the index digest, as dedup does.
+ * Holes: content offsets are cut into 4096-byte blocks aligned to the file's content start (block b is content bytes
+ * [4096 b, 4096 (b + 1))).  Within a range, a block's part inside the range is a hole when all of its bytes are zero;
+ * extents are (content offset, length) pairs of the maximal runs of the other parts, ascending.  They depend only on
+ * the file's bytes and the range: the zero-chunk rule only saves work.
+ * pbsgpu_reader_plan_file_sparse: pbsgpu_reader_plan's outputs and errors for these ranges, leaving out zero chunks.
+ * pbsgpu_reader_read_file_sparse: pbsgpu_reader_read_sparse's outputs, statuses and errors for these ranges: host out
+ * with len[i] bytes reserved at out + out_off[i] for range i's data bytes, packed; ext / ext_first; ext_cap at least
+ * sum ceil(B_i / 2), with B_i the blocks range i touches, checked before any work; a failed range has no extents and
+ * none of its out bytes are written; a corrupt blob never fails the call.  The data chunks' bytes, with the zeros of
+ * the zero chunks in blocks they share with data chunks, are staged on the device, K17 maps their all-zero block
+ * parts, and K14 copies the data extents out. */
+int pbsgpu_reader_plan_file_sparse(pbsgpu_reader *r, const uint64_t *file_off, const uint64_t *file_size,
+                                   const uint64_t *pos, const uint64_t *len, uint32_t n, uint64_t *chunk, uint8_t *digest,
+                                   uint64_t cap, uint64_t *n_out);
+int pbsgpu_reader_read_file_sparse(pbsgpu_reader *r, const uint64_t *file_off, const uint64_t *file_size,
+                                   const uint64_t *pos, const uint64_t *len, uint32_t n, const void *blob_base,
+                                   const uint64_t *blob_off, const uint64_t *blob_len, const uint64_t *blob_chunk,
+                                   uint32_t n_blobs, uint8_t *out, const uint64_t *out_off, uint64_t *ext,
+                                   uint64_t ext_cap, uint64_t *ext_first, int32_t *status, int32_t *blob_status);
+
 /* ---- f3, read side: zip restore ------------------------------------------------------------------------------------
  * Restore as zip (reference internal/pxar/zip.go, RestoreModeZip): files are compressed on the GPU into raw Deflate
  * streams (RFC 1951) and the host writes the zip container around them (APPNOTE 6.3.x, as Go's archive/zip writes it).

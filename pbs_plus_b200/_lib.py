@@ -187,6 +187,9 @@ _SIGNATURES = {
                                    _vp, _vp],
     "pbsgpu_reader_read_sparse": [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp,
                                   C.c_uint64, _vp, _vp, _vp],
+    "pbsgpu_reader_plan_file_sparse": [_vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, C.c_uint64, _u64p],
+    "pbsgpu_reader_read_file_sparse": [_vp, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, C.c_uint32, _vp, _vp,
+                                       _vp, C.c_uint64, _vp, _vp, _vp],
     "pbsgpu_zip_local_header": ([C.POINTER(ZipEntry), _vp, C.c_uint64], C.c_uint64),
     "pbsgpu_zip_data_descriptor": ([C.POINTER(ZipEntry), _vp, C.c_uint64], C.c_uint64),
     "pbsgpu_zip_directory": ([_vp, C.c_uint64, C.c_uint64, _vp, C.c_uint64], C.c_uint64),

@@ -32,7 +32,8 @@ struct pbsgpu_reader {
     std::deque<Slot> ring;
     std::unordered_map<uint64_t, Held> held;
     bool image = false;   // over a fixed index: no pxar headers, PBSGPU_READ_PAYLOAD is refused
-    // sparse calls of an image: the digests of clen zero bytes for the (at most two) chunk lengths, computed on first use
+    // sparse calls: the digests of clen zero bytes for the (at most two) chunk lengths of an image, or for the longest
+    // chunk of a .didx reader, computed on first use
     bool zero_known = false;
     uint64_t zero_len[2] = {0, 0};
     uint8_t zero_dig[2][32];
@@ -145,16 +146,39 @@ template <typename F> static void for_pieces(const pbsgpu_reader *r, uint64_t lo
     }
 }
 
-// The digests of clen zero bytes for the image's two chunk lengths (chunk_size and the last chunk's), plain or keyed with
-// the reader's crypt as the index's digests are: K3 through the SHA-256 batch calls, once per reader.
+// The digests of clen zero bytes, plain or keyed with the reader's crypt as the index's digests are: K3 through the
+// SHA-256 batch calls, once per reader.  An image: its two chunk lengths (chunk_size and the last chunk's).  A .didx
+// reader: its longest chunk length, the one that carries zero runs (a zero window hashes to 0, so a zero run is only
+// cut at the chunker's maximum) -- but only when two or more chunks of that length share a digest.  That digest is one
+// serial SHA-256 chain over the longest length (16 MiB at a 4 MiB average), which costs more than fetching and decoding
+// one chunk, so a digest the index holds once is not worth identifying; without a repeat zero_len[0] stays 0 and no
+// chunk is served by digest (for_pieces never visits a chunk of length 0).
+static bool longest_digest_repeats(const pbsgpu_reader *r, uint64_t longest) {
+    std::vector<const uint8_t *> d;
+    for (uint64_t c = 0; c < r->clen.size(); c++)
+        if (r->clen[c] == longest) d.push_back(r->digests.data() + 32 * c);
+    std::sort(d.begin(), d.end(), [](const uint8_t *a, const uint8_t *b) { return memcmp(a, b, 32) < 0; });
+    for (size_t k = 1; k < d.size(); k++)
+        if (memcmp(d[k - 1], d[k], 32) == 0) return true;
+    return false;
+}
 static int zero_digests(pbsgpu_reader *r) {
     if (r->zero_known || r->ends.empty()) return PBSGPU_OK;
-    r->zero_len[0] = r->clen.front();   // the longest: every chunk but the last is chunk_size
-    r->zero_len[1] = r->clen.back();
+    if (!r->image) {
+        const uint64_t longest = *std::max_element(r->clen.begin(), r->clen.end());
+        if (!longest_digest_repeats(r, longest)) {
+            r->zero_known = true;
+            return PBSGPU_OK;
+        }
+    }
+    // an image's longest is its first: every chunk but the last is chunk_size
+    r->zero_len[0] = r->image ? r->clen.front() : *std::max_element(r->clen.begin(), r->clen.end());
+    r->zero_len[1] = r->image ? r->clen.back() : 0;
+    const uint32_t k = r->image ? 2 : 1;
     const std::vector<uint8_t> zeros(r->zero_len[0]);
     const uint64_t at[2] = {0, 0};
-    if (int rc = r->crypt ? pbsgpu_sha256_keyed_batch(r->ctx, r->crypt, zeros.data(), at, r->zero_len, 2, r->zero_dig[0])
-                          : pbsgpu_sha256_batch(r->ctx, zeros.data(), at, r->zero_len, 2, r->zero_dig[0]))
+    if (int rc = r->crypt ? pbsgpu_sha256_keyed_batch(r->ctx, r->crypt, zeros.data(), at, r->zero_len, k, r->zero_dig[0])
+                          : pbsgpu_sha256_batch(r->ctx, zeros.data(), at, r->zero_len, k, r->zero_dig[0]))
         return rc;
     r->zero_known = true;
     return PBSGPU_OK;
@@ -169,6 +193,12 @@ static bool zero_chunk(const pbsgpu_reader *r, uint64_t c) {
     const int k = r->clen[c] == r->zero_len[0] ? 0 : r->clen[c] == r->zero_len[1] ? 1 : -1;
     return k >= 0 && memcmp(r->digests.data() + 32 * c, r->zero_dig[k], 32) == 0;
 }
+// chunk c of a .didx reader is served by its digest in a file-sparse call (after zero_digests): a zero chunk of the
+// index's longest length, when that length holds a repeated digest.  Its bounds need not be block boundaries: the call stages the zeros of the blocks it shares
+// with data chunks itself.
+static bool file_zero_chunk(const pbsgpu_reader *r, uint64_t c) {
+    return r->clen[c] == r->zero_len[0] && memcmp(r->digests.data() + 32 * c, r->zero_dig[0], 32) == 0;
+}
 
 // The arguments every call checks: flags, and every range (with its PAYLOAD header) inside the archive.
 static int check_ranges(pbsgpu_reader *r, const uint64_t *off, const uint64_t *len, uint32_t n, uint32_t flags) {
@@ -178,6 +208,40 @@ static int check_ranges(pbsgpu_reader *r, const uint64_t *off, const uint64_t *l
     for (uint32_t i = 0; i < n; i++)
         if (off[i] > size || len[i] > size - off[i] || hs > size - off[i] - len[i])
             return fail(r->ctx, PBSGPU_EINVAL, "range %u ends past the archive (%llu bytes)", i, (unsigned long long)size);
+    return PBSGPU_OK;
+}
+// The file-sparse form: a .didx reader, every file (header and content) inside the archive, every range inside its file.
+static int check_file_ranges(pbsgpu_reader *r, const uint64_t *file_off, const uint64_t *file_size, const uint64_t *pos,
+                             const uint64_t *len, uint32_t n) {
+    if (r->image) return fail(r->ctx, PBSGPU_EINVAL, "file sparse: an image has no pxar files");
+    const uint64_t size = pbsgpu_reader_size(r);
+    for (uint32_t i = 0; i < n; i++) {
+        if (file_off[i] > size || 16 > size - file_off[i] || file_size[i] > size - file_off[i] - 16)
+            return fail(r->ctx, PBSGPU_EINVAL, "range %u: its file ends past the archive (%llu bytes)", i, (unsigned long long)size);
+        if (pos[i] > file_size[i] || len[i] > file_size[i] - pos[i])
+            return fail(r->ctx, PBSGPU_EINVAL, "range %u: [pos, pos + len) is not inside its file", i);
+    }
+    return PBSGPU_OK;
+}
+// Does the 16-byte PAYLOAD header h announce `size` content bytes?
+static bool payload_header_ok(const uint8_t *h, uint64_t size) {
+    uint8_t want[16];
+    memcpy(want, PXAR_PAYLOAD_LE, 8);
+    for (int k = 0; k < 8; k++) want[8 + k] = (uint8_t)((16 + size) >> (8 * k));
+    return memcmp(h, want, 16) == 0;
+}
+
+// The plans' common tail: the needed chunks ascending and without repeats, with their digests.
+static int plan_out(pbsgpu_reader *r, std::vector<uint64_t> &need, uint64_t *chunk, uint8_t *digest, uint64_t cap,
+                    uint64_t *n_out) {
+    std::sort(need.begin(), need.end());
+    need.erase(std::unique(need.begin(), need.end()), need.end());
+    *n_out = need.size();
+    if (need.size() > cap) return fail(r->ctx, PBSGPU_ERANGE, "plan capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)need.size());
+    for (size_t k = 0; k < need.size(); k++) {
+        chunk[k] = need[k];
+        if (digest) memcpy(digest + 32 * k, r->digests.data() + 32 * need[k], 32);
+    }
     return PBSGPU_OK;
 }
 
@@ -197,15 +261,24 @@ extern "C" int pbsgpu_reader_plan(pbsgpu_reader *r, const uint64_t *off, const u
         for_pieces(r, off[i], off[i] + hs + len[i], [&](uint64_t c, uint64_t, uint64_t, uint64_t) {
             if (!r->held.count(c) && !(sparse && zero_chunk(r, c))) need.push_back(c);
         });
-    std::sort(need.begin(), need.end());
-    need.erase(std::unique(need.begin(), need.end()), need.end());
-    *n_out = need.size();
-    if (need.size() > cap) return fail(r->ctx, PBSGPU_ERANGE, "plan capacity %llu < %llu chunks", (unsigned long long)cap, (unsigned long long)need.size());
-    for (size_t k = 0; k < need.size(); k++) {
-        chunk[k] = need[k];
-        if (digest) memcpy(digest + 32 * k, r->digests.data() + 32 * need[k], 32);
+    return plan_out(r, need, chunk, digest, cap, n_out);
+}
+
+extern "C" int pbsgpu_reader_plan_file_sparse(pbsgpu_reader *r, const uint64_t *file_off, const uint64_t *file_size,
+                                              const uint64_t *pos, const uint64_t *len, uint32_t n, uint64_t *chunk,
+                                              uint8_t *digest, uint64_t cap, uint64_t *n_out) {
+    if (!r || !n_out || (n && (!file_off || !file_size || !pos || !len)) || (cap && !chunk)) return PBSGPU_EINVAL;
+    Guard g(r->ctx);
+    if (int rc = check_file_ranges(r, file_off, file_size, pos, len, n)) return rc;
+    if (int rc = zero_digests(r)) return rc;
+    std::vector<uint64_t> need;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t a = file_off[i] + 16 + pos[i];   // a range at pos 0 also reads its file's header
+        for_pieces(r, pos[i] ? a : file_off[i], a + len[i], [&](uint64_t c, uint64_t, uint64_t, uint64_t) {
+            if (!r->held.count(c) && !file_zero_chunk(r, c)) need.push_back(c);
+        });
     }
-    return PBSGPU_OK;
+    return plan_out(r, need, chunk, digest, cap, n_out);
 }
 
 namespace {
@@ -381,12 +454,8 @@ extern "C" int pbsgpu_reader_read(pbsgpu_reader *r, const uint64_t *off, const u
         std::vector<uint8_t> hdr(16ull * n);
         if (b.ok()) b.e = cudaMemcpyAsync(hdr.data(), ga.d_hdr, hdr.size(), cudaMemcpyDeviceToHost, b.st);
         if (int rc = b.finish("reader headers")) return rc;
-        for (uint32_t i = 0; i < n; i++) {
-            uint8_t want[16];
-            memcpy(want, PXAR_PAYLOAD_LE, 8);
-            for (int k = 0; k < 8; k++) want[8 + k] = (uint8_t)((16 + len[i]) >> (8 * k));
-            if (status[i] == PBSGPU_DEC_OK && memcmp(hdr.data() + 16ull * i, want, 16) != 0) status[i] = PBSGPU_DEC_BAD_HEADER;
-        }
+        for (uint32_t i = 0; i < n; i++)
+            if (status[i] == PBSGPU_DEC_OK && !payload_header_ok(hdr.data() + 16ull * i, len[i])) status[i] = PBSGPU_DEC_BAD_HEADER;
     }
     return PBSGPU_OK;
 }
@@ -444,6 +513,108 @@ extern "C" int pbsgpu_reader_read_deflate(pbsgpu_reader *r, const uint64_t *off,
     return PBSGPU_OK;
 }
 
+namespace {
+// A staged run of a sparse read: `len` bytes of range `range` at block coordinate `off` (an image offset, or an offset
+// into a file's content) that lie at `soff` in the call's device stage, with soff = off mod 16 so K17's vector loads are
+// aligned on whole blocks.  Two runs of a range are apart by at least one whole hole block, so no block part spans two.
+struct SparseRun { uint64_t off, len, soff; uint32_t range; };
+}  // namespace
+
+// The sparse reads' argument checks: out in host memory, and ext_cap at least sum ceil(B_i / 2), with B_i the block
+// parts of [at[i], at[i] + len[i]) in block coordinates.  bit0[i]: the bit of range i's first block part.
+static int sparse_bits(pbsgpu_reader *r, const uint64_t *at, const uint64_t *len, uint32_t n, const uint8_t *out,
+                       uint64_t ext_cap, const char *what, std::vector<uint64_t> &bit0) {
+    if (n && pbsgpu_is_device_ptr(out)) return fail(r->ctx, PBSGPU_EINVAL, "%s: out must be host memory", what);
+    bit0.assign(n + 1, 0);
+    uint64_t bound = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t parts = len[i] ? (at[i] + len[i] - 1) / ZERO_BLOCK - at[i] / ZERO_BLOCK + 1 : 0;
+        bit0[i + 1] = bit0[i] + parts;
+        bound += (parts + 1) / 2;
+    }
+    if (ext_cap < bound)
+        return fail(r->ctx, PBSGPU_EINVAL, "%s: ext_cap %llu < %llu, the most extents the ranges can have", what,
+                    (unsigned long long)ext_cap, (unsigned long long)bound);
+    return PBSGPU_OK;
+}
+
+// The sparse reads' common tail, once the runs are staged and the statuses known: K17 maps the all-zero block parts of
+// the runs of the ranges that are OK, the extents are the maximal runs of the other block parts, and K14 copies their
+// bytes to the caller's host memory, packed per range.  A block part no run covers keeps the preset bit: a hole.
+static int sparse_extents(pbsgpu_reader *r, Blocking &b, const std::vector<SparseRun> &runs, const uint8_t *dstage,
+                          const uint64_t *at, const std::vector<uint64_t> &bit0, uint32_t n, uint8_t *out,
+                          const uint64_t *out_off, uint64_t *ext, uint64_t *ext_first, const int32_t *status,
+                          const char *what) {
+    pbsgpu_ctx *ctx = r->ctx;
+    const uint32_t nr = (uint32_t)runs.size();
+    std::vector<ZeroRun> zr;
+    std::vector<uint64_t> part_first(1, 0);
+    for (const SparseRun &u : runs) {
+        if (status[u.range] != PBSGPU_DEC_OK) continue;
+        const uint64_t b0 = u.off / ZERO_BLOCK, b1 = (u.off + u.len - 1) / ZERO_BLOCK;
+        zr.push_back({(uint64_t)(uintptr_t)dstage + u.soff, u.off, u.len, bit0[u.range] + b0 - at[u.range] / ZERO_BLOCK});
+        part_first.push_back(part_first.back() + b1 - b0 + 1);
+    }
+    std::vector<uint32_t> bits;
+    if (!zr.empty()) {
+        const uint64_t words = (bit0[n] + 31) / 32;
+        bits.resize(words);
+        uint32_t *d_bits = b.get<uint32_t>(words);
+        const ZeroRun *d_runs = b.upload(zr.data(), zr.size());
+        const uint64_t *d_first = b.upload(part_first.data(), part_first.size());
+        if (!d_bits || !d_runs || !d_first) return fail(ctx, PBSGPU_ENOMEM, "%s: zero map buffers failed", what);
+        if (b.ok()) b.e = cudaMemsetAsync(d_bits, 0xff, words * 4, b.st);
+        if (b.ok()) b.e = launch_zero_map(d_runs, d_first, (uint32_t)zr.size(), part_first.back(), d_bits, ctx->sm_count, b.st);
+        if (b.ok()) b.e = cudaMemcpyAsync(bits.data(), d_bits, words * 4, cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("sparse zero map")) return rc;
+    }
+    // the extents: an extent lies in one run (SparseRun), so its dstage bytes are contiguous
+    std::vector<uint64_t> esrc;   // per extent: its offset in dstage
+    uint64_t ne = 0, host_bytes = 0;
+    if (n) ext_first[0] = 0;
+    for (uint32_t i = 0, k = 0; i < n; i++) {
+        const uint64_t e0 = ne;
+        for (; k < nr && runs[k].range == i; k++) {
+            const SparseRun &u = runs[k];
+            if (status[i] != PBSGPU_DEC_OK) continue;
+            const uint64_t b0 = u.off / ZERO_BLOCK, b1 = (u.off + u.len - 1) / ZERO_BLOCK;
+            for (uint64_t blk = b0; blk <= b1; blk++) {
+                const uint64_t bit = bit0[i] + blk - at[i] / ZERO_BLOCK;
+                if (bits[bit >> 5] >> (bit & 31) & 1) continue;   // a hole
+                const uint64_t lo = std::max(u.off, blk * ZERO_BLOCK), hi = std::min(u.off + u.len, (blk + 1) * ZERO_BLOCK);
+                if (ne > e0 && ext[2 * ne - 2] + ext[2 * ne - 1] == lo) {
+                    ext[2 * ne - 1] += hi - lo;
+                } else {
+                    ext[2 * ne] = lo; ext[2 * ne + 1] = hi - lo;
+                    esrc.push_back(u.soff + (lo - u.off));
+                    ne++;
+                }
+                host_bytes += hi - lo;
+            }
+        }
+        ext_first[i + 1] = ne;
+    }
+    if (ne == 0) return PBSGPU_OK;
+    // K14: the data extents, packed per range, through the host-out staging buffer
+    Gather ga{b, r, out, nullptr};
+    ga.out_dev = false;
+    const uint32_t pcap = (uint32_t)std::min<uint64_t>(ne + 1, READER_PIECE_BATCH) * 2;   // a split piece adds one
+    ga.d_pieces = b.get<ReadPiece>(pcap);
+    ga.d_first = b.get<uint64_t>(pcap + 1);
+    ga.pieces.reserve(pcap);
+    ga.stage_cap = std::min(host_bytes, READER_STAGE_MAX);
+    ga.stage = b.get<uint8_t>(ga.stage_cap);
+    if (!ga.d_pieces || !ga.d_first || !ga.stage) return fail(ctx, PBSGPU_ENOMEM, "%s: gather buffers failed", what);
+    for (uint32_t i = 0; i < n; i++) {
+        uint64_t packed = 0;
+        for (uint64_t e = ext_first[i]; e < ext_first[i + 1]; e++) {
+            if (int rc = ga.add({0, esrc[e], ext[2 * e + 1], out_off[i] + packed, i, false, false}, dstage)) return rc;
+            packed += ext[2 * e + 1];
+        }
+    }
+    return ga.flush();
+}
+
 // The sparse image restore's read: the ranges' data chunks (every chunk but the zero chunks) go through
 // pbsgpu_reader_read into a device stage owned by this call, K17 maps their 4 KiB block parts that are all zero, and K14
 // copies only the data extents of the ranges whose status is OK to the caller's host memory, packed.  Zero chunks
@@ -460,23 +631,12 @@ extern "C" int pbsgpu_reader_read_sparse(pbsgpu_reader *r, const uint64_t *off, 
     Guard g(ctx);
     if (!r->image) return fail(ctx, PBSGPU_EINVAL, "read_sparse: a .didx reader has no sparse read");
     if (int rc = check_ranges(r, off, len, n, flags)) return rc;
-    if (n && pbsgpu_is_device_ptr(out)) return fail(ctx, PBSGPU_EINVAL, "read_sparse: out must be host memory");
-    // bit0[i]: the bit of range i's first block part; a range of B block parts has at most ceil(B / 2) extents
-    std::vector<uint64_t> bit0(n + 1, 0);
-    uint64_t bound = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        const uint64_t parts = len[i] ? (off[i] + len[i] - 1) / ZERO_BLOCK - off[i] / ZERO_BLOCK + 1 : 0;
-        bit0[i + 1] = bit0[i] + parts;
-        bound += (parts + 1) / 2;
-    }
-    if (ext_cap < bound)
-        return fail(ctx, PBSGPU_EINVAL, "read_sparse: ext_cap %llu < %llu, the most extents the ranges can have",
-                    (unsigned long long)ext_cap, (unsigned long long)bound);
+    std::vector<uint64_t> bit0;
+    if (int rc = sparse_bits(r, off, len, n, out, ext_cap, "read_sparse", bit0)) return rc;
     if (int rc = zero_digests(r)) return rc;
-    // the data runs: maximal runs of data chunks within a range, staged at offsets congruent to their image offsets
-    // mod 16 so K17's vector loads are aligned on whole blocks
-    struct Run { uint64_t off, len, soff; uint32_t range; };
-    std::vector<Run> runs;
+    // the data runs: maximal runs of data chunks within a range; the zero chunks between them are whole blocks
+    // (zero_chunk), so every block part lies in one run
+    std::vector<SparseRun> runs;
     uint64_t total = 0;
     for (uint32_t i = 0; i < n; i++)
         for_pieces(r, off[i], off[i] + len[i], [&](uint64_t c, uint64_t, uint64_t l, uint64_t at) {
@@ -505,73 +665,104 @@ extern "C" int pbsgpu_reader_read_sparse(pbsgpu_reader *r, const uint64_t *off, 
     for (uint32_t i = 0; i < n; i++) status[i] = PBSGPU_DEC_OK;
     for (uint32_t k = 0; k < nr; k++)
         if (status[runs[k].range] == PBSGPU_DEC_OK) status[runs[k].range] = rst[k];
-    // K17 over the runs of the ranges that are OK
-    std::vector<ZeroRun> zr;
-    std::vector<uint64_t> part_first(1, 0);
-    for (const Run &u : runs) {
-        if (status[u.range] != PBSGPU_DEC_OK) continue;
-        const uint64_t b0 = u.off / ZERO_BLOCK, b1 = (u.off + u.len - 1) / ZERO_BLOCK;
-        zr.push_back({(uint64_t)(uintptr_t)dstage + u.soff, u.off, u.len, bit0[u.range] + b0 - off[u.range] / ZERO_BLOCK});
-        part_first.push_back(part_first.back() + b1 - b0 + 1);
-    }
-    std::vector<uint32_t> bits;
-    if (!zr.empty()) {
-        const uint64_t words = (bit0[n] + 31) / 32;
-        bits.resize(words);
-        uint32_t *d_bits = b.get<uint32_t>(words);
-        const ZeroRun *d_runs = b.upload(zr.data(), zr.size());
-        const uint64_t *d_first = b.upload(part_first.data(), part_first.size());
-        if (!d_bits || !d_runs || !d_first) return fail(ctx, PBSGPU_ENOMEM, "read_sparse: zero map buffers failed");
-        if (b.ok()) b.e = cudaMemsetAsync(d_bits, 0xff, words * 4, b.st);
-        if (b.ok()) b.e = launch_zero_map(d_runs, d_first, (uint32_t)zr.size(), part_first.back(), d_bits, ctx->sm_count, b.st);
-        if (b.ok()) b.e = cudaMemcpyAsync(bits.data(), d_bits, words * 4, cudaMemcpyDeviceToHost, b.st);
-        if (int rc = b.finish("read_sparse zero map")) return rc;
-    }
-    // the extents: maximal runs of non-hole block parts.  Two runs of a range are apart by at least one zero chunk whose
-    // bounds are block boundaries (zero_chunk), so no block part spans two runs, an extent lies in one run, its dstage
-    // bytes are contiguous, and a range has at most ceil(B / 2) extents.
-    std::vector<uint64_t> esrc;   // per extent: its offset in dstage
-    uint64_t ne = 0, host_bytes = 0;
-    if (n) ext_first[0] = 0;
-    for (uint32_t i = 0, k = 0; i < n; i++) {
-        const uint64_t e0 = ne;
-        for (; k < nr && runs[k].range == i; k++) {
-            const Run &u = runs[k];
-            if (status[i] != PBSGPU_DEC_OK) continue;
-            const uint64_t b0 = u.off / ZERO_BLOCK, b1 = (u.off + u.len - 1) / ZERO_BLOCK;
-            for (uint64_t blk = b0; blk <= b1; blk++) {
-                const uint64_t bit = bit0[i] + blk - off[i] / ZERO_BLOCK;
-                if (bits[bit >> 5] >> (bit & 31) & 1) continue;   // a hole
-                const uint64_t lo = std::max(u.off, blk * ZERO_BLOCK), hi = std::min(u.off + u.len, (blk + 1) * ZERO_BLOCK);
-                if (ne > e0 && ext[2 * ne - 2] + ext[2 * ne - 1] == lo) {
-                    ext[2 * ne - 1] += hi - lo;
-                } else {
-                    ext[2 * ne] = lo; ext[2 * ne + 1] = hi - lo;
-                    esrc.push_back(u.soff + (lo - u.off));
-                    ne++;
-                }
-                host_bytes += hi - lo;
-            }
-        }
-        ext_first[i + 1] = ne;
-    }
-    if (ne == 0) return PBSGPU_OK;
-    // K14: the data extents, packed per range, through the host-out staging buffer
-    Gather ga{b, r, out, nullptr};
-    ga.out_dev = false;
-    const uint32_t pcap = (uint32_t)std::min<uint64_t>(ne + 1, READER_PIECE_BATCH) * 2;   // a split piece adds one
-    ga.d_pieces = b.get<ReadPiece>(pcap);
-    ga.d_first = b.get<uint64_t>(pcap + 1);
-    ga.pieces.reserve(pcap);
-    ga.stage_cap = std::min(host_bytes, READER_STAGE_MAX);
-    ga.stage = b.get<uint8_t>(ga.stage_cap);
-    if (!ga.d_pieces || !ga.d_first || !ga.stage) return fail(ctx, PBSGPU_ENOMEM, "read_sparse gather buffers failed");
+    return sparse_extents(r, b, runs, dstage, off, bit0, n, out, out_off, ext, ext_first, status, "read_sparse");
+}
+
+// The file restore's read: ranges of pxar file contents, sparse in blocks aligned to each file's content start.  Per
+// range, the runs are the data chunks' content bytes widened to whole blocks (clipped to the range) and merged where
+// they touch, so runs are apart by at least one whole block that lies in zero chunks.  The stage is zeroed when a run or
+// a header spans a zero chunk, then the data chunks' pieces land in it through pbsgpu_reader_read; the 16-byte headers
+// of the ranges at pos 0 go to one area after the runs.  The tail is the image form's, with content offsets as block
+// coordinates.  Zero chunks (file_zero_chunk) are neither fetched, decoded nor cached.
+extern "C" int pbsgpu_reader_read_file_sparse(pbsgpu_reader *r, const uint64_t *file_off, const uint64_t *file_size,
+                                              const uint64_t *pos, const uint64_t *len, uint32_t n, const void *blob_base,
+                                              const uint64_t *blob_off, const uint64_t *blob_len, const uint64_t *blob_chunk,
+                                              uint32_t n_blobs, uint8_t *out, const uint64_t *out_off, uint64_t *ext,
+                                              uint64_t ext_cap, uint64_t *ext_first, int32_t *status, int32_t *blob_status) {
+    if (!r || (n && (!file_off || !file_size || !pos || !len || !out || !out_off || !ext_first || !status)) ||
+        (ext_cap && !ext) || (n_blobs && (!blob_base || !blob_off || !blob_len || !blob_chunk)))
+        return PBSGPU_EINVAL;
+    pbsgpu_ctx *ctx = r->ctx;
+    Guard g(ctx);
+    if (int rc = check_file_ranges(r, file_off, file_size, pos, len, n)) return rc;
+    std::vector<uint64_t> bit0;
+    if (int rc = sparse_bits(r, pos, len, n, out, ext_cap, "read_file_sparse", bit0)) return rc;
+    if (int rc = zero_digests(r)) return rc;
+    // the runs, in content offsets
+    std::vector<SparseRun> runs;
     for (uint32_t i = 0; i < n; i++) {
-        uint64_t packed = 0;
-        for (uint64_t e = ext_first[i]; e < ext_first[i + 1]; e++) {
-            if (int rc = ga.add({0, esrc[e], ext[2 * e + 1], out_off[i] + packed, i, false, false}, dstage)) return rc;
-            packed += ext[2 * e + 1];
+        const uint64_t a0 = file_off[i] + 16 + pos[i], end = pos[i] + len[i];
+        for_pieces(r, a0, a0 + len[i], [&](uint64_t c, uint64_t, uint64_t l, uint64_t at) {
+            if (file_zero_chunk(r, c)) return;
+            const uint64_t a = pos[i] + at;
+            const uint64_t lo = std::max(pos[i], a / ZERO_BLOCK * ZERO_BLOCK);
+            const uint64_t hi = std::min(end, (a + l + ZERO_BLOCK - 1) / ZERO_BLOCK * ZERO_BLOCK);
+            if (!runs.empty() && runs.back().range == i && runs.back().off + runs.back().len >= lo)
+                runs.back().len = hi - runs.back().off;
+            else
+                runs.push_back({lo, hi - lo, 0, i});
+        });
+    }
+    if (runs.size() > UINT32_MAX) return fail(ctx, PBSGPU_EINVAL, "read_file_sparse: more than 2^32 - 1 data runs");
+    uint64_t total = 0;
+    for (SparseRun &u : runs) {
+        total += (u.off - total) & 15;
+        u.soff = total;
+        total += u.len;
+    }
+    std::vector<uint32_t> hdr_of;   // the ranges at pos 0, in order: their headers at hbase + 16 k
+    for (uint32_t i = 0; i < n; i++)
+        if (pos[i] == 0) hdr_of.push_back(i);
+    const uint64_t hbase = (total + 15) & ~15ull;
+    total = hbase + 16 * hdr_of.size();
+    // the reads: per range its header, then its runs, each as the maximal runs of data-chunk pieces in it
+    struct Read { uint64_t off, len, soff; uint32_t range; };
+    std::vector<Read> reads;
+    auto stage_span = [&](uint32_t i, uint64_t lo, uint64_t hi, uint64_t soff) {
+        for_pieces(r, lo, hi, [&](uint64_t c, uint64_t, uint64_t l, uint64_t at) {
+            if (file_zero_chunk(r, c)) return;
+            if (!reads.empty() && reads.back().range == i && reads.back().soff + reads.back().len == soff + at &&
+                reads.back().off + reads.back().len == lo + at)
+                reads.back().len += l;
+            else
+                reads.push_back({lo + at, l, soff + at, i});
+        });
+    };
+    for (uint32_t i = 0, k = 0, h = 0; i < n; i++) {
+        if (pos[i] == 0) stage_span(i, file_off[i], file_off[i] + 16, hbase + 16ull * h++);
+        for (; k < runs.size() && runs[k].range == i; k++)
+            stage_span(i, file_off[i] + 16 + runs[k].off, file_off[i] + 16 + runs[k].off + runs[k].len, runs[k].soff);
+    }
+    if (reads.size() > UINT32_MAX) return fail(ctx, PBSGPU_EINVAL, "read_file_sparse: more than 2^32 - 1 data reads");
+    const uint32_t nq = (uint32_t)reads.size();
+    Blocking b(ctx, ctx->streams[0]);
+    uint8_t *dstage = total ? b.get<uint8_t>(total + 16) : nullptr;
+    if (total && !dstage) return fail(ctx, PBSGPU_ENOMEM, "read_file_sparse: device stage of %llu bytes failed", (unsigned long long)total);
+    uint64_t landed = 0, staged = 16 * hdr_of.size();
+    for (const Read &q : reads) landed += q.len;
+    for (const SparseRun &u : runs) staged += u.len;
+    if (landed < staged) {   // runs or headers span zero chunks: the data pieces land on zeros
+        if (b.ok()) b.e = cudaMemsetAsync(dstage, 0, total, b.st);
+        if (int rc = b.finish("read_file_sparse stage")) return rc;
+    }
+    std::vector<uint64_t> ro(nq), rl(nq), rs(nq);
+    std::vector<int32_t> rst(nq);
+    for (uint32_t k = 0; k < nq; k++) { ro[k] = reads[k].off; rl[k] = reads[k].len; rs[k] = reads[k].soff; }
+    if (int rc = pbsgpu_reader_read(r, ro.data(), rl.data(), nq, 0, blob_base, blob_off, blob_len, blob_chunk, n_blobs,
+                                    dstage, rs.data(), rst.data(), blob_status))
+        return rc;
+    // a range's status: its first failing read's (header first, then in archive order), then BAD_HEADER
+    for (uint32_t i = 0; i < n; i++) status[i] = PBSGPU_DEC_OK;
+    for (uint32_t k = 0; k < nq; k++)
+        if (status[reads[k].range] == PBSGPU_DEC_OK) status[reads[k].range] = rst[k];
+    if (!hdr_of.empty()) {
+        std::vector<uint8_t> hdr(16 * hdr_of.size());
+        if (b.ok()) b.e = cudaMemcpyAsync(hdr.data(), dstage + hbase, hdr.size(), cudaMemcpyDeviceToHost, b.st);
+        if (int rc = b.finish("read_file_sparse headers")) return rc;
+        for (size_t h = 0; h < hdr_of.size(); h++) {
+            const uint32_t i = hdr_of[h];
+            if (status[i] == PBSGPU_DEC_OK && !payload_header_ok(hdr.data() + 16 * h, file_size[i])) status[i] = PBSGPU_DEC_BAD_HEADER;
         }
     }
-    return ga.flush();
+    return sparse_extents(r, b, runs, dstage, pos, bit0, n, out, out_off, ext, ext_first, status, "read_file_sparse");
 }

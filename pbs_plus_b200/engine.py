@@ -703,16 +703,37 @@ class Reader(_Handle):
         sparse (a .fidx reader only): leave out the zero chunks, which read_sparse serves without a blob."""
         o, l = Engine._offlen(off, length)
         flags = (_lib.READ_PAYLOAD if payload else 0) | (_lib.READ_SPARSE if sparse else 0)
+        return self._plan(lambda *out: self._eng._L.pbsgpu_reader_plan(self._h, o.ctypes.data, l.ctypes.data, len(o),
+                                                                       flags, *out))
+
+    def _plan(self, call):
+        """A plan call given its trailing (chunk, digest, cap, n_out) arguments: sized first, then filled."""
         n = C.c_uint64()
-        rc = self._eng._L.pbsgpu_reader_plan(self._h, o.ctypes.data, l.ctypes.data, len(o), flags, None, None, 0, C.byref(n))
+        rc = call(None, None, 0, C.byref(n))
         if rc != _lib.ERANGE:
             self._eng._ck(rc)
         chunks = np.zeros(n.value, dtype=np.uint64)
         dig = np.zeros((n.value, 32), dtype=np.uint8)
         if n.value:
-            self._eng._ck(self._eng._L.pbsgpu_reader_plan(self._h, o.ctypes.data, l.ctypes.data, len(o), flags,
-                                                          chunks.ctypes.data, dig.ctypes.data, n.value, C.byref(n)))
+            self._eng._ck(call(chunks.ctypes.data, dig.ctypes.data, n.value, C.byref(n)))
         return chunks, dig
+
+    @staticmethod
+    def _file_ranges(file_off, file_size, pos, length):
+        """File-content ranges -> four u64 arrays of one shape."""
+        a = [np.ascontiguousarray(x, dtype=np.uint64).reshape(-1) for x in (file_off, file_size, pos, length)]
+        if len({x.shape for x in a}) != 1:
+            raise ValueError("file_off, file_size, pos and length must have one entry per range")
+        return a
+
+    def plan_file_sparse(self, file_off, file_size, pos, length):
+        """The chunks that ranges of file contents need and the cache lacks, leaving out the zero chunks
+        (pbsgpu_reader_plan_file_sparse) -> (chunk indices u64[k] ascending, digests u8[k, 32]).  Range i is the content
+        bytes [pos[i], pos[i] + length[i]) of the file whose PAYLOAD header is at file_off[i] and whose size is
+        file_size[i]; a range at pos 0 also reads that header."""
+        fo, fs, p, l = self._file_ranges(file_off, file_size, pos, length)
+        return self._plan(lambda *out: self._eng._L.pbsgpu_reader_plan_file_sparse(
+            self._h, fo.ctypes.data, fs.ctypes.data, p.ctypes.data, l.ctypes.data, len(fo), *out))
 
     def read(self, off, length, blobs, payload: bool = False, out: str = "host"):
         """Read ranges (pbsgpu_reader_read).  `blobs`: {chunk index: DataBlob bytes}, or (base, off[k], len[k], chunk[k])
@@ -762,21 +783,36 @@ class Reader(_Handle):
         back.  `blobs` as in read().  -> (status int32[n], per range (extents [(image offset, length)], packed data
         bytes) or None where the status is not DEC_OK, blob_status int32[k])"""
         o, l = Engine._offlen(off, length)
+        return self._sparse(o, l, blobs, lambda *a: self._eng._L.pbsgpu_reader_read_sparse(
+            self._h, o.ctypes.data, l.ctypes.data, len(o), 0, *a))
+
+    def read_file_sparse(self, file_off, file_size, pos, length, blobs):
+        """Read ranges of file contents sparsely (pbsgpu_reader_read_file_sparse): ranges as in plan_file_sparse, zero
+        chunks need no blob, and per range only the data extents -- the maximal runs of block parts that are not all
+        zero, in 4 KiB blocks aligned to the file's content start -- come back.  A range at pos 0 checks its file's
+        PAYLOAD header.  `blobs` as in read().  -> (status int32[n], per range (extents [(content offset, length)],
+        packed data bytes) or None where the status is not DEC_OK, blob_status int32[k])"""
+        fo, fs, p, l = self._file_ranges(file_off, file_size, pos, length)
+        return self._sparse(p, l, blobs, lambda *a: self._eng._L.pbsgpu_reader_read_file_sparse(
+            self._h, fo.ctypes.data, fs.ctypes.data, p.ctypes.data, l.ctypes.data, len(fo), *a))
+
+    def _sparse(self, at, length, blobs, call):
+        """A sparse read given its block coordinates (at, length) and a call that takes the trailing arguments from
+        the blobs on."""
         base, bo, bl, bc = _blob_args(blobs)
-        n, k = len(o), len(bo)
-        ooff, total = _offsets(l)
+        n, k = len(at), len(bo)
+        ooff, total = _offsets(length)
         buf = self._eng._alloc(total, "host")
         bs = _lib.SPARSE_BLOCK
-        parts = [(int(a) + int(b) - 1) // bs - int(a) // bs + 1 if b else 0 for a, b in zip(o, l)]
+        parts = [(int(a) + int(b) - 1) // bs - int(a) // bs + 1 if b else 0 for a, b in zip(at, length)]
         cap = sum((p + 1) // 2 for p in parts)
         ext = np.zeros((max(1, cap), 2), dtype=np.uint64)
         first = np.zeros(n + 1, dtype=np.uint64)
         status = np.zeros(n, dtype=np.int32)
         bst = np.zeros(k, dtype=np.int32)
-        self._eng._ck(self._eng._L.pbsgpu_reader_read_sparse(
-            self._h, o.ctypes.data, l.ctypes.data, n, 0, _ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k,
-            buf.ctypes.data, ooff.ctypes.data, ext.ctypes.data, cap, first.ctypes.data, status.ctypes.data,
-            bst.ctypes.data))
+        self._eng._ck(call(_ptr(base), bo.ctypes.data, bl.ctypes.data, bc.ctypes.data, k, buf.ctypes.data,
+                           ooff.ctypes.data, ext.ctypes.data, cap, first.ctypes.data, status.ctypes.data,
+                           bst.ctypes.data))
         data = []
         for i in range(n):
             if status[i] != _lib.DEC_OK:

@@ -26,6 +26,7 @@ Two writers:
 
 And for disk images (`.img.fidx` archives): FixedIndexWriter -- fixed-size chunks through the batch call, fed in slices;
 restore_image -- the sparse restore: zero chunks are served by digest and only the data extents are written.
+PayloadReader.RestoreFiles -- the same for the files of a payload stream, restored into a directory.
 
 Restore as zip (reference internal/pxar/zip.go): ZipWriter -- files of a PayloadReader deflated on the GPU
 (pbsgpu_reader_read_deflate) inside a zip container written by pbsgpu_zip_*.
@@ -34,6 +35,7 @@ from __future__ import annotations
 
 import io
 import os
+import stat
 import zlib
 from collections import deque
 from dataclasses import dataclass, field
@@ -463,6 +465,81 @@ class PayloadReader:
         off, size = zip(*files)
         return self._read(list(off), list(size), True)
 
+    def RestoreFiles(self, root: str, entries: list, no_attr: bool = False, slice_bytes: int = 1 << 30) -> None:
+        """Restores entries into the directory `root` (reference restoreNormal / restoreFile / restoreSymlink,
+        internal/pxar/restore.go): DirEntry, FileEntry and SymlinkEntry items, paths relative to root, a directory
+        before what it holds.  File contents are read sparsely (pbsgpu_reader_read_file_sparse): zero chunks are never
+        fetched or decoded, and only the data extents come back.  Each file is opened with O_CREAT | O_TRUNC, gets one
+        os.pwrite per extent and an os.ftruncate to its size, so its all-zero 4 KiB blocks stay holes.  Files up to
+        `slice_bytes` go in batches of about `slice_bytes` file bytes, one plan / fetch / read per batch; a larger file
+        is read in pieces of `slice_bytes` (rounded down to a multiple of 4096).  A file whose type and size match the
+        entry, and its mtime too unless `no_attr`, is not rewritten (shouldUpdateFile).  Unless `no_attr`, files and
+        directories get the entry's permission bits and mtime (owners, xattrs, ACLs and fcaps are not restored).
+        Raises IOError naming the first file that cannot be read and its status."""
+        piece = max(_lib.SPARSE_BLOCK, int(slice_bytes) // _lib.SPARSE_BLOCK * _lib.SPARSE_BLOCK)
+        os.makedirs(root, exist_ok=True)
+        dirs, batch, acc = [], [], 0
+        for e in entries:
+            path = _restore_path(root, e.path)
+            if isinstance(e, DirEntry):
+                os.makedirs(path, exist_ok=True)
+                dirs.append((path, e))
+            elif isinstance(e, SymlinkEntry):
+                _restore_symlink(path, e.target)
+            elif not _should_update(path, e, no_attr):
+                if not no_attr:
+                    _apply_attrs(path, e)
+            elif e.size > piece:
+                self._restore_large(path, e, piece, no_attr)
+            else:
+                if batch and acc + e.size > piece:
+                    self._restore_batch(batch, no_attr)
+                    batch, acc = [], 0
+                batch.append((path, e))
+                acc += e.size
+        self._restore_batch(batch, no_attr)
+        if not no_attr:   # after their contents, deepest first, so writing a file does not move a directory's mtime
+            for path, e in reversed(dirs):
+                _apply_attrs(path, e)
+
+    def _read_file_sparse(self, what: list[tuple[str, "FileEntry"]], pos: list[int], n: list[int]):
+        """One plan, one fetch and one pbsgpu_reader_read_file_sparse of ranges of files -> per range (extents, packed)."""
+        fo, fs = [e.payload_offset for _, e in what], [e.size for _, e in what]
+        chunks, digests = self._reader.plan_file_sparse(fo, fs, pos, n)
+        blobs = {int(c): self._source(bytes(d)) for c, d in zip(chunks, digests)}
+        status, data, _ = self._reader.read_file_sparse(fo, fs, pos, n, blobs)
+        for (path, e), s in zip(what, status):
+            if s != _lib.DEC_OK:
+                raise IOError(f"transfer: restore of {path} (payload offset {e.payload_offset}, {e.size} bytes): "
+                              f"{_DEC_NAMES.get(int(s), int(s))}")
+        return data
+
+    def _restore_batch(self, batch, no_attr: bool) -> None:
+        if not batch:
+            return
+        data = self._read_file_sparse(batch, [0] * len(batch), [e.size for _, e in batch])
+        for (path, e), (extents, packed) in zip(batch, data):
+            fd = os.open(path, os.O_CREAT | os.O_TRUNC | os.O_WRONLY, 0o666)
+            try:
+                _write_extents(fd, extents, packed)
+                os.ftruncate(fd, e.size)
+            finally:
+                os.close(fd)
+            if not no_attr:
+                _apply_attrs(path, e)
+
+    def _restore_large(self, path: str, e: "FileEntry", piece: int, no_attr: bool) -> None:
+        fd = os.open(path, os.O_CREAT | os.O_TRUNC | os.O_WRONLY, 0o666)
+        try:
+            for lo in range(0, e.size, piece):
+                (extents, packed), = self._read_file_sparse([(path, e)], [lo], [min(piece, e.size - lo)])
+                _write_extents(fd, extents, packed)
+            os.ftruncate(fd, e.size)
+        finally:
+            os.close(fd)
+        if not no_attr:
+            _apply_attrs(path, e)
+
     def Close(self) -> None:
         self._reader.close()
         if self._crypt is not None:
@@ -473,6 +550,79 @@ class PayloadReader:
 
     def __exit__(self, *a):
         self.Close()
+
+
+@dataclass
+class DirEntry:
+    """A directory of PayloadReader.RestoreFiles: path relative to the root, st_mode, mtime in seconds."""
+    path: str
+    mode: int
+    mtime: int
+
+
+@dataclass
+class FileEntry:
+    """A regular file of PayloadReader.RestoreFiles: path, st_mode, mtime in seconds, the payload offset of its
+    PAYLOAD header (what the mpxar PAYLOAD_REF stores) and its size."""
+    path: str
+    mode: int
+    mtime: int
+    payload_offset: int
+    size: int
+
+
+@dataclass
+class SymlinkEntry:
+    """A symlink of PayloadReader.RestoreFiles: path and target."""
+    path: str
+    target: str
+
+
+def _restore_path(root: str, rel: str) -> str:
+    """root/rel, refusing a path that leaves root."""
+    parts = rel.replace(os.sep, "/").split("/")
+    if os.path.isabs(rel) or ".." in parts:
+        raise ValueError(f"transfer: restore path {rel!r} leaves the target directory")
+    return os.path.join(root, rel)
+
+
+def _should_update(path: str, e: FileEntry, no_attr: bool) -> bool:
+    """The reference's shouldUpdateFile (internal/pxar/restore.go) for a regular file: rewrite it unless a regular file of the
+    entry's size, and (unless no_attr) its mtime in seconds, is already there."""
+    try:
+        st = os.lstat(path)
+    except FileNotFoundError:
+        return True
+    if stat.S_ISDIR(st.st_mode) or stat.S_ISLNK(st.st_mode) or st.st_size != e.size:
+        return True
+    return not no_attr and int(st.st_mtime) != int(e.mtime)
+
+
+def _restore_symlink(path: str, target: str) -> None:
+    """restoreSymlink: keep a symlink that already points at target, replace one that points elsewhere."""
+    try:
+        if os.readlink(path) == target:
+            return
+        os.remove(path)
+    except OSError:
+        pass
+    os.symlink(target, path)
+
+
+def _apply_attrs(path: str, e) -> None:
+    """applyMeta's permission bits and mtime (atime = mtime)."""
+    os.chmod(path, e.mode & 0o777)
+    os.utime(path, (e.mtime, e.mtime))
+
+
+def _write_extents(fd: int, extents, packed: bytes) -> None:
+    """One os.pwrite per (offset, length) extent of the packed bytes."""
+    view, at = memoryview(packed), 0
+    for eo, el in extents:
+        done = 0
+        while done < el:
+            done += os.pwrite(fd, view[at + done: at + el], eo + done)
+        at += el
 
 
 def restore_image(engine: Engine, fidx: bytes, chunk_source: Callable[[bytes], bytes], fd: int,
@@ -498,13 +648,7 @@ def restore_image(engine: Engine, fidx: bytes, chunk_source: Callable[[bytes], b
                     bad = [f"chunk {int(c)} ({bytes(d).hex()})" for c, d, s in zip(chunks, digests, bst) if s != _lib.DEC_OK]
                     where = bad[0] if bad else f"the slice at {off}"
                     raise IOError(f"transfer: image {where}: {_DEC_NAMES.get(int(status[0]), int(status[0]))}")
-                extents, packed = data[0]
-                view, at = memoryview(packed), 0
-                for eo, el in extents:
-                    done = 0
-                    while done < el:
-                        done += os.pwrite(fd, view[at + done: at + el], eo + done)
-                    at += el
+                _write_extents(fd, *data[0])
             os.ftruncate(fd, size)
         finally:
             reader.close()
